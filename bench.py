@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — UNet denoise steps/sec of the DiffSensei sampling loop on B200 (BASELINE.json metric).
+"""bench.py — UNet denoise steps/sec of the DiffSensei sampling loop on H100 (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # this repo's engine (one process per GPU)
     python bench.py --impl reference --gpus N --steps K --warmup W   # the reference's CPU path on the host cores
@@ -11,8 +11,9 @@ of the SDXL + IP topology (2.9 B params; no checkpoints offline).  N > 1: every 
 (cfg4 = bs 32 over 8 GPUs), no per-step collective; one NCCL all-gather of the final latents outside the timed
 region.  Timing: CUDA events on the launching stream, barrier + synchronize on both sides, max over ranks.
 
-Printed JSON line (rank 0): see the contract in the task statement; extra keys `roofline` (dominant kernel: the
-tcgen05 GEMM at the FF1/GEGLU shape, timed live with CUDA events, against MEASURED_PEAKS.json), `roofline_family`
+Printed JSON line (rank 0): metric, value, unit, steps, warmup and the keys below; `roofline` (dominant kernel: the
+wgmma GEMM at the FF1/GEGLU shape, timed live with CUDA events, against MEASURED_PEAKS.json if present, else the H100
+SXM data-sheet figures), `roofline_family`
 (the same kernel time-weighted over the step's real shape census), `roofline_gn` / `roofline_attn` (the two
 north-star kernels), `roofline_chain` (the GEMM kernel in chain mode: the four linears between two attention kernels as
 one launch), `roofline_cross` (fused text+IP cross-attention against its byte floor), `panel` (MEASURED
@@ -21,6 +22,8 @@ without the hoisted K|V projections), `cfg1_gpu` + `cpu_baseline.cfg1_measured` 
 `gpu_library_baseline` (the torch/cuBLAS/cuDNN/SDPA stack the reference would dispatch — stated, not the product),
 `cpu_baseline`, `e2e`, `clocks`.  `--config cfg1|cfg2|cfg3|cfg5` selects the BASELINE workload (default cfg2, the
 one the metric is quoted on); the reference arm (`--impl reference`) imports only `oracle/`, never the product.
+`--dump-outputs DIR` writes the latents the timed loop produced in its last step (all ranks, in panel order) as
+DIR/latents_<group>.npy (float32).
 """
 from __future__ import annotations
 
@@ -54,11 +57,12 @@ def measured_peaks():
         return {"hbm_gbs": p["hbm_gbs"], "bf16_tflops": p["bf16_tflops"],
                 "bf16_tflops_sustained": p.get("bf16_tflops_sustained", p["bf16_tflops"]), "source": "measured"}
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+        # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s — a ceiling, not a measured rate
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -169,20 +173,10 @@ def event_time_ms(fn, iters, stream_sync=True):
 
 
 # ------------------------------------------------------------------------------------------------ kernel rooflines
-def ncu_traffic():
-    """DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum) of the roofline kernels, from the
-    committed `ncu --set full` capture of tools/profile_kernels.py (profiles/ncu_traffic.json; null if absent)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            return json.load(f)
-    except Exception:
-        return {}
-
-
 def kernel_rooflines(ds, peaks, device):
     """The dominant kernel and the two north-star kernels, each timed alone with CUDA events on the launching
     stream: >= 3 warm-ups, then ROUNDS back-to-back launches that rotate over SETS disjoint input/output buffer
-    sets whose total footprint exceeds the 126 MB L2 (so no launch finds its operands cached, and the host's
+    sets whose total footprint exceeds the 50 MB L2 (so no launch finds its operands cached, and the host's
     per-launch enqueue latency — ~10 us through ctypes — is hidden behind queued work instead of being billed to
     a 30 us kernel).  Reported against the measured BURST peaks (kernel timed alone)."""
     ops = ds.ops
@@ -204,8 +198,7 @@ def kernel_rooflines(ds, peaks, device):
         return e0.elapsed_time(e1) / (rounds * len(calls))
 
     out = {}
-    traffic = ncu_traffic()
-    # dominant kernel: gemm_bf16_tcgen05 at the level-2 FF1/GEGLU shape (60 launches per step, 22.5 of 54.8 TFLOP)
+    # dominant kernel: gemm_bf16_wgmma at the level-2 FF1/GEGLU shape (60 launches per step, 22.5 of 54.8 TFLOP)
     M, N, K = 8192, 10240, 1280
     sets = []
     for i in range(3):                                   # 3 x (21 + 26 + 42 MB) = 267 MB > L2
@@ -216,9 +209,9 @@ def kernel_rooflines(ds, peaks, device):
     b = torch.zeros(N, device=device)
     ms = timed([(lambda s=s: ops.gemm(s[0], s[1], b, epilogue=ops.EPI_GEGLU, out=s[2])) for s in sets], 4)
     flops = 2.0 * M * N * K
-    out["roofline"] = {"kernel": "gemm_bf16_tcgen05<256,2> FF1+GEGLU M8192 N10240 K1280", "bound": "tensor",
+    out["roofline"] = {"kernel": "gemm_bf16_wgmma<256> FF1+GEGLU M8192 N10240 K1280", "bound": "tensor",
                        "achieved": round(flops / ms / 1e9, 1), "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
-                       "frac": round(flops / ms / 1e9 / peaks["bf16_tflops"], 4), "traffic": traffic.get("gemm_ff1"),
+                       "frac": round(flops / ms / 1e9 / peaks["bf16_tflops"], 4),
                        "ms_per_launch": round(ms, 4), "peak_source": peaks["source"] + " burst (kernel timed alone)",
                        "algorithmic_GFLOP": round(flops / 1e9, 1)}
     del sets
@@ -243,11 +236,10 @@ def kernel_rooflines(ds, peaks, device):
                      ((None,) + W[3], dict(ln_stats=st[1], ln_colsum=csq, zero_rows=st[0], out=qkv))])
     ms = timed([(lambda s=s: ops.gemm_chain(s)) for s in sets], 4)
     flops = 2.0 * M * (C4 * C4 + 8 * C4 * C4 + 4 * C4 * C4 + 3 * C4 * C4)
-    out["roofline_chain"] = {"kernel": "gemm_bf16_tcgen05<256,2,chain> attn2.to_out>ff.net.0>ff.net.2>to_qkv, M8192 "
+    out["roofline_chain"] = {"kernel": "gemm_bf16_wgmma<256,chain> attn2.to_out>ff.net.0>ff.net.2>to_qkv, M8192 "
                                        "C1280 (4 linears, one launch)", "bound": "tensor",
                              "achieved": round(flops / ms / 1e9, 1), "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
                              "frac": round(flops / ms / 1e9 / peaks["bf16_tflops"], 4),
-                             "traffic": traffic.get("gemm_chain"),
                              "ms_per_launch": round(ms, 4), "algorithmic_GFLOP": round(flops / 1e9, 1)}
     del sets
     # fused GroupNorm+SiLU at (8, 128, 128, 320): algorithmic bytes = read x + write y.  In the step the statistics
@@ -264,13 +256,13 @@ def kernel_rooflines(ds, peaks, device):
     out["roofline_gn"] = {"kernel": "gn_apply2_kernel (8,128,128,320) bf16: GroupNorm+SiLU from producer-epilogue "
                                     "channel statistics, one pass", "bound": "hbm",
                           "achieved": round(gb / (ms * 1e-3), 1), "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                          "frac": round(gb / (ms * 1e-3) / peaks["hbm_gbs"], 4), "traffic": traffic.get("gn_apply"),
+                          "frac": round(gb / (ms * 1e-3) / peaks["hbm_gbs"], 4),
                           "ms_per_launch": round(ms, 4), "algorithmic_MB": round(gb * 1e3, 1)}
     ms2 = timed([(lambda s=s: ops.groupnorm_silu(s[0], ga, be, 32, 1e-5, True, out=s[1], stats=s[3])) for s in sets], 4)
     out["roofline_gn_two_pass"] = {"kernel": "chan_stats_kernel + gn_apply2_kernel (8,128,128,320) bf16, stand-alone",
                                    "bound": "hbm", "achieved": round(gb / (ms2 * 1e-3), 1), "peak": peaks["hbm_gbs"],
                                    "unit": "GB/s", "frac": round(gb / (ms2 * 1e-3) / peaks["hbm_gbs"], 4),
-                                   "traffic": traffic.get("gn"), "ms_per_launch": round(ms2, 4),
+                                   "ms_per_launch": round(ms2, 4),
                                    "algorithmic_MB": round(gb * 1e3, 1)}
     del sets
     # fused self-attention at level 1: B=8, N=4096, 10 heads (4*N^2*C*B flops)
@@ -281,9 +273,9 @@ def kernel_rooflines(ds, peaks, device):
                      torch.empty(B, Nn, heads * 64, dtype=bf, device=device)))
     ms = timed([(lambda s=s: ops.attention_self(s[0], heads, out=s[1])) for s in sets], 4)
     flops = 4.0 * Nn * Nn * heads * 64 * B
-    out["roofline_attn"] = {"kernel": "flash_attn_v5_kernel B8 N4096 h10 d64", "bound": "tensor",
+    out["roofline_attn"] = {"kernel": "attn_wgmma_kernel (self) B8 N4096 h10 d64", "bound": "tensor",
                             "achieved": round(flops / ms / 1e9, 1), "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
-                            "frac": round(flops / ms / 1e9 / peaks["bf16_tflops"], 4), "traffic": traffic.get("flash"),
+                            "frac": round(flops / ms / 1e9 / peaks["bf16_tflops"], 4),
                             "ms_per_launch": round(ms, 4), "algorithmic_GFLOP": round(flops / 1e9, 1)}
     del sets
     # fused text + masked-IP cross-attention at level 1 (B8 N4096 h10): FLOP-light (157 keys) -> bounded by moving Q in
@@ -297,10 +289,10 @@ def kernel_rooflines(ds, peaks, device):
     ms = timed([(lambda s=s: ops.attention_cross_ip(s[0], s[1], s[2], bb, heads, 1.0, 0.6, 16, 16, out=s[3]))
                 for s in sets], 4)
     gb = 4.0 * B * Nn * C / 1e9
-    out["roofline_cross"] = {"kernel": "cross_ip_attn kernel B8 N4096 h10 (77 text + 80 IP keys, bbox mask in-kernel)",
+    out["roofline_cross"] = {"kernel": "attn_wgmma_kernel (cross+IP) B8 N4096 h10 (77 text + 80 IP keys, bbox mask in-kernel)",
                              "bound": "hbm", "achieved": round(gb / (ms * 1e-3), 1), "peak": peaks["hbm_gbs"],
                              "unit": "GB/s", "frac": round(gb / (ms * 1e-3) / peaks["hbm_gbs"], 4),
-                             "traffic": traffic.get("cross"), "ms_per_launch": round(ms, 4),
+                             "ms_per_launch": round(ms, 4),
                              "algorithmic_MB": round(gb * 1e3, 1),
                              "flops_frac_of_tensor_peak": round(4.0 * Nn * 157 * C * B / ms / 1e9 / peaks["bf16_tflops"], 4)}
     return out
@@ -467,7 +459,7 @@ def run_reference(args):
 # ------------------------------------------------------------------------------------------------ GPU-library baseline
 @torch.no_grad()
 def library_baseline(dev, steps=3, warmup=2, log=lambda *a: None):
-    """NOT the product path and not a target: the oracle modules in bf16 on the B200 with
+    """NOT the product path and not a target: the oracle modules in bf16 on the H100 with
     ``F.scaled_dot_product_attention`` — the cuBLAS / cuDNN / flash-attention kernels the reference itself would
     dispatch on a GPU (SURVEY §2.1), including its Python mask builder with its host syncs — timed for the cfg2 step
     so that "matches or beats the path the reference actually runs" has a measured denominator."""
@@ -523,7 +515,7 @@ def library_baseline(dev, steps=3, warmup=2, log=lambda *a: None):
 
 # ------------------------------------------------------------------------------------------------ our arm
 def family_roofline(ds, stepper, peaks, reps=2):
-    """Time-weighted roofline of the tcgen05 GEMM family over the REAL shape census of one step: every ds_gemm_bf16 /
+    """Time-weighted roofline of the wgmma GEMM family over the REAL shape census of one step: every ds_gemm_bf16 /
     ds_gemm_chain / ds_conv3x3_nhwc launch of an eager step is bracketed by CUDA events; achieved = sum(2*M*N*K) /
     sum(time)."""
     ops = ds.ops
@@ -596,7 +588,7 @@ def family_roofline(ds, stepper, peaks, reps=2):
     ach = tot_fl / tot_ms / 1e9
     worst = sorted(((k, d[2] / (d[1] / d[0]) / 1e9, d[1] / reps) for k, d in agg.items() if d[1] / reps > 0.25),
                    key=lambda x: x[1])[:4]
-    return {"kernel": "gemm_bf16_tcgen05 family (all ds_gemm_bf16 / ds_gemm_chain / ds_conv3x3_nhwc launches of one "
+    return {"kernel": "gemm_bf16_wgmma family (all ds_gemm_bf16 / ds_gemm_chain / ds_conv3x3_nhwc launches of one "
                       "cfg2 step)",
             "bound": "tensor", "achieved": round(ach, 1), "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
             "frac": round(ach / peaks["bf16_tflops"], 4),
@@ -662,6 +654,10 @@ def run_ours(args):
     with ClockSampler(local) as clk:
         ms = event_time_ms(lambda i: step_all(args.warmup + i), args.steps)
         barrier()
+    if args.dump_outputs:                         # the whole batch in panel order, as a caller receives it
+        lats = [parallel.gather_latents(st.latents_nchw(), [g[0]] * world) for st, g in zip(steppers, groups)]
+        if rank == 0:
+            dump_outputs(args.dump_outputs, lats)
     ms = parallel.max_over_ranks(ms, dev)
     steps_per_sec = world * 1e3 / ms
     clocks = clk.summary()
@@ -814,7 +810,7 @@ def run_ours(args):
                            "parallelism": f"dp{world}: one global batch of {bs_total * world} panels, contiguous shards of "
                                           f"{bs_total} per GPU (parallel.shard_range), no per-step collective, final "
                                           "latents all-gathered in panel order",
-                           "l2": "working set per step (5.8 GB weights + activations) >> 126 MB L2; no explicit flush",
+                           "l2": "working set per step (5.8 GB weights + activations) >> 50 MB L2; no explicit flush",
                            "hoisted": "text/IP K|V projections (0.86 TFLOP/step) and time embeddings are computed "
                                       "once per panel, outside the timed step (inside the measured `panel` leg)"},
                 "panels_per_sec": round(world * bs_total * 1e3 / (ms * T_STEPS), 4),
@@ -849,6 +845,15 @@ def run_ours(args):
     return 0
 
 
+def dump_outputs(out_dir: str, latents) -> None:
+    """The timed path's result of its last step — the latents of each panel group, all-gathered over the ranks in
+    panel order — as float32 .npy files, one per group ([bs * gpus, 4, h, w]; 1 MB per GPU for cfg2)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for k, lat in enumerate(latents):
+        np.save(os.path.join(out_dir, f"latents_{k}.npy"), lat.float().cpu().numpy())
+
+
 _JSON_FD = None
 
 
@@ -881,6 +886,8 @@ def main():
                     help="concurrent kernel chains per GPU (default: DS_CHAINS env, else 2)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-kernel-rooflines", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the latents of the last timed step to DIR/latents_<group>.npy (float32)")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3

@@ -1,4 +1,4 @@
-"""diffsensei_b200 — B200-native (sm_100a) engine for DiffSensei's UNet sampling loop.
+"""diffsensei_b200 — H100-native (sm_90a) engine for DiffSensei's UNet sampling loop.
 
 Public surface (mirrors the reference's, SURVEY.md §8b):
     UNetMangaEngine        <- src/models/unet.py            UNetMangaModel
@@ -10,7 +10,7 @@ Public surface (mirrors the reference's, SURVEY.md §8b):
     DiffSenseiPipeline     <- src/pipelines/pipeline_diffsensei.py  (denoise loop)
     ops                    -- tensor-level wrappers over the C ABI in include/dsengine.h
 
-Importing the package loads ``libdsengine.so`` (built in-tree for sm_100a); it fails loudly if the library is
+Importing the package loads ``libdsengine.so`` (built in-tree for sm_90a); it fails loudly if the library is
 missing, and nothing in here falls back to PyTorch compute or to the test oracle.
 """
 from . import _lib  # noqa: F401  (loads libdsengine.so or raises ImportError)

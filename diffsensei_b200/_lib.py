@@ -2,7 +2,7 @@
 
 The library is built in-tree by ``__graft_entry__.build()`` / ``make -C diffsensei_b200/csrc``.  There is no
 fallback of any kind: if the shared object is missing the import fails loudly, and on a machine without an
-sm_100 GPU every compute entry point returns DS_ERR_CUDA, which ``check`` turns into a ``DsEngineError``.
+sm_90 GPU every compute entry point returns DS_ERR_CUDA, which ``check`` turns into a ``DsEngineError``.
 """
 from __future__ import annotations
 

@@ -13,7 +13,7 @@ Same class names, constructor arguments, parameters and call signature as
 so they can be installed on a stock diffusers ``UNet2DConditionModel`` with ``set_attn_processor`` (the
 innermost drop-in seam, SURVEY.md §8b) — ``load_ip_adapter``'s ``ModuleList(unet.attn_processors.values())``
 state-dict indexing (src/models/utils.py:46-48) keeps working because both are ``nn.Module`` s with the same
-parameter names.  The arithmetic runs in libdsengine: one fused-QKV tcgen05 GEMM + the flash kernel for
+parameter names.  The arithmetic runs in libdsengine: one fused-QKV wgmma GEMM + the flash kernel for
 self-attention; for cross-attention the text / IP K|V projections (cached per conditioning tensor), ONE fused
 kernel for both softmaxes, the bbox mask and the ``scale`` blend, and the output projection with its bias
 (and optional residual) in the GEMM epilogue.  bf16, head_dim 64, 3-D hidden states — the SDXL configuration;

@@ -55,8 +55,8 @@ bool get_device(DeviceInfo* out) {
     have[dev] = true;
   }
   *out = cache[dev];
-  if (out->cc_major != 10) {
-    set_error("device compute capability %d.%d is not sm_100: libdsengine is built for sm_100a only", out->cc_major,
+  if (out->cc_major != 9 || out->cc_minor != 0) {
+    set_error("device compute capability %d.%d is not sm_90: libdsengine is built for sm_90a only", out->cc_major,
               out->cc_minor);
     return false;
   }

@@ -1,10 +1,8 @@
-// ds_common.cuh — sm_100a device primitives shared by every kernel in libdsengine.
+// ds_common.cuh — sm_90a device primitives shared by every kernel in libdsengine.
 //
-// Thin inline-PTX wrappers for the Blackwell execution model: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (TMEM alloc / mma / commit / ld) and the
-// shared-memory matrix descriptors tcgen05.mma consumes.  Nothing here is
-// derived from the reference (it ships no native code, SURVEY.md §2.1); bit
-// layouts follow the PTX ISA for sm_100a.
+// Thin inline-PTX wrappers for the Hopper execution model: mbarrier and TMA (cp.async.bulk.tensor); the warpgroup
+// MMA wrappers live in wgmma.cuh.  Nothing here is derived from the reference (it ships no native code, SURVEY.md
+// §2.1); bit layouts follow the PTX ISA for sm_90a.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -12,8 +10,6 @@
 #include <stdint.h>
 
 namespace ds {
-
-constexpr int kNumSMs = 148;
 
 // ----------------------------------------------------------------------------------------------
 // small helpers
@@ -42,8 +38,7 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 }
 
 // bf16 pack on the INTEGER pipe: round-half-up on the 16 dropped mantissa bits (differs from RNE only on exact
-// ties, no bias that matters) + one PRMT.  cvt.rn.bf16x2.f32 (F2FP) issues at the XU/MUFU rate (16/clk/SM) and was
-// the co-limiter of the exp-bound softmax loops and of GroupNorm-apply (profiles/r01_ncu_summary.md).
+// ties, no bias that matters) + one PRMT, instead of cvt.rn.bf16x2.f32, which issues at the lower XU rate.
 // Inf stays Inf, NaN stays NaN; finite inputs only lose <= 0.5 ulp(bf16).
 __device__ __forceinline__ uint32_t pack_bf16_alu(float lo, float hi) {
   const uint32_t a = __float_as_uint(lo) + 0x8000u;
@@ -53,7 +48,7 @@ __device__ __forceinline__ uint32_t pack_bf16_alu(float lo, float hi) {
 
 // ----------------------------------------------------------------------------------------------
 // Programmatic dependent launch (PDL).  A kernel launched with programmaticStreamSerializationAllowed may start
-// (and run its prologue: barrier init, TMEM alloc, tensor-map prefetch) while its predecessor in the stream / graph
+// (and run its prologue: barrier init, tensor-map prefetch) while its predecessor in the stream / graph
 // is still draining; pdl_wait() blocks until the predecessor grid has completed and its memory is visible, and must
 // precede the first global-memory access.  pdl_launch_dependents() lets OUR successor start early likewise.
 // ----------------------------------------------------------------------------------------------
@@ -69,7 +64,7 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void fence_mbar_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// generic-proxy writes (st.shared) -> visible to the async proxy (TMA / tcgen05.mma operand reads)
+// generic-proxy writes (st.shared) -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -134,250 +129,9 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
 }
 
 // ----------------------------------------------------------------------------------------------
-// CTA-pair (cluster of 2) helpers for tcgen05 cta_group::2
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {  // every thread of both CTAs
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
-  // default semantics (release at CTA scope): a cluster-scope release here costs a membar + L1 invalidate per
-  // call and throttled the peer's TMA producer loop to one stage per ~1600 cycles (profiles: gemm pair A/B)
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-// In a CTA pair the peer's shared window differs in bit 24 of the shared::cluster address; clearing it addresses
-// the LEADER's (rank 0) copy of a barrier — the 2-SM TMA variants post their bytes there.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(m), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-// the same, multicast: the box lands at `dst`'s offset in every CTA of `mask`, its bytes on the barrier of each
-// destination's pair leader
-__device__ __forceinline__ void tma_load_2d_pair_mc(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                    uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster "
-      "[%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
-      "l"(m), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                                 int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(m), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_dst, uint32_t ncols) {  // one warp in EACH CTA of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem, 128 rows in each CTA] (+)= A[smem of both CTAs, M=256] * B[smem of both CTAs, N split]; leader CTA issues
-__device__ __forceinline__ void umma_ss_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit: arrive on the barrier at this offset in BOTH CTAs of the pair once all prior MMAs completed
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(static_cast<uint16_t>(3))
-      : "memory");
-}
-
-// commit with an explicit CTA mask (clusters of two pairs)
-__device__ __forceinline__ void umma_commit_mask(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-// ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, loads
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {  // whole warp, ncols pow2 >= 32
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]; one thread issues for the whole CTA.
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// ---- "elected" variants: to be executed by a fully CONVERGED warp.  One lane (elect.sync) issues the instruction;
-// the operands are computed by all lanes in converged code, so ptxas keeps them in uniform registers.  Issuing from
-// inside an `if (lane == 0)` region instead makes ptxas wrap every tcgen05 instruction in an ELECT / BRA.U.ANY
-// "waterfall" (~50 cycles per MMA: profiles/r02_ncu_summary.md), which is what bounded the flash kernel's short
-// (32-cycle) MMAs.
-__device__ __forceinline__ void umma_ss_e(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, q;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_ts_e(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, q;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_e(uint64_t* bar) {
-  asm volatile(
-      "{\n"
-      ".reg .pred q;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n"
-      "}\n" ::"r"(smem_u32(bar))
-      : "memory");
-}
-
-// Arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed.
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: 32 lanes x 32 consecutive 32-bit columns; thread t of the warp receives lane
-// (base_lane + t).  A warp may only touch lanes [32*(warp_id%4), +32).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// registers -> TMEM (same lane/column mapping as tmem_ld*)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-      "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (64-bit) for tcgen05.mma operands, 128-byte swizzle.
-//   bits [0,14)  start address >> 4          bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4     bits [46,48) version = 1 (sm_100)
-//   bits [61,64) layout type: 2 = SWIZZLE_128B
-// K-major operand ([rows][64 bf16] tile, 128 B per row, written by TMA with SWIZZLE_128B):
-//   8-row groups are 1024 B apart (SBO); LBO is unused for swizzled K-major layouts.
-//   Stepping K by 16 elements (one UMMA) advances the start address by 32 B.
-// MN-major operand ([k rows][64 bf16] tile, the 64-wide MN extent contiguous):
-//   8 k-rows form one 1024 B swizzle atom (SBO); LBO would step to the next 64 MN elements (unused,
-//   MN <= 64 per atom here).  Stepping K by 16 rows advances the start address by 2048 B.
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
-// Instruction descriptor (32-bit) for kind::f16 with bf16 inputs and fp32 accumulation.
-//   [4,6) D format (1 = f32)  [7,10) A format (1 = bf16)  [10,13) B format (1 = bf16)
-//   [15] A major (0 = K)      [16] B major (0 = K, 1 = MN)
-//   [17,23) N >> 3            [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
-
-// ----------------------------------------------------------------------------------------------
 // math
 // ----------------------------------------------------------------------------------------------
-// x * sigmoid(x) with two MUFU ops (ex2 + rcp); a full-precision divide made gn_apply XU/issue-bound (profiles/r01)
+// x * sigmoid(x) with two MUFU ops (ex2 + rcp) instead of a full-precision divide
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 // x * sigmoid(x) = 0.5 x (1 + tanh(x/2)) with ONE MUFU op (tanh.approx, abs err ~5e-4 on tanh => |err| <= 2.5e-4 |x|,
 // below the bf16 rounding of the result for |x| < 16).  Used where the op is otherwise XU-bound (GroupNorm apply).
@@ -409,8 +163,8 @@ __device__ __forceinline__ float gelu_erf_fast(float x) {
 
 // erf-GELU as x * sigmoid(2 k (x + a x^3 + b x^5)) with (k, a, b) fitted to x * Phi(x): |abs err| <= 2.6e-5 for every
 // x (the classic tanh form with b = 0 is 4.7e-4), i.e. >= 10x below the bf16 rounding of the GEGLU product it feeds.
-// 7 FP + 2 MUFU instead of the 15 FP + 2 MUFU of gelu_erf_fast: the GEGLU epilogue was the co-limiter of the FF1
-// GEMM (tensor pipe 66 %, profiles/r01_ncu_flash_v3.md).  The quintic changes sign beyond |x| ~ 11: clamp to +-10
+// 7 FP + 2 MUFU instead of the 15 FP + 2 MUFU of gelu_erf_fast, which keeps the GEGLU epilogue of the FF1 GEMM
+// short.  The quintic changes sign beyond |x| ~ 11: clamp to +-10
 // (sigmoid is saturated to 1 - 3e-9 there).
 __device__ __forceinline__ float gelu_sig5(float x) {
   const float xc = fminf(fmaxf(x, -10.0f), 10.0f);

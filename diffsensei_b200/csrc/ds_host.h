@@ -18,7 +18,7 @@ extern std::atomic<uint64_t> g_launches;
 inline void count_launch(uint64_t n = 1) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
 // Device properties of the current device (cached). Fails (returns false + error text) when the
-// current device is not an sm_100 part — there is no fallback path.
+// current device is not an sm_90 part — there is no fallback path.
 struct DeviceInfo {
   int num_sms;
   int cc_major;

@@ -1,6 +1,6 @@
 // encoder_kernels.cu — what the conditioning encoders need beyond the UNet's kernels (SURVEY.md §8f ranks 2-3:
 // the CLIP ViT-H and Magi ViT-MAE image encoders of prepare_ip_image_embeds, src/pipelines/pipeline_diffsensei.py:125-128,
-// and the two SDXL CLIP text encoders of encode_prompt, :232-245).  Their linears / MLPs run on the tcgen05 GEMM
+// and the two SDXL CLIP text encoders of encode_prompt, :232-245).  Their linears / MLPs run on the wgmma GEMM
 // (ds_gemm_bf16, bias / GELU / quick-GELU / residual epilogues) and their LayerNorms on ds_layernorm; this file adds
 //   ds_attention_small : softmax(scale * Q K^T [+ causal mask]) V for SHORT sequences (<= 320 keys) and any head
 //                        width that is a multiple of 8 up to 128 — 77 text tokens (causal), 197 / 257 image tokens, heads

@@ -14,8 +14,7 @@ namespace ds {
 __global__ void conv_in_kernel(const uint2* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
                                uint4* __restrict__ out, int H, int W, int Cout, int grp_per_cta) {
   // Work item = 4 consecutive output pixels of one row x 8 output channels: every weight read from shared memory
-  // feeds 4 FMAs (the one-pixel version re-read all 36 x 8 weights per output vector and was bound by the
-  // shared-memory port: 403 us for 84 MB of output).
+  // feeds 4 FMAs (a one-pixel version would re-read all 36 x 8 weights per output vector from shared memory).
   extern __shared__ float sw[];  // [36][Cout] then bias [Cout]
   float* sb = sw + 36 * Cout;
   for (int i = threadIdx.x; i < 36 * Cout; i += blockDim.x) {
@@ -221,7 +220,7 @@ extern "C" int ds_conv_in_3x3(const void* x, const float* w, const float* bias, 
 }
 
 // im2col of the 4-channel latent for a 3x3 / pad 1 conv: A[b*HW + p][tap*4 + c] = x[b][y+r-1][x+s-1][c] (zero outside
-// the image), taps 0..8 = (r, s) row-major, columns 36..63 zero -> one K = 64 block of the tcgen05 GEMM.  16 threads
+// the image), taps 0..8 = (r, s) row-major, columns 36..63 zero -> one K = 64 block of the wgmma GEMM.  16 threads
 // per pixel, 8 bytes each: every 128-byte row of A is one coalesced store.
 __global__ void im2col_latent_kernel(const uint2* __restrict__ x, uint2* __restrict__ a, int H, int W, long long total) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;  // (pixel, tap slot)

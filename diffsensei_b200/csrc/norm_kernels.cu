@@ -4,7 +4,7 @@
 // coalesced decomposition is by PIXEL RANGE, not by group: a CTA streams a contiguous run of pixels (all
 // channels, 16-byte vectors, every thread pinned to the same 8 channels).
 //   statistics : per-(sample, CHANNEL) {sum, sum of squares} in fp64, [B][C][2].  Normally they come for free from
-//                the epilogue of the GEMM / conv that PRODUCED the tensor (gemm_tcgen05.cu, `chan_stats`); tensors
+//                the epilogue of the GEMM / conv that PRODUCED the tensor (gemm_wgmma.cu, `chan_stats`); tensors
 //                without such a producer (conv_in output, unaligned shapes) get them from chan_stats_kernel.
 //                Per-channel (not per-group) sums make them composable: the statistics of torch.cat([h, skip], 1)
 //                are the two tensors' statistics side by side, whatever the group boundaries of the result.
@@ -410,7 +410,7 @@ extern "C" int ds_groupnorm_apply(const void* x1, const double* stats1, int C1, 
   static const int tt = gn_env("DS_GN_THREADS", 256, 64, 1024);
   static const int unroll = gn_env("DS_GN_UNROLL", 8, 4, 8);
   static const int max_occ = gn_env("DS_GN_OCC", 8, 1, 16);
-  static const int l2_hint = gn_env("DS_GN_L2HINT", 0, 0, 1);  // measured: plain loads 35.4 us vs evict_first 36.1 us
+  static const int l2_hint = gn_env("DS_GN_L2HINT", 0, 0, 1);  // default: plain loads
   GnPlan pl;
   DS_REQUIRE(gn_plan(B, HW, C, tt, unroll, &pl), "ds_groupnorm_apply: tensor too large");
   const size_t smem = static_cast<size_t>(C) * 2 * sizeof(double) + static_cast<size_t>(groups) * 2 * sizeof(float);

@@ -1,11 +1,11 @@
 // vae_kernels.cu — the three small kernels the AutoencoderKL decoder needs beyond the UNet's (everything else in the
-// decoder — 3x3 convs, GroupNorm+SiLU, linears, nearest upsample — runs on the kernels in gemm_tcgen05.cu /
+// decoder — 3x3 convs, GroupNorm+SiLU, linears, nearest upsample — runs on the kernels in gemm_wgmma.cu /
 // norm_kernels.cu / glue_kernels.cu):
 //   ds_latent_pointwise : latents / scaling_factor -> post_quant_conv (1x1, 4 -> 4) -> NHWC bf16
 //                         (src/pipelines/pipeline_diffsensei.py:346-361; diffusers AutoencoderKL.decode)
 //   ds_softmax_rows     : P = softmax(scale * S) row-wise, fp32 scores in, bf16 probabilities out — the mid-block
 //                         attention of the decoder has ONE head of width 512 over all H*W tokens (no flash kernel for
-//                         that head size: QK^T and PV run as plain tcgen05 GEMMs with this kernel between them)
+//                         that head size: QK^T and PV run as plain wgmma GEMMs with this kernel between them)
 //   ds_image_postprocess: (x / 2 + 0.5).clamp(0, 1), NHWC bf16 -> NCHW fp32 (VaeImageProcessor.postprocess/denormalize)
 // All three are HBM-bound one-pass kernels.
 #include "ds_common.cuh"

@@ -1,4 +1,4 @@
-"""Conditioning encoders on the B200 kernels (SURVEY.md §8f ranks 2 and 3).
+"""Conditioning encoders on the H100 kernels (SURVEY.md §8f ranks 2 and 3).
 
 What ``DiffSenseiPipeline.__call__`` runs before the denoise loop (src/pipelines/pipeline_diffsensei.py):
   * ``encode_prompt`` (:232-245, inherited from diffusers' StableDiffusionXLPipeline): the two SDXL text encoders —
@@ -11,7 +11,7 @@ What ``DiffSenseiPipeline.__call__`` runs before the denoise loop (src/pipelines
     (``pixel_values`` in: the PIL resize / normalise of the image processors is host-side preprocessing)
 
 All four are pre-LayerNorm transformer encoders; one stack implementation serves them: LayerNorm (ds_layernorm) ->
-fused q|k|v projection (tcgen05 GEMM + bias) -> short-sequence attention (ds_attention_small: 77 causal text tokens,
+fused q|k|v projection (wgmma GEMM + bias) -> short-sequence attention (ds_attention_small: 77 causal text tokens,
 197 / 257 image tokens, head widths 64 and 80) -> output projection + residual (GEMM epilogue) -> LayerNorm -> MLP
 (GELU / quick-GELU in the first GEMM's epilogue, residual in the second's).  They load the Hugging Face
 ``transformers`` state dicts unchanged, and are tested against those very classes executed on the same weights

@@ -209,7 +209,7 @@ def zero_(t: torch.Tensor) -> torch.Tensor:
 
 
 def gemm(*a, **kw) -> torch.Tensor:
-    """out[..., Nout] = epilogue(a[..., K] @ w[N, K]^T) on tcgen05 — one launch; see ``_gemm_args`` for the
+    """out[..., Nout] = epilogue(a[..., K] @ w[N, K]^T) on wgmma — one launch; see ``_gemm_args`` for the
     arguments."""
     args, out = _gemm_args(*a, **kw)
     check(lib.ds_gemm_bf16(C.byref(args), _stream()), "ds_gemm_bf16")
@@ -224,6 +224,10 @@ def gemm_chain_max() -> int:
     return int(lib.ds_gemm_chain_max())
 
 
+# A chain launch spins on dependency counters across its CTAs, so all of them must be resident: it needs the whole GPU.
+# DenoiseStepper turns chains off while it runs kernels of several streams concurrently (separate launches instead,
+# bit-identical results).
+GEMM_CHAINS = True
 _CHAIN_SLOTS = 72          # torch hands out streams from two pools of 32 per device (+ the default stream)
 
 
@@ -264,7 +268,7 @@ def gemm_chain(calls, min_links: int = 2, enable: bool = True) -> list:
             a = (prepared[-1][1],) + tuple(a[1:])
         prepared.append(_gemm_args(*a, **kw))
     M = prepared[0][0].M
-    ok = enable and min_links <= len(prepared) <= gemm_chain_max() and 128 < M <= _CHAIN_ROW_BLOCKS * 128
+    ok = enable and GEMM_CHAINS and min_links <= len(prepared) <= gemm_chain_max() and 128 < M <= _CHAIN_ROW_BLOCKS * 128
     for i, (g, _) in enumerate(prepared):
         ok = ok and g.M == M and not g.out_fp32 and not g.chan_stats and not g.a2
         ok = ok and (g.N // 2 if g.epilogue == EPI_GEGLU else g.N) % 8 == 0
@@ -434,7 +438,7 @@ def conv_in(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], out:
 
 def im2col_latent(x: torch.Tensor) -> torch.Tensor:
     """3x3 / pad 1 patches of the 4-channel latent: NHWC bf16 [B,H,W,4] -> [B*H*W, 64] bf16 (36 real columns), the A
-    operand of conv_in as a K = 64 tcgen05 GEMM against ``weights.pack_conv_in``."""
+    operand of conv_in as a K = 64 wgmma GEMM against ``weights.pack_conv_in``."""
     _req(x, bf16, "im2col_latent.x", 4)
     B, H, W, Cin = x.shape
     if Cin != 4:

@@ -1,4 +1,4 @@
-"""DiffSenseiPipeline — the sampling loop of the reference pipeline on the B200 engine.
+"""DiffSenseiPipeline — the sampling loop of the reference pipeline on the H100 engine.
 
 Mirrors ``src/pipelines/pipeline_diffsensei.py``:
   * ``register_manga_modules`` (:73-79), ``check_inputs`` (:81-102, same ValueErrors), ``set_ip_scale`` (:172-178)
@@ -325,10 +325,9 @@ class DenoiseStepper:
         self._host_in = None
         # Independent batch rows (the CFG halves, the panels) CAN run as `chains` concurrent kernel chains on separate
         # streams (graph branches), meant to back-fill the idle SMs of every kernel's last wave (flops-weighted tile
-        # efficiency of one cfg2 step: 0.80, tools/shape_census.py).  MEASURED on B200 (cfg2, graph replay): 1 chain
-        # 67.6 ms/step, 2 chains 76.7, 4 chains 76.9 — the half-size launches lose more to their own tails and
-        # per-launch fixed costs than back-filling recovers (1-CTA/SM persistent GEMMs cannot co-reside).  Default
-        # therefore stays 1; DS_CHAINS / `chains=` keep the path for var-res buckets whose panels differ in size.
+        # efficiency of one cfg2 step: 0.80, tools/shape_census.py).  Half-size launches pay their own tails and
+        # per-launch fixed costs, and the 1-CTA/SM persistent GEMMs cannot co-reside, so the default is 1;
+        # DS_CHAINS / `chains=` keep the path for var-res buckets whose panels differ in size.
         B2 = self.model_in.shape[0]
         want = int(os.environ.get("DS_CHAINS", "1")) if chains is None else int(chains)
         self.chains = max(1, min(want, B2))
@@ -392,8 +391,11 @@ class DenoiseStepper:
         else:
             main = torch.cuda.current_stream(self.dev)
             eps = self._eps
-            prev_splitk, ops.SPLITK = ops.SPLITK, False   # one split-K workspace per device: never shared by
-            try:                                           # kernels that may overlap (also keeps it out of the capture)
+            # one split-K workspace per device: never shared by kernels that may overlap (also keeps it out of the
+            # capture); GEMM chains need every SM resident, which concurrent streams do not guarantee
+            prev_splitk, ops.SPLITK = ops.SPLITK, False
+            prev_chains, ops.GEMM_CHAINS = ops.GEMM_CHAINS, False
+            try:
                 for k, (s, e) in enumerate(self._parts):
                     st = main if k == 0 else self._side[k - 1]
                     if k:
@@ -406,6 +408,7 @@ class DenoiseStepper:
                     main.wait_stream(st)                       # join before the CFG blend needs both halves
             finally:
                 ops.SPLITK = prev_splitk
+                ops.GEMM_CHAINS = prev_chains
         ops.cfg_ddim_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance)   # :332-337 (+ :315 of next)
 
     @torch.no_grad()

@@ -3,7 +3,7 @@
 Mirrors ``src/models/resampler.py`` (Resampler :79-144, PerceiverAttention :32-76, FeedForward :11-18): same
 constructor keywords as ``scripts/demo/gradio_wo_mllm.py:174-185``, same ``forward(x, magi_image_embeds)``
 -> (bsz, num_dummy + max_num_ips*num_queries, output_dim), ``dtype()`` is a METHOD (resampler.py:143-144),
-same state-dict keys.  All arithmetic goes through libdsengine: tcgen05 GEMMs (the GELU of the FF fused into
+same state-dict keys.  All arithmetic goes through libdsengine: wgmma GEMMs (the GELU of the FF fused into
 the first GEMM's epilogue, residual adds into the second's / to_out's), ds_layernorm, and the flash kernel for
 the 16 x 274 perceiver attention.  Runs twice per panel, outside the denoise loop (pipeline :133,135).
 """

@@ -1,4 +1,4 @@
-"""UNetMangaEngine — the B200-native denoiser behind the reference's ``UNetMangaModel`` surface.
+"""UNetMangaEngine — the H100-native denoiser behind the reference's ``UNetMangaModel`` surface.
 
 Mirrors ``src/models/unet.py`` of jianzongwu/DiffSensei:
   * ``set_manga_modules(max_num_ips, num_vision_tokens, max_num_dialogs)``   (:44-86)
@@ -6,7 +6,7 @@ Mirrors ``src/models/unet.py`` of jianzongwu/DiffSensei:
   * ``forward(sample, timestep, encoder_hidden_states, added_cond_kwargs, cross_attention_kwargs,
               dialog_bbox, return_dict)``                                    (:116-347)
   * ``load_state_dict`` with the reference's key names, ``.config``, ``.dtype``, ``.attn_processors``
-Every arithmetic op runs in a hand-written sm_100a kernel through the libdsengine C ABI (``ops``); torch
+Every arithmetic op runs in a hand-written sm_90a kernel through the libdsengine C ABI (``ops``); torch
 provides device memory and the stream.  Activations are bf16 NHWC inside; the NCHW <-> NHWC conversion
 happens once at each end on the 4-channel latent.
 
@@ -33,8 +33,8 @@ from .weights import (bf, colsum_bf16, fold_layernorm, fp, pack_conv3x3, pack_co
 # The linears between two attention kernels of a BasicTransformerBlock (attn1.to_out -> attn2.to_q, and attn2.to_out ->
 # ff.net.0 -> ff.net.2 -> the next block's to_qkv) run as ONE persistent launch each (ops.gemm_chain): same tiles and K
 # order as separate launches, so the UNet output only moves by the tile-width dependence of the LayerNorm statistics'
-# fp32 partial sums (last bit).  MEASURED (B200, cfg2, same box, 2 runs each): 60.43 / 60.67 ms per step with
-# separate launches, 59.74 / 59.39 ms chained (687 -> 418 launches).  DS_GEMM_CHAIN=0 restores one launch per linear.
+# fp32 partial sums (last bit).  A chain saves the launch, prologue and drain of every linear but its first.
+# DS_GEMM_CHAIN=0 restores one launch per linear.
 _CHAIN = os.environ.get("DS_GEMM_CHAIN", "1") not in ("", "0")
 # shape rule for the chains (see _transformer); DS_GEMM_CHAIN_RULE="long_rows,short_rows,short_c,long_c" overrides
 _CHAIN_LONG_MIN_ROWS, _CHAIN_SHORT_MIN_ROWS, _CHAIN_SHORT_MIN_C, _CHAIN_LONG_MIN_C = (
@@ -374,11 +374,10 @@ class UNetMangaEngine:
                                       zero_rows=st[(k + 1) % 3])
 
         # The linears between two attention kernels go to ops.gemm_chain — ONE persistent launch per run where that
-        # is faster, separate launches (same calls, same order) where it is not.  MEASURED (tools/chain_bench.py,
-        # B200): the 3/4-link run attn2.to_out -> ff.net.0 (GEGLU) -> ff.net.2 -> next attn1.to_qkv wins from
-        # M = 4096 rows up (C1280: 207 -> 197 us at M4096, 412 -> 365 at M8192; C640: 89.2 -> 87.9 at M4096, 147 -> 134
-        # at M8192) and loses 1-5 % below; the 2-link runs (proj_in -> to_qkv, attn1.to_out -> attn2.to_q) only win
-        # at C1280 / M8192 (60.7 -> 57.9 us) and lose 3-8 % elsewhere.
+        # is expected to be faster, separate launches (same calls, same order) elsewhere: the 3/4-link run
+        # attn2.to_out -> ff.net.0 (GEGLU) -> ff.net.2 -> next attn1.to_qkv from M = 4096 rows up, the 2-link runs
+        # (proj_in -> to_qkv, attn1.to_out -> attn2.to_q) only at C1280 / M8192 — tools/chain_bench.py measures the
+        # crossover; DS_GEMM_CHAIN_RULE moves it.
         long_run = _CHAIN and Cc >= _CHAIN_LONG_MIN_C and _CHAIN_LONG_MIN_ROWS <= M <= 65536
         short_run = _CHAIN and Cc >= _CHAIN_SHORT_MIN_C and _CHAIN_SHORT_MIN_ROWS <= M <= 65536
         b0 = t.blocks[0]

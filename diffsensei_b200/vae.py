@@ -1,4 +1,4 @@
-"""VaeDecoderEngine — the AutoencoderKL decoder behind ``vae.decode`` on the B200 kernels (SURVEY.md §8f rank 1).
+"""VaeDecoderEngine — the AutoencoderKL decoder behind ``vae.decode`` on the H100 kernels (SURVEY.md §8f rank 1).
 
 Mirrors what ``src/pipelines/pipeline_diffsensei.py:339-367`` uses of diffusers' ``AutoencoderKL``:
 ``vae.config.scaling_factor`` / ``force_upcast`` / ``latents_mean`` / ``latents_std``, ``vae.dtype``,
@@ -6,9 +6,9 @@ Mirrors what ``src/pipelines/pipeline_diffsensei.py:339-367`` uses of diffusers'
 ``image_processor.postprocess`` (``decode_image`` fuses the three).  Loads diffusers' AutoencoderKL state dict
 (``post_quant_conv.*`` and ``decoder.*``; ``encoder.*`` / ``quant_conv.*`` are ignored).
 
-Same kernel family as the UNet at 8x the spatial size: every 3x3 conv is the tcgen05 implicit GEMM with its GroupNorm
+Same kernel family as the UNet at 8x the spatial size: every 3x3 conv is the wgmma implicit GEMM with its GroupNorm
 statistics taken in the epilogue, every GroupNorm(+SiLU) is one read/write pass, the 1x1 shortcuts and the attention
-projections are tcgen05 GEMMs.  The mid-block attention is ONE head of width 512 over all H*W latent tokens — outside
+projections are wgmma GEMMs.  The mid-block attention is ONE head of width 512 over all H*W latent tokens — outside
 the flash kernel's head_dim 64 — so it runs per image as QK^T (fp32 scores) -> ``ds_softmax_rows`` -> PV on the same GEMM
 kernel.  The fp32-upcast rule of the reference (:340-344: the fp16 VAE overflows) is moot here: activations are
 bf16 (fp32 range), accumulation / normalisation / softmax in fp32; tolerance stated in tests/test_vae_gpu.py.
@@ -119,7 +119,7 @@ class VaeDecoderEngine:
 
     def _attention(self, x, st, pool):
         """diffusers Attention(heads=1, dim_head=C, residual_connection=True) via AttnProcessor2_0: per image
-        softmax(Q K^T / sqrt(C)) V on the tcgen05 GEMM (fp32 scores) + ds_softmax_rows."""
+        softmax(Q K^T / sqrt(C)) V on the wgmma GEMM (fp32 scores) + ds_softmax_rows."""
         a, g = self.attn, self.cfg.norm_num_groups
         B, H, W, C = x.shape
         N = H * W

@@ -1,4 +1,4 @@
-/* dsengine.h — C ABI of libdsengine.so, the sm_100a kernel library behind diffsensei_b200.
+/* dsengine.h — C ABI of libdsengine.so, the sm_90a kernel library behind diffsensei_b200.
  *
  * The reference (jianzongwu/DiffSensei) has no FFI: every kernel on its UNet sampling path is a
  * PyTorch library call.  Each entry point below therefore names the reference call site whose
@@ -13,7 +13,7 @@
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it, nothing synchronises;
  *   - no entry point allocates device memory: scratch is passed in by the caller;
  *   - return value 0 = ok, otherwise a DS_ERR_* code; ds_last_error() gives the message
- *     (thread-local).  There is no CPU fallback: on a box without an sm_100 device every compute
+ *     (thread-local).  There is no CPU fallback: on a box without an sm_90 device every compute
  *     entry point returns DS_ERR_CUDA.
  */
 #ifndef DSENGINE_H_
@@ -91,7 +91,7 @@ int ds_ip_mask(const float* bbox, float* mask, int B, int N, double aspect_ratio
                int num_dummy, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * bf16 GEMM on tcgen05 tensor cores, TMA-fed, fp32 accumulation in TMEM.      [tensor-bound]
+ * bf16 GEMM on wgmma tensor cores, TMA-fed, fp32 accumulation in registers.   [tensor-bound]
  *   out[M][Nout] = epilogue( A[M][K] * W[N][K]^T )
  * Replaces every nn.Linear on the path: attn.to_q/to_k/to_v/to_out (src/models/attention_processor.py:
  * 56,63-64,84,207,225-226,245-246,261), diffusers FeedForward/GEGLU, Transformer2D proj_in/proj_out,
@@ -117,14 +117,14 @@ int ds_ip_mask(const float* bbox, float* mask, int B, int N, double aspect_ratio
  *             bf16 outputs with 16-byte rows only.  zero_rows != NULL: the call also resets that [M][2] buffer (the first n-tile of
  *             every m-tile does it), which lets a chain of GEMMs rotate three statistics buffers without any
  *             memset node: the consumer of buffer k clears buffer k+2.
- * Split-K tail: the kernel is persistent (one CTA pair per two SMs, static round-robin over 256 x BN output tiles);
- *   when the tile count is not a multiple of the resident pairs, the tiles of the partial last round are cut along
- *   K into slices that run on different pairs, reduced in fp32 through `splitk_ws` (vector red.global.add) and
+ * Split-K tail: the kernel is persistent (one CTA per SM, static round-robin over 128 x BN output tiles);
+ *   when the tile count is not a multiple of the resident CTAs, the tiles of the partial last round are cut along
+ *   K into slices that run on different CTAs, reduced in fp32 through `splitk_ws` (vector red.global.add) and
  *   finished by whichever slice arrives last.  The caller provides a 16-byte aligned workspace that is ALL ZERO on
  *   entry (ds_gemm_splitk_ws_bytes() bytes cover every shape; the kernel leaves it all zero again) and must not be
  *   shared by GEMMs running concurrently on different streams.  NULL simply disables the feature.
  * Mixed-width schedule (default on, DS_GEMM_TAIL=0 disables): when the last round of the persistent schedule would
- *   fill less than ~45 % of the CTA pairs, the m-rows that fall into it run as 128-column units (twice as many, half
+ *   fill less than ~45 % of the CTAs, the m-rows that fall into it run as 128-column units (twice as many, half
  *   as long) appended to the 256-column units of the same launch, instead of paying a whole round for a handful of
  *   tiles.  Results are bit-identical to the plain schedule (same K order per output element).
  * Constraints: K % 8 == 0, lda % 8 == 0 (16-byte TMA strides). M, N, K tails are handled by TMA
@@ -183,19 +183,19 @@ int64_t ds_gemm_splitk_ws_bytes(void);
  * (the BasicTransformerBlock sequences attn.to_out -> attn2.to_q and attn2.to_out -> ff.net.0 -> ff.net.2 -> next
  * attn1.to_qkv of diffusers' BasicTransformerBlock.forward, each a torch.nn.Linear call in the reference; the
  * LayerNorms between them are folded as in ds_gemm_bf16).  Results are bit-identical to n ds_gemm_bf16 calls: same
- * tiles, same K order; only the schedule differs — the CTA pairs walk the problems back to back and a tile of problem
+ * tiles, same K order; only the schedule differs — the CTAs walk the problems back to back and a tile of problem
  * q+1 on row block m starts as soon as all column tiles of problem q for those 128 rows are written (a counter per
  * (problem, row block) in `dep`), so launch / prologue / drain are paid once and the partial last round of one
  * problem is filled with the first tiles of the next.  Every problem: same M > 128, bf16 output with 16-byte
  * addressable rows, no chan_stats, no split-K; residual / ln_stats / row_stats_out / zero_rows may refer to buffers
  * written by EARLIER problems of the chain for the same rows.
- * dep: dep_len >= ds_gemm_chain_max() * 2 * ceil(M / 256) + 1 ints, ALL ZERO on entry; the kernel leaves them all
+ * dep: dep_len >= ds_gemm_chain_max() * ceil(M / 128) + 1 ints, ALL ZERO on entry; the kernel leaves them all
  *      zero again (no memset between launches or graph replays); not to be shared by chains running concurrently. */
 int ds_gemm_chain(const ds_gemm_args* args, int n, int* dep, int dep_len, void* stream);
 int ds_gemm_chain_max(void);
 
 /* ---------------------------------------------------------------------------------------------
- * 3x3 convolution, padding 1, stride 1 or 2, NHWC bf16, as an implicit GEMM on tcgen05:
+ * 3x3 convolution, padding 1, stride 1 or 2, NHWC bf16, as an implicit GEMM on wgmma:
  * the A operand is gathered by 4-D TMA tiles (one 8x16-pixel patch x 64 channels per filter tap;
  * the halo / zero padding is TMA out-of-bounds fill), never materialised.       [tensor-bound]
  * Replaces nn.Conv2d 3x3 in diffusers ResnetBlock2D.conv1/conv2, Downsample2D.conv (stride 2),

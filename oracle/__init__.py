@@ -1,7 +1,7 @@
 """CPU oracle for the DiffSensei UNet sampling path — TEST INFRASTRUCTURE ONLY.
 
 This package is a plain-PyTorch (CPU, fp32) restatement of the arithmetic on the reference's hot
-path (SURVEY.md §8a).  It exists so that the sm_100a kernels in ``diffsensei_b200`` can be checked
+path (SURVEY.md §8a).  It exists so that the sm_90a kernels in ``diffsensei_b200`` can be checked
 against the reference's results.  Only ``tests/``, ``__graft_entry__.smoke()`` and the
 ``cpu_baseline`` / ``--impl reference`` legs of ``bench.py`` may import it; the product package
 ``diffsensei_b200`` never does (tests/test_no_oracle_leak.py enforces this).

@@ -10,7 +10,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine that has one)")
     # the C-ABI library must exist before the package can be imported; build it once if it is missing
     if not os.path.exists(os.path.join(ROOT, "diffsensei_b200", "libdsengine.so")):
         import __graft_entry__

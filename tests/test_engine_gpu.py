@@ -201,27 +201,28 @@ def test_pipeline_call_surface(tiny):
 
 def test_resampler_matches_executed_reference():
     import diffsensei_b200 as ds
-    g = torch.load(os.path.join(GOLDEN, "resampler_tiny.pt"), weights_only=False)
+    from test_oracle_golden import resampler_tiny_case
+    g, sd, x, magi = resampler_tiny_case()
     res = ds.ResamplerEngine(**g["kwargs"], device=DEV)
-    res.load_state_dict(g["state_dict"])
-    out = res(g["x"], g["magi"])
+    res.load_state_dict(sd)
+    out = res(x, magi)
     assert out.shape == (1, 80, 128) and res.dtype() == bf16
     assert rel_l2(out.float(), g["out"]) < 2e-2
-    assert rel_l2(res(torch.zeros_like(g["x"]), torch.zeros_like(g["magi"])).float(), g["out_zero"]) < 2e-2
+    assert rel_l2(res(torch.zeros_like(x), torch.zeros_like(magi)).float(), g["out_zero"]) < 2e-2
 
 
 def test_resampler_shipped_config_matches_executed_reference():
     """The Resampler at the SHIPPED size (dim 1280, depth 4, 20 heads, 4 x (257 + 1) image tokens, 84 M params) on the
     GPU vs the reference's own resampler.py executed on the same seeded weights (tests/golden/resampler_full.pt)."""
     import diffsensei_b200 as ds
-    from test_oracle_golden import resampler_full_case
+    from test_oracle_golden import golden_pair, resampler_full_case
     g, sd, x, magi = resampler_full_case()
     res = ds.ResamplerEngine(**g["kwargs"], device=DEV)
     res.load_state_dict(sd)
     out = res(x, magi)
     assert out.shape == (1, 80, 2048)
-    e1 = rel_l2(out.float(), g["out"])
-    e0 = rel_l2(res(torch.zeros_like(x), torch.zeros_like(magi)).float(), g["out_zero"])
+    e1 = rel_l2(*golden_pair(out.float(), g["out"]))
+    e0 = rel_l2(*golden_pair(res(torch.zeros_like(x), torch.zeros_like(magi)).float(), g["out_zero"]))
     print(f"shipped-config Resampler vs executed reference: rel-L2 {e1:.3e} (zero inputs: {e0:.3e})")
     assert e1 < 2e-2 and e0 < 2e-2
 
@@ -233,14 +234,15 @@ def test_qwen_resampler_matches_executed_reference(name):
     width 160 and LayerNorms over 5120 features."""
     import diffsensei_b200 as ds
     from oracle.qwen_resampler import seeded_case
+    from test_oracle_golden import golden_pair
     g = torch.load(os.path.join(GOLDEN, "qwen_resampler.pt"), weights_only=False)[name]
     _m, sd, x = seeded_case(g["kwargs"], g["seed"])
     eng = ds.QwenResamplerEngine(**g["kwargs"], device=DEV)
     eng.load_state_dict(sd)
     out = eng(x)
-    err = rel_l2(out.float(), g["out"])
+    err = rel_l2(*golden_pair(out.float(), g["out"]))     # golden_pair also checks the full output shape
     print(f"QwenResampler[{name}] vs executed reference: rel-L2 {err:.3e}")
-    assert out.shape == g["out"].shape and err < 1.5e-2
+    assert err < 1.5e-2
 
 
 def test_smoke_entry_point():

@@ -12,7 +12,7 @@ run in bf16 through torch's library kernels (what the reference's own bf16 GPU p
 The fp32 oracle runs ON THE GPU here (plain torch modules, TF32 off) because an SDXL forward on the box's host cores
 costs minutes of leased GPU time; `test_gpu_fp32_oracle_equals_cpu_oracle` pins that run to the CPU oracle first.
 Tolerances (BASELINE.md §3): UNet output rel-L2 <= 3e-2 per forward; 50-step final-latent drift <= 1e-1 and
-reported.  Results are written to gpurun_out/parity_full.json (committed copy: profiles/r02_parity_full.json).
+reported.  With DS_PARITY_OUT=<dir> set, the measured errors are also written to <dir>/parity_full.json.
 """
 import json
 import os
@@ -29,7 +29,9 @@ RESULTS = {}
 
 
 def _dump():
-    out = os.path.join(ROOT, "gpurun_out")
+    out = os.environ.get("DS_PARITY_OUT")
+    if not out:
+        return
     os.makedirs(out, exist_ok=True)
     with open(os.path.join(out, "parity_full.json"), "w") as f:
         json.dump(RESULTS, f, indent=1, sort_keys=True)

@@ -396,8 +396,8 @@ def test_conv_producer_channel_stats(ops, B, H, W, Cin, Cout, stride):
 
 
 def test_gemm_tail_launch_is_bit_identical_to_wide_tiles(ops):
-    """M 8192 x N 1280 is 160 wide tiles on 74 CTA pairs: the call runs the last m-rows as BN=128 tiles in a second
-    launch (ds_gemm_bf16 'tail launch').  Every output element accumulates the same k-blocks in the same order, so
+    """M 8192 x N 1280 is 320 wide tiles on 132 CTAs: the call runs the last m-rows as 128-column units of the same
+    launch (mixed-width schedule).  Every output element accumulates the same k-blocks in the same order, so
     those rows must equal the same rows computed on their own (15 wide tiles, no split)."""
     M, N, K = 8192, 1280, 640
     a = _r(M, K, seed=11).to(DEV)
@@ -486,7 +486,7 @@ def test_gemm_chain_is_bit_identical_to_separate_launches(ops, C, M):
     bit, launch after launch (the kernel hands its counters back zeroed), including odd row-block counts."""
     build = _block_links(ops, C, M, seed=C + M)
     links, h_ref, st_ref = build()
-    # the reference: the same four GEMMs as four launches of the same tile geometry (<256, 2> tiles; the row statistics
+    # the reference: the same four GEMMs as four launches of the same tile geometry (128 x 256 tiles; the row statistics
     # are fp64 sums of per-tile fp32 partials, so they depend — in the last bit — on the tile widths)
     prev, want = None, []
     for args, kw in links:

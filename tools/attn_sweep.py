@@ -36,7 +36,7 @@ for (B, N, h) in ((8, 4096, 10), (8, 1024, 20)):
     out.append("cross B%%d N%%d h%%d %%.1fus %%.0fGB/s" %% (B, N, h, ms * 1e3, 4.0 * B * N * C / ms / 1e6))
 print(" | ".join(out))
 ''' % ROOT
-variants = sys.argv[1:] or ["", "DS_CROSS_PIPE=0", "DS_FLASH_POLY=1", "DS_FLASH_POLY=2", "DS_FLASH_POLY=3"]
+variants = sys.argv[1:] or [""]
 for v in variants:
     env = dict(os.environ)
     for kv in filter(None, v.split(",")):

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Per-shape timing of the tcgen05 GEMM / conv kernel at the shapes that dominate a cfg2 step, under environment
+"""Per-shape timing of the wgmma GEMM / conv kernel at the shapes that dominate a cfg2 step, under environment
 variants (each in its own process: the knobs are read once).  Rotating buffer sets larger than the L2.
     python tools/gemm_sweep.py [variant ...]     variants: KEY=VAL[,KEY=VAL]   default: a built-in list"""
 import os

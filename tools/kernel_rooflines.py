@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """The three kernel-roofline measurements of bench.py alone (no UNet step): prints one JSON line.
-Env switches read by libdsengine apply (DS_FLASH, DS_FLASH_POLY, DS_GN_L2HINT, DS_GEMM_BN, DS_GEMM_PAIR)."""
+Env switches read by libdsengine apply (DS_GN_L2HINT, DS_GEMM_BN)."""
 import json
 import os
 import sys

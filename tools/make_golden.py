@@ -75,6 +75,16 @@ class StubAttn:
                 "to_out_b": self.to_out[0].bias.detach().clone()}
 
 
+def sampled(out: torch.Tensor, n: int = 8192, seed: int = 7):
+    """A fixed seeded sample of a large output (flat indices + fp32 values) so every fixture stays far below 1 MB;
+    outputs of at most `n` elements are stored whole."""
+    out = out.detach().float()
+    if out.numel() <= n:
+        return out
+    idx = torch.randperm(out.numel(), generator=torch.Generator().manual_seed(seed))[:n].sort().values
+    return {"shape": tuple(out.shape), "idx": idx.to(torch.int32), "vals": out.reshape(-1)[idx].clone()}
+
+
 @torch.no_grad()
 def main():
     os.makedirs(OUT, exist_ok=True)
@@ -163,25 +173,27 @@ def main():
     torch.save(cases, f"{OUT}/dialog_embed.pt")
 
     # ------------------------------------------------------------------ Resampler (tiny config)
-    torch.manual_seed(3)
-    kw = dict(dim=128, depth=2, dim_head=64, heads=2, num_queries=16, num_dummy_tokens=16, embedding_dim=64,
-              magi_embedding_dim=32, output_dim=128, ff_mult=4)
+    # weights and inputs are regenerated from the seeds on both sides (tests/test_oracle_golden.py::resampler_tiny_case)
+    sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+    from diffsensei_b200.config import RESAMPLER, RESAMPLER_TINY
+    from diffsensei_b200.weights import random_state_dict, resampler_param_shapes
+    import dataclasses
+    kw = dataclasses.asdict(RESAMPLER_TINY)
     model = rs.Resampler(**kw).eval()
-    x = torch.randn(1, 4, 33, 64)
-    magi = torch.randn(1, 4, 32)
+    sdt = random_state_dict(resampler_param_shapes(RESAMPLER_TINY), seed=44, device="cpu")
+    model.load_state_dict({k: v.to(torch.bfloat16).float() for k, v in sdt.items()})
+    gt = torch.Generator().manual_seed(45)
+    x = torch.randn(1, 4, 33, 64, generator=gt).to(torch.bfloat16).float()
+    magi = torch.randn(1, 4, 32, generator=gt).to(torch.bfloat16).float()
     x[0, 2:] = 0
     magi[0, 2:] = 0
-    torch.save({"kwargs": kw, "state_dict": model.state_dict(), "x": x, "magi": magi, "out": model(x, magi),
+    torch.save({"kwargs": kw, "weight_seed": 44, "input_seed": 45, "n_real": 2, "out": model(x, magi),
                 "out_zero": model(torch.zeros_like(x), torch.zeros_like(magi))}, f"{OUT}/resampler_tiny.pt")
     # ------------------------------------------------------------------ Resampler at the SHIPPED config
     # (configs/model/diffsensei.yaml + scripts/demo/gradio_wo_mllm.py:174-185: 83,978,752 params).  The weights
     # (336 MB) and inputs are NOT stored: both sides regenerate them from the seeds below with
-    # diffsensei_b200.weights.random_state_dict / torch.Generator (same torch build on the GPU box); only the
-    # reference's outputs are committed.
-    sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-    from diffsensei_b200.config import RESAMPLER
-    from diffsensei_b200.weights import random_state_dict, resampler_param_shapes
-    import dataclasses
+    # diffsensei_b200.weights.random_state_dict / torch.Generator (same torch build on the GPU box); only a fixed
+    # seeded sample of the reference's outputs is committed (sampled()).
     kwf = dataclasses.asdict(RESAMPLER)
     full = rs.Resampler(**kwf).eval()
     print("Resampler(shipped config) params:", sum(p.numel() for p in full.parameters()))
@@ -193,8 +205,8 @@ def main():
     mf = torch.randn(1, 4, 768, generator=gx).to(torch.bfloat16).float()
     xf[0, 3:] = 0                                                        # 3 real characters, 1 padded (:131-132)
     mf[0, 3:] = 0
-    torch.save({"kwargs": kwf, "weight_seed": 42, "input_seed": 43, "n_real": 3, "out": full(xf, mf),
-                "out_zero": full(torch.zeros_like(xf), torch.zeros_like(mf))}, f"{OUT}/resampler_full.pt")
+    torch.save({"kwargs": kwf, "weight_seed": 42, "input_seed": 43, "n_real": 3, "out": sampled(full(xf, mf)),
+                "out_zero": sampled(full(torch.zeros_like(xf), torch.zeros_like(mf)))}, f"{OUT}/resampler_full.pt")
     # ------------------------------------------------------------------ QwenResampler (MLLM adaptor, §8f-4)
     # configs/model/diffsensei.yaml agent.input_resampler / output_resampler + a small one; weights / inputs are
     # regenerated from seeds on both sides (tests/test_oracle_golden.py::qwen_case), only outputs are stored
@@ -219,7 +231,7 @@ def main():
                 sdq[k] = (torch.randn(v.shape, generator=gq) * v.shape[-1] ** -0.5).to(torch.bfloat16).float()
         m.load_state_dict(sdq)
         xq = torch.randn(2, kw["grid_size"] ** 2, kw["kv_dim"], generator=gq).to(torch.bfloat16).float()
-        qcases[name] = {"kwargs": kw, "seed": 50, "out": m(xq)}
+        qcases[name] = {"kwargs": kw, "seed": 50, "out": sampled(m(xq))}
     torch.save(qcases, f"{OUT}/qwen_resampler.pt")
     for f in sorted(os.listdir(OUT)):
         print(f, os.path.getsize(os.path.join(OUT, f)))

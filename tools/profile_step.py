@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """One EAGER (non-graph) denoise step at BASELINE cfg2 for `ncu --metrics gpu__time_duration.sum` launch lists.
-Usage on the GPU box (B200_PROFILING.md recipe):
+Usage on the GPU box:
   ncu --metrics gpu__time_duration.sum --clock-control none --profile-from-start off --csv \
       --log-file gpurun_out/launches.csv python tools/profile_step.py
 The profiled range (cudaProfilerStart/Stop) is exactly one step: UNet forward + fused CFG/DDIM update."""

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """CPU-only census of every GEMM / conv / attention launch in one cfg2 UNet forward (shape-only stand-ins for ops.*),
-with a wave-quantisation model of the persistent tcgen05 GEMM: units = ceil(M/256) x ceil(N/BN) CTA-pair tiles over
-`pairs` co-resident pairs."""
+with a wave-quantisation model of the persistent wgmma GEMM: units = ceil(M/128) x ceil(N/BN) CTA tiles over
+`ctas` co-resident CTAs (one per SM)."""
 import collections, math, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -55,16 +55,16 @@ B = 8
 cond = unet_mod.Conditions(kv_text=[None] * eng.num_cross_layers, kv_ip=[None] * eng.num_cross_layers, bbox=None, aspect_ratio=1.0, batch=B)
 eng.forward_nhwc(E(B, 128, 128, 4), E(B, eng.temb_total, dtype=torch.float32), cond)
 
-pairs = int(os.environ.get("PAIRS", "74"))
+ctas = int(os.environ.get("CTAS", "132"))
 tot = 0.0; rows = []
 for (kind, key), (n, fl) in log.items():
     if kind in ("gemm", "conv"):
         M, N, K = key[0], key[1], key[2]
         best = None
         for bn in (256, 128):
-            units = math.ceil(M / 256) * math.ceil(N / bn)
-            waves = math.ceil(units / pairs)
-            eff = (M * N) / (waves * pairs * 256 * bn)
+            units = math.ceil(M / 128) * math.ceil(N / bn)
+            waves = math.ceil(units / ctas)
+            eff = (M * N) / (waves * ctas * 128 * bn)
             if best is None or eff > best[1]: pass
             rows.append((kind, key, n, fl, bn, units, waves, eff))
         tot += n * fl
