@@ -4,8 +4,6 @@
 #include <mutex>
 #include <string>
 
-#include <cstdlib>
-
 #include "ds_host.h"
 
 namespace ds {
@@ -20,14 +18,6 @@ void set_error(const char* fmt, ...) {
   vsnprintf(buf, sizeof(buf), fmt, ap);
   va_end(ap);
   t_last_error = buf;
-}
-
-bool pdl_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("DS_PDL");
-    return e ? atoi(e) != 0 : true;
-  }();
-  return on;
 }
 
 bool get_device(DeviceInfo* out) {

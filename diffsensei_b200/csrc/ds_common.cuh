@@ -104,10 +104,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory");
 }
-// L2 prefetch of a tile (no shared-memory destination, no barrier)
-__device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* m, int c0, int c1) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(m), "r"(c0), "r"(c1) : "memory");
-}
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"

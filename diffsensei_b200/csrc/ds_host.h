@@ -63,11 +63,11 @@ inline int device_slot() {
     ::ds::count_launch();                                                            \
   } while (0)
 
-// DS_PDL=0 disables programmatic dependent launch (A/B timing); default on.  Fills one launch attribute.
-bool pdl_enabled();
+// Fills one launch attribute: programmatic dependent launch (the kernel's prologue may overlap the previous kernel's
+// tail).
 inline void pdl_attr(cudaLaunchAttribute* a) {
   a->id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  a->val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+  a->val.programmaticStreamSerializationAllowed = 1;
 }
 
 // bf16 tensor map (tile mode, 128-byte swizzle, zero OOB fill). dims/strides innermost first;

@@ -86,8 +86,6 @@ struct GemmParams {
   // 1: the weight operand is constant data (never written by a kernel that may still be in flight), so the producer
   // may request its first tiles BEFORE griddepcontrol.wait.  0 (e.g. K / V^T of the VAE attention used as `w`): after.
   int w_const;
-  int n_block;      // > 0: wide units are ordered in column blocks of n_block n-tiles (m-major inside a block), see run_gemm
-  int l2_prefetch;  // k-blocks of weight tile the producer requests into the L2 ahead of its smem ring (0 = off)
   // second A operand: k-blocks [k1_iters, num_k_iters) of a plain GEMM come from tmA2 (the channel concatenation
   // [a | a2] along K is never materialised); k1_iters == num_k_iters: off
   int k1_iters;
@@ -257,21 +255,8 @@ gemm_bf16_wgmma(const __grid_constant__ GemmLaunch<MAXQ> L) {
   // unit -> (m-tile, first weight row of its columns, tile width)
   auto unit_geom = [&](int unit, int& m_tile, int& n_org, int& bn) {
     if (unit < p.wide_units) {
-      int k;
-      if (p.n_block > 0) {
-        // column-blocked order: the CTAs resident at one time cover ~(CTAs / n_block) row blocks x n_block column
-        // tiles — fewer distinct operand tiles in flight, more identical requests at the L2
-        const int per_blk = p.wide_m_tiles * p.n_block;
-        const int nb = unit / per_blk;
-        const int r = unit - nb * per_blk;
-        const int left = p.num_n_tiles - nb * p.n_block;
-        const int wcur = left < p.n_block ? left : p.n_block;
-        m_tile = r / wcur;
-        k = nb * p.n_block + (r - m_tile * wcur);
-      } else {
-        m_tile = unit / p.num_n_tiles;
-        k = unit - m_tile * p.num_n_tiles;
-      }
+      m_tile = unit / p.num_n_tiles;
+      const int k = unit - m_tile * p.num_n_tiles;
       n_org = k * BN;
       bn = (p.last_narrow && k == p.num_n_tiles - 1) ? kNarrowBN : BN;
     } else {
@@ -329,18 +314,7 @@ gemm_bf16_wgmma(const __grid_constant__ GemmLaunch<MAXQ> L) {
           x0 = (rem % p.tiles_x) * kConvTileW;
         }
         const CUtensorMap* bm = narrow ? &tmB2 : &tmB;
-        if (p.l2_prefetch > 0 && it + it_step < it_end) {
-          // the first weight blocks of this CTA's NEXT item, requested into the L2 a whole item early
-          const int nxt = MAXQ > 1 ? __ldg(sched_items + it + it_step) : it + it_step;
-          int u2, k02, k12, t2, mt2, no2, bn2;
-          decode(nxt, u2, k02, k12, t2);
-          unit_geom(u2, mt2, no2, bn2);
-          const CUtensorMap* bm2 = (bn2 != BN) ? &tmB2 : &tmB;
-          const int npf = (k12 - k02) < p.l2_prefetch ? (k12 - k02) : p.l2_prefetch;
-          for (int i = 0; i < npf; ++i) tma_prefetch_2d(bm2, (k02 + i) * kBK, no2);
-        }
         for (int kb = k0; kb < k1; ++kb) {
-          if (p.l2_prefetch > 0 && kb + p.l2_prefetch < k1) tma_prefetch_2d(bm, (kb + p.l2_prefetch) * kBK, n_org);
           mbar_wait(&empty_bar[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full_bar[stage], stage_bytes);
           if (p.conv) {
@@ -788,41 +762,43 @@ gemm_bf16_wgmma(const __grid_constant__ GemmLaunch<MAXQ> L) {
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-// Co-resident CTAs of gemm_bf16_wgmma<BN, *, *> on the current device: the schedule is persistent with a static stride,
-// so every CTA must be resident — one per SM.  Cached per device.
-template <int BN>
-static int resident_groups(int num_sms) {
-  static int cache[kMaxDevices] = {};
-  int& g = cache[device_slot()];
-  if (g == 0) {
-    int per_sm = 0;
-    (void)cudaFuncSetAttribute(gemm_bf16_wgmma<BN, false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               GemmCfg<BN>::kSmemBytes);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gemm_bf16_wgmma<BN, false, 1>, kGemmThreads,
-                                                      GemmCfg<BN>::kSmemBytes) != cudaSuccess || per_sm < 1)
-      per_sm = 1;
-    (void)cudaGetLastError();
-    g = num_sms;
-    if (getenv("DS_DEBUG"))
-      fprintf(stderr, "[dsengine] gemm<%d>: %d co-resident CTAs (%d per SM possible), %d SMs\n", BN, g, per_sm, num_sms);
-  }
-  return g;
-}
+// One prepared problem: tensor maps {A, B, C, R, A2, B2}, parameters and the tile shape run_gemm chose for it.
+struct PreparedGemm {
+  CUtensorMap tm[6];
+  GemmParams p;
+  int bn;
+};
 
-template <int BN, bool STATS>
-static int launch_gemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
-                         const CUtensorMap& tmR, const CUtensorMap& tmA2, const CUtensorMap& tmB2,
-                         const GemmParams& p_in, int num_sms, cudaStream_t stream, void* splitk_ws,
-                         long long splitk_ws_bytes) {
-  GemmParams p = p_in;
-  using Cfg = GemmCfg<BN>;
+// Launches gemm_bf16_wgmma<BN, STATS, MAXQ> on `groups` CTAs with programmatic dependent launch.  The schedule is
+// persistent with a static stride, so every CTA must be resident: callers pass at most one CTA per SM.  The dynamic
+// shared-memory opt-in is set once per device for each instantiation.
+template <int BN, bool STATS, int MAXQ>
+static int launch_wgmma(const GemmLaunch<MAXQ>& L, int groups, cudaStream_t stream, const char* name) {
   const int slot = device_slot();
   static bool attr_set[kMaxDevices] = {};  // per device; benign race: idempotent
   if (!attr_set[slot]) {
-    DS_CUDA_OK(cudaFuncSetAttribute(gemm_bf16_wgmma<BN, STATS, 1>,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    DS_CUDA_OK(cudaFuncSetAttribute(gemm_bf16_wgmma<BN, STATS, MAXQ>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    GemmCfg<BN>::kSmemBytes));
     attr_set[slot] = true;
   }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(groups);
+  cfg.blockDim = dim3(kGemmThreads);
+  cfg.dynamicSmemBytes = GemmCfg<BN>::kSmemBytes;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  pdl_attr(&attr[0]);
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  DS_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_wgmma<BN, STATS, MAXQ>, L));
+  DS_LAUNCH_OK(name);
+  return DS_OK;
+}
+
+template <int BN, bool STATS>
+static int launch_gemm_t(const PreparedGemm& g, int num_sms, cudaStream_t stream, void* splitk_ws,
+                         long long splitk_ws_bytes) {
+  GemmParams p = g.p;
   const int m_groups = p.num_m_tiles;
   const bool mixed = p.nt_narrow > 0;  // run_gemm chose the mixed-width tail (BN == 256 only)
   if (!mixed) {
@@ -831,16 +807,7 @@ static int launch_gemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const C
     p.nt_narrow = 0;
   }
   const int units = mixed ? p.wide_units + (m_groups - p.wide_m_tiles) * p.nt_narrow : m_groups * p.num_n_tiles;
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  pdl_attr(&attr[0]);
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  const int max_groups = resident_groups<BN>(num_sms);
-  const int groups = units < max_groups ? units : max_groups;
+  const int groups = units < num_sms ? units : num_sms;
   // split-K tail (see GemmParams): the units of the partial last wave are cut along K so that every CTA gets a slice.
   // Needs the bf16 TMA epilogue, no GEGLU (its accumulator pairs value | gate columns) and a caller-provided zeroed
   // workspace.  The fp32 reductions through the L2 and the second epilogue pass cost a fixed amount per launch, so it
@@ -871,31 +838,16 @@ static int launch_gemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const C
       }
     }
   }
-  cfg.gridDim = dim3(groups);
   GemmLaunch<1> L;
-  L.tm[0][0] = tmA;
-  L.tm[0][1] = tmB;
-  L.tm[0][2] = tmC;
-  L.tm[0][3] = tmR;
-  L.tm[0][4] = tmA2;
-  L.tm[0][5] = tmB2;
+  for (int i = 0; i < 6; ++i) L.tm[0][i] = g.tm[i];
   L.p[0] = p;
   L.nq = 1;
   L.dep = nullptr;
   L.dep_stride = 0;
   L.sched = nullptr;
   L.sched_items = 0;
-  DS_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_wgmma<BN, STATS, 1>, L));
-  DS_LAUNCH_OK("gemm_bf16_wgmma");
-  return DS_OK;
+  return launch_wgmma<BN, STATS, 1>(L, groups, stream, "gemm_bf16_wgmma");
 }
-
-// One prepared problem: tensor maps {A, B, C, R, A2, B2}, parameters and the tile shape run_gemm chose for it.
-struct PreparedGemm {
-  CUtensorMap tm[6];
-  GemmParams p;
-  int bn;
-};
 
 // Static schedule of a chain: which CTA runs which units, in which order.  Round-robin per problem (what a single
 // launch does) leaves every problem's partial last round on the same low-numbered CTAs; here the units of ALL
@@ -909,17 +861,11 @@ struct ChainSchedule {
   int items_off = 0;
 };
 
+constexpr double kChainAlpha = 6.0;  // per-unit fixed cost of the schedule's cost model, in k-blocks
+
 static int chain_schedule(const PreparedGemm* pr, int n, int groups, cudaStream_t stream, ChainSchedule* out) {
   static std::mutex mu;
   static std::map<std::vector<int>, ChainSchedule> cache[kMaxDevices];
-  static const double alpha = [] {
-    const char* e = getenv("DS_CHAIN_ALPHA");
-    return e ? atof(e) : 6.0;
-  }();
-  static const int uniform = [] {  // DS_CHAIN_SCHED=rr: every unit costs the same (round-robin continued across problems)
-    const char* e = getenv("DS_CHAIN_SCHED");
-    return (e && e[0] == 'r') ? 1 : 0;
-  }();
   std::vector<int> key = {groups, n};
   for (int q = 0; q < n; ++q) {
     key.push_back(pr[q].p.total_items);
@@ -943,7 +889,7 @@ static int chain_schedule(const PreparedGemm* pr, int n, int groups, cudaStream_
   for (int g = 0; g < groups; ++g) free_at.push({0.0, g});
   int total = 0;
   for (int q = 0; q < n; ++q) {
-    const double cost = uniform ? 1.0 : static_cast<double>(pr[q].p.num_k_iters) + alpha;
+    const double cost = static_cast<double>(pr[q].p.num_k_iters) + kChainAlpha;
     for (int u = 0; u < pr[q].p.total_items; ++u) {
       Slot s = free_at.top();
       free_at.pop();
@@ -974,15 +920,6 @@ static int chain_schedule(const PreparedGemm* pr, int n, int groups, cudaStream_
 // ds_gemm_chain: n dependent GEMMs (problem q+1 reads problem q's output rows) as ONE persistent launch of
 // 128 x 256 tiles; see GemmLaunch.  `dep` = kMaxChain * dep_stride + 1 zeroed ints the kernel hands back zeroed.
 static int launch_chain(PreparedGemm* pr, int n, int* dep, int dep_len, int num_sms, cudaStream_t stream) {
-  constexpr int BN = 256;
-  using Cfg = GemmCfg<BN>;
-  const int slot = device_slot();
-  static bool attr_set[kMaxDevices] = {};
-  if (!attr_set[slot]) {
-    DS_CUDA_OK(cudaFuncSetAttribute(gemm_bf16_wgmma<BN, false, kMaxChain>,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_set[slot] = true;
-  }
   GemmLaunch<kMaxChain> L;
   const int m_groups = pr[0].p.num_m_tiles;
   int max_units = 0;
@@ -1009,45 +946,26 @@ static int launch_chain(PreparedGemm* pr, int n, int* dep, int dep_len, int num_
   L.dep_stride = m_groups;
   DS_REQUIRE(kMaxChain * L.dep_stride + 1 <= dep_len,
              "ds_gemm_chain: dependency buffer too small (%d ints for %d row blocks)", dep_len, L.dep_stride);
-  const int max_groups = resident_groups<BN>(num_sms);
-  const int groups = max_units < max_groups ? max_units : max_groups;
+  const int groups = max_units < num_sms ? max_units : num_sms;
   ChainSchedule sc;
   const int rc = chain_schedule(pr, n, groups, stream, &sc);
   if (rc != DS_OK) return rc;
   L.sched = sc.dev;
   L.sched_items = sc.items_off;
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  pdl_attr(&attr[0]);
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  cfg.gridDim = dim3(groups);
-  DS_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_wgmma<BN, false, kMaxChain>, L));
-  DS_LAUNCH_OK("gemm_bf16_wgmma(chain)");
-  return DS_OK;
+  return launch_wgmma<256, false, kMaxChain>(L, groups, stream, "gemm_bf16_wgmma(chain)");
 }
 
 template <int BN>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
-                       const CUtensorMap& tmR, const CUtensorMap& tmA2, const CUtensorMap& tmB2, const GemmParams& p,
-                       int num_sms, cudaStream_t stream, void* splitk_ws, long long splitk_ws_bytes) {
+static int launch_gemm(const PreparedGemm& g, int num_sms, cudaStream_t stream, void* splitk_ws,
+                       long long splitk_ws_bytes) {
   // the statistics epilogue is a separate instantiation: the default one keeps its register budget
-  if (p.chan_stats)
-    return launch_gemm_t<BN, true>(tmA, tmB, tmC, tmR, tmA2, tmB2, p, num_sms, stream, splitk_ws, splitk_ws_bytes);
-  return launch_gemm_t<BN, false>(tmA, tmB, tmC, tmR, tmA2, tmB2, p, num_sms, stream, splitk_ws, splitk_ws_bytes);
+  if (g.p.chan_stats) return launch_gemm_t<BN, true>(g, num_sms, stream, splitk_ws, splitk_ws_bytes);
+  return launch_gemm_t<BN, false>(g, num_sms, stream, splitk_ws, splitk_ws_bytes);
 }
 
 static int pick_bn(int N, int epilogue) {
   if (epilogue == DS_EPI_GEGLU) return 256;
   if (N <= 128) return 128;
-  static const int bn_env = [] {  // DS_GEMM_BN=128|256 forces the tile width (A/B timing); default: heuristic below
-    const char* e = getenv("DS_GEMM_BN");
-    return e ? atoi(e) : 0;
-  }();
-  if (bn_env == 128 || bn_env == 192 || bn_env == 256) return bn_env;
   // wide tiles read less shared memory per MMA (the A slice is shared by more columns), so BN = 256 is the default;
   // BN = 192 (3 x 64-column blocks) is used where it trims >= 15 % of the padded columns.
   const int c256 = ((N + 255) / 256) * 256, c192 = ((N + 191) / 192) * 192;
@@ -1118,30 +1036,14 @@ static int prepare_gemm(const CUtensorMap& tmA, const CUtensorMap& tmA2, const v
     return e ? atoi(e) : 0;
   }();
   if (!early_w_env) p.w_const = 0;
-  // opt-in
-  static const int l2pf_env = [] {  // DS_GEMM_L2PF = k-blocks of weights requested into the L2 ahead of the smem ring
-    const char* e = getenv("DS_GEMM_L2PF");
-    return e ? atoi(e) : 0;
-  }();
-  p.l2_prefetch = l2pf_env;
-  // DS_GEMM_NBLOCK = w: order the units in column blocks of w n-tiles when a problem has more than w of them
-  static const int nblock_env = [] {
-    const char* e = getenv("DS_GEMM_NBLOCK");
-    return e ? atoi(e) : 0;
-  }();
   p.num_n_tiles = (p.N + bn - 1) / bn;
-  p.n_block = (nblock_env > 0 && p.num_n_tiles > nblock_env) ? nblock_env : 0;
   p.wide_units = 0;
   p.wide_m_tiles = 0;
   p.nt_narrow = 0;
   // narrow last n-tile: when the last BN-wide tile of a row would hold <= 128 real columns (N = 640 -> 256|256|128,
   // N = 320 -> 192|128, N = 1920 -> 7 x 256|128) it runs as a 128-column unit: same unit count, no padded MMAs
-  static const int narrow_env = [] {
-    const char* e = getenv("DS_GEMM_NARROW_LAST");
-    return e ? atoi(e) : 1;
-  }();
   p.last_narrow = 0;
-  if (narrow_env && bn > kNarrowBN && p.epilogue != DS_EPI_GEGLU) {
+  if (bn > kNarrowBN && p.epilogue != DS_EPI_GEGLU) {
     const int last_cols = p.N - (p.num_n_tiles - 1) * bn;
     if (last_cols <= kNarrowBN) p.last_narrow = 1;
   }
@@ -1156,7 +1058,7 @@ static int prepare_gemm(const CUtensorMap& tmA, const CUtensorMap& tmA2, const v
   }();
   if (tail_env && !chain && bn == 256 && p.epilogue != DS_EPI_GEGLU && p.N % 128 == 0 &&
       !p.last_narrow) {
-    const int G = resident_groups<256>(dev.num_sms);
+    const int G = dev.num_sms;  // one persistent CTA per SM
     const int mp = p.num_m_tiles, nt = p.num_n_tiles;
     const int units = mp * nt;
     const int full = units / G, rem = units - full * G;
@@ -1205,11 +1107,9 @@ static int run_gemm(const CUtensorMap& tmA_in, const CUtensorMap& tmA2_in, const
   PreparedGemm g;
   const int rc = prepare_gemm(tmA_in, tmA2_in, w, ldw, p_in, conv_B, stream, row_stats_zeroed, false, dev, &g);
   if (rc != DS_OK) return rc;
-  const CUtensorMap &tmA = g.tm[0], &tmB = g.tm[1], &tmC = g.tm[2], &tmR = g.tm[3], &tmA2 = g.tm[4], &tmB2 = g.tm[5];
-  const GemmParams& p = g.p;
-  if (g.bn == 256) return launch_gemm<256>(tmA, tmB, tmC, tmR, tmA2, tmB2, p, dev.num_sms, stream, splitk_ws, splitk_ws_bytes);
-  if (g.bn == 192) return launch_gemm<192>(tmA, tmB, tmC, tmR, tmA2, tmB2, p, dev.num_sms, stream, splitk_ws, splitk_ws_bytes);
-  return launch_gemm<128>(tmA, tmB, tmC, tmR, tmA2, tmB2, p, dev.num_sms, stream, splitk_ws, splitk_ws_bytes);
+  if (g.bn == 256) return launch_gemm<256>(g, dev.num_sms, stream, splitk_ws, splitk_ws_bytes);
+  if (g.bn == 192) return launch_gemm<192>(g, dev.num_sms, stream, splitk_ws, splitk_ws_bytes);
+  return launch_gemm<128>(g, dev.num_sms, stream, splitk_ws, splitk_ws_bytes);
 }
 
 // argument checks + A tensor map(s) + GemmParams of one ds_gemm_args (shared by ds_gemm_bf16 and ds_gemm_chain)

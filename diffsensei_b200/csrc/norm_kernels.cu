@@ -16,24 +16,23 @@
 // Replaces diffusers ResnetBlock2D.norm1/norm2+SiLU, Transformer2DModel.norm, conv_norm_out+conv_act
 // (reached from src/models/unet.py:251-261,281-290,316-338) and BasicTransformerBlock / Resampler LayerNorms
 // (src/models/resampler.py:14,40-41,104).
-#include <cstdlib>
-
 #include "ds_common.cuh"
 #include "ds_host.h"
 
 namespace ds {
 
+// Launch shape: threads per CTA of the apply and statistics kernels, the apply kernel's independent 16-byte loads in
+// flight per thread, and its cap on resident CTAs per SM.
+constexpr int kGnApplyThreads = 256;
+constexpr int kGnStatsThreads = 512;
+constexpr int kGnUnroll = 8;
+constexpr int kGnMaxOcc = 8;
+
 // L2 residency control for the two-pass GroupNorm: the stats pass marks x evict_last so that the apply pass
-// re-reads it from the 126 MB L2 instead of HBM (x of the largest cfg2 tensor is 84 MB); the apply pass reads x
-// evict_first (dead after this read) so the y write stream displaces x's consumed lines first.
+// re-reads it from the L2 instead of HBM; the apply pass reads x with the evict_normal policy.
 __device__ __forceinline__ uint64_t l2_policy_evict_last() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
   return p;
 }
 __device__ __forceinline__ uint64_t l2_policy_normal() {
@@ -144,7 +143,7 @@ template <bool kSilu, int kU>
 __global__ void gn_apply2_kernel(const uint4* __restrict__ x1, const uint4* __restrict__ x2, uint4* __restrict__ y,
                                  const double* __restrict__ st1, const double* __restrict__ st2,
                                  const float* __restrict__ gamma, const float* __restrict__ beta, int HW, int C1, int C2,
-                                 int groups, float eps, int items_per_sample, int ipx, int total_items, int l2_hint) {
+                                 int groups, float eps, int items_per_sample, int ipx, int total_items) {
   extern __shared__ double shd[];  // [C][2] channel sums of the current sample, then [groups][2] {mean, rstd}
   const int C = C1 + C2;
   const int cv = C >> 3, cv1 = C1 >> 3;
@@ -173,8 +172,7 @@ __global__ void gn_apply2_kernel(const uint4* __restrict__ x1, const uint4* __re
     be[j] = __ldg(beta + cvec * 8 + j);
   }
   pdl_wait();  // x and the statistics come from the predecessor
-  // x is dead after this read (evict_first); y stays for the consumer conv.  l2_hint == 0: plain loads (A/B knob)
-  const uint64_t pol = l2_hint ? l2_policy_evict_first() : l2_policy_normal();
+  const uint64_t pol = l2_policy_normal();
   // group coefficients of sample b: channel sums -> smem -> 32 threads fold cpg channels each, in order
   auto load_coeffs = [&](int b) {
     __syncthreads();                                 // previous sample's coefficients no longer in use
@@ -340,11 +338,6 @@ static bool gn_plan(int B, int HW, int C, int target_threads, int sweeps, GnPlan
   pl->total_items = static_cast<int>(t);
   return true;
 }
-static int gn_env(const char* name, int dflt, int lo, int hi) {
-  const char* e = getenv(name);
-  const int v = e ? atoi(e) : dflt;
-  return v >= lo && v <= hi ? v : dflt;
-}
 }  // namespace
 
 extern "C" int ds_channel_stats(const void* x, double* stats, int B, int HW, int C, void* stream) {
@@ -356,9 +349,8 @@ extern "C" int ds_channel_stats(const void* x, double* stats, int B, int HW, int
   DeviceInfo dev;
   if (!get_device(&dev)) return DS_ERR_CUDA;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  static const int tt = gn_env("DS_GN_STATS_THREADS", 512, 64, 1024);
   GnPlan pl;
-  DS_REQUIRE(gn_plan(B, HW, C, tt, 8, &pl), "ds_channel_stats: tensor too large");
+  DS_REQUIRE(gn_plan(B, HW, C, kGnStatsThreads, 8, &pl), "ds_channel_stats: tensor too large");
   const size_t smem = static_cast<size_t>(pl.rpb) * C * 2 * sizeof(float);
   static size_t attr[kMaxDevices] = {};
   if (smem > 48 * 1024 && smem > attr[device_slot()]) {
@@ -407,22 +399,12 @@ extern "C" int ds_groupnorm_apply(const void* x1, const double* stats1, int C1, 
   DeviceInfo dev;
   if (!get_device(&dev)) return DS_ERR_CUDA;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  static const int tt = gn_env("DS_GN_THREADS", 256, 64, 1024);
-  static const int unroll = gn_env("DS_GN_UNROLL", 8, 4, 8);
-  static const int max_occ = gn_env("DS_GN_OCC", 8, 1, 16);
-  static const int l2_hint = gn_env("DS_GN_L2HINT", 0, 0, 1);  // default: plain loads
   GnPlan pl;
-  DS_REQUIRE(gn_plan(B, HW, C, tt, unroll, &pl), "ds_groupnorm_apply: tensor too large");
+  DS_REQUIRE(gn_plan(B, HW, C, kGnApplyThreads, kGnUnroll, &pl), "ds_groupnorm_apply: tensor too large");
   const size_t smem = static_cast<size_t>(C) * 2 * sizeof(double) + static_cast<size_t>(groups) * 2 * sizeof(float);
-  const void* fn;
-  if (unroll == 8)
-    fn = apply_silu ? reinterpret_cast<const void*>(gn_apply2_kernel<true, 8>)
-                    : reinterpret_cast<const void*>(gn_apply2_kernel<false, 8>);
-  else
-    fn = apply_silu ? reinterpret_cast<const void*>(gn_apply2_kernel<true, 4>)
-                    : reinterpret_cast<const void*>(gn_apply2_kernel<false, 4>);
-  static size_t attr[kMaxDevices][4] = {};
-  size_t& a = attr[device_slot()][(unroll == 8 ? 2 : 0) + (apply_silu ? 1 : 0)];
+  auto* fn = apply_silu ? gn_apply2_kernel<true, kGnUnroll> : gn_apply2_kernel<false, kGnUnroll>;
+  static size_t attr[kMaxDevices][2] = {};
+  size_t& a = attr[device_slot()][apply_silu ? 1 : 0];
   if (smem > 48 * 1024 && smem > a) {
     DS_CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     a = smem;
@@ -432,7 +414,7 @@ extern "C" int ds_groupnorm_apply(const void* x1, const double* stats1, int C1, 
     (void)cudaGetLastError();
     occ = 1;
   }
-  if (occ > max_occ) occ = max_occ;
+  if (occ > kGnMaxOcc) occ = kGnMaxOcc;
   const long long g = static_cast<long long>(occ) * dev.num_sms;
   const int grid = static_cast<int>(g < pl.total_items ? g : pl.total_items);
   cudaLaunchConfig_t cfg = {};
@@ -444,18 +426,9 @@ extern "C" int ds_groupnorm_apply(const void* x1, const double* stats1, int C1, 
   pdl_attr(&lattr[0]);
   cfg.attrs = lattr;
   cfg.numAttrs = 1;
-  const uint4* a1 = static_cast<const uint4*>(x1);
-  const uint4* a2 = static_cast<const uint4*>(x2);
-  uint4* yp = static_cast<uint4*>(y);
-#define DS_GN_LAUNCH(S, U)                                                                                         \
-  DS_CUDA_OK(cudaLaunchKernelEx(&cfg, gn_apply2_kernel<S, U>, a1, a2, yp, stats1, stats2, gamma, beta, HW, C1, C2, \
-                                groups, eps, pl.items_per_sample, pl.ipx, pl.total_items, l2_hint))
-  if (unroll == 8) {
-    if (apply_silu) DS_GN_LAUNCH(true, 8); else DS_GN_LAUNCH(false, 8);
-  } else {
-    if (apply_silu) DS_GN_LAUNCH(true, 4); else DS_GN_LAUNCH(false, 4);
-  }
-#undef DS_GN_LAUNCH
+  DS_CUDA_OK(cudaLaunchKernelEx(&cfg, fn, static_cast<const uint4*>(x1), static_cast<const uint4*>(x2),
+                                static_cast<uint4*>(y), stats1, stats2, gamma, beta, HW, C1, C2, groups, eps,
+                                pl.items_per_sample, pl.ipx, pl.total_items));
   DS_LAUNCH_OK("gn_apply2_kernel");
   return DS_OK;
 }

@@ -51,7 +51,7 @@ for (B, H, W, Ci, Co, res, stats) in CONVS:
     out.append("conv %%dx%%d %%d->%%d%%s%%s %%.1fus %%.0fTF" %% (H, W, Ci, Co, "+res" if res else "", "+stats" if stats else "", ms * 1e3, 2.0 * 9 * Ci * Co * B * H * W / ms / 1e9))
 print("\n    ".join(out))
 ''' % ROOT
-variants = sys.argv[1:] or ["", "DS_GEMM_TAIL=0", "DS_GEMM_BN=256", "DS_PDL=0"]
+variants = sys.argv[1:] or ["", "DS_GEMM_TAIL=0"]
 for v in variants:
     env = dict(os.environ)
     for kv in filter(None, v.split(",")):
