@@ -8,6 +8,7 @@ Public surface (mirrors the reference's, SURVEY.md §8b):
     ClipTextEncoderEngine, ClipVisionEncoderEngine, VitMaeEncoderEngine  <- transformers CLIP / ViT-MAE encoders as
                               used by encode_prompt (:232-245) and prepare_ip_image_embeds (:125-128)
     DiffSenseiPipeline     <- src/pipelines/pipeline_diffsensei.py  (denoise loop)
+    AgentEngine, LlamaEngine  <- src/models/mllm/seed_x.py ContinuousLVLM (greedy LLaMA generate of the MLLM agent)
     ops                    -- tensor-level wrappers over the C ABI in include/dsengine.h
 
 Importing the package loads ``libdsengine.so`` (built in-tree for sm_90a); it fails loudly if the library is
@@ -15,9 +16,10 @@ missing, and nothing in here falls back to PyTorch compute or to the test oracle
 """
 from . import _lib  # noqa: F401  (loads libdsengine.so or raises ImportError)
 from . import ops  # noqa: F401
+from .agent import AgentEngine, LlamaEngine  # noqa: F401
 from .attention_processor import AttnProcessor2_0, MaskedIPAttnProcessor2_0  # noqa: F401
-from .config import (RESAMPLER, RESAMPLER_TINY, SDXL_MANGA, SDXL_VAE, TINY, TINY_VAE, ResamplerConfig, UNetConfig,  # noqa: F401
-                     VaeConfig)
+from .config import (AGENT_TINY, LLAMA2_13B, RESAMPLER, RESAMPLER_TINY, SDXL_MANGA, SDXL_VAE, TINY, TINY_VAE, ResamplerConfig, UNetConfig,  # noqa: F401
+                     AgentConfig, VaeConfig)
 from .encoders import (CLIP_L_TEXT, CLIP_VIT_H, MAGI_VIT_MAE, OPENCLIP_BIGG_TEXT, ClipTextEncoderEngine,  # noqa: F401
                        ClipVisionEncoderEngine, EncoderConfig, VitMaeEncoderEngine)
 from .pipeline import DiffSenseiPipeline  # noqa: F401

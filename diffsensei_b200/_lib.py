@@ -84,6 +84,12 @@ SIGNATURES = {
     "ds_latent_pointwise": [_vp, _vp, _vp, _vp, _f, _i, _i, _vp],
     "ds_softmax_rows": [_vp, _vp, _i, _i, _i64, _i64, _f, _vp],
     "ds_image_postprocess": [_vp, _vp, _i, _i, _i, _vp],
+    "ds_gemv_bf16": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],
+    "ds_rmsnorm": [_vp, _vp, _vp, _i, _i, _f, _vp],
+    "ds_rope_kv_append": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp],
+    "ds_attention_kv": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _i, _i, _vp],
+    "ds_silu_mul": [_vp, _vp, _i, _i, _vp],
+    "ds_agent_next_token": [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _vp],
 }
 OTHER_EXPORTS = ("ds_version", "ds_last_error", "ds_launch_count", "ds_groupnorm_scratch_floats",
                  "ds_gemm_splitk_ws_bytes")

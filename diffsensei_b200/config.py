@@ -85,4 +85,33 @@ class VaeConfig:
 
 
 SDXL_VAE = VaeConfig()
+
+
+@dataclass(frozen=True)
+class AgentConfig:
+    """LlamaForCausalLM of the MLLM agent (src/models/mllm/modeling_llama_xformer.py:152-168, LLaMA-2-13B).  SEED-X adds
+    image and box tokens to the vocabulary, so ``vocab_size`` comes from the checkpoint and has no default."""
+    vocab_size: int
+    hidden_size: int = 5120
+    intermediate_size: int = 13824
+    num_hidden_layers: int = 40
+    num_attention_heads: int = 40
+    rms_norm_eps: float = 1e-5
+    rope_theta: float = 10000.0
+    max_position_embeddings: int = 4096
+    bos_token_id: int = 1
+    eos_token_id: int = 2
+
+    @property
+    def head_dim(self) -> int:
+        return self.hidden_size // self.num_attention_heads
+
+
+def LLAMA2_13B(vocab_size: int) -> AgentConfig:
+    return AgentConfig(vocab_size=vocab_size)
+
+
+# two layers of width 256 (two heads of 128): the CPU reference runs in well under a second
+AGENT_TINY = AgentConfig(vocab_size=1000, hidden_size=256, intermediate_size=688, num_hidden_layers=2,
+                         num_attention_heads=2, max_position_embeddings=512)
 TINY_VAE = VaeConfig(block_out_channels=(64, 64, 128, 128))

@@ -625,6 +625,130 @@ def embed_tokens(ids: torch.Tensor, tok_emb: torch.Tensor, pos_emb: torch.Tensor
     return out
 
 
+# ---------------------------------------------------------------------------------------------- LLaMA decoder (agent)
+def gemv(x: torch.Tensor, w: torch.Tensor, residual: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+         out_fp32: bool = False) -> torch.Tensor:
+    """out[M, N] = x[M, K] @ w[N, K]^T (+ residual) for 1 <= M <= 8 rows: the weight-streaming decode linear
+    (ds_gemv_bf16).  ``out`` may be ``residual`` itself (in-place residual add)."""
+    _req(x, bf16, "gemv.x")
+    _req(w, bf16, "gemv.w", 2)
+    K = x.shape[-1]
+    M = x.numel() // K
+    N = w.shape[0]
+    if w.shape[1] != K:
+        raise DsEngineError(f"gemv: x has K={K} but w is {tuple(w.shape)}")
+    if out is None:
+        out = torch.empty(M, N, dtype=f32 if out_fp32 else bf16, device=x.device)
+    else:
+        _req(out, f32 if out_fp32 else bf16, "gemv.out")
+        if out.numel() != M * N:
+            raise DsEngineError("gemv: out must hold M*N elements")
+    if residual is not None:
+        _req(residual, bf16, "gemv.residual")
+        if residual.numel() != M * N:
+            raise DsEngineError("gemv: residual must hold M*N elements")
+    check(lib.ds_gemv_bf16(x.data_ptr(), w.data_ptr(), _ptr(residual), out.data_ptr(), M, N, K, int(out_fp32),
+                           _stream()), "ds_gemv_bf16")
+    return out
+
+
+def rmsnorm(x: torch.Tensor, gamma: torch.Tensor, eps: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """LlamaRMSNorm over the last dim: bf16 in / out, fp32 ``gamma``."""
+    _req(x, bf16, "rmsnorm.x")
+    _req(gamma, f32, "rmsnorm.gamma", 1)
+    Cc = x.shape[-1]
+    if gamma.numel() != Cc:
+        raise DsEngineError("rmsnorm: gamma must have C elements")
+    out = torch.empty_like(x) if out is None else _req(out, bf16, "rmsnorm.out")
+    if out.numel() != x.numel():
+        raise DsEngineError("rmsnorm: out must match x")
+    check(lib.ds_rmsnorm(x.data_ptr(), gamma.data_ptr(), out.data_ptr(), x.numel() // Cc, Cc, float(eps), _stream()),
+          "ds_rmsnorm")
+    return out
+
+
+def rope_kv_append(qkv: torch.Tensor, kv_layer: torch.Tensor, pos: torch.Tensor, heads: int, theta: float,
+                   q_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Rotary embedding of the fused projection ``qkv`` [M, 3*heads*D] at positions ``pos[0] + m`` (``pos``: int32
+    device tensor): returns rotated q [M, heads*D] and appends rotated k / v to ``kv_layer`` [2, heads, L_max, D]."""
+    _req(qkv, bf16, "rope_kv_append.qkv")
+    _req(kv_layer, bf16, "rope_kv_append.kv_layer", 4)
+    _req(pos, torch.int32, "rope_kv_append.pos")
+    _, H, L_max, D = kv_layer.shape
+    M = qkv.numel() // qkv.shape[-1]
+    if H != heads or qkv.shape[-1] != 3 * H * D:
+        raise DsEngineError("rope_kv_append: qkv must be [M, 3*heads*D] for a [2, heads, L_max, D] cache")
+    q_out = torch.empty(M, H * D, dtype=bf16, device=qkv.device) if q_out is None else _req(q_out, bf16, "rope.q_out")
+    check(lib.ds_rope_kv_append(qkv.data_ptr(), q_out.data_ptr(), kv_layer.data_ptr(), pos.data_ptr(), M, H, D, L_max,
+                                float(theta), _stream()), "ds_rope_kv_append")
+    return q_out
+
+
+ATTN_KV_CHUNK = 256            # keys per split of ds_attention_kv when several splits run
+
+
+def attention_kv_splits(M: int, L_max: int) -> int:
+    """Key splits ds_attention_kv runs with: a decode row (M == 1) spreads its keys over many CTAs; a prefill already
+    has M * heads CTAs, so each row takes its keys in one split."""
+    return -(-L_max // ATTN_KV_CHUNK) if M == 1 else 1
+
+
+def attention_kv(q: torch.Tensor, kv_layer: torch.Tensor, pos: torch.Tensor, ws: Optional[torch.Tensor] = None,
+                 out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """softmax(q K^T / sqrt(D)) V of query rows at positions pos[0] + m against cache keys 0 .. pos[0] + m:
+    q [M, heads*D] bf16, ``kv_layer`` [2, heads, L_max, D]; ``ws`` fp32 workspace (allocated when None)."""
+    _req(q, bf16, "attention_kv.q")
+    _req(kv_layer, bf16, "attention_kv.kv_layer", 4)
+    _req(pos, torch.int32, "attention_kv.pos")
+    _, H, L_max, D = kv_layer.shape
+    M = q.numel() // (H * D)
+    if q.shape[-1] != H * D:
+        raise DsEngineError("attention_kv: q must be [M, heads*D]")
+    splits = attention_kv_splits(M, L_max)
+    chunk = -(-L_max // splits)
+    need = M * H * splits * (D + 2)
+    if ws is None:
+        ws = torch.empty(need, dtype=f32, device=q.device)
+    _req(ws, f32, "attention_kv.ws")
+    out = torch.empty(M, H * D, dtype=bf16, device=q.device) if out is None else _req(out, bf16, "attention_kv.out")
+    check(lib.ds_attention_kv(q.data_ptr(), kv_layer.data_ptr(), out.data_ptr(), ws.data_ptr(), ws.numel() * 4,
+                              pos.data_ptr(), M, H, D, L_max, chunk, _stream()), "ds_attention_kv")
+    return out
+
+
+def silu_mul(gate_up: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """silu(g) * u of the fused [M, 2I] = [g | u] projection -> [M, I]."""
+    _req(gate_up, bf16, "silu_mul.gate_up")
+    I2 = gate_up.shape[-1]
+    M = gate_up.numel() // I2
+    out = torch.empty(M, I2 // 2, dtype=bf16, device=gate_up.device) if out is None else _req(out, bf16, "silu_mul.out")
+    check(lib.ds_silu_mul(gate_up.data_ptr(), out.data_ptr(), M, I2 // 2, _stream()), "ds_silu_mul")
+    return out
+
+
+def agent_next_token(logits: torch.Tensor, img_ids: torch.Tensor, state: torch.Tensor, out_ids: torch.Tensor,
+                     max_new: int, eos: int, embed: torch.Tensor, next_x: torch.Tensor,
+                     hidden_src: Optional[torch.Tensor], hidden: torch.Tensor) -> None:
+    """One greedy step at batch 1 on the device (include/dsengine.h ds_agent_next_token): ``logits`` fp32 [V] are
+    rewritten in place by the image-token rule; ``state`` int32 {pos, generated, done, last token}."""
+    _req(logits, f32, "agent_next_token.logits")
+    _req(img_ids, torch.int32, "agent_next_token.img_ids")
+    _req(state, torch.int32, "agent_next_token.state")
+    _req(out_ids, torch.int32, "agent_next_token.out_ids")
+    _req(embed, bf16, "agent_next_token.embed", 2)
+    _req(next_x, bf16, "agent_next_token.next_x")
+    _req(hidden, bf16, "agent_next_token.hidden", 2)
+    V, Cc = embed.shape
+    if logits.numel() != V or next_x.numel() != Cc or hidden.shape[1] != Cc or state.numel() < 4 or \
+            out_ids.numel() < max_new:
+        raise DsEngineError("agent_next_token: shape mismatch")
+    if hidden_src is not None:
+        _req(hidden_src, bf16, "agent_next_token.hidden_src")
+    check(lib.ds_agent_next_token(logits.data_ptr(), V, img_ids.data_ptr(), img_ids.numel(), state.data_ptr(),
+                                  out_ids.data_ptr(), int(max_new), int(eos), embed.data_ptr(), next_x.data_ptr(),
+                                  _ptr(hidden_src), hidden.data_ptr(), Cc, _stream()), "ds_agent_next_token")
+
+
 # ---------------------------------------------------------------------------------------------- VAE decoder helpers
 def latent_pointwise(latents: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], inv_scale: float) -> torch.Tensor:
     """(latents * inv_scale) through a 1x1 conv 4 -> 4: fp32 NCHW [B,4,H,W] -> bf16 NHWC [B,H,W,4]."""

@@ -20,7 +20,7 @@ from typing import Dict, List, Tuple
 
 import torch
 
-from .config import ResamplerConfig, UNetConfig, VaeConfig
+from .config import AgentConfig, ResamplerConfig, UNetConfig, VaeConfig
 
 Shape = Tuple[int, ...]
 
@@ -191,8 +191,49 @@ def vae_decoder_param_shapes(vc: VaeConfig) -> Dict[str, Shape]:
     return sh
 
 
+def agent_param_shapes(ac: AgentConfig) -> Dict[str, Shape]:
+    """transformers ``LlamaForCausalLM`` keys (no biases)."""
+    C, I, V = ac.hidden_size, ac.intermediate_size, ac.vocab_size
+    sh: Dict[str, Shape] = {"model.embed_tokens.weight": (V, C)}
+    for i in range(ac.num_hidden_layers):
+        p = f"model.layers.{i}"
+        for nm in ("q_proj", "k_proj", "v_proj", "o_proj"):
+            sh[f"{p}.self_attn.{nm}.weight"] = (C, C)
+        sh[f"{p}.mlp.gate_proj.weight"] = (I, C)
+        sh[f"{p}.mlp.up_proj.weight"] = (I, C)
+        sh[f"{p}.mlp.down_proj.weight"] = (C, I)
+        sh[f"{p}.input_layernorm.weight"] = (C,)
+        sh[f"{p}.post_attention_layernorm.weight"] = (C,)
+    sh["model.norm.weight"] = (C,)
+    sh["lm_head.weight"] = (V, C)
+    return sh
+
+
+def agent_packing(ac: AgentConfig) -> Dict[str, Tuple[str, int]]:
+    """Where each LLaMA checkpoint tensor lands in the engine's packed weights: key -> (packed name, first row).
+    q|k|v are fused into one [3C][C] projection (``layers.{i}.qkv``) and gate|up into one [2I][C]
+    (``layers.{i}.gate_up``), so a decode step streams each layer in four GEMVs; every other tensor keeps its shape
+    (``row`` 0).  Packed names: ``embed``, ``norm``, ``lm_head``, ``layers.{i}.{qkv,o,gate_up,down,ln1,ln2}``."""
+    C, I = ac.hidden_size, ac.intermediate_size
+    pk: Dict[str, Tuple[str, int]] = {"model.embed_tokens.weight": ("embed", 0), "model.norm.weight": ("norm", 0),
+                                      "lm_head.weight": ("lm_head", 0)}
+    for i in range(ac.num_hidden_layers):
+        p, q = f"model.layers.{i}", f"layers.{i}"
+        for j, nm in enumerate(("q_proj", "k_proj", "v_proj")):
+            pk[f"{p}.self_attn.{nm}.weight"] = (f"{q}.qkv", j * C)
+        pk[f"{p}.self_attn.o_proj.weight"] = (f"{q}.o", 0)
+        pk[f"{p}.mlp.gate_proj.weight"] = (f"{q}.gate_up", 0)
+        pk[f"{p}.mlp.up_proj.weight"] = (f"{q}.gate_up", I)
+        pk[f"{p}.mlp.down_proj.weight"] = (f"{q}.down", 0)
+        pk[f"{p}.input_layernorm.weight"] = (f"{q}.ln1", 0)
+        pk[f"{p}.post_attention_layernorm.weight"] = (f"{q}.ln2", 0)
+    return pk
+
+
 def _is_norm(key: str) -> bool:
     parts = key.split(".")
+    if parts[-2:-1] and parts[-2] in ("input_layernorm", "post_attention_layernorm"):     # LLaMA RMSNorms
+        return True
     return any(p.startswith("norm") or p in ("conv_norm_out", "group_norm") for p in parts[-2:-1]) or \
         (len(parts) >= 2 and parts[-2] == "0" and "layers" in parts)   # Resampler FF LayerNorm "layers.i.1.0"
 

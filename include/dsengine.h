@@ -348,6 +348,45 @@ int ds_attention_small(const void* q, const void* k, const void* v, void* out, i
 int ds_embed_tokens(const int* ids, const void* tok_emb, const void* pos_emb, void* out, int B, int L, int C, int vocab,
                     void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * LLaMA decoder of the MLLM agent (SURVEY.md §8f-4: ContinuousLVLM.generate, src/models/mllm/seed_x.py:90-171, over
+ * LlamaForCausalLM of src/models/mllm/modeling_llama_xformer.py).  Every kernel that depends on the sequence position
+ * reads it from a DEVICE int32 (`pos`), so one captured graph serves every decode step.
+ *   ds_gemv_bf16       : y[M][N] = x[M][K] W[N][K]^T (+ residual[M][N]), bf16 in, fp32 accumulation, bf16 or fp32
+ *                        (out_fp32) out, 1 <= M <= 8, K % 8 == 0, M*K*2 bytes <= 227 KB.  W is streamed once with
+ *                        16-byte non-allocating loads; x is staged in shared memory.  y may alias residual.
+ *                        The decode linears (fused q|k|v, o_proj, fused gate|up, down_proj, lm_head).  [HBM-bound]
+ *   ds_rmsnorm         : LlamaRMSNorm: y = x * rsqrt(mean(x^2) + eps) * gamma, fp32 statistics, one rounding to
+ *                        bf16; x / y bf16 [rows][C], gamma fp32 [C]; C % 8 == 0, C <= 8192.
+ *   ds_rope_kv_append  : qkv bf16 [M][3][H][D] (the fused projection); row m has position *pos + m.  Rotates q and k
+ *                        (rotate-half, inv_freq = theta^(-2i/D) in fp32), writes q_out bf16 [M][H][D] and appends the
+ *                        rotated k and v to kv_layer bf16 [2][H][L_max][D] (one layer of a [layer][2][H][L_max][D]
+ *                        cache).  Rows at positions >= L_max are skipped.  D = 64 or 128.
+ *   ds_attention_kv    : out[m] = softmax(q[m] K^T / sqrt(D)) V over cache keys 0 .. *pos + m (bottom-right causal),
+ *                        q / out bf16 [M][H][D].  Keys are cut into ceil(L_max / chunk) splits of `chunk` keys that
+ *                        run on separate CTAs (splits past the current length exit at once) and a combine pass merges
+ *                        them; ws: fp32 workspace of >= M * H * splits * (D + 2) * 4 bytes.  D = 64 or 128.
+ *   ds_silu_mul        : out[m][i] = silu(g[m][i]) * u[m][i] from gate_up bf16 [M][2I] = [g | u]; I % 8 == 0.
+ *   ds_agent_next_token: one greedy step at batch 1.  state: int32 {pos, generated, done, last token}.  When done is
+ *                        set the call changes nothing.  Otherwise: hidden[pos] = hidden_src (bf16 [C], skipped when
+ *                        NULL); the image-token rule of AutoImageTokenGenerationProcessor (src/models/mllm/
+ *                        generation.py:18-30) on logits fp32 [V], IN PLACE: if `last` is in img_ids[0 .. n_img-2],
+ *                        the next entry's score becomes max + 10, else the scores of img_ids[1 ..] become 0.0; then
+ *                        tok = argmax (first index on ties); out_ids[generated] = tok; next_x = embed[tok] (bf16
+ *                        [V][C]); pos += 1; generated += 1; last = tok; done = (tok == eos || generated >= max_new).
+ * --------------------------------------------------------------------------------------------- */
+int ds_gemv_bf16(const void* x, const void* w, const void* residual, void* y, int M, int N, int K, int out_fp32,
+                 void* stream);
+int ds_rmsnorm(const void* x, const float* gamma, void* y, int rows, int C, float eps, void* stream);
+int ds_rope_kv_append(const void* qkv, void* q_out, void* kv_layer, const int* pos, int M, int H, int D, int L_max,
+                      float theta, void* stream);
+int ds_attention_kv(const void* q, const void* kv_layer, void* out, float* ws, int64_t ws_bytes, const int* pos, int M,
+                    int H, int D, int L_max, int chunk, void* stream);
+int ds_silu_mul(const void* gate_up, void* out, int M, int I, void* stream);
+int ds_agent_next_token(float* logits, int V, const int* img_ids, int n_img, int* state, int* out_ids, int max_new,
+                        int eos, const void* embed, void* next_x, const void* hidden_src, void* hidden, int C,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif

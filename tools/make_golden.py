@@ -11,7 +11,8 @@ Nothing is copied into this repository: the reference code is imported/executed 
 its seeded inputs and outputs are saved.  /root/reference does not exist on the GPU box, so the fixtures are
 committed; re-run this script only in the build container:
 
-    python tools/make_golden.py
+    python tools/make_golden.py            # every fixture
+    python tools/make_golden.py agent      # tests/golden/agent_generate.pt only
 """
 from __future__ import annotations
 
@@ -237,5 +238,135 @@ def main():
         print(f, os.path.getsize(os.path.join(OUT, f)))
 
 
+class StubTokenizer:
+    """A LlamaTokenizer stand-in for the agent fixture: ``encode`` puts the leading sentencepiece "▁" piece in front
+    (what the reference's ``encode(EOI_TOKEN)[1]`` relies on); ``<img>``, ``<img_00000>`` .. and ``</img>`` are single
+    ids; any other character is one id."""
+    SPACE, BOI, IMG0, EOI = 29, 900, 901, 965
+
+    def encode(self, s, add_special_tokens=False):
+        ids, i = [self.SPACE], 0
+        while i < len(s):
+            if s.startswith("<img>", i):
+                ids.append(self.BOI); i += 5
+            elif s.startswith("</img>", i):
+                ids.append(self.EOI); i += 6
+            elif s.startswith("<img_", i):
+                ids.append(self.IMG0 + int(s[i + 5:i + 10])); i += 11
+            else:
+                ids.append(100 + ord(s[i]) % 50); i += 1
+        return ids
+
+    def decode(self, ids, skip_special_tokens=True):
+        return " ".join(str(int(x)) for x in ids)
+
+
+AGENT_LLAMA = dict(vocab_size=1000, hidden_size=256, intermediate_size=688, num_hidden_layers=2, num_attention_heads=2,
+                   max_position_embeddings=512, rms_norm_eps=1e-5, bos_token_id=1, eos_token_id=2, pad_token_id=0)
+
+
+@torch.no_grad()
+def agent_golden():
+    """tests/golden/agent_generate.pt: the reference's ContinuousLVLM.generate + AutoImageTokenGenerationProcessor +
+    QwenResampler EXECUTED on a seeded tiny transformers LlamaForCausalLM (oracle.agent.seeded_llama regenerates it)."""
+    sys.path.insert(0, REF)
+    sys.path.insert(1, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+    from src.models.mllm.seed_x import ContinuousLVLM
+    from src.models.qwen_resampler import QwenResampler
+    from oracle.agent import image_token_rule, seeded_llama, seeded_qwen_sd
+    tok = StubTokenizer()
+    img_ids = tok.encode("<img>" + "".join(f"<img_{i:05d}>" for i in range(64)) + "</img>")
+    rkw_in = dict(grid_size=8, embed_dim=256, num_heads=4, kv_dim=64)
+    rkw_out = dict(grid_size=8, embed_dim=64, num_heads=4, kv_dim=256)
+    cases = []
+    # (name, llm seed, prompt text ids, ends in <img>, max_new_tokens, eos override)
+    for name, seed, ends_boi, max_new, eos in (("free", 3, False, 120, 2), ("forced", 4, True, 100, 2),
+                                                ("max_new", 5, True, 40, 2)):
+        llm, _ = seeded_llama(AGENT_LLAMA, seed)
+        llm.generation_config.eos_token_id = eos
+        torch.manual_seed(seed + 100)
+        inp, outp = QwenResampler(**rkw_in).eval(), QwenResampler(**rkw_out).eval()
+        g = torch.Generator().manual_seed(seed + 200)
+        for m, kw in ((inp, rkw_in), (outp, rkw_out)):
+            sd = seeded_qwen_sd(kw, g)
+            assert list(sd) == list(m.state_dict()), "state-dict order differs from the restatement"
+            m.load_state_dict(sd)
+        text = [100 + (7 * k + seed) % 50 for k in range(10)]
+        ids = [1] + text + [tok.BOI] + list(range(tok.IMG0, tok.IMG0 + 64)) + [tok.EOI] + [110] + \
+            ([tok.BOI] if ends_boi else [120])
+        ids = torch.tensor([ids])
+        cmp = torch.zeros_like(ids, dtype=torch.bool)
+        cmp[0, 12:76] = True
+        img = torch.randn(1, 64, 64, generator=g).to(torch.bfloat16).float()
+        agent = ContinuousLVLM(llm, inp, outp).eval()
+        o = agent.generate(tok, input_ids=ids, image_embeds=img, ids_cmp_mask=cmp, max_new_tokens=max_new,
+                           num_img_gen_tokens=64)
+        # top-2 margins of the free steps, teacher-forced over the reference's own raw sequence
+        emb = llm.get_input_embeddings()(ids).clone()
+        emb[cmp] = inp(img).reshape(-1, 256)
+        seq_raw = _raw_sequence(llm, ids, emb, img_ids, eos, max_new)
+        full = torch.cat([emb, llm.get_input_embeddings()(seq_raw[None, :-1])], 1)
+        logits = llm(inputs_embeds=full).logits[0, ids.shape[1] - 1:].float()
+        margins, last = {}, int(ids[0, -1])
+        for t in range(seq_raw.numel()):
+            s = image_token_rule(last, logits[t].clone(), img_ids)
+            if last not in img_ids[:-1]:
+                top = s.topk(2).values
+                margins[t] = float(top[0] - top[1])
+            last = int(seq_raw[t])
+        cases.append({"name": name, "llm_seed": seed, "llama": AGENT_LLAMA, "resampler_seed": seed + 200,
+                      "input_resampler": rkw_in, "output_resampler": rkw_out, "input_ids": ids, "ids_cmp_mask": cmp,
+                      "image_embeds": img, "img_ids": img_ids, "eos": eos, "max_new_tokens": max_new,
+                      "raw_ids": seq_raw, "output_ids": o["output_ids"].clone(), "ids_gen_mask": o["ids_gen_mask"],
+                      "num_gen_imgs": o["num_gen_imgs"], "img_gen_feat": o["img_gen_feat"], "margins": margins})
+        print(name, "new tokens", o["output_ids"].numel(), "images", o["num_gen_imgs"],
+              "min free margin", min(margins.values()) if margins else None)
+    # canned: llm.generate returns fixed sequences / hidden states; EOIs at 30 (< 64: skipped), 100 and 170
+    n_new, C = 180, 256
+    gc = torch.Generator().manual_seed(9)
+    prompt = torch.tensor([[1, 101, 102, 103]])
+    new = torch.randint(100, 150, (n_new,), generator=gc)
+    for e in (30, 100, 170):
+        new[e] = tok.EOI
+    hid = [torch.randn(1, prompt.shape[1], C, generator=gc)] + [torch.randn(1, 1, C, generator=gc)
+                                                                  for _ in range(n_new - 1)]
+
+    class CannedLLM(torch.nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.emb = torch.nn.Embedding(1000, C)
+            self.dtype_ = torch.float32
+
+        @property
+        def dtype(self):
+            return torch.float32
+
+        def get_input_embeddings(self):
+            return self.emb
+
+        def generate(self, input_ids=None, **kw):
+            return types.SimpleNamespace(sequences=torch.cat([input_ids, new[None]], 1),
+                                         hidden_states=tuple((h,) for h in hid))
+
+    torch.manual_seed(10)
+    outp = QwenResampler(**rkw_out).eval()
+    agent = ContinuousLVLM(CannedLLM(), QwenResampler(**rkw_in).eval(), outp).eval()
+    o = agent.generate(tok, input_ids=prompt, max_new_tokens=n_new, num_img_gen_tokens=64)
+    canned = {"prompt": prompt, "new_ids": new, "hidden_seed": 9,
+              "img_ids": img_ids, "output_ids": o["output_ids"].clone(), "ids_gen_mask": o["ids_gen_mask"],
+              "num_gen_imgs": o["num_gen_imgs"], "text": o["text"],
+              "run_feats": torch.stack([torch.cat([h[0] for h in hid], 0)[prompt.shape[1]:][s:s + 64]
+                                        for s in (36, 106)])}
+    torch.save({"cases": cases, "canned": canned}, f"{OUT}/agent_generate.pt")
+    print("agent_generate.pt", os.path.getsize(f"{OUT}/agent_generate.pt"))
+
+
+def _raw_sequence(llm, ids, emb, img_ids, eos, max_new):
+    from oracle.agent import greedy
+    return greedy(llm, ids, emb, img_ids, eos, max_new)[0]
+
+
 if __name__ == "__main__":
+    if sys.argv[1:] == ["agent"]:
+        sys.exit(agent_golden())
     sys.exit(main())
