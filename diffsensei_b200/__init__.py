@@ -8,6 +8,8 @@ Public surface (mirrors the reference's, SURVEY.md §8b):
     ClipTextEncoderEngine, ClipVisionEncoderEngine, VitMaeEncoderEngine  <- transformers CLIP / ViT-MAE encoders as
                               used by encode_prompt (:232-245) and prepare_ip_image_embeds (:125-128)
     DiffSenseiPipeline     <- src/pipelines/pipeline_diffsensei.py  (denoise loop)
+    DDIMScheduler, EulerDiscreteScheduler, scheduler_from_config  <- the diffusers schedulers a checkpoint's
+                              scheduler_config.json may name (SDXL-base configuration only)
     AgentEngine, LlamaEngine  <- src/models/mllm/seed_x.py ContinuousLVLM (greedy LLaMA generate of the MLLM agent)
     ops                    -- tensor-level wrappers over the C ABI in include/dsengine.h
 
@@ -24,7 +26,7 @@ from .encoders import (CLIP_L_TEXT, CLIP_VIT_H, MAGI_VIT_MAE, OPENCLIP_BIGG_TEXT
                        ClipVisionEncoderEngine, EncoderConfig, VitMaeEncoderEngine)
 from .pipeline import DiffSenseiPipeline  # noqa: F401
 from .resampler import QwenResamplerEngine, ResamplerEngine  # noqa: F401
-from .scheduler import DDIMScheduler  # noqa: F401
+from .scheduler import DDIMScheduler, EulerDiscreteScheduler, scheduler_from_config  # noqa: F401
 from .unet import UNet2DConditionOutput, UNetMangaEngine  # noqa: F401
 from .vae import VaeDecoderEngine  # noqa: F401
 

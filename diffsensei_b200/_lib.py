@@ -78,6 +78,7 @@ SIGNATURES = {
     "ds_silu": [_vp, _vp, _i64, _vp],
     "ds_timestep_embedding": [_vp, _vp, _i, _i, _vp],
     "ds_cfg_ddim_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp],
+    "ds_cfg_euler_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp],
     "ds_resampler_attn": [_vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "ds_attention_small": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i64, _i64, _i64, _i64, _f, _i, _vp],
     "ds_embed_tokens": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],

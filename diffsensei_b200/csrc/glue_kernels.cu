@@ -1,6 +1,6 @@
 // glue_kernels.cu — small HBM-bound kernels around the tensor-core ops: conv_in (Cin = 4), layout changes at
 // the diffusers-facing boundary, nearest upsample, channel concat, SiLU, sinusoidal timestep features, and the
-// fused CFG + DDIM update.  All vectorised to 16-byte accesses where the shape allows.
+// fused CFG + DDIM and CFG + Euler updates.  All vectorised to 16-byte accesses where the shape allows.
 #include "ds_common.cuh"
 #include "ds_host.h"
 
@@ -192,6 +192,40 @@ __global__ void cfg_ddim_kernel(const uint2* __restrict__ noise_pred, float4* __
   model_in[n_pix + i] = o;
 }
 
+// ------------------------------------------------------------------------------------------------
+// CFG blend + Euler step (s_churn = 0, epsilon prediction) + the next step's scale_model_input,
+// src/pipelines/pipeline_diffsensei.py:315-317,332-337.  coef = {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1)}.
+// Every operation is rounded on its own (no FMA contraction), in diffusers' order, so the update is the one its
+// fp32 eager ops compute.  C == 4: one thread per pixel (8-byte bf16 vectors, 16-byte fp32 vector).
+// ------------------------------------------------------------------------------------------------
+__global__ void cfg_euler_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
+                                 uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
+                                 long long n_pix /* bs*HW */) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n_pix) return;
+  const float sigma = coef[0], sigma_next = coef[1], in_div = coef[2];
+  const float dt = __fsub_rn(sigma_next, sigma);
+  const uint2 eu = __ldg(noise_pred + i);          // uncond half
+  const uint2 et = __ldg(noise_pred + n_pix + i);  // text half
+  const float u[4] = {bf16_lo(eu.x), bf16_hi(eu.x), bf16_lo(eu.y), bf16_hi(eu.y)};
+  const float tt[4] = {bf16_lo(et.x), bf16_hi(et.x), bf16_lo(et.y), bf16_hi(et.y)};
+  float4 x = latents[i];
+  float xv[4] = {x.x, x.y, x.z, x.w};
+  float sv[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float eps = __fadd_rn(u[j], __fmul_rn(guidance, __fsub_rn(tt[j], u[j])));
+    const float x0 = __fsub_rn(xv[j], __fmul_rn(sigma, eps));
+    const float d = __fdiv_rn(__fsub_rn(xv[j], x0), sigma);
+    xv[j] = __fadd_rn(xv[j], __fmul_rn(d, dt));
+    sv[j] = __fdiv_rn(xv[j], in_div);
+  }
+  latents[i] = make_float4(xv[0], xv[1], xv[2], xv[3]);
+  const uint2 o = make_uint2(pack_bf16(sv[0], sv[1]), pack_bf16(sv[2], sv[3]));
+  model_in[i] = o;
+  model_in[n_pix + i] = o;
+}
+
 }  // namespace ds
 
 using namespace ds;
@@ -345,5 +379,19 @@ extern "C" int ds_cfg_ddim_step(const void* noise_pred, float* latents, void* mo
       static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
       guidance, n_pix);
   DS_LAUNCH_OK("cfg_ddim_kernel");
+  return DS_OK;
+}
+
+extern "C" int ds_cfg_euler_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
+                                 float guidance, int bs, int HW, int C, void* stream) {
+  DS_REQUIRE(noise_pred && latents && model_in && coef, "ds_cfg_euler_step: NULL pointer");
+  DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "ds_cfg_euler_step: only C == 4 latents are supported (got C=%d)", C);
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  const long long n_pix = static_cast<long long>(bs) * HW;
+  cfg_euler_kernel<<<static_cast<unsigned>((n_pix + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
+      guidance, n_pix);
+  DS_LAUNCH_OK("cfg_euler_kernel");
   return DS_OK;
 }

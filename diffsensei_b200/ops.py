@@ -573,6 +573,21 @@ def cfg_ddim_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: to
                                float(guidance), bs, H * W, Cc, _stream()), "ds_cfg_ddim_step")
 
 
+def cfg_euler_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
+                    guidance: float) -> None:
+    """In place: latents (fp32 NHWC [bs,H,W,4]) <- Euler(CFG(noise_pred)); model_in (bf16 [2bs,H,W,4]) <-
+    cat[x / coef[2]]*2.  coef: fp32 {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1)} on the device."""
+    _req(noise_pred, bf16, "cfg_euler_step.noise_pred", 4)
+    _req(latents, f32, "cfg_euler_step.latents", 4)
+    _req(model_in, bf16, "cfg_euler_step.model_in", 4)
+    _req(coef, f32, "cfg_euler_step.coef", 1)
+    bs, H, W, Cc = latents.shape
+    if noise_pred.shape != (2 * bs, H, W, Cc) or model_in.shape != (2 * bs, H, W, Cc) or coef.numel() < 3:
+        raise DsEngineError("cfg_euler_step: shape mismatch")
+    check(lib.ds_cfg_euler_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(),
+                                float(guidance), bs, H * W, Cc, _stream()), "ds_cfg_euler_step")
+
+
 # ---------------------------------------------------------------------------------------------- encoder helpers
 def attention_small(qkv: torch.Tensor, heads: int, causal: bool = False, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """softmax(Q K^T / sqrt(d) [+ causal]) V from a fused projection ``qkv`` [B, N, 3*heads*d] (N <= 320, d % 8 == 0,

@@ -13,28 +13,31 @@ the reference's keyword surface but takes their OUTPUTS as tensors (``prompt_emb
 
 Loop structure on the GPU (one process per GPU, one stream):
   once per panel : K|V projections of text and IP tokens for all cross-attention layers, time-embedding
-                   row-bias table for all T steps, (alpha_t, alpha_prev) table
-  per step       : ONE CUDA-graph replay = UNet forward (NHWC bf16) + fused CFG/DDIM update, preceded by two
-                   tiny device-to-device copies that select this step's row of the two tables.
+                   row-bias table for all T steps, the scheduler's coefficient table
+  per step       : ONE CUDA-graph replay = UNet forward (NHWC bf16) + the scheduler's fused CFG update (DDIM or
+                   Euler), preceded by two tiny device-to-device copies that select this step's row of the two tables.
+The scheduler is ``pipe.scheduler``: DDIM by default, or whichever ``scheduler_from_config`` returns for a
+checkpoint's scheduler config.
 """
 from __future__ import annotations
 
 import os
 
 from types import SimpleNamespace
-from typing import List, Optional
+from typing import List, Optional, Union
 
 import torch
 
 from . import ops
-from .scheduler import DDIMScheduler
+from .scheduler import DDIMScheduler, EulerDiscreteScheduler
 from .unet import UNetMangaEngine
 
 bf16, f32 = torch.bfloat16, torch.float32
 
 
 class DiffSenseiPipeline:
-    def __init__(self, unet: UNetMangaEngine, scheduler: Optional[DDIMScheduler] = None, vae_scale_factor: int = 8,
+    def __init__(self, unet: UNetMangaEngine,
+                 scheduler: Optional[Union[DDIMScheduler, EulerDiscreteScheduler]] = None, vae_scale_factor: int = 8,
                  default_sample_size: int = 128, vae=None, text_encoder=None, text_encoder_2=None, image_encoder=None):
         self.unet = unet
         self.vae = vae                      # VaeDecoderEngine (or None: latents out only)
@@ -47,7 +50,8 @@ class DiffSenseiPipeline:
         self.image_proj_model = None
         self.magi_image_encoder = None
         self._guidance_scale = 5.0
-        # captured steppers, keyed by everything a CUDA graph bakes in (shapes, T, guidance, ip scales, dialog mode):
+        # captured steppers, keyed by everything a CUDA graph bakes in (shapes, T, guidance, ip scales, dialog mode,
+        # scheduler class and config):
         # panels of one shape re-use the graph and only refill its static buffers (DenoiseStepper.load_panel)
         self._steppers = {}
         self.max_cached_steppers = 8
@@ -179,7 +183,8 @@ class DiffSenseiPipeline:
         (no re-capture), otherwise a new one is built and cached."""
         key = (tuple(latents.shape), tuple(prompt_embeds.shape), None if dialog_bbox is None else
                (tuple(dialog_bbox.shape), dialog_bbox.dtype == bf16), float(aspect_ratio), int(num_inference_steps),
-               float(guidance_scale), self.unet.scales_key(), chains, self.unet._ip_weights_version())
+               float(guidance_scale), self.unet.scales_key(), chains, self.unet._ip_weights_version(),
+               type(self.scheduler).__name__, tuple(sorted(self.scheduler.config.items())))
         st = self._steppers.get(key)
         if st is None:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
@@ -259,12 +264,15 @@ class DiffSenseiPipeline:
         if guidance_scale <= 1.0:
             raise ValueError("guidance_scale <= 1 disables classifier-free guidance on the reference "
                              "(pipeline_diffsensei.py:315-334: text-only batch, no blend); the engine's denoise step is "
-                             "the fused CFG + DDIM update and does not implement the guidance-free variant")
+                             "the fused CFG + scheduler update and does not implement the guidance-free variant")
         self._guidance_scale = guidance_scale
         self.set_ip_scale(ip_scale)
         dev = self.unet.device
+        self.scheduler.set_timesteps(num_inference_steps, device=dev)    # :248 (init_noise_sigma depends on it)
         if latents is None:
             latents = self.prepare_latents(num_samples, self.unet.config.in_channels, height, width, generator)
+        else:
+            latents = latents * self.scheduler.init_noise_sigma          # diffusers' prepare_latents
         neg_img, img, neg_bbox, bbox = self.prepare_ip_image_embeds(clip_image_embeds, magi_image_embeds,
                                                                     ip_image_embeds, list(ip_bbox), num_samples)
         aspect_ratio = latents.shape[-2] / latents.shape[-1]                            # :272
@@ -298,8 +306,10 @@ class DenoiseStepper:
     """Per-panel state of the denoise loop (pipeline_diffsensei.py:306-337), resident on one GPU.
 
     Construction does everything that is timestep-invariant: the K|V projections of the text / IP tokens for all
-    cross-attention layers, the time-embedding row-bias table and the DDIM coefficient table for all T steps, and
-    (``use_graph``) captures ONE iteration — UNet forward + fused CFG/DDIM update — into a CUDA graph.
+    cross-attention layers, the time-embedding row-bias table and the scheduler's coefficient table for all T steps,
+    and (``use_graph``) captures ONE iteration — UNet forward + the scheduler's fused CFG update — into a CUDA graph.
+    Departure: the latents stay an fp32 master copy between steps, where the reference casts ``prev_sample`` back to
+    the UNet dtype.
     ``step(i)`` runs iteration i on device-resident latents; ``step_host(i, x)`` is the same call with HOST
     buffers (pinned fp32 NCHW latents in, updated latents out), i.e. what a caller on the other side of the
     plugin boundary sees.
@@ -314,7 +324,9 @@ class DenoiseStepper:
         self.num_inference_steps = int(num_inference_steps)
         self.aspect_ratio = float(aspect_ratio)
         self.timesteps = pipe.scheduler.set_timesteps(num_inference_steps, device=dev)
-        self.coef_table = pipe.scheduler.coefficient_table(dev)                         # [T, 2]
+        self.coef_table = pipe.scheduler.coefficient_table(dev)                         # [T, 2] DDIM, [T, 3] Euler
+        # scale_model_input's divisor per step; dividing by a device element is a true division, as in the kernels
+        self.in_div = torch.tensor(pipe.scheduler.model_input_divisors(), dtype=f32, device=dev)
         self.cond = None
         self.lat = self.model_in = self.db = self.temb_table = None
         self.round_bf16 = True
@@ -365,16 +377,17 @@ class DenoiseStepper:
         self.cond = unet.prepare_conditions(prompt_embeds.to(dev), bbox, self.aspect_ratio, out=self.cond)
         self.temb_table = unet.time_rowbias_table(self.timesteps, add_text_embeds, add_time_ids)   # [T, 2bs, sumC]
         lat = latents.to(device=dev, dtype=f32).permute(0, 2, 3, 1).contiguous()         # fp32 NHWC master copy
+        x = lat / self.in_div[0]                                                        # :317 (x / 1.0 for DDIM)
         first = self.lat is None
         if first:
             self.lat = lat
-            self.model_in = torch.cat([lat, lat]).to(bf16).contiguous()                 # :315 (first step only)
+            self.model_in = torch.cat([x, x]).to(bf16).contiguous()                     # :315 (first step only)
         else:
             if lat.shape != self.lat.shape or (dialog_bbox is None) != (self.db is None):
                 raise ValueError("load_panel: latent shape / dialog_bbox presence differs from the captured panel")
             self.lat.copy_(lat)
-            self.model_in[:bs].copy_(lat)
-            self.model_in[bs:].copy_(lat)
+            self.model_in[:bs].copy_(x)
+            self.model_in[bs:].copy_(x)
         if dialog_bbox is not None:
             rb = dialog_bbox.dtype == bf16
             db = dialog_bbox.to(device=dev, dtype=f32).contiguous()
@@ -409,7 +422,7 @@ class DenoiseStepper:
             finally:
                 ops.SPLITK = prev_splitk
                 ops.GEMM_CHAINS = prev_chains
-        ops.cfg_ddim_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance)   # :332-337 (+ :315 of next)
+        self.scheduler.fused_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance)  # :332-337, :315-317
 
     @torch.no_grad()
     def step(self, i: int) -> None:
@@ -429,8 +442,9 @@ class DenoiseStepper:
         nhwc = self._host_in.permute(0, 2, 3, 1)
         self.lat.copy_(nhwc)
         bs = self.lat.shape[0]
-        self.model_in[:bs].copy_(nhwc)
-        self.model_in[bs:].copy_(nhwc)
+        x = nhwc / self.in_div[i]                                                       # step i's scale_model_input
+        self.model_in[:bs].copy_(x)
+        self.model_in[bs:].copy_(x)
         self.step(i)
         out_host.copy_(self.lat.permute(0, 3, 1, 2), non_blocking=True)                 # D2H
         torch.cuda.current_stream(self.dev).synchronize()

@@ -1,16 +1,32 @@
-"""DDIM schedule (host side).  The reference uses whatever scheduler the checkpoint ships
-(src/pipelines/pipeline_diffsensei.py:50,248-249,317,337); BASELINE.json fixes DDIM, so this mirrors diffusers'
-``DDIMScheduler`` under the SDXL scheduler config: scaled_linear betas 0.00085..0.012 over 1000 train steps,
-epsilon prediction, ``timestep_spacing="leading"``, ``steps_offset=1``, ``set_alpha_to_one=False``, no clipping,
-eta = 0.  ``scale_model_input`` is the identity and ``init_noise_sigma`` is 1 for DDIM.  The per-step update
-itself runs on the GPU, fused with the CFG blend (``ds_cfg_ddim_step``); this class only produces the
-timesteps and the (alpha_prod_t, alpha_prod_t_prev) table the kernel reads.
+"""Schedulers (host side).  The reference uses whatever scheduler the checkpoint ships
+(src/pipelines/pipeline_diffsensei.py:50,248-249,317,337).  Two are implemented, each under the scheduler config of
+stable-diffusion-xl-base-1.0 (scaled_linear betas 0.00085..0.012 over 1000 train steps, epsilon prediction,
+``timestep_spacing="leading"``, ``steps_offset=1``):
+
+* ``DDIMScheduler`` mirrors diffusers' ``DDIMScheduler`` with ``set_alpha_to_one=False``, no clipping, eta = 0.
+  ``scale_model_input`` is the identity and ``init_noise_sigma`` is 1.  BASELINE.json fixes it; it is the default.
+* ``EulerDiscreteScheduler`` mirrors diffusers' ``EulerDiscreteScheduler`` with ``interpolation_type="linear"``,
+  ``use_karras_sigmas=False`` and ``s_churn=0`` (no noise injection), the scheduler SDXL-base ships.
+
+``scheduler_from_config`` picks one from a checkpoint's ``scheduler/scheduler_config.json``, the way diffusers does,
+and rejects any class or value whose arithmetic is not implemented here.
+
+The per-step update itself runs on the GPU, fused with the CFG blend and the next step's input scaling
+(``ds_cfg_ddim_step`` / ``ds_cfg_euler_step``); these classes produce the timesteps, the per-step coefficient table
+the kernel reads (``coefficient_table``) and the divisor of the first step's UNet input (``model_input_divisors``).
 """
 from __future__ import annotations
 
 from typing import List, Tuple
 
 import torch
+
+from . import ops
+
+# stable-diffusion-xl-base-1.0 scheduler/scheduler_config.json, the values both classes implement
+_SDXL = {"num_train_timesteps": 1000, "beta_start": 0.00085, "beta_end": 0.012, "beta_schedule": "scaled_linear",
+         "trained_betas": None, "prediction_type": "epsilon", "timestep_spacing": "leading", "steps_offset": 1,
+         "rescale_betas_zero_snr": False}
 
 
 class DDIMScheduler:
@@ -25,6 +41,8 @@ class DDIMScheduler:
         self.steps_offset = steps_offset
         self.timesteps: List[int] = []
         self.num_inference_steps = 0
+        self.config = dict(_SDXL, num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
+                           steps_offset=steps_offset, set_alpha_to_one=False, clip_sample=False)
 
     def set_timesteps(self, num_inference_steps: int, device=None) -> List[int]:
         ratio = self.num_train_timesteps // num_inference_steps
@@ -44,3 +62,96 @@ class DDIMScheduler:
     def coefficient_table(self, device) -> torch.Tensor:
         """fp32 [T, 2] device tensor of (alpha_prod_t, alpha_prod_t_prev) in loop order."""
         return torch.tensor([self.coefficients(t) for t in self.timesteps], dtype=torch.float32, device=device)
+
+    def model_input_divisors(self) -> List[float]:
+        """scale_model_input(x, timesteps[i]) == x / model_input_divisors()[i]: the identity for DDIM."""
+        return [1.0] * len(self.timesteps)
+
+    def fused_step_(self, noise_pred, latents, model_in, coef, guidance: float) -> None:
+        ops.cfg_ddim_step_(noise_pred, latents, model_in, coef, guidance)
+
+
+class EulerDiscreteScheduler:
+    """diffusers' ``EulerDiscreteScheduler`` under the SDXL-base config, all schedule arithmetic in fp32:
+    sigma(t) = sqrt((1 - alpha_bar_t) / alpha_bar_t); sigma_i = sigma(timesteps[i]) with a final 0 appended;
+    scale_model_input(x, timesteps[i]) = x / sqrt(sigma_i^2 + 1); step: x0 = x - sigma_i * eps,
+    d = (x - x0) / sigma_i, x' = x + d * (sigma_{i+1} - sigma_i)."""
+
+    def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.00085, beta_end: float = 0.012,
+                 steps_offset: int = 1):
+        betas = torch.linspace(beta_start ** 0.5, beta_end ** 0.5, num_train_timesteps, dtype=torch.float32) ** 2
+        alphas_cumprod = torch.cumprod(1.0 - betas, dim=0)
+        self.train_sigmas = ((1 - alphas_cumprod) / alphas_cumprod) ** 0.5          # sigma(t), t = 0..999
+        self.num_train_timesteps = num_train_timesteps
+        self.steps_offset = steps_offset
+        self.timesteps: List[int] = []
+        self.num_inference_steps = 0
+        self.sigmas = torch.cat([self.train_sigmas.flip(0), torch.zeros(1)])        # before set_timesteps
+        self.config = dict(_SDXL, num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
+                           steps_offset=steps_offset, interpolation_type="linear", use_karras_sigmas=False)
+
+    @property
+    def init_noise_sigma(self) -> float:
+        """Standard deviation of the initial noise: sqrt(max sigma^2 + 1), diffusers' rule for "leading" spacing."""
+        return float((self.sigmas.max() ** 2 + 1) ** 0.5)
+
+    def set_timesteps(self, num_inference_steps: int, device=None) -> List[int]:
+        ratio = self.num_train_timesteps // num_inference_steps
+        self.num_inference_steps = num_inference_steps
+        self.timesteps = [int(round(i * ratio)) + self.steps_offset for i in reversed(range(num_inference_steps))]
+        # interpolation_type="linear" evaluated at integer timesteps is the table entry itself
+        self.sigmas = torch.cat([self.train_sigmas[self.timesteps], torch.zeros(1)])
+        return self.timesteps
+
+    def _divisors(self) -> torch.Tensor:
+        return (self.sigmas ** 2 + 1) ** 0.5                                          # fp32 [T + 1]
+
+    def scale_model_input(self, sample, timestep):
+        return sample / self._divisors()[self.timesteps.index(int(timestep))]
+
+    def coefficient_table(self, device) -> torch.Tensor:
+        """fp32 [T, 3] device tensor of (sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1)) in loop order; the last
+        column divides the updated latents into the next step's UNet input."""
+        return torch.stack([self.sigmas[:-1], self.sigmas[1:], self._divisors()[1:]], dim=1).to(device)
+
+    def model_input_divisors(self) -> List[float]:
+        """scale_model_input(x, timesteps[i]) == x / model_input_divisors()[i] (fp32 values)."""
+        return self._divisors()[:-1].tolist()
+
+    def fused_step_(self, noise_pred, latents, model_in, coef, guidance: float) -> None:
+        ops.cfg_euler_step_(noise_pred, latents, model_in, coef, guidance)
+
+
+# (key, value implemented here, diffusers' default when the config omits the key) for every key that changes the
+# arithmetic of the class
+_COMMON_KEYS = [("num_train_timesteps", 1000, 1000), ("beta_start", 0.00085, 0.0001), ("beta_end", 0.012, 0.02),
+                ("beta_schedule", "scaled_linear", "linear"), ("trained_betas", None, None),
+                ("prediction_type", "epsilon", "epsilon"), ("steps_offset", 1, 0),
+                ("rescale_betas_zero_snr", False, False)]
+_CLASS_KEYS = {
+    "DDIMScheduler": (DDIMScheduler, [("timestep_spacing", "leading", "leading"), ("set_alpha_to_one", False, True),
+                                      ("clip_sample", False, True), ("thresholding", False, False)]),
+    "EulerDiscreteScheduler": (EulerDiscreteScheduler, [
+        ("timestep_spacing", "leading", "linspace"), ("interpolation_type", "linear", "linear"),
+        ("use_karras_sigmas", False, False), ("use_exponential_sigmas", False, False),
+        ("use_beta_sigmas", False, False), ("timestep_type", "discrete", "discrete"),
+        ("final_sigmas_type", "zero", "zero")]),
+}
+
+
+def scheduler_from_config(config: dict):
+    """The scheduler a diffusers ``scheduler_config.json`` dict names (``_class_name``), checked key by key against
+    the SDXL-base configuration this engine implements.  A key the config omits takes diffusers' default for that
+    class.  Any other class, or any other value of a key that changes the arithmetic, raises ``ValueError`` naming
+    the key: there is no fallback to a different scheduler."""
+    name = config.get("_class_name")
+    if name not in _CLASS_KEYS:
+        raise ValueError(f"scheduler config: _class_name={name!r} is not supported "
+                         f"(supported: {', '.join(sorted(_CLASS_KEYS))})")
+    cls, keys = _CLASS_KEYS[name]
+    for key, want, default in _COMMON_KEYS + keys:
+        got = config.get(key, default)
+        if got != want:
+            raise ValueError(f"scheduler config: {name} with {key}={got!r} is not supported (this engine implements "
+                             f"{key}={want!r})")
+    return cls()

@@ -307,6 +307,24 @@ int ds_timestep_embedding(const float* t, void* out, int rows, int dim, void* st
 int ds_cfg_ddim_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
                      int bs, int HW, int C, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * CFG blend + Euler (EulerDiscreteScheduler, s_churn = 0, epsilon-prediction) update + the next
+ * step's scale_model_input, fused.                                                 [HBM-bound]
+ * Replaces src/pipelines/pipeline_diffsensei.py:315-317,332-337 (chunk, u + g*(t-u), scheduler.step,
+ * the torch.cat([latents]*2) and scheduler.scale_model_input for the next step), fp32, each operation
+ * rounded separately in this order:
+ *   eps     = e_uncond + guidance * (e_text - e_uncond)
+ *   x0      = x - sigma * eps
+ *   d       = (x - x0) / sigma
+ *   x_new   = x + d * (sigma_next - sigma)
+ *   noise_pred : bf16 NHWC [2*bs][H][W][4] (uncond half first)
+ *   latents    : fp32 [bs][H][W][4] updated in place (fp32 master copy)
+ *   model_in   : bf16 NHWC [2*bs][H][W][4] — x_new / sqrt(sigma_next^2 + 1) for both CFG halves
+ *   coef       : device pointer to 3 floats {sigma, sigma_next, sqrt(sigma_next^2 + 1)} for this step
+ * --------------------------------------------------------------------------------------------- */
+int ds_cfg_euler_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
+                      int bs, int HW, int C, void* stream);
+
 /* Perceiver attention of the character Resampler: 16 latent queries x (n_kv) keys per (character, head),
  * q and k each pre-scaled by dim_head^-0.25, fp32 softmax (src/models/resampler.py:64-74).
  *   q: bf16 [Bc][nq][C], kv: bf16 [Bc][n_kv][2*C] (k | v), out: bf16 [Bc][nq][C]; C = heads*64 */
