@@ -7,6 +7,8 @@ Public surface (mirrors the reference's, SURVEY.md §8b):
     VaeDecoderEngine       <- diffusers AutoencoderKL.decode as used by pipeline_diffsensei.py:339-363
     ClipTextEncoderEngine, ClipVisionEncoderEngine, VitMaeEncoderEngine  <- transformers CLIP / ViT-MAE encoders as
                               used by encode_prompt (:232-245) and prepare_ip_image_embeds (:125-128)
+    CLIPImageProcessor, ViTImageProcessor  <- transformers' image processors as constructed by
+                              pipeline_diffsensei.py:70-71 (shipped defaults; resize / normalise on the GPU)
     DiffSenseiPipeline     <- src/pipelines/pipeline_diffsensei.py  (denoise loop)
     DDIMScheduler, EulerDiscreteScheduler, scheduler_from_config  <- the diffusers schedulers a checkpoint's
                               scheduler_config.json may name (SDXL-base configuration only)
@@ -24,6 +26,7 @@ from .config import (AGENT_TINY, LLAMA2_13B, RESAMPLER, RESAMPLER_TINY, SDXL_MAN
                      AgentConfig, VaeConfig)
 from .encoders import (CLIP_L_TEXT, CLIP_VIT_H, MAGI_VIT_MAE, OPENCLIP_BIGG_TEXT, ClipTextEncoderEngine,  # noqa: F401
                        ClipVisionEncoderEngine, EncoderConfig, VitMaeEncoderEngine)
+from .image_processor import CLIPImageProcessor, ViTImageProcessor  # noqa: F401
 from .pipeline import DiffSenseiPipeline  # noqa: F401
 from .resampler import QwenResamplerEngine, ResamplerEngine  # noqa: F401
 from .scheduler import DDIMScheduler, EulerDiscreteScheduler, scheduler_from_config  # noqa: F401

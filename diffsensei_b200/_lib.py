@@ -85,6 +85,7 @@ SIGNATURES = {
     "ds_latent_pointwise": [_vp, _vp, _vp, _vp, _f, _i, _i, _vp],
     "ds_softmax_rows": [_vp, _vp, _i, _i, _i64, _i64, _f, _vp],
     "ds_image_postprocess": [_vp, _vp, _i, _i, _i, _vp],
+    "ds_image_preprocess": [_vp, _vp, _vp, _i, _i, _vp, _vp, _i64, _vp],
     "ds_gemv_bf16": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "ds_rmsnorm": [_vp, _vp, _vp, _i, _i, _f, _vp],
     "ds_rope_kv_append": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp],
@@ -93,7 +94,7 @@ SIGNATURES = {
     "ds_agent_next_token": [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _vp],
 }
 OTHER_EXPORTS = ("ds_version", "ds_last_error", "ds_launch_count", "ds_groupnorm_scratch_floats",
-                 "ds_gemm_splitk_ws_bytes")
+                 "ds_gemm_splitk_ws_bytes", "ds_image_preprocess_scratch_bytes")
 
 
 def _load() -> C.CDLL:
@@ -113,6 +114,8 @@ def _load() -> C.CDLL:
     lib.ds_groupnorm_scratch_floats.restype = C.c_int64
     lib.ds_gemm_splitk_ws_bytes.argtypes = []
     lib.ds_gemm_splitk_ws_bytes.restype = C.c_int64
+    lib.ds_image_preprocess_scratch_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int]
+    lib.ds_image_preprocess_scratch_bytes.restype = C.c_int64
     return lib
 
 

@@ -1,0 +1,272 @@
+// image_kernels.cu — the CLIP / ViT image processors of the reference (CLIPImageProcessor, ViTImageProcessor with
+// their shipped defaults, src/pipelines/pipeline_diffsensei.py:70-71,125-126) on the GPU: uint8 RGB HWC images of any
+// size in, the fp32 NCHW [n][3][224][224] pixel values the vision encoders read out.
+//
+// The resize restates Pillow's 8-bit separable resampler bit for bit (transformers' PIL backend calls
+// Image.resize(size, resample) with no box and no reducing_gap):
+//   per output index xx, in double:  scale = in/out, fs = max(scale, 1), support = filter_support * fs,
+//     center = (xx + 0.5) * scale, xmin = max((int)(center - support + 0.5), 0),
+//     xmax = min((int)(center + support + 0.5), in) - xmin, w[x] = filter((x + xmin - center + 0.5) * (1/fs)),
+//     w /= sum(w) (summed in x order; skipped when the sum is 0), k[x] = (int)(w * 2^22 +- 0.5)
+//   per pass: acc = 2^21 + sum u8 * k, out = clamp(acc >> 22, 0, 255); horizontal pass first into a uint8
+//   intermediate, then the vertical pass; a pass whose size does not change is skipped.
+// Every double / float operation is an explicit round-to-nearest intrinsic, so no FMA contraction can change a
+// coefficient or a normalised value.  CLIP: shortest edge -> 224 bicubic (a = -0.5), centre crop 224 x 224 — only
+// the 224 kept columns and rows are ever resampled (each output index has its own coefficients, so this is the same
+// arithmetic as resize-then-crop).  ViT: 224 x 224 bilinear.  Then float32(u8 * (1/255 as double)) and
+// (x - mean) / std in fp32.
+//
+// Three launches per batch of up to kMaxImages images: coefficient tables, horizontal pass, vertical pass fused with
+// crop / rescale / normalise.  Tables and the intermediate live in the caller's scratch; the tap count per output
+// index is not bounded by anything but the image size.
+#include <cmath>
+#include <vector>
+
+#include "ds_host.h"
+
+namespace ds {
+
+constexpr int kOut = 224;          // crop / resize target of both processors
+constexpr int kMaxImages = 16;     // images per launch (descriptors travel as kernel parameters)
+constexpr int kMaxSide = 65535;
+constexpr int kPrecisionBits = 22;
+
+struct ImgDesc {
+  long long src;                       // byte offset of the image in `src`
+  long long coef_h, coef_v, inter;     // byte offsets into scratch
+  int H, W;                            // source size
+  int rh, rw;                          // resized size (before the crop)
+  int top, left;                       // crop origin in resized coordinates
+  int kh, kv;                          // taps per output index of each pass; 0: pass skipped
+};
+
+struct ImgBatch {
+  ImgDesc d[kMaxImages];
+  int n;
+  int bicubic;
+};
+
+__constant__ float kClipMean[3] = {static_cast<float>(0.48145466), static_cast<float>(0.4578275),
+                                   static_cast<float>(0.40821073)};
+__constant__ float kClipStd[3] = {static_cast<float>(0.26862954), static_cast<float>(0.26130258),
+                                  static_cast<float>(0.27577711)};
+
+__device__ __forceinline__ double resample_filter(double x, bool bicubic) {
+  if (x < 0.0) x = -x;
+  if (bicubic) {  // a = -0.5: ((a + 2) x - (a + 3)) x x + 1 on [0, 1), (((x - 5) x + 8) x - 4) a on [1, 2)
+    if (x < 1.0) return __dadd_rn(__dmul_rn(__dmul_rn(__dsub_rn(__dmul_rn(1.5, x), 2.5), x), x), 1.0);
+    if (x < 2.0) return __dmul_rn(__dsub_rn(__dmul_rn(__dadd_rn(__dmul_rn(__dsub_rn(x, 5.0), x), 8.0), x), 4.0), -0.5);
+    return 0.0;
+  }
+  return x < 1.0 ? __dsub_rn(1.0, x) : 0.0;
+}
+
+__device__ __forceinline__ int clip8(int acc) { return min(max(acc >> kPrecisionBits, 0), 255); }
+
+// grid (n, 2 axes), kOut threads: thread t writes {xmin, xmax, k[0 .. ksize)} of output index first + t.
+__global__ void image_coef_kernel(ImgBatch b, unsigned char* __restrict__ scratch) {
+  const ImgDesc& d = b.d[blockIdx.x];
+  const bool vert = blockIdx.y == 1;
+  const int ksize = vert ? d.kv : d.kh;
+  if (ksize == 0) return;
+  const int in = vert ? d.H : d.W, out = vert ? d.rh : d.rw;
+  const int xx = (vert ? d.top : d.left) + static_cast<int>(threadIdx.x);
+  int* row = reinterpret_cast<int*>(scratch + (vert ? d.coef_v : d.coef_h)) + threadIdx.x * (2 + ksize);
+  const bool bicubic = b.bicubic != 0;
+  const double scale = __ddiv_rn(static_cast<double>(in), static_cast<double>(out));
+  const double fs = scale < 1.0 ? 1.0 : scale;
+  const double support = __dmul_rn(bicubic ? 2.0 : 1.0, fs);
+  const double center = __dmul_rn(__dadd_rn(static_cast<double>(xx), 0.5), scale);
+  const double ss = __ddiv_rn(1.0, fs);
+  const int xmin = max(__double2int_rz(__dadd_rn(__dsub_rn(center, support), 0.5)), 0);
+  const int xmax = min(min(__double2int_rz(__dadd_rn(__dadd_rn(center, support), 0.5)), in) - xmin, ksize);
+  double ww = 0.0;
+  for (int x = 0; x < xmax; ++x)
+    ww = __dadd_rn(ww, resample_filter(__dmul_rn(__dadd_rn(__dsub_rn(static_cast<double>(x + xmin), center), 0.5), ss),
+                                       bicubic));
+  for (int x = 0; x < xmax; ++x) {
+    double w = resample_filter(__dmul_rn(__dadd_rn(__dsub_rn(static_cast<double>(x + xmin), center), 0.5), ss), bicubic);
+    if (ww != 0.0) w = __ddiv_rn(w, ww);
+    row[2 + x] = __double2int_rz(__dadd_rn(w < 0.0 ? -0.5 : 0.5, __dmul_rn(w, static_cast<double>(1 << kPrecisionBits))));
+  }
+  row[0] = xmin;
+  row[1] = xmax;
+}
+
+// grid (x-blocks, n): every source row, the kOut kept output columns, 3 channels -> uint8 intermediate [H][kOut][3].
+__global__ void image_hpass_kernel(ImgBatch b, const unsigned char* __restrict__ src, unsigned char* __restrict__ scratch) {
+  const ImgDesc& d = b.d[blockIdx.y];
+  if (d.kh == 0) return;
+  const long long total = static_cast<long long>(d.H) * kOut;
+  const int* coef = reinterpret_cast<const int*>(scratch + d.coef_h);
+  unsigned char* inter = scratch + d.inter;
+  const unsigned char* img = src + d.src;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long y = i / kOut;
+    const int x = static_cast<int>(i - y * kOut);
+    const int* k = coef + x * (2 + d.kh);
+    const int xmin = k[0], xmax = k[1];
+    const unsigned char* p = img + (y * d.W + xmin) * 3;
+    int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
+    for (int t = 0; t < xmax; ++t) {
+      const int w = k[2 + t];
+      a0 += p[3 * t] * w;
+      a1 += p[3 * t + 1] * w;
+      a2 += p[3 * t + 2] * w;
+    }
+    unsigned char* o = inter + i * 3;
+    o[0] = static_cast<unsigned char>(clip8(a0));
+    o[1] = static_cast<unsigned char>(clip8(a1));
+    o[2] = static_cast<unsigned char>(clip8(a2));
+  }
+}
+
+// grid (kOut*kOut/256, n): one output pixel per thread — vertical pass (or the crop rows), rescale, normalise, NCHW.
+__global__ void image_vpass_normalise_kernel(ImgBatch b, const unsigned char* __restrict__ src,
+                                             const unsigned char* __restrict__ scratch, float* __restrict__ out) {
+  const ImgDesc& d = b.d[blockIdx.y];
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= kOut * kOut) return;
+  const int y = i / kOut, x = i - (i / kOut) * kOut;
+  const unsigned char* base;
+  long long pitch;
+  if (d.kh) {
+    base = scratch + d.inter + x * 3;
+    pitch = kOut * 3;
+  } else {
+    base = src + d.src + static_cast<long long>(d.left + x) * 3;
+    pitch = static_cast<long long>(d.W) * 3;
+  }
+  int v[3];
+  if (d.kv) {
+    const int* k = reinterpret_cast<const int*>(scratch + d.coef_v) + y * (2 + d.kv);
+    const int ymin = k[0], ymax = k[1];
+    int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
+    for (int t = 0; t < ymax; ++t) {
+      const unsigned char* p = base + (ymin + t) * pitch;
+      const int w = k[2 + t];
+      a0 += p[0] * w;
+      a1 += p[1] * w;
+      a2 += p[2] * w;
+    }
+    v[0] = clip8(a0);
+    v[1] = clip8(a1);
+    v[2] = clip8(a2);
+  } else {
+    const unsigned char* p = base + (d.top + y) * pitch;
+    v[0] = p[0];
+    v[1] = p[1];
+    v[2] = p[2];
+  }
+  float* o = out + static_cast<long long>(blockIdx.y) * 3 * kOut * kOut + i;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float f = __double2float_rn(__dmul_rn(static_cast<double>(v[c]), 1.0 / 255.0));
+    const float mean = b.bicubic ? kClipMean[c] : 0.5f, stdv = b.bicubic ? kClipStd[c] : 0.5f;
+    o[c * kOut * kOut] = __fdiv_rn(__fsub_rn(f, mean), stdv);
+  }
+}
+
+// Host plan shared by the size query and the entry point: resized size, crop, taps per pass and scratch offsets
+// (every section 16-byte aligned).  Returns false on an unsupported size.
+static bool plan_images(const int* sizes, int n, int mode, ImgDesc* descs, long long* total) {
+  long long cur = 0;
+  auto take = [&cur](long long bytes) {
+    const long long at = cur;
+    cur += (bytes + 15) / 16 * 16;
+    return at;
+  };
+  for (int i = 0; i < n; ++i) {
+    const int H = sizes[2 * i], W = sizes[2 * i + 1];
+    if (H < 1 || W < 1 || H > kMaxSide || W > kMaxSide) return false;
+    ImgDesc d{};
+    d.H = H;
+    d.W = W;
+    double support;
+    if (mode == DS_IMG_CLIP) {  // transformers get_resize_output_image_size(shortest_edge=224, default_to_square=False)
+      const int s = W <= H ? W : H, l = W <= H ? H : W;
+      const int nl = static_cast<int>(static_cast<double>(static_cast<long long>(kOut) * l) / static_cast<double>(s));
+      d.rh = W <= H ? nl : kOut;
+      d.rw = W <= H ? kOut : nl;
+      d.top = (d.rh - kOut) / 2;
+      d.left = (d.rw - kOut) / 2;
+      support = 2.0;
+    } else {
+      d.rh = d.rw = kOut;
+      support = 1.0;
+    }
+    auto taps = [support](int in, int out) {
+      double fs = static_cast<double>(in) / static_cast<double>(out);
+      if (fs < 1.0) fs = 1.0;
+      return static_cast<int>(std::ceil(support * fs)) * 2 + 1;
+    };
+    d.kh = d.rw != W ? taps(W, d.rw) : 0;
+    d.kv = d.rh != H ? taps(H, d.rh) : 0;
+    d.coef_h = d.kh ? take(4LL * kOut * (2 + d.kh)) : 0;
+    d.coef_v = d.kv ? take(4LL * kOut * (2 + d.kv)) : 0;
+    d.inter = d.kh ? take(3LL * kOut * H) : 0;
+    if (descs) descs[i] = d;
+  }
+  *total = cur;
+  return true;
+}
+
+}  // namespace ds
+
+extern "C" int64_t ds_image_preprocess_scratch_bytes(const int* sizes, int n, int mode) {
+  long long total = 0;
+  if (!sizes || n < 1 || (mode != DS_IMG_CLIP && mode != DS_IMG_VIT) || !ds::plan_images(sizes, n, mode, nullptr, &total))
+    return -1;
+  return total;
+}
+
+extern "C" int ds_image_preprocess(const uint8_t* src, const int64_t* offsets, const int* sizes, int n, int mode,
+                                   float* out, void* scratch, int64_t scratch_bytes, void* stream) {
+  using namespace ds;
+  DS_REQUIRE(src && offsets && sizes && out && n > 0, "ds_image_preprocess: bad arguments");
+  DS_REQUIRE(mode == DS_IMG_CLIP || mode == DS_IMG_VIT, "ds_image_preprocess: unknown mode %d", mode);
+  DS_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3) == 0, "ds_image_preprocess: out must be 4-byte aligned");
+  for (int i = 0; i < n; ++i) {
+    DS_REQUIRE(sizes[2 * i] >= 1 && sizes[2 * i + 1] >= 1 && sizes[2 * i] <= kMaxSide && sizes[2 * i + 1] <= kMaxSide,
+               "ds_image_preprocess: image %d is %d x %d; sides must be in [1, %d]", i, sizes[2 * i], sizes[2 * i + 1],
+               kMaxSide);
+    DS_REQUIRE(offsets[i] >= 0, "ds_image_preprocess: negative offset for image %d", i);
+  }
+  long long need = 0;
+  std::vector<ImgDesc> all(n);
+  plan_images(sizes, n, mode, all.data(), &need);
+  DS_REQUIRE(need == 0 || (scratch && scratch_bytes >= need && (reinterpret_cast<uintptr_t>(scratch) & 15) == 0),
+             "ds_image_preprocess: needs %lld bytes of 16-byte aligned scratch (ds_image_preprocess_scratch_bytes), "
+             "got %lld", need, static_cast<long long>(scratch_bytes));
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  unsigned char* scr = static_cast<unsigned char*>(scratch);
+  for (int first = 0; first < n; first += kMaxImages) {
+    ImgBatch b;
+    b.n = n - first < kMaxImages ? n - first : kMaxImages;
+    b.bicubic = mode == DS_IMG_CLIP;
+    bool any_resize = false;
+    long long max_rows = 0;  // rows of the tallest image that needs the horizontal pass
+    for (int j = 0; j < b.n; ++j) {
+      b.d[j] = all[first + j];
+      b.d[j].src = offsets[first + j];
+      any_resize |= b.d[j].kh || b.d[j].kv;
+      if (b.d[j].kh && b.d[j].H > max_rows) max_rows = b.d[j].H;
+    }
+    if (any_resize) {
+      image_coef_kernel<<<dim3(b.n, 2), kOut, 0, st>>>(b, scr);
+      DS_LAUNCH_OK("image_coef_kernel");
+    }
+    if (max_rows) {
+      const long long blocks = (max_rows * kOut + 255) / 256;
+      image_hpass_kernel<<<dim3(static_cast<unsigned>(blocks < 2048 ? blocks : 2048), b.n), 256, 0, st>>>(b, src, scr);
+      DS_LAUNCH_OK("image_hpass_kernel");
+    }
+    image_vpass_normalise_kernel<<<dim3(kOut * kOut / 256, b.n), 256, 0, st>>>(
+        b, src, scr, out + static_cast<long long>(first) * 3 * kOut * kOut);
+    DS_LAUNCH_OK("image_vpass_normalise_kernel");
+  }
+  return DS_OK;
+}

@@ -8,7 +8,7 @@ What ``DiffSenseiPipeline.__call__`` runs before the denoise loop (src/pipelines
   * ``prepare_ip_image_embeds`` (:125-128): ``CLIPVisionModelWithProjection`` (ViT-H/14) read at
     ``hidden_states[-2]`` (257 x 1280 per character crop) and the Magi ``ViTMAEModel`` read at
     ``last_hidden_state[:, 0]`` (768).            -> ``ClipVisionEncoderEngine`` / ``VitMaeEncoderEngine``
-    (``pixel_values`` in: the PIL resize / normalise of the image processors is host-side preprocessing)
+    (``pixel_values`` in: the image processors that make them are in image_processor.py)
 
 All four are pre-LayerNorm transformer encoders; one stack implementation serves them: LayerNorm (ds_layernorm) ->
 fused q|k|v projection (wgmma GEMM + bias) -> short-sequence attention (ds_attention_small: 77 causal text tokens,

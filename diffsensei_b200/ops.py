@@ -800,4 +800,58 @@ def image_postprocess(x: torch.Tensor) -> torch.Tensor:
     return out
 
 
+# ---------------------------------------------------------------------------------------------- image processors
+IMG_MODES = {"clip": 0, "vit": 1}     # DS_IMG_CLIP / DS_IMG_VIT
+IMG_SIZE = 224
+
+
+def _img_sizes(sizes) -> "C.Array":
+    flat = [int(v) for hw in sizes for v in hw]
+    return (C.c_int * len(flat))(*flat)
+
+
+def image_preprocess_scratch_bytes(sizes, mode: str) -> int:
+    """Bytes of scratch ds_image_preprocess needs for images of ``sizes`` [(height, width), ...] (host arithmetic)."""
+    if mode not in IMG_MODES:
+        raise DsEngineError(f"image_preprocess: mode must be one of {sorted(IMG_MODES)}, got {mode!r}")
+    n = int(lib.ds_image_preprocess_scratch_bytes(_img_sizes(sizes), len(sizes), IMG_MODES[mode]))
+    if n < 0:
+        raise DsEngineError(f"image_preprocess: unsupported image sizes {list(sizes)} (sides must be in [1, 65535])")
+    return n
+
+
+def image_preprocess(src: torch.Tensor, sizes, mode: str, offsets=None, out: Optional[torch.Tensor] = None,
+                     scratch: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The CLIP (``mode="clip"``) or ViT (``"vit"``) image processor's resize / crop / rescale / normalise:
+    uint8 RGB HWC images packed in the 1-D CUDA tensor ``src`` (image i is ``sizes[i]`` = (height, width) at byte
+    ``offsets[i]``; packed back to back when ``offsets`` is None) -> fp32 [n, 3, 224, 224] pixel values."""
+    _req(src, torch.uint8, "image_preprocess.src", 1)
+    sizes = [(int(h), int(w)) for h, w in sizes]
+    n = len(sizes)
+    if n == 0:
+        raise DsEngineError("image_preprocess: no images")
+    if offsets is None:
+        offsets, at = [], 0
+        for h, w in sizes:
+            offsets.append(at)
+            at += h * w * 3
+    offsets = [int(o) for o in offsets]
+    if len(offsets) != n:
+        raise DsEngineError("image_preprocess: one offset per image")
+    for (h, w), o in zip(sizes, offsets):
+        if o < 0 or o + h * w * 3 > src.numel():
+            raise DsEngineError(f"image_preprocess: a {h} x {w} x 3 image at byte {o} overruns src ({src.numel()} bytes)")
+    need = image_preprocess_scratch_bytes(sizes, mode)
+    if scratch is None:
+        scratch = torch.empty(max(need, 16), dtype=torch.uint8, device=src.device)
+    _req(scratch, torch.uint8, "image_preprocess.scratch", 1)
+    shape = (n, 3, IMG_SIZE, IMG_SIZE)
+    out = torch.empty(shape, dtype=f32, device=src.device) if out is None else _req(out, f32, "image_preprocess.out", 4)
+    if tuple(out.shape) != shape:
+        raise DsEngineError(f"image_preprocess: out must be {shape}")
+    check(lib.ds_image_preprocess(src.data_ptr(), (C.c_int64 * n)(*offsets), _img_sizes(sizes), n, IMG_MODES[mode],
+                                  out.data_ptr(), scratch.data_ptr(), scratch.numel(), _stream()), "ds_image_preprocess")
+    return out
+
+
 launch_count = _lib.launch_count

@@ -7,9 +7,11 @@ Mirrors ``src/pipelines/pipeline_diffsensei.py``:
     repeat to ``num_samples``; ``prepare_dialog_bbox`` (:156-170)
   * the CFG denoise loop (:293-337) — ``denoise``: the hot path.
   * VAE decode + image post-process (:339-363) — ``VaeDecoderEngine`` (vae.py), ``output_type`` "pt" / "np" / "pil".
-Out of scope (SURVEY.md §8f ranks 2-4): the SDXL text encoders and the CLIP / Magi image encoders.  ``__call__`` keeps
-the reference's keyword surface but takes their OUTPUTS as tensors (``prompt_embeds`` ..., ``clip_image_embeds`` /
-``magi_image_embeds``); passing a raw ``prompt`` string without embeddings raises, it does not fall back to anything.
+``__call__`` keeps the reference's keyword surface.  A raw ``prompt`` string needs the two CLIP tokenizers
+(``tokenizer=`` / ``tokenizer_2=``, host objects) and the text-encoder engines; ``ip_images`` need the image-encoder
+engines and run through the two image processors on the GPU (image_processor.py).  Without them the encoders' inputs
+(token ids, pixel values) or outputs (``prompt_embeds`` ..., ``clip_image_embeds`` / ``magi_image_embeds``) can be
+passed instead; a raw prompt or image without what it needs raises, it does not fall back to anything.
 
 Loop structure on the GPU (one process per GPU, one stream):
   once per panel : K|V projections of text and IP tokens for all cross-attention layers, time-embedding
@@ -29,6 +31,7 @@ from typing import List, Optional, Union
 import torch
 
 from . import ops
+from .image_processor import CLIPImageProcessor, ViTImageProcessor
 from .scheduler import DDIMScheduler, EulerDiscreteScheduler
 from .unet import UNetMangaEngine
 
@@ -38,12 +41,17 @@ bf16, f32 = torch.bfloat16, torch.float32
 class DiffSenseiPipeline:
     def __init__(self, unet: UNetMangaEngine,
                  scheduler: Optional[Union[DDIMScheduler, EulerDiscreteScheduler]] = None, vae_scale_factor: int = 8,
-                 default_sample_size: int = 128, vae=None, text_encoder=None, text_encoder_2=None, image_encoder=None):
+                 default_sample_size: int = 128, vae=None, text_encoder=None, text_encoder_2=None, image_encoder=None,
+                 tokenizer=None, tokenizer_2=None):
         self.unet = unet
         self.vae = vae                      # VaeDecoderEngine (or None: latents out only)
         self.text_encoder = text_encoder    # ClipTextEncoderEngine (CLIP-L) / (OpenCLIP bigG, with projection)
         self.text_encoder_2 = text_encoder_2
         self.image_encoder = image_encoder  # ClipVisionEncoderEngine (ViT-H/14)
+        self.tokenizer = tokenizer          # transformers CLIPTokenizer of each text encoder (host objects)
+        self.tokenizer_2 = tokenizer_2
+        self.clip_image_processor = CLIPImageProcessor()                # pipeline_diffsensei.py:70-71
+        self.magi_image_processor = ViTImageProcessor()
         self.scheduler = scheduler or DDIMScheduler()
         self.vae_scale_factor = vae_scale_factor
         self.default_sample_size = default_sample_size
@@ -86,10 +94,32 @@ class DiffSenseiPipeline:
     def set_ip_scale(self, scale):
         self.unet.set_ip_scale(scale)
 
+    def tokenize_prompt(self, prompt: str, prompt_2=None, negative_prompt=None, negative_prompt_2=None):
+        """The tokenizer half of diffusers' SDXL ``encode_prompt`` (pipeline_diffsensei.py:232-245): each prompt padded
+        to ``model_max_length`` and truncated; ``prompt_2`` defaults to ``prompt``.  ``negative_prompt=None`` gives no
+        negative ids, i.e. zero negative embeddings (``force_zeros_for_empty_prompt``); otherwise it defaults to "" and
+        ``negative_prompt_2`` to ``negative_prompt``, tokenized to the prompt's length.
+        Returns (ids, ids_2, negative_ids, negative_ids_2) int64 [1, L] tensors, the negatives None or both set."""
+        if self.tokenizer is None or self.tokenizer_2 is None:
+            raise ValueError("tokenize_prompt needs tokenizer and tokenizer_2")
+        for name, p in (("prompt_2", prompt_2), ("negative_prompt", negative_prompt),
+                        ("negative_prompt_2", negative_prompt_2)):
+            if p is not None and not isinstance(p, str):
+                raise ValueError(f"`{name}` has to be of type `str` but is {type(p)}")
+        prompt_2 = prompt_2 or prompt
+        tok = lambda t, p, n: t(p, padding="max_length", max_length=n, truncation=True, return_tensors="pt").input_ids
+        ids = tok(self.tokenizer, prompt, self.tokenizer.model_max_length)
+        ids_2 = tok(self.tokenizer_2, prompt_2, self.tokenizer_2.model_max_length)
+        if negative_prompt is None:
+            return ids, ids_2, None, None
+        negative_prompt_2 = negative_prompt_2 or negative_prompt
+        return ids, ids_2, tok(self.tokenizer, negative_prompt, ids.shape[1]), \
+            tok(self.tokenizer_2, negative_prompt_2, ids.shape[1])
+
     @torch.no_grad()
     def encode_prompt_ids(self, input_ids, input_ids_2, negative_input_ids=None, negative_input_ids_2=None):
-        """``encode_prompt`` (pipeline_diffsensei.py:232-245; diffusers StableDiffusionXLPipeline) from TOKEN IDS — the
-        two tokenizers' vocabulary files are host-side assets outside the hot path.  Both encoders are read at
+        """``encode_prompt`` (pipeline_diffsensei.py:232-245; diffusers StableDiffusionXLPipeline) from TOKEN IDS
+        (``tokenize_prompt`` makes them from strings).  Both encoders are read at
         ``hidden_states[-2]`` and concatenated (768 + 1280 = 2048 features); the pooled embedding is the second
         encoder's projected EOS feature.  No negative ids: zeros (SDXL-base ``force_zeros_for_empty_prompt``)."""
         if self.text_encoder is None or self.text_encoder_2 is None:
@@ -116,6 +146,15 @@ class DiffSenseiPipeline:
         clip = self.image_encoder(clip_pixel_values, output_hidden_states=True).hidden_states[-2].unsqueeze(0)
         magi = self.magi_image_encoder(magi_pixel_values).last_hidden_state[:, 0].unsqueeze(0)
         return clip, magi
+
+    @torch.no_grad()
+    def preprocess_ip_images(self, ip_images):
+        """The processor half of ``prepare_ip_image_embeds`` (:125-126) on the GPU: PIL images (or uint8 RGB HWC arrays
+        / tensors) -> the CLIP and Magi ``pixel_values``, fp32 [n, 3, 224, 224] each."""
+        dev = self.unet.device
+        ip_images = [self.clip_image_processor.to_device(im, dev) for im in ip_images]   # decode + upload once
+        return (self.clip_image_processor(images=ip_images, return_tensors="pt").pixel_values,
+                self.magi_image_processor(images=ip_images, return_tensors="pt").pixel_values)
 
     def prepare_ip_image_embeds(self, clip_image_embeds: torch.Tensor, magi_image_embeds: torch.Tensor,
                                 ip_image_embeds: Optional[torch.Tensor], ip_bbox: List[List[float]], num_samples: int):
@@ -223,7 +262,7 @@ class DiffSenseiPipeline:
                  original_size=None, crops_coords_top_left=(0, 0), target_size=None, min_size_step: int = 8,
                  ip_images=(), ip_image_embeds: Optional[torch.Tensor] = None, ip_bbox=(), ip_scale: float = 1.0,
                  dialog_bbox=(),
-                 # outputs of the out-of-scope encoders (SURVEY.md §8f), required instead of raw prompt / images:
+                 # outputs of the conditioning encoders, instead of a raw prompt / images:
                  prompt_embeds: Optional[torch.Tensor] = None, negative_prompt_embeds: Optional[torch.Tensor] = None,
                  pooled_prompt_embeds: Optional[torch.Tensor] = None,
                  negative_pooled_prompt_embeds: Optional[torch.Tensor] = None,
@@ -236,6 +275,16 @@ class DiffSenseiPipeline:
         width = width or self.default_sample_size * self.vae_scale_factor
         original_size = original_size or (height, width)
         target_size = target_size or (height, width)
+        if len(ip_images) > 0:
+            if ip_image_embeds is not None:
+                raise ValueError("`ip_images` and `ip_image_embeds` can not be input together!")
+            if clip_pixel_values is not None or magi_pixel_values is not None or clip_image_embeds is not None or \
+                    magi_image_embeds is not None:
+                raise ValueError("`ip_images` and pixel values / image embeddings can not be input together!")
+        if prompt_embeds is None and prompt_input_ids is None and isinstance(prompt, str) and \
+                self.tokenizer is not None and self.tokenizer_2 is not None:
+            prompt_input_ids, prompt_input_ids_2, negative_prompt_input_ids, negative_prompt_input_ids_2 = \
+                self.tokenize_prompt(prompt, prompt_2, negative_prompt, negative_prompt_2)
         if prompt_embeds is None and prompt_input_ids is not None:
             prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds, negative_pooled_prompt_embeds = \
                 self.encode_prompt_ids(prompt_input_ids, prompt_input_ids_2 if prompt_input_ids_2 is not None
@@ -249,9 +298,17 @@ class DiffSenseiPipeline:
                 "pass prompt_input_ids (+ prompt_input_ids_2) with the text-encoder engines registered, or "
                 "prompt_embeds / negative_prompt_embeds / pooled_prompt_embeds / negative_pooled_prompt_embeds")
         if len(ip_images) > 0:
-            raise NotImplementedError("PIL images need the CLIP / Magi image processors (host-side resize + normalise): "
-                                      "pass clip_pixel_values / magi_pixel_values with the image-encoder engines "
-                                      "registered, or clip_image_embeds / magi_image_embeds")
+            if len(ip_images) != len(ip_bbox):
+                raise ValueError(f"`ip_images` must have the same length as `ip_bbox`. But they are in length "
+                                 f"{len(ip_images)} and {len(ip_bbox)}!")
+            if self.image_encoder is None or self.magi_image_encoder is None:
+                raise NotImplementedError("ip_images need the image-encoder engines: DiffSenseiPipeline(..., "
+                                          "image_encoder=ClipVisionEncoderEngine) and register_manga_modules("
+                                          "magi_image_encoder=VitMaeEncoderEngine, ...); or pass clip_image_embeds / "
+                                          "magi_image_embeds")
+            m = self.unet.cfg.max_num_ips                                  # :112-114
+            ip_bbox = list(ip_bbox)[:m]
+            clip_image_embeds, magi_image_embeds = self.encode_ip_images(*self.preprocess_ip_images(list(ip_images)[:m]))
         if output_type not in ("latent", "pt", "np", "pil"):
             raise ValueError(f"output_type must be one of latent / pt / np / pil, got {output_type!r}")
         if output_type != "latent" and self.vae is None:

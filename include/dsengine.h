@@ -366,6 +366,26 @@ int ds_attention_small(const void* q, const void* k, const void* v, void* out, i
 int ds_embed_tokens(const int* ids, const void* tok_emb, const void* pos_emb, void* out, int B, int L, int C, int vocab,
                     void* stream);
 
+/* Image processors of prepare_ip_image_embeds (src/pipelines/pipeline_diffsensei.py:70-71,125-126: transformers'
+ * CLIPImageProcessor / ViTImageProcessor, shipped defaults, PIL backend), bit-exact:
+ *   DS_IMG_CLIP : shortest edge -> 224 (long edge int(224 * long / short)), Pillow bicubic, centre crop 224 x 224,
+ *                 (x / 255 - OPENAI_CLIP_MEAN) / OPENAI_CLIP_STD
+ *   DS_IMG_VIT  : 224 x 224, Pillow bilinear, (x / 255 - 0.5) / 0.5
+ * The resize is Pillow's 8-bit fixed-point resampler (22-bit coefficients, horizontal pass into a uint8
+ * intermediate, then vertical; a pass whose size does not change is skipped); see image_kernels.cu.
+ *   src     : uint8 RGB HWC images packed in one buffer; image i starts at byte offsets[i]
+ *   offsets : HOST int64 [n];  sizes: HOST int32 [n][2] {height, width}, each side in [1, 65535]
+ *   out     : fp32 NCHW [n][3][224][224]
+ *   scratch : ds_image_preprocess_scratch_bytes(sizes, n, mode) bytes, 16-byte aligned (coefficient tables and the
+ *             uint8 intermediate; no fixed tap limit).  The query is pure host arithmetic; it returns -1 for
+ *             arguments the entry point rejects.
+ * Three launches per 16 images. */
+#define DS_IMG_CLIP 0
+#define DS_IMG_VIT 1
+int64_t ds_image_preprocess_scratch_bytes(const int* sizes, int n, int mode);
+int ds_image_preprocess(const uint8_t* src, const int64_t* offsets, const int* sizes, int n, int mode, float* out,
+                        void* scratch, int64_t scratch_bytes, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * LLaMA decoder of the MLLM agent (SURVEY.md §8f-4: ContinuousLVLM.generate, src/models/mllm/seed_x.py:90-171, over
  * LlamaForCausalLM of src/models/mllm/modeling_llama_xformer.py).  Every kernel that depends on the sequence position
