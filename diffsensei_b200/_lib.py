@@ -85,6 +85,7 @@ SIGNATURES = {
     "ds_latent_pointwise": [_vp, _vp, _vp, _vp, _f, _i, _i, _vp],
     "ds_softmax_rows": [_vp, _vp, _i, _i, _i64, _i64, _f, _vp],
     "ds_image_postprocess": [_vp, _vp, _i, _i, _i, _vp],
+    "ds_attention_single_head": [_vp, _vp, _vp, _vp, _i, _i, _i, _i64, _vp],
     "ds_image_preprocess": [_vp, _vp, _vp, _i, _i, _vp, _vp, _i64, _vp],
     "ds_gemv_bf16": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "ds_rmsnorm": [_vp, _vp, _vp, _i, _i, _f, _vp],

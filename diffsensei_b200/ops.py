@@ -791,6 +791,37 @@ def softmax_rows(S: torch.Tensor, scale: float, out: Optional[torch.Tensor] = No
     return out
 
 
+ATTN_SINGLE_HEAD_DIMS = (128, 512)
+
+
+def attention_single_head(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor,
+                          out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """softmax(Q K^T / sqrt(D)) V per image, one head, one launch: q / k / v bf16 [B, N, D] with D in (128, 512),
+    unit column stride and one shared row stride (column slices of a wider projection are fine) -> dense bf16
+    [B, N, D].  Any N >= 1; no [N, N] buffer (ds_attention_single_head)."""
+    for t, nm in ((q, "q"), (k, "k"), (v, "v")):
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == bf16 and t.dim() == 3 and t.stride(2) == 1):
+            raise DsEngineError(f"attention_single_head.{nm}: expected a 3-D CUDA bf16 tensor with unit column stride")
+        _on_current_device(t, f"attention_single_head.{nm}")
+        if t.shape != q.shape:
+            raise DsEngineError(f"attention_single_head: {nm} is {tuple(t.shape)} but q is {tuple(q.shape)}")
+        if t.stride(1) != q.stride(1) or (t.shape[0] > 1 and t.stride(0) != t.shape[1] * t.stride(1)):
+            raise DsEngineError(f"attention_single_head.{nm}: q / k / v must share one row stride, images "
+                                "N * row stride apart")
+    B, N, D = q.shape
+    if D not in ATTN_SINGLE_HEAD_DIMS:
+        raise DsEngineError(f"attention_single_head: head width {D} is not supported {ATTN_SINGLE_HEAD_DIMS}")
+    if out is None:
+        out = torch.empty(B, N, D, dtype=bf16, device=q.device)
+    else:
+        _req(out, bf16, "attention_single_head.out")
+        if out.numel() != B * N * D:
+            raise DsEngineError("attention_single_head: out must hold B * N * D elements")
+    check(lib.ds_attention_single_head(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, N, D, q.stride(1),
+                                       _stream()), "ds_attention_single_head")
+    return out
+
+
 def image_postprocess(x: torch.Tensor) -> torch.Tensor:
     """clamp(x / 2 + 0.5, 0, 1): bf16 NHWC [B,H,W,C] -> fp32 NCHW [B,C,H,W]."""
     _req(x, bf16, "image_postprocess.x", 4)

@@ -9,9 +9,10 @@ Mirrors what ``src/pipelines/pipeline_diffsensei.py:339-367`` uses of diffusers'
 Same kernel family as the UNet at 8x the spatial size: every 3x3 conv is the wgmma implicit GEMM with its GroupNorm
 statistics taken in the epilogue, every GroupNorm(+SiLU) is one read/write pass, the 1x1 shortcuts and the attention
 projections are wgmma GEMMs.  The mid-block attention is ONE head of width 512 over all H*W latent tokens — outside
-the flash kernel's head_dim 64 — so it runs per image as QK^T (fp32 scores) -> ``ds_softmax_rows`` -> PV on the same GEMM
-kernel.  The fp32-upcast rule of the reference (:340-344: the fp16 VAE overflows) is moot here: activations are
-bf16 (fp32 range), accumulation / normalisation / softmax in fp32; tolerance stated in tests/test_vae_gpu.py.
+the flash kernel's head_dim 64 — so it runs on its own single-head flash kernel (``ds_attention_single_head``), one
+launch for the batch, any H*W.  The fp32-upcast rule of the reference (:340-344: the fp16 VAE overflows) is moot
+here: activations are bf16 (fp32 range), accumulation / normalisation / softmax in fp32; tolerance stated in
+tests/test_vae_gpu.py.
 """
 from __future__ import annotations
 
@@ -118,24 +119,14 @@ class VaeDecoderEngine:
         return ops.conv3x3(h, r.w2, r.b2, residual=sc, chan_stats=st2), st2
 
     def _attention(self, x, st, pool):
-        """diffusers Attention(heads=1, dim_head=C, residual_connection=True) via AttnProcessor2_0: per image
-        softmax(Q K^T / sqrt(C)) V on the wgmma GEMM (fp32 scores) + ds_softmax_rows."""
+        """diffusers Attention(heads=1, dim_head=C, residual_connection=True) via AttnProcessor2_0:
+        softmax(Q K^T / sqrt(C)) V of every image in one ds_attention_single_head launch."""
         a, g = self.attn, self.cfg.norm_num_groups
         B, H, W, C = x.shape
         N = H * W
-        if N % 8 != 0:
-            raise NotImplementedError(f"VaeDecoderEngine: H*W = {N} latent tokens must be a multiple of 8")
         hn = ops.groupnorm_apply(x, st, a.gn[0], a.gn[1], g, 1e-6, False).view(B * N, C)
         q, k, v = ops.gemm(hn, a.wq, a.bq), ops.gemm(hn, a.wk, a.bk), ops.gemm(hn, a.wv, a.bv)
-        o = torch.empty(B * N, C, dtype=bf16, device=x.device)
-        S = torch.empty(N, N, dtype=f32, device=x.device)
-        P = torch.empty(N, N, dtype=bf16, device=x.device)
-        for b in range(B):
-            rows = slice(b * N, (b + 1) * N)
-            ops.gemm(q[rows], k[rows], out=S, out_fp32=True, w_const=False)          # S = Q K^T  (fp32)
-            ops.softmax_rows(S, C ** -0.5, out=P)
-            vT = ops.nhwc_to_nchw(v[rows].view(1, N, 1, C), bf16).view(C, N)         # V^T: K-major B operand
-            ops.gemm(P, vT, out=o[rows], w_const=False)                              # O = P V
+        o = ops.attention_single_head(q.view(B, N, C), k.view(B, N, C), v.view(B, N, C)).view(B * N, C)
         ost = pool.take(C) if N % 128 == 0 else None
         out = ops.gemm(o, a.wo, a.bo, residual=x.view(B * N, C), chan_stats=ost,
                        stats_rows_per_sample=N if ost is not None else 0)

@@ -347,6 +347,18 @@ int ds_latent_pointwise(const float* latents, const float* w, const float* bias,
 int ds_softmax_rows(const float* S, void* P, int rows, int n, int64_t lds, int64_t ldp, float scale, void* stream);
 int ds_image_postprocess(const void* x, float* out, int B, int HW, int C, void* stream);
 
+/* The decoder's mid-block attention (diffusers Attention(heads=1, dim_head=D)) in ONE launch for the whole batch:
+ *   out[b] = softmax(q[b] k[b]^T / sqrt(D)) v[b]                                                     [compute-bound]
+ *   q / k / v : bf16 [B][N][ld] — rows of D elements with one shared row stride ld (elements, >= D, a multiple of 8),
+ *               images N * ld apart, so column slices of one fused q|k|v projection may be passed as they are
+ *   out       : bf16 [B][N][D], dense
+ *   D = 128 or 512 (the last block_out_channels of TINY_VAE / SDXL's VAE); any other D returns DS_ERR_INVALID.
+ *   Any N >= 1 and B <= 65535; pointers 16-byte aligned.  fp32 scores, running max / sum and accumulation, P rounded
+ *   to bf16 before the PV product.  No scratch memory: a flash (online-softmax) pass over 32-key tiles.
+ * Replaces the decoder's QK^T GEMM -> ds_softmax_rows -> PV GEMM, which materialised the [N][N] scores. */
+int ds_attention_single_head(const void* q, const void* k, const void* v, void* out, int B, int N, int D, int64_t ld,
+                             void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Conditioning-encoder helpers (SURVEY.md §8f ranks 2-3: CLIP ViT-H / Magi ViT-MAE image encoders,
  * src/pipelines/pipeline_diffsensei.py:125-128, and the two SDXL CLIP text encoders of encode_prompt, :232-245).
