@@ -12,6 +12,10 @@
 //   ds_attention_kv     : split-KV attention of M query rows against the cache (bottom-right causal) + combine pass
 //   ds_silu_mul         : silu(gate) * up of the fused gate|up projection
 //   ds_agent_next_token : the image-token logits rule + greedy argmax + stop flag + next input row, on the device
+// and, for B <= 8 sequences decoded together (one row each, each with its own position and cache slice):
+//   ds_rope_kv_append_rows, ds_attention_kv_rows, ds_agent_next_token_rows
+// The per-row arithmetic of each *_rows kernel is the same __device__ function its batch-1 kernel calls, so a row
+// computes bit for bit what the batch-1 decode computes for that sequence alone.
 // Every kernel is launched with programmatic dependent launch and waits for its predecessor before its first access
 // to global memory.
 #include "ds_common.cuh"
@@ -161,17 +165,12 @@ rmsnorm_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ ga
 }
 
 // ----------------------------------------------------------------------------------------------- RoPE + KV append
-__global__ void __launch_bounds__(256)
-rope_kv_append_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ q_out,
-                      __nv_bfloat16* __restrict__ kv, const int* __restrict__ pos_ptr, int H, int D, int L_max,
-                      float theta) {
-  pdl_wait();
-  pdl_launch_dependents();
-  const int m = blockIdx.x;
-  const int p = *pos_ptr + m;
-  if (p < 0 || p >= L_max) return;
+// One row at position p: rotates q and k of `row` ([3][H][D]), writes q to qo and appends k / v at row p of the
+// [2][H][L_max][D] cache kv.  Shared by the prefill / batch-1 kernel and the one-sequence-per-row kernel.
+__device__ __forceinline__ void rope_kv_append_row(const __nv_bfloat16* __restrict__ row, __nv_bfloat16* __restrict__ qo,
+                                                   __nv_bfloat16* __restrict__ kv, int p, int H, int D, int L_max,
+                                                   float theta) {
   const int half = D / 2, C = H * D;
-  const __nv_bfloat16* row = qkv + static_cast<size_t>(m) * 3 * C;
   for (int t = threadIdx.x; t < H * half; t += blockDim.x) {
     const int h = t / half, i = t - h * half;
     // inv_freq = theta^(-2i/D) in fp32, angle = p * inv_freq in fp32 (LlamaRotaryEmbedding)
@@ -181,7 +180,6 @@ rope_kv_append_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __re
     const int a = h * D + i, b = a + half;
     const float q1 = __bfloat162float(row[a]), q2 = __bfloat162float(row[b]);
     const float k1 = __bfloat162float(row[C + a]), k2 = __bfloat162float(row[C + b]);
-    __nv_bfloat16* qo = q_out + static_cast<size_t>(m) * C;
     qo[a] = __float2bfloat16_rn(q1 * c - q2 * s);
     qo[b] = __float2bfloat16_rn(q2 * c + q1 * s);
     __nv_bfloat16* kr = kv + (static_cast<size_t>(h) * L_max + p) * D;
@@ -195,33 +193,57 @@ rope_kv_append_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __re
   }
 }
 
+// row m of one sequence at position *pos_ptr + m (prefill and batch-1 decode)
+__global__ void __launch_bounds__(256)
+rope_kv_append_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ q_out,
+                      __nv_bfloat16* __restrict__ kv, const int* __restrict__ pos_ptr, int H, int D, int L_max,
+                      float theta) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int m = blockIdx.x;
+  const int p = *pos_ptr + m;
+  if (p < 0 || p >= L_max) return;
+  const int C = H * D;
+  rope_kv_append_row(qkv + static_cast<size_t>(m) * 3 * C, q_out + static_cast<size_t>(m) * C, kv, p, H, D, L_max,
+                     theta);
+}
+
+// row b is its own sequence at position pos[b * pos_stride], with its cache slice at kv + b * seq_stride
+__global__ void __launch_bounds__(256)
+rope_kv_append_rows_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ q_out,
+                           __nv_bfloat16* __restrict__ kv, long long seq_stride, const int* __restrict__ pos,
+                           int pos_stride, int H, int D, int L_cap, float theta) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int b = blockIdx.x;
+  const int p = pos[static_cast<size_t>(b) * pos_stride];
+  if (p < 0 || p >= L_cap) return;
+  const int C = H * D;
+  rope_kv_append_row(qkv + static_cast<size_t>(b) * 3 * C, q_out + static_cast<size_t>(b) * C, kv + b * seq_stride,
+                     p, H, D, L_cap, theta);
+}
+
 // ----------------------------------------------------------------------------------------------- attention
 constexpr int kAttnWarps = 4;
 constexpr int kAttnMaxVec = 4;   // D / 32 values per lane: D = 128 -> 4, D = 64 -> 2
 
-// One CTA per (split, head, query row): its warps stride over the split's keys with an online softmax per warp,
-// merge in shared memory, and leave {max, sum, o[D]} of the split in the workspace for the combine pass.
+// Keys j0 .. j1-1 of one split for one (query row, head): the CTA's warps stride over the keys with an online softmax
+// per warp, merge in shared memory, and leave {max, sum, o[D]} of the split in `part` for the combine pass.
+// qr: the row's q of this head [D]; kh / vh: this head's keys / values [L][D].
 template <int DV>
-__global__ void __launch_bounds__(kAttnWarps * 32)
-attention_kv_split_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kv,
-                          float* __restrict__ ws, const int* __restrict__ pos_ptr, int H, int L_max, int chunk,
-                          int splits, float scale) {
+__device__ __forceinline__ void attention_kv_split_part(const __nv_bfloat16* __restrict__ qr,
+                                                        const __nv_bfloat16* __restrict__ kh,
+                                                        const __nv_bfloat16* __restrict__ vh, float* __restrict__ part,
+                                                        int j0, int j1, float scale) {
   constexpr int D = DV * 32;
   __shared__ float s_m[kAttnWarps], s_l[kAttnWarps];
   __shared__ float s_o[kAttnWarps][D];
-  pdl_wait();
-  pdl_launch_dependents();
-  const int split = blockIdx.x, h = blockIdx.y, m = blockIdx.z;
-  const int nkeys = min(*pos_ptr + m + 1, L_max);       // bottom-right causal: row m sees keys 0 .. pos0 + m
-  const int j0 = split * chunk, j1 = min(j0 + chunk, nkeys);
-  if (j0 >= j1) return;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float qf[DV];
-  const __nv_bfloat16* qr = q + (static_cast<size_t>(m) * H + h) * D + lane * DV;
 #pragma unroll
-  for (int i = 0; i < DV; ++i) qf[i] = __bfloat162float(qr[i]) * scale;
-  const __nv_bfloat16* kb = kv + static_cast<size_t>(h) * L_max * D + lane * DV;
-  const __nv_bfloat16* vb = kb + static_cast<size_t>(H) * L_max * D;
+  for (int i = 0; i < DV; ++i) qf[i] = __bfloat162float(qr[lane * DV + i]) * scale;
+  const __nv_bfloat16* kb = kh + lane * DV;
+  const __nv_bfloat16* vb = vh + lane * DV;
   float mx = -INFINITY, l = 0.f, o[DV];
 #pragma unroll
   for (int i = 0; i < DV; ++i) o[i] = 0.f;
@@ -267,21 +289,14 @@ attention_kv_split_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat
 #pragma unroll
     for (int i = 0; i < DV; ++i) acc[i] += s_o[w][lane * DV + i] * f;
   }
-  float* part = ws + ((static_cast<size_t>(m) * H + h) * splits + split) * (D + 2);
   if (lane == 0) { part[0] = M_; part[1] = L_; }
 #pragma unroll
   for (int i = 0; i < DV; ++i) part[2 + lane * DV + i] = acc[i];
 }
 
-__global__ void attention_kv_combine_kernel(const float* __restrict__ ws, __nv_bfloat16* __restrict__ out,
-                                            const int* __restrict__ pos_ptr, int H, int D, int L_max, int chunk,
-                                            int splits) {
-  pdl_wait();
-  pdl_launch_dependents();
-  const int h = blockIdx.x, m = blockIdx.y, d = threadIdx.x;
-  const int nkeys = min(*pos_ptr + m + 1, L_max);
-  const int used = min((nkeys + chunk - 1) / chunk, splits);
-  const float* base = ws + (static_cast<size_t>(m) * H + h) * splits * (D + 2);
+// Merges the `used` split partials at `base` (stride D + 2) into element d of the output row.
+__device__ __forceinline__ void attention_kv_combine_part(const float* __restrict__ base, __nv_bfloat16* __restrict__ o,
+                                                          int used, int D, int d) {
   float M_ = -INFINITY;
   for (int s = 0; s < used; ++s) M_ = fmaxf(M_, base[s * (D + 2)]);
   float L_ = 0.f, acc = 0.f;
@@ -290,7 +305,68 @@ __global__ void attention_kv_combine_kernel(const float* __restrict__ ws, __nv_b
     L_ += base[s * (D + 2) + 1] * f;
     acc += base[s * (D + 2) + 2 + d] * f;
   }
-  out[(static_cast<size_t>(m) * H + h) * D + d] = __float2bfloat16_rn(acc / L_);
+  o[d] = __float2bfloat16_rn(acc / L_);
+}
+
+// One CTA per (split, head, query row) of one sequence; row m sees keys 0 .. *pos_ptr + m (bottom-right causal).
+template <int DV>
+__global__ void __launch_bounds__(kAttnWarps * 32)
+attention_kv_split_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kv,
+                          float* __restrict__ ws, const int* __restrict__ pos_ptr, int H, int L_max, int chunk,
+                          int splits, float scale) {
+  constexpr int D = DV * 32;
+  pdl_wait();
+  pdl_launch_dependents();
+  const int split = blockIdx.x, h = blockIdx.y, m = blockIdx.z;
+  const int nkeys = min(*pos_ptr + m + 1, L_max);
+  const int j0 = split * chunk, j1 = min(j0 + chunk, nkeys);
+  if (j0 >= j1) return;
+  const __nv_bfloat16* kh = kv + static_cast<size_t>(h) * L_max * D;
+  attention_kv_split_part<DV>(q + (static_cast<size_t>(m) * H + h) * D, kh, kh + static_cast<size_t>(H) * L_max * D,
+                              ws + ((static_cast<size_t>(m) * H + h) * splits + split) * (D + 2), j0, j1, scale);
+}
+
+__global__ void attention_kv_combine_kernel(const float* __restrict__ ws, __nv_bfloat16* __restrict__ out,
+                                            const int* __restrict__ pos_ptr, int H, int D, int L_max, int chunk,
+                                            int splits) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int h = blockIdx.x, m = blockIdx.y;
+  const int nkeys = min(*pos_ptr + m + 1, L_max);
+  const int used = min((nkeys + chunk - 1) / chunk, splits);
+  attention_kv_combine_part(ws + (static_cast<size_t>(m) * H + h) * splits * (D + 2),
+                            out + (static_cast<size_t>(m) * H + h) * D, used, D, threadIdx.x);
+}
+
+// One CTA per (split, head, row b); row b is its own sequence: keys 0 .. pos[b * pos_stride] of the cache slice at
+// kv + b * seq_stride.  With the same chunk, every split covers the same keys as the batch-1 decode's.
+template <int DV>
+__global__ void __launch_bounds__(kAttnWarps * 32)
+attention_kv_rows_split_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kv,
+                               long long seq_stride, float* __restrict__ ws, const int* __restrict__ pos,
+                               int pos_stride, int H, int L_cap, int chunk, int splits, float scale) {
+  constexpr int D = DV * 32;
+  pdl_wait();
+  pdl_launch_dependents();
+  const int split = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int nkeys = min(pos[static_cast<size_t>(b) * pos_stride] + 1, L_cap);
+  const int j0 = split * chunk, j1 = min(j0 + chunk, nkeys);
+  if (j0 >= j1) return;
+  const __nv_bfloat16* kh = kv + b * seq_stride + static_cast<size_t>(h) * L_cap * D;
+  attention_kv_split_part<DV>(q + (static_cast<size_t>(b) * H + h) * D, kh, kh + static_cast<size_t>(H) * L_cap * D,
+                              ws + ((static_cast<size_t>(b) * H + h) * splits + split) * (D + 2), j0, j1, scale);
+}
+
+__global__ void attention_kv_rows_combine_kernel(const float* __restrict__ ws, __nv_bfloat16* __restrict__ out,
+                                                 const int* __restrict__ pos, int pos_stride, int H, int D, int L_cap,
+                                                 int chunk, int splits) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int h = blockIdx.x, b = blockIdx.y;
+  const int nkeys = min(pos[static_cast<size_t>(b) * pos_stride] + 1, L_cap);
+  const int used = min((nkeys + chunk - 1) / chunk, splits);
+  attention_kv_combine_part(ws + (static_cast<size_t>(b) * H + h) * splits * (D + 2),
+                            out + (static_cast<size_t>(b) * H + h) * D, used, D, threadIdx.x);
 }
 
 // ----------------------------------------------------------------------------------------------- SiLU * up
@@ -338,15 +414,12 @@ __device__ __forceinline__ void block_argmax(const float* s, int V, float* sv, i
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(kTokThreads)
-agent_next_token_kernel(float* logits, int V, const int* __restrict__ img_ids, int n_img, int* state,
-                        int* __restrict__ out_ids, int max_new, int eos, const uint4* __restrict__ embed,
-                        uint4* __restrict__ next_x, const uint4* __restrict__ hidden_src, uint4* __restrict__ hidden,
-                        int C8) {
-  __shared__ float sv[kTokThreads / 32];
-  __shared__ int si[kTokThreads / 32];
-  pdl_wait();
-  pdl_launch_dependents();
+// One greedy step of one sequence (the ds_agent_next_token contract); sv / si: the block's shared argmax scratch.
+__device__ __forceinline__ void agent_next_token_row(float* logits, int V, const int* __restrict__ img_ids, int n_img,
+                                                     int* state, int* __restrict__ out_ids, int max_new, int eos,
+                                                     const uint4* __restrict__ embed, uint4* __restrict__ next_x,
+                                                     const uint4* __restrict__ hidden_src, uint4* __restrict__ hidden,
+                                                     int C8, float* sv, int* si) {
   // state: {pos, generated, done, last token}
   const int pos = state[0], n = state[1], done = state[2], last = state[3];
   if (done) return;
@@ -376,6 +449,37 @@ agent_next_token_kernel(float* logits, int V, const int* __restrict__ img_ids, i
     state[2] = (tok == eos || n + 1 >= max_new) ? 1 : 0;
     state[3] = tok;
   }
+}
+
+__global__ void __launch_bounds__(kTokThreads)
+agent_next_token_kernel(float* logits, int V, const int* __restrict__ img_ids, int n_img, int* state,
+                        int* __restrict__ out_ids, int max_new, int eos, const uint4* __restrict__ embed,
+                        uint4* __restrict__ next_x, const uint4* __restrict__ hidden_src, uint4* __restrict__ hidden,
+                        int C8) {
+  __shared__ float sv[kTokThreads / 32];
+  __shared__ int si[kTokThreads / 32];
+  pdl_wait();
+  pdl_launch_dependents();
+  agent_next_token_row(logits, V, img_ids, n_img, state, out_ids, max_new, eos, embed, next_x, hidden_src, hidden, C8,
+                       sv, si);
+}
+
+// One CTA per row b, each its own sequence: logits[b], state[b], out_ids[b] (stride max_new), next_x[b],
+// hidden[b] (stride hidden_stride8 uint4s) and hidden_src[b]; img_ids, eos and max_new are shared.
+__global__ void __launch_bounds__(kTokThreads)
+agent_next_token_rows_kernel(float* logits, int V, const int* __restrict__ img_ids, int n_img, int* state,
+                             int* __restrict__ out_ids, int max_new, int eos, const uint4* __restrict__ embed,
+                             uint4* __restrict__ next_x, const uint4* __restrict__ hidden_src,
+                             uint4* __restrict__ hidden, long long hidden_stride8, int C8) {
+  __shared__ float sv[kTokThreads / 32];
+  __shared__ int si[kTokThreads / 32];
+  pdl_wait();
+  pdl_launch_dependents();
+  const int b = blockIdx.x;
+  agent_next_token_row(logits + static_cast<size_t>(b) * V, V, img_ids, n_img, state + 4 * b,
+                       out_ids + static_cast<size_t>(b) * max_new, max_new, eos, embed,
+                       next_x + static_cast<size_t>(b) * C8, hidden_src ? hidden_src + static_cast<size_t>(b) * C8 : nullptr,
+                       hidden + b * hidden_stride8, C8, sv, si);
 }
 
 template <typename Kern, typename... Args>
@@ -484,6 +588,52 @@ extern "C" int ds_attention_kv(const void* q, const void* kv_layer, void* out, f
                     static_cast<const float*>(ws), static_cast<__nv_bfloat16*>(out), pos, H, D, L_max, chunk, splits);
 }
 
+extern "C" int ds_rope_kv_append_rows(const void* qkv, void* q_out, void* kv, int64_t seq_stride, const int* pos,
+                                      int pos_stride, int B, int H, int D, int L_cap, float theta, void* stream) {
+  using namespace ds;
+  DS_REQUIRE(qkv && q_out && kv && pos, "ds_rope_kv_append_rows: NULL pointer");
+  DS_REQUIRE(B > 0 && H > 0 && L_cap > 0 && pos_stride >= 0 && (D == 64 || D == 128),
+             "ds_rope_kv_append_rows: bad shape (D = 64 or 128)");
+  DS_REQUIRE(seq_stride >= 2LL * H * L_cap * D || B == 1, "ds_rope_kv_append_rows: seq_stride < 2 * H * L_cap * D");
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  return launch_pdl("rope_kv_append_rows_kernel", rope_kv_append_rows_kernel, dim3(B), dim3(256), 0, stream,
+                    static_cast<const __nv_bfloat16*>(qkv), static_cast<__nv_bfloat16*>(q_out),
+                    static_cast<__nv_bfloat16*>(kv), static_cast<long long>(seq_stride), pos, pos_stride, H, D, L_cap,
+                    theta);
+}
+
+extern "C" int ds_attention_kv_rows(const void* q, const void* kv, int64_t seq_stride, void* out, float* ws,
+                                    int64_t ws_bytes, const int* pos, int pos_stride, int B, int H, int D, int L_cap,
+                                    int chunk, void* stream) {
+  using namespace ds;
+  DS_REQUIRE(q && kv && out && ws && pos, "ds_attention_kv_rows: NULL pointer");
+  DS_REQUIRE(B > 0 && B <= 65535 && H > 0 && H <= 65535 && L_cap > 0 && chunk > 0 && pos_stride >= 0 &&
+                 (D == 64 || D == 128),
+             "ds_attention_kv_rows: bad shape (D = 64 or 128)");
+  DS_REQUIRE(seq_stride >= 2LL * H * L_cap * D || B == 1, "ds_attention_kv_rows: seq_stride < 2 * H * L_cap * D");
+  const int splits = (L_cap + chunk - 1) / chunk;
+  const int64_t need = static_cast<int64_t>(B) * H * splits * (D + 2) * 4;
+  DS_REQUIRE(ws_bytes >= need, "ds_attention_kv_rows: workspace of %lld bytes < %lld",
+             static_cast<long long>(ws_bytes), static_cast<long long>(need));
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  const float scale = 1.0f / sqrtf(static_cast<float>(D));
+  const auto* qq = static_cast<const __nv_bfloat16*>(q);
+  const auto* kk = static_cast<const __nv_bfloat16*>(kv);
+  const long long ss = seq_stride;
+  int rc = D == 128 ? launch_pdl("attention_kv_rows_split_kernel", attention_kv_rows_split_kernel<4>,
+                                 dim3(splits, H, B), dim3(kAttnWarps * 32), 0, stream, qq, kk, ss, ws, pos, pos_stride,
+                                 H, L_cap, chunk, splits, scale)
+                    : launch_pdl("attention_kv_rows_split_kernel", attention_kv_rows_split_kernel<2>,
+                                 dim3(splits, H, B), dim3(kAttnWarps * 32), 0, stream, qq, kk, ss, ws, pos, pos_stride,
+                                 H, L_cap, chunk, splits, scale);
+  if (rc != DS_OK) return rc;
+  return launch_pdl("attention_kv_rows_combine_kernel", attention_kv_rows_combine_kernel, dim3(H, B), dim3(D), 0,
+                    stream, static_cast<const float*>(ws), static_cast<__nv_bfloat16*>(out), pos, pos_stride, H, D,
+                    L_cap, chunk, splits);
+}
+
 extern "C" int ds_silu_mul(const void* gate_up, void* out, int M, int I, void* stream) {
   using namespace ds;
   DS_REQUIRE(gate_up && out && M > 0 && I > 0 && I % 8 == 0, "ds_silu_mul: bad arguments (I %% 8 == 0)");
@@ -511,4 +661,22 @@ extern "C" int ds_agent_next_token(float* logits, int V, const int* img_ids, int
                     V, img_ids, n_img, state, out_ids, max_new, eos, static_cast<const uint4*>(embed),
                     static_cast<uint4*>(next_x), static_cast<const uint4*>(hidden_src), static_cast<uint4*>(hidden),
                     C / 8);
+}
+
+extern "C" int ds_agent_next_token_rows(float* logits, int V, const int* img_ids, int n_img, int* state, int* out_ids,
+                                        int max_new, int eos, const void* embed, void* next_x, const void* hidden_src,
+                                        void* hidden, int64_t hidden_stride, int C, int B, void* stream) {
+  using namespace ds;
+  DS_REQUIRE(logits && state && out_ids && embed && next_x && hidden && V > 0 && max_new > 0 && B > 0,
+             "ds_agent_next_token_rows: bad arguments");
+  DS_REQUIRE(n_img >= 0 && (n_img == 0 || img_ids), "ds_agent_next_token_rows: img_ids missing");
+  DS_REQUIRE(C > 0 && C % 8 == 0 && hidden_stride >= C && hidden_stride % 8 == 0 && aligned16(embed) &&
+                 aligned16(next_x) && aligned16(hidden) && (!hidden_src || aligned16(hidden_src)),
+             "ds_agent_next_token_rows: C %% 8 == 0, hidden_stride %% 8 == 0 and 16-byte aligned rows");
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  return launch_pdl("agent_next_token_rows_kernel", agent_next_token_rows_kernel, dim3(B), dim3(kTokThreads), 0,
+                    stream, logits, V, img_ids, n_img, state, out_ids, max_new, eos, static_cast<const uint4*>(embed),
+                    static_cast<uint4*>(next_x), static_cast<const uint4*>(hidden_src), static_cast<uint4*>(hidden),
+                    static_cast<long long>(hidden_stride / 8), C / 8);
 }

@@ -764,6 +764,107 @@ def agent_next_token(logits: torch.Tensor, img_ids: torch.Tensor, state: torch.T
                                   _ptr(hidden_src), hidden.data_ptr(), Cc, _stream()), "ds_agent_next_token")
 
 
+# B sequences decoded together, one row each (LlamaEngine.generate_ids_batch); B is bounded by ds_gemv_bf16's M
+ROWS_MAX = 8
+
+
+def _req_pos_rows(pos: torch.Tensor, B: int, name: str) -> int:
+    """``pos``: int32 CUDA [B] view (e.g. column 0 of a [B, 4] state); returns its element stride."""
+    if not isinstance(pos, torch.Tensor) or not pos.is_cuda or pos.dtype != torch.int32 or pos.dim() != 1 or \
+            pos.numel() != B or (B > 1 and pos.stride(0) < 1):
+        raise DsEngineError(f"{name}: expected an int32 CUDA [B={B}] tensor (any positive stride)")
+    _on_current_device(pos, name)
+    return pos.stride(0) if B > 1 else 1
+
+
+def _req_kv_rows(kv: torch.Tensor, name: str):
+    """``kv``: bf16 [B, 2, H, L_cap, D] whose per-row slices are contiguous; returns (B, H, L_cap, D)."""
+    if not isinstance(kv, torch.Tensor) or not kv.is_cuda or kv.dtype != bf16 or kv.dim() != 5 or \
+            not kv[0].is_contiguous():
+        raise DsEngineError(f"{name}: expected a bf16 CUDA [B, 2, H, L_cap, D] cache with contiguous row slices")
+    _on_current_device(kv, name)
+    B, two, H, L_cap, D = kv.shape
+    if two != 2 or not 1 <= B <= ROWS_MAX or (B > 1 and kv.stride(0) < 2 * H * L_cap * D):
+        raise DsEngineError(f"{name}: cache shape {tuple(kv.shape)} / strides {kv.stride()}: need 1 <= B <= "
+                            f"{ROWS_MAX} and non-overlapping [2, H, L_cap, D] slices")
+    return B, H, L_cap, D
+
+
+def rope_kv_append_rows(qkv: torch.Tensor, kv: torch.Tensor, pos: torch.Tensor, heads: int, theta: float,
+                        q_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``rope_kv_append`` for B sequences at once: row b of ``qkv`` [B, 3*heads*D] is at position ``pos[b]`` and
+    appends to its own slice ``kv[b]`` ([B, 2, heads, L_cap, D]); returns rotated q [B, heads*D]."""
+    _req(qkv, bf16, "rope_kv_append_rows.qkv", 2)
+    B, H, L_cap, D = _req_kv_rows(kv, "rope_kv_append_rows.kv")
+    ps = _req_pos_rows(pos, B, "rope_kv_append_rows.pos")
+    if H != heads or tuple(qkv.shape) != (B, 3 * H * D):
+        raise DsEngineError(f"rope_kv_append_rows: qkv must be [{B}, {3 * H * D}], got {tuple(qkv.shape)}")
+    q_out = torch.empty(B, H * D, dtype=bf16, device=qkv.device) if q_out is None else \
+        _req(q_out, bf16, "rope_kv_append_rows.q_out")
+    if q_out.numel() != B * H * D:
+        raise DsEngineError("rope_kv_append_rows: q_out must hold B*heads*D elements")
+    check(lib.ds_rope_kv_append_rows(qkv.data_ptr(), q_out.data_ptr(), kv.data_ptr(), kv.stride(0), pos.data_ptr(), ps,
+                                     B, H, D, L_cap, float(theta), _stream()), "ds_rope_kv_append_rows")
+    return q_out
+
+
+def attention_kv_rows_ws_floats(B: int, heads: int, L_cap: int, D: int) -> int:
+    return B * heads * (L_cap // ATTN_KV_CHUNK) * (D + 2)
+
+
+def attention_kv_rows(q: torch.Tensor, kv: torch.Tensor, pos: torch.Tensor, ws: Optional[torch.Tensor] = None,
+                      out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``attention_kv`` for B sequences at once: row b of ``q`` [B, heads*D] attends over keys 0 .. pos[b] of its own
+    slice ``kv[b]``.  ``L_cap`` must be a multiple of ATTN_KV_CHUNK, so the splits are the batch-1 decode's."""
+    _req(q, bf16, "attention_kv_rows.q", 2)
+    B, H, L_cap, D = _req_kv_rows(kv, "attention_kv_rows.kv")
+    ps = _req_pos_rows(pos, B, "attention_kv_rows.pos")
+    if tuple(q.shape) != (B, H * D):
+        raise DsEngineError(f"attention_kv_rows: q must be [{B}, {H * D}], got {tuple(q.shape)}")
+    if L_cap % ATTN_KV_CHUNK:
+        raise DsEngineError(f"attention_kv_rows: L_cap {L_cap} is not a multiple of {ATTN_KV_CHUNK}")
+    if ws is None:
+        ws = torch.empty(attention_kv_rows_ws_floats(B, H, L_cap, D), dtype=f32, device=q.device)
+    _req(ws, f32, "attention_kv_rows.ws")
+    out = torch.empty(B, H * D, dtype=bf16, device=q.device) if out is None else _req(out, bf16, "attention_kv_rows.out")
+    if out.numel() != B * H * D:
+        raise DsEngineError("attention_kv_rows: out must hold B*heads*D elements")
+    check(lib.ds_attention_kv_rows(q.data_ptr(), kv.data_ptr(), kv.stride(0), out.data_ptr(), ws.data_ptr(),
+                                   ws.numel() * 4, pos.data_ptr(), ps, B, H, D, L_cap, ATTN_KV_CHUNK, _stream()),
+          "ds_attention_kv_rows")
+    return out
+
+
+def agent_next_token_rows(logits: torch.Tensor, img_ids: torch.Tensor, state: torch.Tensor, out_ids: torch.Tensor,
+                          max_new: int, eos: int, embed: torch.Tensor, next_x: torch.Tensor,
+                          hidden_src: Optional[torch.Tensor], hidden: torch.Tensor) -> None:
+    """``agent_next_token`` for B sequences at once, each on its own row: ``logits`` fp32 [B, V], ``state`` int32
+    [B, 4], ``out_ids`` int32 [B, max_new], ``next_x`` bf16 [B, C], ``hidden`` bf16 [B, L, C], ``hidden_src`` bf16
+    [B, C] or None; ``img_ids``, ``eos`` and ``max_new`` are shared.  A row whose done flag is set changes nothing."""
+    _req(logits, f32, "agent_next_token_rows.logits", 2)
+    _req(img_ids, torch.int32, "agent_next_token_rows.img_ids")
+    _req(state, torch.int32, "agent_next_token_rows.state", 2)
+    _req(out_ids, torch.int32, "agent_next_token_rows.out_ids", 2)
+    _req(embed, bf16, "agent_next_token_rows.embed", 2)
+    _req(next_x, bf16, "agent_next_token_rows.next_x", 2)
+    _req(hidden, bf16, "agent_next_token_rows.hidden", 3)
+    V, Cc = embed.shape
+    B = logits.shape[0]
+    if not 1 <= B <= ROWS_MAX:
+        raise DsEngineError(f"agent_next_token_rows: need 1 <= B <= {ROWS_MAX}, got {B}")
+    if tuple(logits.shape) != (B, V) or tuple(state.shape) != (B, 4) or tuple(out_ids.shape) != (B, max_new) or \
+            tuple(next_x.shape) != (B, Cc) or hidden.shape[0] != B or hidden.shape[2] != Cc:
+        raise DsEngineError("agent_next_token_rows: shape mismatch")
+    if hidden_src is not None:
+        _req(hidden_src, bf16, "agent_next_token_rows.hidden_src", 2)
+        if tuple(hidden_src.shape) != (B, Cc):
+            raise DsEngineError("agent_next_token_rows: hidden_src must be [B, C]")
+    check(lib.ds_agent_next_token_rows(logits.data_ptr(), V, img_ids.data_ptr(), img_ids.numel(), state.data_ptr(),
+                                       out_ids.data_ptr(), int(max_new), int(eos), embed.data_ptr(), next_x.data_ptr(),
+                                       _ptr(hidden_src), hidden.data_ptr(), hidden.stride(0), Cc, B, _stream()),
+          "ds_agent_next_token_rows")
+
+
 # ---------------------------------------------------------------------------------------------- VAE decoder helpers
 def latent_pointwise(latents: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], inv_scale: float) -> torch.Tensor:
     """(latents * inv_scale) through a 1x1 conv 4 -> 4: fp32 NCHW [B,4,H,W] -> bf16 NHWC [B,H,W,4]."""

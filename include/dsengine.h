@@ -424,6 +424,19 @@ int ds_image_preprocess(const uint8_t* src, const int64_t* offsets, const int* s
  *                        the next entry's score becomes max + 10, else the scores of img_ids[1 ..] become 0.0; then
  *                        tok = argmax (first index on ties); out_ids[generated] = tok; next_x = embed[tok] (bf16
  *                        [V][C]); pos += 1; generated += 1; last = tok; done = (tok == eos || generated >= max_new).
+ * B sequences decoded together, one row each (B <= 8 in the engine, the GEMV's limit).  Row b has its own position
+ * pos[b * pos_stride] (device int32; the engine passes its [B][4] state with pos_stride 4) and its own cache slice
+ * kv + b * seq_stride elements, laid out [2][H][L_cap][D].  Each row computes what the batch-1 kernel computes for
+ * that sequence alone, bit for bit (same split boundaries when `chunk` is the batch-1 decode's).
+ *   ds_rope_kv_append_rows  : ds_rope_kv_append of row b of qkv bf16 [B][3][H][D] at position pos[b]: q_out[b],
+ *                             k / v appended at row pos[b] of its slice.  Rows at positions >= L_cap are skipped.
+ *   ds_attention_kv_rows    : out[b] = softmax(q[b] K_b^T / sqrt(D)) V_b over keys 0 .. pos[b] of slice b; q / out
+ *                             bf16 [B][H][D].  ceil(L_cap / chunk) splits per (row, head) and a combine pass; ws:
+ *                             fp32 workspace of >= B * H * splits * (D + 2) * 4 bytes.  D = 64 or 128.
+ *   ds_agent_next_token_rows: ds_agent_next_token for every row b on its own: logits fp32 [B][V], state int32 [B][4],
+ *                             out_ids int32 [B][max_new], next_x bf16 [B][C], hidden bf16 rows of row b at hidden +
+ *                             b * hidden_stride elements (hidden_stride % 8 == 0), hidden_src bf16 [B][C] or NULL.
+ *                             img_ids, eos and max_new are shared.  A row whose done is set changes nothing.
  * --------------------------------------------------------------------------------------------- */
 int ds_gemv_bf16(const void* x, const void* w, const void* residual, void* y, int M, int N, int K, int out_fp32,
                  void* stream);
@@ -436,6 +449,13 @@ int ds_silu_mul(const void* gate_up, void* out, int M, int I, void* stream);
 int ds_agent_next_token(float* logits, int V, const int* img_ids, int n_img, int* state, int* out_ids, int max_new,
                         int eos, const void* embed, void* next_x, const void* hidden_src, void* hidden, int C,
                         void* stream);
+int ds_rope_kv_append_rows(const void* qkv, void* q_out, void* kv, int64_t seq_stride, const int* pos, int pos_stride,
+                           int B, int H, int D, int L_cap, float theta, void* stream);
+int ds_attention_kv_rows(const void* q, const void* kv, int64_t seq_stride, void* out, float* ws, int64_t ws_bytes,
+                         const int* pos, int pos_stride, int B, int H, int D, int L_cap, int chunk, void* stream);
+int ds_agent_next_token_rows(float* logits, int V, const int* img_ids, int n_img, int* state, int* out_ids, int max_new,
+                             int eos, const void* embed, void* next_x, const void* hidden_src, void* hidden,
+                             int64_t hidden_stride, int C, int B, void* stream);
 
 #ifdef __cplusplus
 }
