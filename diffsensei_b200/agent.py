@@ -304,6 +304,22 @@ class LlamaEngine:
         return bb
 
 
+def mllm_inputs(prompt: str, tokenizer, num_img_tokens: int = 64):
+    """The demo's agent prompt for one panel (scripts/demo/gradio.py:36-57): BOS, then ``prompt``, a newline,
+    ``<img>`` + ``num_img_tokens`` x ``<img_i>`` + ``</img>`` and a newline.  Returns (input_ids int64 [L],
+    ids_cmp_mask bool [L]); the mask covers the image ids between the first ``<img>`` and ``</img>``, the rows that
+    ``AgentEngine`` replaces by ``input_resampler(image_embeds)``."""
+    image_tokens = BOI_TOKEN + "".join(IMG_TOKEN.format(i) for i in range(num_img_tokens)) + EOI_TOKEN
+    ids = torch.tensor([tokenizer.bos_token_id] + list(tokenizer.encode(prompt + "\n" + image_tokens + "\n",
+                                                                        add_special_tokens=False)), dtype=torch.long)
+    boi = tokenizer.encode(BOI_TOKEN, add_special_tokens=False)[1]       # [1]: past the leading "▁" piece
+    eoi = tokenizer.encode(EOI_TOKEN, add_special_tokens=False)[1]
+    mask = torch.zeros_like(ids, dtype=torch.bool)
+    first_boi, first_eoi = int(torch.where(ids == boi)[0][0]), int(torch.where(ids == eoi)[0][0])
+    mask[first_boi + 1:first_eoi] = True
+    return ids, mask
+
+
 def image_runs(generate_ids: torch.Tensor, eoi_token_id: int, image_gen_ids: Sequence[int], num_img_gen_tokens: int):
     """The post-processing of seed_x.py:139-159 on the new ids (1-D int64, CPU): every ``</img>`` at index >= N starts
     an image run at index - N, whose ids become ``image_gen_ids`` and whose ``ids_gen_mask`` is set.  Returns

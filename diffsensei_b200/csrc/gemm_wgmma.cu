@@ -1050,14 +1050,16 @@ static int prepare_gemm(const CUtensorMap& tmA, const CUtensorMap& tmA2, const v
   // ---- mixed-width schedule: when the last round of the persistent schedule would fill less than ~45 % of the CTAs,
   // the m-rows that fall into it are cut into 128-column units instead (twice as many, half as long; same kernel, same
   // launch: the MMA width, the B box and the epilogue's column range are per unit) and appended after the wide units,
-  // so the round-robin hands them to the CTAs that would otherwise idle.  Bit-identical results (same K order per
-  // output element).  DS_GEMM_TAIL=0: off.
+  // so the round-robin hands them to the CTAs that would otherwise idle.  Bit-identical outputs (same K order per
+  // output element).  Not with row_stats_out: a unit sums its rows' statistics in fp32 over its own columns before the
+  // fp64 add, so a row in a narrow unit would get differently rounded LayerNorm statistics, and whether the schedule
+  // runs depends on M — a sample's statistics would change with the batch it runs in.  DS_GEMM_TAIL=0: off.
   static const int tail_env = [] {
     const char* e = getenv("DS_GEMM_TAIL");
     return e ? atoi(e) : 1;
   }();
   if (tail_env && !chain && bn == 256 && p.epilogue != DS_EPI_GEGLU && p.N % 128 == 0 &&
-      !p.last_narrow) {
+      !p.last_narrow && !p.row_stats_out) {
     const int G = dev.num_sms;  // one persistent CTA per SM
     const int mp = p.num_m_tiles, nt = p.num_n_tiles;
     const int units = mp * nt;

@@ -60,9 +60,9 @@ __device__ __forceinline__ void gn_item_range(int total_items, int& i0, int& i1)
 }
 
 // Per-(sample, channel) {sum, sum of squares} of a [B][HW][C] bf16 tensor -> fp64 [B][C][2] (accumulated: the caller
-// zeroes it).  Threads keep fp32 partials over <= a few hundred pixels, the CTA's pixel rows are combined in a fixed
-// order in shared memory and every channel adds ONE fp64 pair per (CTA, sample) — fp64 sums of a few hundred fp32
-// partials are exact, so the result does not depend on the arrival order.
+// zeroes it).  Threads keep fp32 partials over one item's pixels, the CTA's pixel rows are combined in a fixed order
+// in shared memory and every channel adds ONE fp64 pair per item — fp64 sums of a few hundred fp32 partials are
+// exact, so the result does not depend on the arrival order.
 __global__ void chan_stats_kernel(const uint4* __restrict__ x, double* __restrict__ stats, int HW, int C,
                                   int items_per_sample, int ipx, int total_items) {
   extern __shared__ float shs[];  // [rpb][C][2]
@@ -111,16 +111,12 @@ __global__ void chan_stats_kernel(const uint4* __restrict__ x, double* __restric
     }
     __syncthreads();
   };
-  reset();
   const uint64_t pol = l2_policy_evict_last();  // the GroupNorm apply pass that follows re-reads x
-  int cur_b = i0 / items_per_sample;
   for (int it = i0; it < i1; ++it) {
+    // one fp32 partial per ITEM: an item's pixels and their order depend only on (HW, C), never on which CTA holds
+    // the item or how many samples share the launch, so a sample's statistics are the same bits at any batch size
     const int b = it / items_per_sample;
-    if (b != cur_b) {  // CTA-uniform
-      flush(cur_b);
-      reset();
-      cur_b = b;
-    }
+    reset();
     const int p0 = (it - b * items_per_sample) * ipx;
     const int p1 = min(p0 + ipx, HW);
     const uint4* base = x + (static_cast<size_t>(b) * HW) * cv + cvec;
@@ -133,8 +129,8 @@ __global__ void chan_stats_kernel(const uint4* __restrict__ x, double* __restric
       for (int k = 0; k < 8; ++k) accum(u[k]);
     }
     for (; p < p1; p += rpb) accum(ldg_hint(base + static_cast<size_t>(p) * cv, pol));
+    flush(b);
   }
-  flush(cur_b);
 }
 
 // GroupNorm(+SiLU) apply from per-channel statistics; x = [x1 | x2] along channels (x2 may be NULL).

@@ -12,6 +12,7 @@ Mirrors ``src/pipelines/pipeline_diffsensei.py``:
 engines and run through the two image processors on the GPU (image_processor.py).  Without them the encoders' inputs
 (token ids, pixel values) or outputs (``prompt_embeds`` ..., ``clip_image_embeds`` / ``magi_image_embeds``) can be
 passed instead; a raw prompt or image without what it needs raises, it does not fall back to anything.
+``generate_page`` runs the panels of a page together (one front-end pass, one denoise per group of same-size panels).
 
 Loop structure on the GPU (one process per GPU, one stream):
   once per panel : K|V projections of text and IP tokens for all cross-attention layers, time-embedding
@@ -36,6 +37,72 @@ from .scheduler import DDIMScheduler, EulerDiscreteScheduler
 from .unet import UNetMangaEngine
 
 bf16, f32 = torch.bfloat16, torch.float32
+
+# generate_page: what a captured stepper bakes in is the same for the whole page; everything else is per panel
+PAGE_KEYS = frozenset({"num_inference_steps", "guidance_scale", "ip_scale", "output_type", "use_graph",
+                       "max_batch_panels"})
+PANEL_KEYS = frozenset({
+    "prompt", "prompt_2", "negative_prompt", "negative_prompt_2", "height", "width", "num_samples", "generator",
+    "latents", "original_size", "crops_coords_top_left", "target_size", "min_size_step", "ip_images",
+    "ip_image_embeds", "clip_image_embeds", "magi_image_embeds", "clip_pixel_values", "magi_pixel_values", "ip_bbox",
+    "dialog_bbox", "prompt_embeds", "negative_prompt_embeds", "pooled_prompt_embeds", "negative_pooled_prompt_embeds",
+    "prompt_input_ids", "prompt_input_ids_2", "negative_prompt_input_ids", "negative_prompt_input_ids_2"})
+PAGE_MAX_ROWS = 8       # samples per page denoise: a UNet batch of 16 rows, as __call__(num_samples=8)
+
+
+def plan_page(shapes, max_batch_panels: int = PAGE_MAX_ROWS) -> List[List[int]]:
+    """The denoise chunks of a page.  ``shapes`` holds one (num_samples, h, w) per panel, h x w its latent size.
+    Panels of one latent size form a group, groups in order of first appearance; a group splits into consecutive
+    chunks of at most ``max_batch_panels`` samples, and a panel's samples are never split (a panel with more samples
+    than the cap is a chunk of its own).  Returns the panel indices of every chunk."""
+    cap = int(max_batch_panels)
+    if cap < 1:
+        raise ValueError(f"max_batch_panels must be >= 1, got {max_batch_panels}")
+    groups = {}
+    for i, (_, h, w) in enumerate(shapes):
+        groups.setdefault((int(h), int(w)), []).append(i)
+    chunks = []
+    for idx in groups.values():
+        cur, rows = [], 0
+        for i in idx:
+            k = int(shapes[i][0])
+            if cur and rows + k > cap:
+                chunks.append(cur)
+                cur, rows = [], 0
+            cur.append(i)
+            rows += k
+        chunks.append(cur)
+    return chunks
+
+
+def _stacked(fn, xs):
+    """``fn`` on the row-concatenation of the tensors ``xs``, once per distinct trailing shape; ``fn`` returns a tuple
+    of batch-major tensors.  Returns, per x, the tuple of its rows of every output."""
+    out, groups = [None] * len(xs), {}
+    for i, x in enumerate(xs):
+        groups.setdefault(tuple(x.shape[1:]), []).append(i)
+    for idx in groups.values():
+        res = fn(torch.cat([xs[i] for i in idx]))
+        r0 = 0
+        for i in idx:
+            r1 = r0 + xs[i].shape[0]
+            out[i] = tuple(t[r0:r1] for t in res)
+            r0 = r1
+    return out
+
+
+def _postprocess(image: torch.Tensor, output_type: str):
+    """The decoded fp32 NCHW [0, 1] images as ``output_type`` asks ("latent" / "pt": unchanged)."""
+    if output_type == "np":
+        return image.permute(0, 2, 3, 1).cpu().numpy()
+    if output_type == "pil":
+        try:
+            from PIL import Image
+        except ImportError as e:
+            raise RuntimeError("output_type='pil' needs Pillow; use 'pt' or 'np'") from e
+        arr = (image.permute(0, 2, 3, 1).cpu().numpy() * 255).round().astype("uint8")
+        return [Image.fromarray(a) for a in arr]
+    return image
 
 
 class DiffSenseiPipeline:
@@ -347,16 +414,308 @@ class DiffSenseiPipeline:
             return SimpleNamespace(images=final, latents=final)
         # pipeline_diffsensei.py:339-363: latents / scaling_factor -> vae.decode -> image_processor.postprocess
         image = self.vae.decode_image(final)                                            # fp32 NCHW in [0, 1]
-        if output_type == "np":
-            image = image.permute(0, 2, 3, 1).cpu().numpy()
-        elif output_type == "pil":
-            try:
-                from PIL import Image
-            except ImportError as e:
-                raise RuntimeError("output_type='pil' needs Pillow; use 'pt' or 'np'") from e
-            arr = (image.permute(0, 2, 3, 1).cpu().numpy() * 255).round().astype("uint8")
-            image = [Image.fromarray(a) for a in arr]
-        return SimpleNamespace(images=image, latents=final)
+        return SimpleNamespace(images=_postprocess(image, output_type), latents=final)
+
+    # ------------------------------------------------------------------------------ a page of panels
+    @torch.no_grad()
+    def generate_page(self, panels: List[dict], *, num_inference_steps: int = 40, guidance_scale: float = 5.0,
+                      ip_scale: float = 1.0, output_type: str = "latent", use_graph: bool = True,
+                      max_batch_panels: int = PAGE_MAX_ROWS, agent=None, tokenizer_mllm=None,
+                      mllm_scale: float = 0.4, max_new_tokens: int = 500) -> List[SimpleNamespace]:
+        """Several panels of a page in one call.  ``panels`` holds one dict per panel with the per-panel keywords of
+        ``__call__`` (``PANEL_KEYS``); the keywords here are the same for the whole page.  Returns one
+        ``SimpleNamespace(images=..., latents=...)`` per panel, in panel order, each ``torch.equal`` to
+        ``pipe(**panel, <the page keywords>)`` run alone: every kernel on the path gives a row the same bits whatever
+        the batch around it.
+
+        The front end runs once per page: each text encoder on the stacked token ids of every panel (positives and
+        string negatives), the two image processors and each image encoder on every panel's character images, and the
+        character Resampler on [panels + 1, max_num_ips, ...] (the last row is the all-zero negative every panel
+        shares; one call per distinct encoder sequence length, so a panel without characters, which the reference pads
+        with 257 zero tokens, joins the 257-token call).  Panels whose latents have the same size are then denoised
+        together, ``max_batch_panels`` samples (latent rows) at most per denoise: the default 8 keeps the UNet batch
+        at the 16 rows of ``__call__(num_samples=8)``.  Each chunk is one ``denoise`` (a cached stepper is refilled
+        when the chunk's shapes repeat) and one batched VAE decode.
+
+        Initial noise: each panel draws its latents from its own ``generator``, with the solo call's shape; panels
+        without a generator draw from the global RNG in panel order, as the same calls made one after another would.
+
+        ``agent=`` (an ``AgentEngine``, with ``tokenizer_mllm``) runs the demo's MLLM composition
+        (scripts/demo/gradio.py:85-129) for every panel: the character images, padded to ``max_num_ips`` with black
+        224² images (encoded, not zeroed) and truncated to it, go through the encoders and the Resampler; the agent
+        decodes every panel's ``mllm_inputs(prompt)`` with those embeddings (``generate_batch``, ``max_new_tokens``);
+        its image features are blended as ``feat * mllm_scale + embeds * (1 - mllm_scale)``, and the blend is
+        denoised as ``ip_image_embeds`` with ``ip_images=[]`` and ``ip_bbox`` padded with zero boxes."""
+        if not isinstance(panels, (list, tuple)) or len(panels) == 0:
+            raise ValueError("generate_page needs a non-empty list of panel dicts")
+        panels = [dict(p) for p in panels]
+        for i, p in enumerate(panels):
+            for k in p:
+                if k in PAGE_KEYS:
+                    raise ValueError(f"panel {i}: `{k}` is the same for the whole page; pass it to generate_page")
+                if k not in PANEL_KEYS:
+                    raise ValueError(f"panel {i}: unknown key `{k}`")
+        if output_type not in ("latent", "pt", "np", "pil"):
+            raise ValueError(f"output_type must be one of latent / pt / np / pil, got {output_type!r}")
+        if output_type != "latent" and self.vae is None:
+            raise ValueError("output_type other than 'latent' needs a VAE decoder: DiffSenseiPipeline(..., vae=...)")
+        if guidance_scale <= 1.0:
+            raise ValueError("guidance_scale <= 1 disables classifier-free guidance; the engine's denoise step is the "
+                             "fused CFG + scheduler update and does not implement the guidance-free variant")
+        if int(max_batch_panels) < 1:
+            raise ValueError(f"max_batch_panels must be >= 1, got {max_batch_panels}")
+        if agent is not None:
+            self._check_agent_panels(panels, tokenizer_mllm)
+            for i, p in enumerate(panels):          # the panels' own checks too, before the agent's decode
+                self._panel_job(i, p)
+            panels = self._agent_panels(panels, agent, tokenizer_mllm, mllm_scale, max_new_tokens)
+        jobs = [self._panel_job(i, p) for i, p in enumerate(panels)]        # host checks and tokenization only
+
+        # ---- front end, once per page
+        dev = self.unet.device
+        text = _stacked(lambda ids: (self.text_encoder(ids, output_hidden_states=True).hidden_states[-2],),
+                        [x for j in jobs if j.ids is not None for x in (j.ids[0], j.ids[2]) if x is not None])
+        text_2 = _stacked(lambda ids: (lambda o: (o.hidden_states[-2], o[0]))(
+                          self.text_encoder_2(ids, output_hidden_states=True)),
+                          [x for j in jobs if j.ids is not None for x in (j.ids[1], j.ids[3]) if x is not None])
+        for j in jobs:
+            if j.ids is None:
+                continue
+            (h1,), (h2, pooled) = text.pop(0), text_2.pop(0)
+            j.pe, j.pp = torch.cat([h1, h2], dim=-1), pooled
+            if j.ids[2] is None:
+                j.npe, j.npp = torch.zeros_like(j.pe), torch.zeros_like(j.pp)
+            else:
+                (h1,), (h2, pooled) = text.pop(0), text_2.pop(0)
+                j.npe, j.npp = torch.cat([h1, h2], dim=-1), pooled
+        self._encode_page_images(jobs)
+        m, nv = self.unet.cfg.max_num_ips, self.unet.cfg.num_vision_tokens
+        for j, (img, neg) in zip(jobs, self._character_embeds([(j.clip, j.magi) for j in jobs])):
+            if j.ip_image_embeds is not None:                                          # :143-145
+                e = j.ip_image_embeds[:m]
+                img = img.clone()
+                img[0, nv:(1 + e.shape[0]) * nv, :] = e.reshape(1, -1, e.shape[-1]).to(img)
+            j.img, j.neg_img = img, neg
+
+        # ---- noise and per-panel condition rows, then one denoise + one decode per chunk
+        self._guidance_scale = guidance_scale
+        self.set_ip_scale(ip_scale)
+        self.scheduler.set_timesteps(num_inference_steps, device=dev)
+        for j in jobs:                                                     # panel order: the global RNG's order
+            if j.latents is None:
+                j.latents = self.prepare_latents(j.ns, self.unet.config.in_channels, j.height, j.width, j.generator)
+            else:
+                j.latents = j.latents * self.scheduler.init_noise_sigma
+        results = [None] * len(jobs)
+        for chunk in plan_page([(j.ns,) + tuple(j.latents.shape[-2:]) for j in jobs], max_batch_panels):
+            rows = [self._panel_rows(jobs[i]) for i in chunk]
+            cat = lambda k: torch.cat([r[0][k] for r in rows] + [r[1][k] for r in rows], dim=0)
+            lat = torch.cat([jobs[i].latents for i in chunk], dim=0)
+            final = self.denoise(lat, cat("pe"), cat("te"), cat("ti"), cat("bbox"), lat.shape[-2] / lat.shape[-1],
+                                 cat("db"), num_inference_steps, guidance_scale, use_graph=use_graph)
+            image = self.vae.decode_image(final) if output_type != "latent" else final
+            r0 = 0
+            for i in chunk:
+                r1 = r0 + jobs[i].ns
+                results[i] = SimpleNamespace(images=_postprocess(image[r0:r1], output_type), latents=final[r0:r1])
+                r0 = r1
+        return results
+
+    def _panel_job(self, i: int, p: dict) -> SimpleNamespace:
+        """One panel's arguments resolved as ``__call__`` resolves them, with its ValueErrors prefixed by the panel
+        index; runs on the host only (tokenization included), so a bad panel fails before any GPU work."""
+        g = lambda k, d=None: p.get(k, d)
+        try:
+            height = g("height") or self.default_sample_size * self.vae_scale_factor
+            width = g("width") or self.default_sample_size * self.vae_scale_factor
+            ip_images, ip_bbox = list(g("ip_images", ())), list(g("ip_bbox", ()))
+            ip_image_embeds = g("ip_image_embeds")
+            if len(ip_images) > 0:
+                if ip_image_embeds is not None:
+                    raise ValueError("`ip_images` and `ip_image_embeds` can not be input together!")
+                if any(g(k) is not None for k in ("clip_pixel_values", "magi_pixel_values", "clip_image_embeds",
+                                                  "magi_image_embeds")):
+                    raise ValueError("`ip_images` and pixel values / image embeddings can not be input together!")
+            ids = None
+            if g("prompt_embeds") is None:
+                if g("prompt_input_ids") is None and isinstance(g("prompt"), str) and \
+                        self.tokenizer is not None and self.tokenizer_2 is not None:
+                    ids = self.tokenize_prompt(g("prompt"), g("prompt_2"), g("negative_prompt"),
+                                               g("negative_prompt_2"))
+                elif g("prompt_input_ids") is not None:
+                    ids = (g("prompt_input_ids"), g("prompt_input_ids_2"), g("negative_prompt_input_ids"),
+                           g("negative_prompt_input_ids_2"))
+                if ids is None:
+                    self.check_inputs(g("prompt"), g("prompt_2"), ip_images, ip_image_embeds, ip_bbox)
+                    raise NotImplementedError(
+                        "raw prompt strings need the CLIP tokenizers (tokenizer= / tokenizer_2=): pass "
+                        "prompt_input_ids with the text-encoder engines registered, or the prompt embeddings")
+                if self.text_encoder is None or self.text_encoder_2 is None:
+                    raise ValueError("encode_prompt_ids needs text_encoder and text_encoder_2 engines")
+                as_ids = lambda t: None if t is None else torch.as_tensor(t)
+                # negative_prompt_input_ids_2 without negative_prompt_input_ids: zero negatives, as in __call__
+                ids = (as_ids(ids[0]), as_ids(ids[1] if ids[1] is not None else ids[0]), as_ids(ids[2]),
+                       None if ids[2] is None else as_ids(ids[3] if ids[3] is not None else ids[2]))
+            m = self.unet.cfg.max_num_ips
+            clip_pv = magi_pv = None
+            n_real = 0
+            if len(ip_images) > 0:
+                if len(ip_images) != len(ip_bbox):
+                    raise ValueError(f"`ip_images` must have the same length as `ip_bbox`. But they are in length "
+                                     f"{len(ip_images)} and {len(ip_bbox)}!")
+                if self.image_encoder is None or self.magi_image_encoder is None:
+                    raise NotImplementedError("ip_images need the image-encoder engines (image_encoder= and "
+                                              "register_manga_modules(magi_image_encoder=...)); or pass "
+                                              "clip_image_embeds / magi_image_embeds")
+                ip_images, ip_bbox = ip_images[:m], ip_bbox[:m]
+                n_real = len(ip_images)
+            elif g("clip_image_embeds") is None and g("clip_pixel_values") is not None:
+                if self.image_encoder is None or self.magi_image_encoder is None:
+                    raise ValueError("encode_ip_images needs image_encoder and magi_image_encoder engines")
+                clip_pv, magi_pv = torch.as_tensor(g("clip_pixel_values")), torch.as_tensor(g("magi_pixel_values"))
+                n_real = clip_pv.shape[0]
+            elif g("clip_image_embeds") is not None:
+                n_real = g("clip_image_embeds").shape[1]
+            num_ips = len(ip_image_embeds) if ip_image_embeds is not None else n_real
+            if num_ips != len(ip_bbox):
+                raise ValueError(f"`ip_images` must have the same length as `ip_bbox`. But they are in length "
+                                 f"{num_ips} and {len(ip_bbox)}!")
+        except (ValueError, NotImplementedError) as e:
+            raise type(e)(f"panel {i}: {e}") from e
+        ns = int(g("num_samples", 1))
+        return SimpleNamespace(
+            index=i, ns=ns, height=height, width=width, generator=g("generator"), latents=g("latents"), ids=ids,
+            pe=g("prompt_embeds"), npe=g("negative_prompt_embeds"), pp=g("pooled_prompt_embeds"),
+            npp=g("negative_pooled_prompt_embeds"), ip_images=ip_images, clip_pv=clip_pv, magi_pv=magi_pv,
+            clip=g("clip_image_embeds"), magi=g("magi_image_embeds"), ip_image_embeds=ip_image_embeds,
+            ip_bbox=ip_bbox, dialog_bbox=list(g("dialog_bbox", ())),
+            time_ids=list(g("original_size") or (height, width)) + list(g("crops_coords_top_left", (0, 0))) +
+            list(g("target_size") or (height, width)))
+
+    def _encode_page_images(self, jobs) -> None:
+        """Every panel's character images through the two processors and each image encoder once; panels given
+        pixel values join the encoder calls.  Sets ``clip`` (1, n, S, D) / ``magi`` (1, n, Dm) on those panels."""
+        dev = self.unet.device
+        images = [self.clip_image_processor.to_device(im, dev) for j in jobs for im in j.ip_images]  # upload once
+        if images:
+            clip_all = self.clip_image_processor(images=images, return_tensors="pt").pixel_values
+            magi_all = self.magi_image_processor(images=images, return_tensors="pt").pixel_values
+            r0 = 0
+            for j in jobs:
+                if j.ip_images:
+                    r1 = r0 + len(j.ip_images)
+                    j.clip_pv, j.magi_pv = clip_all[r0:r1], magi_all[r0:r1]
+                    r0 = r1
+        enc = [j for j in jobs if j.clip is None and j.clip_pv is not None]
+        if not enc:
+            return
+        clip = _stacked(lambda pv: (self.image_encoder(pv, output_hidden_states=True).hidden_states[-2],),
+                        [j.clip_pv.to(dev) for j in enc])
+        magi = _stacked(lambda pv: (self.magi_image_encoder(pv).last_hidden_state[:, 0],),
+                        [j.magi_pv.to(dev) for j in enc])
+        for j, (c,), (mg,) in zip(enc, clip, magi):
+            j.clip, j.magi = c.unsqueeze(0), mg.unsqueeze(0)
+
+    def _character_embeds(self, chars):
+        """``prepare_ip_image_embeds``' Resampler passes (:118-135) for a page: ``chars`` holds one (clip (1, n, S, D),
+        magi (1, n, Dm)) per panel, or (None, None) for a panel without characters.  Each panel's characters are
+        truncated / zero-padded to ``max_num_ips`` and all panels of one sequence length S go through the Resampler in
+        one call, together with the all-zero row that is every such panel's negative (a panel without characters is
+        all zeros on both branches, with S = 257).  Returns one (image_embeds, negative_image_embeds) pair per panel,
+        (1, T, D) bf16 rows of the shared output: clone before writing."""
+        m, dev = self.unet.cfg.max_num_ips, self.unet.device
+        rc = getattr(self.image_proj_model, "rc", None)
+        groups = {}
+        for i, (clip, magi) in enumerate(chars):
+            if clip is None or magi is None:
+                if rc is None:
+                    raise ValueError(f"panel {i}: a panel without character references needs an image_proj_model "
+                                     "that exposes its ResamplerConfig (`.rc`) to size the zero embeddings")
+                key = (257, rc.embedding_dim, rc.magi_embedding_dim)
+            else:
+                key = (clip.shape[2], clip.shape[3], magi.shape[-1])
+            groups.setdefault(key, []).append(i)
+        out = [None] * len(chars)
+        for (S, D, Dm), idx in groups.items():
+            real = [i for i in idx if chars[i][0] is not None and chars[i][1] is not None]
+            clip = torch.zeros(len(real) + 1, m, S, D, dtype=bf16, device=dev)
+            magi = torch.zeros(len(real) + 1, m, Dm, dtype=bf16, device=dev)
+            for r, i in enumerate(real):
+                c, mg = chars[i]
+                n = min(c.shape[1], m)
+                clip[r, :n] = c[0, :n].to(dev).to(bf16)       # the dtype cast the Resampler applies, element by element
+                magi[r, :n] = mg[0, :n].to(dev).to(bf16)
+            emb = self.image_proj_model(clip, magi)
+            neg = emb[-1:]
+            for i in idx:
+                out[i] = (emb[real.index(i):real.index(i) + 1] if i in real else neg, neg)
+        return out
+
+    def _panel_rows(self, j):
+        """One panel's [negative, positive] condition rows, each repeated to its ``num_samples`` (:293-304)."""
+        dev, ns = self.unet.device, j.ns
+        m = self.unet.cfg.max_num_ips
+        ip_bbox = [list(b) for b in j.ip_bbox[:m]]
+        while len(ip_bbox) < m:
+            ip_bbox.append([0.0, 0.0, 0.0, 0.0])                                       # :121-122
+        bbox = torch.tensor(ip_bbox, dtype=f32).unsqueeze(0).to(dev)
+        neg_db, db = self.prepare_dialog_bbox(j.dialog_bbox, ns)
+        rep = lambda t: t.to(dev).repeat(ns, 1, 1) if t.dim() == 3 else t.to(dev).repeat(ns, 1)
+        ti = torch.tensor([j.time_ids], dtype=f32, device=dev).repeat(ns, 1)
+        side = lambda pe, pp, img, bb, d: dict(pe=torch.cat([rep(pe).to(bf16), rep(img).to(bf16)], dim=1),
+                                               te=rep(pp), ti=ti, bbox=rep(bb), db=d)
+        return (side(j.npe, j.npp, j.neg_img, torch.zeros_like(bbox), neg_db), side(j.pe, j.pp, j.img, bbox, db))
+
+    def _check_agent_panels(self, panels, tokenizer_mllm) -> None:
+        """The host-only checks of the ``agent=`` path."""
+        if tokenizer_mllm is None:
+            raise ValueError("agent= needs tokenizer_mllm")
+        if self.image_encoder is None or self.magi_image_encoder is None or self.image_proj_model is None:
+            raise ValueError("agent= needs the image encoders and the character Resampler registered")
+        for i, p in enumerate(panels):
+            if not isinstance(p.get("prompt"), str):
+                raise ValueError(f"panel {i}: agent= needs a `prompt` string")
+            for k in ("ip_image_embeds", "clip_image_embeds", "magi_image_embeds", "clip_pixel_values",
+                      "magi_pixel_values", "prompt_embeds", "prompt_input_ids"):
+                if p.get(k) is not None:
+                    raise ValueError(f"panel {i}: agent= takes `prompt` and `ip_images`, not `{k}`")
+            if len(p.get("ip_images", ())) != len(p.get("ip_bbox", ())):
+                raise ValueError(f"panel {i}: `ip_images` must have the same length as `ip_bbox`. But they are in "
+                                 f"length {len(p.get('ip_images', ()))} and {len(p.get('ip_bbox', ()))}!")
+
+    def _agent_panels(self, panels, agent, tokenizer_mllm, mllm_scale, max_new_tokens):
+        """The demo's MLLM composition (scripts/demo/gradio.py:85-129) for every panel at once; returns the panels as
+        the pipeline then runs them: ``ip_images=[]``, ``ip_image_embeds`` = the blend, ``ip_bbox`` padded."""
+        from .agent import mllm_inputs
+        m, nv = self.unet.cfg.max_num_ips, self.unet.cfg.num_vision_tokens
+        dev = self.unet.device
+        black = torch.zeros(224, 224, 3, dtype=torch.uint8, device=dev)                # gradio.py:87-90
+        images = [[self.clip_image_processor.to_device(im, dev) for im in list(p.get("ip_images", ()))[:m]]
+                  for p in panels]
+        images = [ims + [black] * (m - len(ims)) for ims in images]
+        flat = [im for ims in images for im in ims]
+        clip_pv = self.clip_image_processor(images=flat, return_tensors="pt").pixel_values
+        magi_pv = self.magi_image_processor(images=flat, return_tensors="pt").pixel_values
+        clip = self.image_encoder(clip_pv, output_hidden_states=True).hidden_states[-2]
+        magi = self.magi_image_encoder(magi_pv).last_hidden_state[:, 0]
+        chars = [(clip[k * m:(k + 1) * m].unsqueeze(0), magi[k * m:(k + 1) * m].unsqueeze(0))
+                 for k in range(len(panels))]
+        embeds = [img[:, nv:, :] for img, _ in self._character_embeds(chars)]         # gradio.py:96-97
+        prompts = [mllm_inputs(p["prompt"], tokenizer_mllm) for p in panels]
+        outs = agent.generate_batch(tokenizer=tokenizer_mllm, input_ids=[ids[None] for ids, _ in prompts],
+                                    image_embeds=embeds, ids_cmp_mask=[mask[None] for _, mask in prompts],
+                                    max_new_tokens=max_new_tokens,
+                                    num_img_gen_tokens=agent.output_resampler.num_queries)
+        out_panels = []
+        for i, (p, o, e) in enumerate(zip(panels, outs, embeds)):
+            if o["num_gen_imgs"] != 1:
+                raise ValueError(f"panel {i}: the agent generated {o['num_gen_imgs']} images (num_gen_imgs); the "
+                                 "mllm_scale blend needs exactly one")
+            blend = o["img_gen_feat"].view(m, nv, -1) * mllm_scale + e.view(m, nv, -1) * (1 - mllm_scale)  # :108-109
+            bbox = [list(b) for b in list(p.get("ip_bbox", ()))[:m]]
+            bbox += [[0.0, 0.0, 0.0, 0.0]] * (m - len(bbox))
+            out_panels.append({**p, "ip_images": [], "ip_image_embeds": blend, "ip_bbox": bbox})
+        return out_panels
 
 
 class DenoiseStepper:

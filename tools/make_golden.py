@@ -13,6 +13,7 @@ committed; re-run this script only in the build container:
 
     python tools/make_golden.py            # every fixture
     python tools/make_golden.py agent      # tests/golden/agent_generate.pt only
+    python tools/make_golden.py mllm       # tests/golden/mllm_inputs.pt only
 """
 from __future__ import annotations
 
@@ -35,13 +36,14 @@ def load_module(name: str, path: str):
     return mod
 
 
-def lift_function(path: str, func_name: str):
-    """Compile one function definition out of a module that cannot be imported (missing diffusers)."""
+def lift_function(path: str, func_name: str, **module_globals):
+    """Compile one function definition out of a module that cannot be imported (missing diffusers); the function
+    sees ``torch`` and ``module_globals`` as its module's globals."""
     tree = ast.parse(open(path).read())
     for node in ast.walk(tree):
         if isinstance(node, ast.FunctionDef) and node.name == func_name:
             mod = ast.Module(body=[node], type_ignores=[])
-            ns = {"torch": torch}
+            ns = {"torch": torch, **module_globals}
             exec(compile(mod, path, "exec"), ns)
             return ns[func_name]
     raise KeyError(func_name)
@@ -243,6 +245,7 @@ class StubTokenizer:
     (what the reference's ``encode(EOI_TOKEN)[1]`` relies on); ``<img>``, ``<img_00000>`` .. and ``</img>`` are single
     ids; any other character is one id."""
     SPACE, BOI, IMG0, EOI = 29, 900, 901, 965
+    bos_token_id = 1
 
     def encode(self, s, add_special_tokens=False):
         ids, i = [self.SPACE], 0
@@ -366,7 +369,23 @@ def _raw_sequence(llm, ids, emb, img_ids, eos, max_new):
     return greedy(llm, ids, emb, img_ids, eos, max_new)[0]
 
 
+MLLM_PROMPTS = ["", "a manga panel", "two girls talk on a rooftop at night,\nwind", "<img> inside a prompt"]
+
+
+def mllm_golden():
+    """tests/golden/mllm_inputs.pt: the demo's ``get_mllm_inputs`` (scripts/demo/gradio.py:36-57, lifted out of the
+    gradio module) EXECUTED on ``StubTokenizer`` for ``MLLM_PROMPTS``."""
+    get_mllm_inputs = lift_function(f"{REF}/scripts/demo/gradio.py", "get_mllm_inputs", BOI_TOKEN="<img>",
+                                    EOI_TOKEN="</img>", IMG_TOKEN="<img_{:05d}>")
+    cases = [{"prompt": p, **dict(zip(("input_ids", "ids_cmp_mask"), get_mllm_inputs(p, StubTokenizer())))}
+             for p in MLLM_PROMPTS]
+    torch.save(cases, f"{OUT}/mllm_inputs.pt")
+    print("mllm_inputs.pt", os.path.getsize(f"{OUT}/mllm_inputs.pt"))
+
+
 if __name__ == "__main__":
     if sys.argv[1:] == ["agent"]:
         sys.exit(agent_golden())
+    if sys.argv[1:] == ["mllm"]:
+        sys.exit(mllm_golden())
     sys.exit(main())
