@@ -5,6 +5,8 @@ Public surface (mirrors the reference's, SURVEY.md §8b):
     AttnProcessor2_0, MaskedIPAttnProcessor2_0  <- src/models/attention_processor.py
     ResamplerEngine        <- src/models/resampler.py       Resampler
     VaeDecoderEngine       <- diffusers AutoencoderKL.decode as used by pipeline_diffsensei.py:339-363
+    VaeEncoderEngine, VaeImageProcessor  <- diffusers AutoencoderKL.encode + VaeImageProcessor.preprocess, for
+                              img2img (``DiffSenseiPipeline(vae_encoder=...)(image=..., strength=...)``)
     ClipTextEncoderEngine, ClipVisionEncoderEngine, VitMaeEncoderEngine  <- transformers CLIP / ViT-MAE encoders as
                               used by encode_prompt (:232-245) and prepare_ip_image_embeds (:125-128)
     CLIPImageProcessor, ViTImageProcessor  <- transformers' image processors as constructed by
@@ -26,11 +28,11 @@ from .config import (AGENT_TINY, LLAMA2_13B, RESAMPLER, RESAMPLER_TINY, SDXL_MAN
                      AgentConfig, VaeConfig)
 from .encoders import (CLIP_L_TEXT, CLIP_VIT_H, MAGI_VIT_MAE, OPENCLIP_BIGG_TEXT, ClipTextEncoderEngine,  # noqa: F401
                        ClipVisionEncoderEngine, EncoderConfig, VitMaeEncoderEngine)
-from .image_processor import CLIPImageProcessor, ViTImageProcessor  # noqa: F401
+from .image_processor import CLIPImageProcessor, VaeImageProcessor, ViTImageProcessor  # noqa: F401
 from .pipeline import DiffSenseiPipeline  # noqa: F401
 from .resampler import QwenResamplerEngine, ResamplerEngine  # noqa: F401
-from .scheduler import DDIMScheduler, EulerDiscreteScheduler, scheduler_from_config  # noqa: F401
+from .scheduler import DDIMScheduler, EulerDiscreteScheduler, get_timesteps, scheduler_from_config  # noqa: F401
 from .unet import UNet2DConditionOutput, UNetMangaEngine  # noqa: F401
-from .vae import VaeDecoderEngine  # noqa: F401
+from .vae import VaeDecoderEngine, VaeEncoderEngine  # noqa: F401
 
 __version__ = "0.1.0"

@@ -37,7 +37,7 @@ class Conv3x3Args(C.Structure):
                 ("B", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("Cin", C.c_int32), ("Cout", C.c_int32),
                 ("stride", C.c_int32), ("rowbias_ld", C.c_int32), ("out_fp32", C.c_int32), ("out_scale", C.c_float),
                 ("splitk_ws", C.c_void_p), ("splitk_ws_bytes", C.c_int64), ("chan_stats", C.c_void_p),
-                ("upsample2", C.c_int32)]
+                ("upsample2", C.c_int32), ("pad_bottom_right", C.c_int32)]
 
 
 class CrossIpArgs(C.Structure):
@@ -87,6 +87,9 @@ SIGNATURES = {
     "ds_image_postprocess": [_vp, _vp, _i, _i, _i, _vp],
     "ds_attention_single_head": [_vp, _vp, _vp, _vp, _i, _i, _i, _i64, _vp],
     "ds_image_preprocess": [_vp, _vp, _vp, _i, _i, _vp, _vp, _i64, _vp],
+    "ds_vae_image_preprocess": [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _i64, _vp],
+    "ds_vae_image_pack": [_vp, _vp, _vp, _i, _i, _i, _vp],
+    "ds_vae_posterior": [_vp, _vp, _vp, _vp, _f, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _vp],
     "ds_gemv_bf16": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "ds_rmsnorm": [_vp, _vp, _vp, _i, _i, _f, _vp],
     "ds_rope_kv_append": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp],
@@ -98,7 +101,8 @@ SIGNATURES = {
     "ds_agent_next_token_rows": [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i64, _i, _i, _vp],
 }
 OTHER_EXPORTS = ("ds_version", "ds_last_error", "ds_launch_count", "ds_groupnorm_scratch_floats",
-                 "ds_gemm_splitk_ws_bytes", "ds_image_preprocess_scratch_bytes")
+                 "ds_gemm_splitk_ws_bytes", "ds_image_preprocess_scratch_bytes",
+                 "ds_vae_image_preprocess_scratch_bytes")
 
 
 def _load() -> C.CDLL:
@@ -120,6 +124,8 @@ def _load() -> C.CDLL:
     lib.ds_gemm_splitk_ws_bytes.restype = C.c_int64
     lib.ds_image_preprocess_scratch_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int]
     lib.ds_image_preprocess_scratch_bytes.restype = C.c_int64
+    lib.ds_vae_image_preprocess_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
+    lib.ds_vae_image_preprocess_scratch_bytes.restype = C.c_int64
     return lib
 
 

@@ -1316,7 +1316,7 @@ extern "C" int ds_conv3x3_nhwc(const ds_conv3x3_args* a, void* stream) {
     // conv3x3(nearest_x2(x)) as FOUR 2x2 convolutions of x, one per output-pixel parity (a, b): the 3x3 taps that read
     // the same low-resolution pixel are pre-summed (weights.pack_conv3x3_up2), so the op does 16 instead of 36 MACs per
     // (low-res pixel, Cin, Cout) and the upsampled tensor is never written.  Phase (a, b) writes pixels (2i+a, 2j+b).
-    DS_REQUIRE(a->stride == 1 && !a->residual && !a->rowbias && !a->out_fp32 && a->Cout % 8 == 0 &&
+    DS_REQUIRE(a->stride == 1 && !a->pad_bottom_right && !a->residual && !a->rowbias && !a->out_fp32 && a->Cout % 8 == 0 &&
                    (reinterpret_cast<uintptr_t>(a->out) & 15) == 0,
                "ds_conv3x3_nhwc: upsample2 needs stride 1, bf16 output with Cout %% 8 == 0, no residual / rowbias");
     const size_t wph = static_cast<size_t>(a->Cout) * 4 * a->Cin;  // elements per phase: [Cout][2][2][Cin]
@@ -1328,6 +1328,15 @@ extern "C" int ds_conv3x3_nhwc(const ds_conv3x3_args* a, void* stream) {
       if (rc != DS_OK) return rc;
     }
     return DS_OK;
+  }
+  if (a->pad_bottom_right) {
+    // diffusers Downsample2D(padding=0) of the VAE encoder: F.pad(x, (0, 1, 0, 1)) then a stride-2 conv without
+    // padding.  Output pixel i reads input rows / columns 2i .. 2i+2: the tap window starts at offset 0 instead of -1,
+    // and the one padded row and column are the tensor map's out-of-bounds zero fill.
+    DS_REQUIRE(a->stride == 2 && a->H >= 2 && a->W >= 2,
+               "ds_conv3x3_nhwc: pad_bottom_right needs stride 2 and H, W >= 2 (got stride %d, %d x %d)", a->stride,
+               a->H, a->W);
+    return conv_launch(a, a->w, a->out, a->H / 2, a->W / 2, 3, 3, 0, 0, 1, st);
   }
   const int Ho = (a->H - 1) / a->stride + 1;
   const int Wo = (a->W - 1) / a->stride + 1;

@@ -19,6 +19,11 @@
 // Three launches per batch of up to kMaxImages images: coefficient tables, horizontal pass, vertical pass fused with
 // crop / rescale / normalise.  Tables and the intermediate live in the caller's scratch; the tap count per output
 // index is not bounded by anything but the image size.
+//
+// The same resampler also serves the AutoencoderKL encoder's preprocessing (ds_vae_image_preprocess: Pillow LANCZOS
+// to any size, then 2 * u8 / 255 - 1), with host-built tap tables; see the section below plan_images.
+#include <cuda_bf16.h>
+
 #include <cmath>
 #include <vector>
 
@@ -212,6 +217,171 @@ static bool plan_images(const int* sizes, int n, int mode, ImgDesc* descs, long 
   return true;
 }
 
+// ------------------------------------------------------------------------------------------------
+// VAE image preprocessing (diffusers VaeImageProcessor.preprocess, default config: Pillow LANCZOS resize to the
+// panel size, float32(u8) / 255, 2x - 1).  Same fixed-point two-pass resampler as above, any output size.  The
+// Lanczos taps need sin(), and one ulp of a device sin() can flip a 22-bit coefficient, so the coefficient tables are
+// built on the HOST with the host libm's sin — the function Pillow's precompute_coeffs calls, in the same double
+// arithmetic — and copied into the scratch; the kernels only do the integer passes.
+constexpr double kLanczosSupport = 3.0;
+
+static double sinc_filter(double x) {
+  if (x == 0.0) return 1.0;
+  x = x * M_PI;
+  return std::sin(x) / x;
+}
+
+static double lanczos_filter(double x) {
+  if (-3.0 <= x && x < 3.0) return sinc_filter(x) * sinc_filter(x / 3.0);
+  return 0.0;
+}
+
+static int lanczos_taps(int in, int out) {
+  double fs = static_cast<double>(in) / static_cast<double>(out);
+  if (fs < 1.0) fs = 1.0;
+  return static_cast<int>(std::ceil(kLanczosSupport * fs)) * 2 + 1;
+}
+
+// {xmin, xmax, k[0 .. ksize)} per output index, as Pillow's precompute_coeffs + normalize_coeffs_8bpc.
+static void lanczos_coeffs(int in, int out, int ksize, int* table) {
+  const double scale = static_cast<double>(in) / static_cast<double>(out);
+  const double fs = scale < 1.0 ? 1.0 : scale;
+  const double support = kLanczosSupport * fs;
+  const double ss = 1.0 / fs;
+  std::vector<double> k(ksize);
+  for (int xx = 0; xx < out; ++xx) {
+    const double center = (xx + 0.5) * scale;
+    int xmin = static_cast<int>(center - support + 0.5);
+    if (xmin < 0) xmin = 0;
+    int xmax = static_cast<int>(center + support + 0.5);
+    if (xmax > in) xmax = in;
+    xmax -= xmin;
+    double ww = 0.0;
+    for (int x = 0; x < xmax; ++x) {
+      k[x] = lanczos_filter((x + xmin - center + 0.5) * ss);
+      ww += k[x];
+    }
+    int* row = table + static_cast<size_t>(xx) * (2 + ksize);
+    row[0] = xmin;
+    row[1] = xmax;
+    for (int x = 0; x < ksize; ++x) {
+      double w = x < xmax ? k[x] : 0.0;
+      if (x < xmax && ww != 0.0) w /= ww;
+      row[2 + x] = w < 0 ? static_cast<int>(-0.5 + w * (1 << kPrecisionBits))
+                         : static_cast<int>(0.5 + w * (1 << kPrecisionBits));
+    }
+  }
+}
+
+struct VaePlan {
+  int kh, kv;                          // taps per output index of each pass; 0: pass skipped
+  long long coef_h, coef_v, inter, total;
+};
+
+static VaePlan plan_vae(int H, int W, int oh, int ow) {
+  VaePlan p{};
+  long long cur = 0;
+  auto take = [&cur](long long bytes) {
+    const long long at = cur;
+    cur += (bytes + 15) / 16 * 16;
+    return at;
+  };
+  p.kh = ow != W ? lanczos_taps(W, ow) : 0;
+  p.kv = oh != H ? lanczos_taps(H, oh) : 0;
+  p.coef_h = p.kh ? take(4LL * ow * (2 + p.kh)) : 0;
+  p.coef_v = p.kv ? take(4LL * oh * (2 + p.kv)) : 0;
+  p.inter = p.kh ? take(3LL * ow * H) : 0;
+  p.total = cur;
+  return p;
+}
+
+// every source row, the ow output columns, 3 channels -> uint8 intermediate [H][ow][3]
+__global__ void vae_image_hpass_kernel(const unsigned char* __restrict__ img, const int* __restrict__ coef,
+                                       unsigned char* __restrict__ inter, int W, int ow, int kh, long long total) {
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long y = i / ow;
+    const int x = static_cast<int>(i - y * ow);
+    const int* k = coef + static_cast<size_t>(x) * (2 + kh);
+    const int xmin = k[0], xmax = k[1];
+    const unsigned char* p = img + (y * W + xmin) * 3;
+    int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
+    for (int t = 0; t < xmax; ++t) {
+      const int w = k[2 + t];
+      a0 += p[3 * t] * w;
+      a1 += p[3 * t + 1] * w;
+      a2 += p[3 * t + 2] * w;
+    }
+    unsigned char* o = inter + i * 3;
+    o[0] = static_cast<unsigned char>(clip8(a0));
+    o[1] = static_cast<unsigned char>(clip8(a1));
+    o[2] = static_cast<unsigned char>(clip8(a2));
+  }
+}
+
+// one output pixel per thread: vertical pass (or a copy), float32(u8) / 255, 2x - 1 -> fp32 NCHW and / or bf16 NHWC
+// with a zero 4th channel (the input of the encoder's conv_in)
+__global__ void vae_image_vpass_kernel(const unsigned char* __restrict__ base, long long pitch,
+                                       const int* __restrict__ coef, int kv, int oh, int ow, float* __restrict__ out,
+                                       uint2* __restrict__ out4) {
+  const long long hw = static_cast<long long>(oh) * ow;
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= hw) return;
+  const int y = static_cast<int>(i / ow), x = static_cast<int>(i - static_cast<long long>(y) * ow);
+  const unsigned char* col = base + static_cast<long long>(x) * 3;
+  int v[3];
+  if (kv) {
+    const int* k = coef + static_cast<size_t>(y) * (2 + kv);
+    const int ymin = k[0], ymax = k[1];
+    int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
+    for (int t = 0; t < ymax; ++t) {
+      const unsigned char* p = col + (ymin + t) * pitch;
+      const int w = k[2 + t];
+      a0 += p[0] * w;
+      a1 += p[1] * w;
+      a2 += p[2] * w;
+    }
+    v[0] = clip8(a0);
+    v[1] = clip8(a1);
+    v[2] = clip8(a2);
+  } else {
+    const unsigned char* p = col + y * pitch;
+    v[0] = p[0];
+    v[1] = p[1];
+    v[2] = p[2];
+  }
+  float o[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    o[c] = __fsub_rn(__fmul_rn(2.0f, __fdiv_rn(static_cast<float>(v[c]), 255.0f)), 1.0f);
+    if (out) out[c * hw + i] = o[c];
+  }
+  if (out4) {
+    __nv_bfloat162 lo = __floats2bfloat162_rn(o[0], o[1]), hi = __floats2bfloat162_rn(o[2], 0.0f);
+    out4[i] = make_uint2(*reinterpret_cast<uint32_t*>(&lo), *reinterpret_cast<uint32_t*>(&hi));
+  }
+}
+
+// float NCHW [B][3][HW] -> (normalize ? 2x - 1 : x) as fp32 NCHW (may alias x) and / or bf16 NHWC with a zero 4th channel
+__global__ void vae_image_pack_kernel(const float* x, float* out, uint2* __restrict__ out4, int HW, int normalize,
+                                      long long total) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;  // pixel of (batch, hw)
+  if (i >= total) return;
+  const long long b = i / HW;
+  const long long p = i - b * HW;
+  float o[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const long long at = (b * 3 + c) * HW + p;
+    o[c] = normalize ? __fsub_rn(__fmul_rn(2.0f, x[at]), 1.0f) : x[at];
+    if (out) out[at] = o[c];
+  }
+  if (out4) {
+    __nv_bfloat162 lo = __floats2bfloat162_rn(o[0], o[1]), hi = __floats2bfloat162_rn(o[2], 0.0f);
+    out4[i] = make_uint2(*reinterpret_cast<uint32_t*>(&lo), *reinterpret_cast<uint32_t*>(&hi));
+  }
+}
+
 }  // namespace ds
 
 extern "C" int64_t ds_image_preprocess_scratch_bytes(const int* sizes, int n, int mode) {
@@ -268,5 +438,74 @@ extern "C" int ds_image_preprocess(const uint8_t* src, const int64_t* offsets, c
         b, src, scr, out + static_cast<long long>(first) * 3 * kOut * kOut);
     DS_LAUNCH_OK("image_vpass_normalise_kernel");
   }
+  return DS_OK;
+}
+
+extern "C" int64_t ds_vae_image_preprocess_scratch_bytes(int H, int W, int out_h, int out_w) {
+  if (H < 1 || W < 1 || H > ds::kMaxSide || W > ds::kMaxSide || out_h < 1 || out_w < 1 || out_h > ds::kMaxSide ||
+      out_w > ds::kMaxSide)
+    return -1;
+  return ds::plan_vae(H, W, out_h, out_w).total;
+}
+
+extern "C" int ds_vae_image_preprocess(const uint8_t* src, int H, int W, int out_h, int out_w, float* out,
+                                       void* out_nhwc4, void* scratch, int64_t scratch_bytes, void* stream) {
+  using namespace ds;
+  DS_REQUIRE(src && (out || out_nhwc4), "ds_vae_image_preprocess: bad arguments");
+  DS_REQUIRE(H >= 1 && W >= 1 && H <= kMaxSide && W <= kMaxSide && out_h >= 1 && out_w >= 1 && out_h <= kMaxSide &&
+                 out_w <= kMaxSide,
+             "ds_vae_image_preprocess: %d x %d -> %d x %d; sides must be in [1, %d]", H, W, out_h, out_w, kMaxSide);
+  DS_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3) == 0 && (reinterpret_cast<uintptr_t>(out_nhwc4) & 7) == 0,
+             "ds_vae_image_preprocess: out must be 4-byte and out_nhwc4 8-byte aligned");
+  const VaePlan p = plan_vae(H, W, out_h, out_w);
+  DS_REQUIRE(p.total == 0 || (scratch && scratch_bytes >= p.total && (reinterpret_cast<uintptr_t>(scratch) & 15) == 0),
+             "ds_vae_image_preprocess: needs %lld bytes of 16-byte aligned scratch "
+             "(ds_vae_image_preprocess_scratch_bytes), got %lld", p.total, static_cast<long long>(scratch_bytes));
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  unsigned char* scr = static_cast<unsigned char*>(scratch);
+  // host-built tap tables (pageable source: the copy is staged before the call returns)
+  std::vector<int> table;
+  if (p.kh) {
+    table.assign(static_cast<size_t>(out_w) * (2 + p.kh), 0);
+    lanczos_coeffs(W, out_w, p.kh, table.data());
+    DS_CUDA_OK(cudaMemcpyAsync(scr + p.coef_h, table.data(), table.size() * 4, cudaMemcpyHostToDevice, st));
+  }
+  if (p.kv) {
+    table.assign(static_cast<size_t>(out_h) * (2 + p.kv), 0);
+    lanczos_coeffs(H, out_h, p.kv, table.data());
+    DS_CUDA_OK(cudaMemcpyAsync(scr + p.coef_v, table.data(), table.size() * 4, cudaMemcpyHostToDevice, st));
+  }
+  const unsigned char* base = src;
+  long long pitch = 3LL * W;
+  if (p.kh) {
+    const long long total = static_cast<long long>(H) * out_w;
+    const long long blocks = (total + 255) / 256;
+    vae_image_hpass_kernel<<<static_cast<unsigned>(blocks < 4096 ? blocks : 4096), 256, 0, st>>>(
+        src, reinterpret_cast<const int*>(scr + p.coef_h), scr + p.inter, W, out_w, p.kh, total);
+    DS_LAUNCH_OK("vae_image_hpass_kernel");
+    base = scr + p.inter;
+    pitch = 3LL * out_w;
+  }
+  const long long hw = static_cast<long long>(out_h) * out_w;
+  vae_image_vpass_kernel<<<static_cast<unsigned>((hw + 255) / 256), 256, 0, st>>>(
+      base, pitch, reinterpret_cast<const int*>(scr + p.coef_v), p.kv, out_h, out_w, out,
+      static_cast<uint2*>(out_nhwc4));
+  DS_LAUNCH_OK("vae_image_vpass_kernel");
+  return DS_OK;
+}
+
+extern "C" int ds_vae_image_pack(const float* x, float* out, void* out_nhwc4, int B, int HW, int normalize,
+                                 void* stream) {
+  using namespace ds;
+  DS_REQUIRE(x && (out || out_nhwc4) && B > 0 && HW > 0, "ds_vae_image_pack: bad arguments");
+  DS_REQUIRE((reinterpret_cast<uintptr_t>(out_nhwc4) & 7) == 0, "ds_vae_image_pack: out_nhwc4 must be 8-byte aligned");
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  const long long total = static_cast<long long>(B) * HW;
+  vae_image_pack_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      x, out, static_cast<uint2*>(out_nhwc4), HW, normalize, total);
+  DS_LAUNCH_OK("vae_image_pack_kernel");
   return DS_OK;
 }

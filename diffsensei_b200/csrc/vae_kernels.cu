@@ -7,7 +7,11 @@
 //                         attention of the decoder has ONE head of width 512 over all H*W tokens (no flash kernel for
 //                         that head size: QK^T and PV run as plain wgmma GEMMs with this kernel between them)
 //   ds_image_postprocess: (x / 2 + 0.5).clamp(0, 1), NHWC bf16 -> NCHW fp32 (VaeImageProcessor.postprocess/denormalize)
-// All three are HBM-bound one-pass kernels.
+// and one the encoder needs after its conv_out:
+//   ds_vae_posterior    : quant_conv (1x1, 8 -> 8) -> DiagonalGaussianDistribution sample / mode -> * scaling_factor
+//                         -> repeat to num_samples -> scheduler.add_noise (diffusers AutoencoderKL.encode and
+//                         StableDiffusionXLImg2ImgPipeline.prepare_latents)
+// All four are HBM-bound one-pass kernels.
 #include "ds_common.cuh"
 #include "ds_host.h"
 
@@ -88,6 +92,54 @@ __global__ void image_postprocess_kernel(const __nv_bfloat16* __restrict__ x, fl
   out[i] = fminf(fmaxf(fmaf(v, 0.5f, 0.5f), 0.f), 1.f);
 }
 
+// The AutoencoderKL posterior from the encoder's conv_out (fp32 NHWC [B][HW][8]), one pixel per thread:
+//   moments = quant_conv(x) (1x1, 8 -> 8, fp32), mean = moments[0:4], logvar = clamp(moments[4:8], -30, 20),
+//   z = mean + exp(0.5 * logvar) * eps (eps NULL: z = mean, DiagonalGaussianDistribution.mode()), z *= scale,
+//   then for each of the `repeat` copies r: out[b * repeat + r] = c0 * z + c1 * noise[b * repeat + r] (noise NULL:
+//   out = z).  Each fp32 operation is rounded on its own, as torch's eager ops are.  All planes fp32 NCHW.
+__global__ void vae_posterior_kernel(const float* __restrict__ x, const float* __restrict__ w,
+                                     const float* __restrict__ bias, const float* __restrict__ eps, float scale,
+                                     const float* __restrict__ noise, const float* __restrict__ coef, int repeat,
+                                     float* __restrict__ mean_out, float* __restrict__ logvar_out,
+                                     float* __restrict__ out, int HW, long long total) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;  // pixel of (batch, hw)
+  if (i >= total) return;
+  const long long b = i / HW;
+  const long long p = i - b * HW;
+  const float4* src = reinterpret_cast<const float4*>(x + i * 8);
+  const float4 u0 = src[0], u1 = src[1];
+  const float in[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
+  float m[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    float a = __ldg(bias + k);
+#pragma unroll
+    for (int c = 0; c < 8; ++c) a = fmaf(__ldg(w + k * 8 + c), in[c], a);
+    m[k] = a;
+  }
+  float c0 = 1.0f, c1 = 0.0f;
+  if (noise) {
+    c0 = __ldg(coef);
+    c1 = __ldg(coef + 1);
+  }
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    const long long at = (b * 4 + c) * HW + p;
+    const float mu = m[c];
+    const float lv = fminf(fmaxf(m[4 + c], -30.0f), 20.0f);
+    if (mean_out) mean_out[at] = mu;
+    if (logvar_out) logvar_out[at] = lv;
+    float z = mu;
+    if (eps) z = __fadd_rn(mu, __fmul_rn(expf(__fmul_rn(0.5f, lv)), eps[at]));
+    z = __fmul_rn(scale, z);
+    if (!out) continue;
+    for (int r = 0; r < repeat; ++r) {
+      const long long o = ((b * repeat + r) * 4 + c) * HW + p;
+      out[o] = noise ? __fadd_rn(__fmul_rn(c0, z), __fmul_rn(c1, noise[o])) : z;
+    }
+  }
+}
+
 }  // namespace ds
 
 extern "C" int ds_latent_pointwise(const float* latents, const float* w, const float* bias, void* out,
@@ -137,5 +189,22 @@ extern "C" int ds_image_postprocess(const void* x, float* out, int B, int HW, in
   image_postprocess_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(x), out, HW, C, total);
   DS_LAUNCH_OK("image_postprocess_kernel");
+  return DS_OK;
+}
+
+extern "C" int ds_vae_posterior(const float* x, const float* w, const float* bias, const float* eps, float scale,
+                                const float* noise, const float* coef, int repeat, float* mean, float* logvar,
+                                float* out, int B, int HW, void* stream) {
+  using namespace ds;
+  DS_REQUIRE(x && w && bias && B > 0 && HW > 0 && repeat >= 1 && (mean || logvar || out),
+             "ds_vae_posterior: bad arguments");
+  DS_REQUIRE(!noise || (coef && out), "ds_vae_posterior: noise needs coef and out");
+  DS_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "ds_vae_posterior: x must be 16-byte aligned");
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  const long long total = static_cast<long long>(B) * HW;
+  vae_posterior_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      x, w, bias, eps, scale, noise, coef, repeat, mean, logvar, out, HW, total);
+  DS_LAUNCH_OK("vae_posterior_kernel");
   return DS_OK;
 }

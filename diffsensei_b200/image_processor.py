@@ -108,3 +108,68 @@ class ViTImageProcessor(_DeviceImageProcessor):
     mode = "vit"
     defaults = dict(do_resize=True, size={"height": 224, "width": 224}, resample=_BILINEAR, do_rescale=True,
                     rescale_factor=1 / 255, do_normalize=True, image_mean=(0.5, 0.5, 0.5), image_std=(0.5, 0.5, 0.5))
+
+
+class VaeImageProcessor:
+    """diffusers ``VaeImageProcessor(vae_scale_factor=8)`` with its default configuration (``do_resize=True``,
+    ``resample="lanczos"``, ``do_normalize=True``), the preprocessing of SDXL img2img, on the GPU.
+
+    ``preprocess(image, height=None, width=None)`` returns fp32 NCHW [1, 3, h, w] in [-1, 1]:
+      * target size: ``height`` / ``width`` if given, else the image's own, each rounded down to a multiple of 8
+        (``get_default_height_width``);
+      * a PIL image or uint8 RGB HWC array / tensor is converted to RGB (as the character images are), resized with
+        Pillow's LANCZOS filter when its size differs (``ds_vae_image_preprocess``, bit-exact with Pillow), then
+        ``float32(u8) / 255`` and ``2x - 1``;
+      * a float NCHW tensor of batch 1 must already be at a multiple-of-8 size (float inputs are not resized); it is
+        normalised with ``2x - 1`` only if its minimum is >= 0, diffusers' rule.
+    """
+    defaults = dict(do_resize=True, vae_scale_factor=8, resample="lanczos", do_normalize=True)
+
+    def __init__(self, device: Optional[torch.device] = None, **kwargs):
+        _DeviceImageProcessor._check(self, kwargs)
+        self.vae_scale_factor = 8
+        self.device = device
+
+    @staticmethod
+    def _is_float_tensor(image) -> bool:
+        return isinstance(image, torch.Tensor) and image.is_floating_point()
+
+    def get_default_height_width(self, image, height: Optional[int] = None, width: Optional[int] = None):
+        """(height, width): the given ones, else the image's, each rounded down to a multiple of 8."""
+        if self._is_float_tensor(image):
+            ih, iw = image.shape[-2:]
+        elif hasattr(image, "size") and not isinstance(image, (torch.Tensor, np.ndarray)):
+            iw, ih = image.size                                        # PIL
+        else:
+            ih, iw = image.shape[:2]
+        height = int(height) if height is not None else int(ih)
+        width = int(width) if width is not None else int(iw)
+        f = self.vae_scale_factor
+        height, width = height - height % f, width - width % f
+        if height < f or width < f:
+            raise ValueError(f"image / panel size {height} x {width} (after rounding down to a multiple of {f}) is "
+                             "too small")
+        return height, width
+
+    def _prepare(self, image, height, width, want_nchw: bool, want_nhwc4: bool):
+        dev = self.device or torch.device("cuda", torch.cuda.current_device())
+        h, w = self.get_default_height_width(image, height, width)
+        if self._is_float_tensor(image):
+            x = image if image.dim() == 4 else image.unsqueeze(0)
+            if x.dim() != 4 or x.shape[0] != 1 or x.shape[1] != 3:
+                raise ValueError(f"a float image must be an NCHW tensor of batch 1 with 3 channels, got "
+                                 f"{tuple(image.shape)}")
+            if tuple(x.shape[-2:]) != (h, w):
+                raise ValueError(f"a float image tensor is not resized: it must already be {h} x {w} (a multiple of "
+                                 f"8), got {tuple(x.shape[-2:])}")
+            x = x.to(device=dev, dtype=torch.float32).contiguous()
+            return ops.vae_image_pack(x, normalize=bool(x.min() >= 0), want_nchw=want_nchw, want_nhwc4=want_nhwc4)
+        u8 = _DeviceImageProcessor.to_device(image, dev)
+        return ops.vae_image_preprocess(u8, h, w, want_nchw=want_nchw, want_nhwc4=want_nhwc4)
+
+    def preprocess(self, image, height: Optional[int] = None, width: Optional[int] = None) -> torch.Tensor:
+        return self._prepare(image, height, width, True, False)[0]
+
+    def preprocess_nhwc4(self, image, height: Optional[int] = None, width: Optional[int] = None) -> torch.Tensor:
+        """The same image as bf16 NHWC [1, h, w, 4] with a zero 4th channel: the encoder's conv_in input."""
+        return self._prepare(image, height, width, False, True)[1]

@@ -371,10 +371,13 @@ def _gemm_args(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = 
 def conv3x3(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, *, stride: int = 1,
             rowbias: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None,
             out: Optional[torch.Tensor] = None, out_fp32: bool = False,
-            chan_stats: Optional[torch.Tensor] = None, upsample2: bool = False) -> torch.Tensor:
+            chan_stats: Optional[torch.Tensor] = None, upsample2: bool = False,
+            pad_bottom_right: bool = False) -> torch.Tensor:
     """3x3 / pad 1 conv on NHWC bf16 ``x``; ``w`` is packed [Cout, 3, 3, Cin] bf16 (weights.pack_conv3x3).
     ``upsample2``: conv3x3(nearest_x2(x)) without the upsampled tensor — ``w`` is then the phase-decomposed
-    [4, Cout, 2, 2, Cin] packing of ``weights.pack_conv3x3_up2`` and the output is [B, 2H, 2W, Cout]."""
+    [4, Cout, 2, 2, Cin] packing of ``weights.pack_conv3x3_up2`` and the output is [B, 2H, 2W, Cout].
+    ``pad_bottom_right`` (stride 2 only): the VAE encoder's Downsample2D — pad (0, 1, 0, 1), then no padding — with
+    output [B, H // 2, W // 2, Cout]."""
     _req(x, bf16, "conv3x3.x", 4)
     B, H, W, Cin = x.shape
     if upsample2:
@@ -389,6 +392,10 @@ def conv3x3(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = Non
         if tuple(w.shape[1:]) != (3, 3, Cin):
             raise DsEngineError(f"conv3x3: w must be [Cout,3,3,{Cin}], got {tuple(w.shape)}")
         Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
+        if pad_bottom_right:
+            if stride != 2 or H < 2 or W < 2:
+                raise DsEngineError("conv3x3(pad_bottom_right): stride 2 and H, W >= 2 only")
+            Ho, Wo = H // 2, W // 2
     if bias is not None:
         _req(bias, f32, "conv3x3.bias", 1)
     if rowbias is not None:
@@ -415,7 +422,7 @@ def conv3x3(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = Non
                        rowbias_ld=0 if rowbias is None else rowbias.stride(0),
                        out_fp32=int(out_fp32), out_scale=0.0, splitk_ws=_ptr(ws),
                        splitk_ws_bytes=0 if ws is None else ws.numel() * 4, chan_stats=_ptr(chan_stats),
-                       upsample2=int(bool(upsample2)))
+                       upsample2=int(bool(upsample2)), pad_bottom_right=int(bool(pad_bottom_right)))
     check(lib.ds_conv3x3_nhwc(C.byref(args), _stream()), "ds_conv3x3_nhwc")
     return out
 
@@ -932,6 +939,50 @@ def image_postprocess(x: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def vae_posterior(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, *, eps: Optional[torch.Tensor] = None,
+                  scale: float = 1.0, noise: Optional[torch.Tensor] = None, coef: Optional[torch.Tensor] = None,
+                  repeat: int = 1, want_mean: bool = False, want_logvar: bool = False, want_out: bool = True):
+    """The encoder's posterior from its conv_out ``x`` fp32 NHWC [B, h, w, 8]: quant_conv (``w`` fp32 [8, 8], ``bias``
+    [8]) -> mean / clamped logvar -> ``scale * (mean + exp(logvar / 2) * eps)`` (``eps`` None: the mean) -> repeated
+    ``repeat`` times -> ``coef[0] * z + coef[1] * noise`` (``noise`` fp32 NCHW [B * repeat, 4, h, w], ``coef`` a
+    2-element fp32 CUDA tensor).  Returns (mean, logvar, out), fp32 NCHW, None where not asked for."""
+    _req(x, f32, "vae_posterior.x", 4)
+    B, h, w_, c8 = x.shape
+    if c8 != 8:
+        raise DsEngineError("vae_posterior: x must have 8 channels (mean | logvar before quant_conv)")
+    _req(w, f32, "vae_posterior.w", 2)
+    _req(bias, f32, "vae_posterior.bias", 1)
+    if tuple(w.shape) != (8, 8) or bias.numel() != 8:
+        raise DsEngineError("vae_posterior: w must be [8, 8] and bias [8]")
+    repeat = int(repeat)
+    if repeat < 1:
+        raise DsEngineError("vae_posterior: repeat must be >= 1")
+    if eps is not None:
+        _req(eps, f32, "vae_posterior.eps", 4)
+        if tuple(eps.shape) != (B, 4, h, w_):
+            raise DsEngineError(f"vae_posterior: eps must be {(B, 4, h, w_)}")
+    if noise is not None:
+        _req(noise, f32, "vae_posterior.noise", 4)
+        if tuple(noise.shape) != (B * repeat, 4, h, w_):
+            raise DsEngineError(f"vae_posterior: noise must be {(B * repeat, 4, h, w_)}")
+        if coef is None:
+            raise DsEngineError("vae_posterior: noise needs coef")
+        _req(coef, f32, "vae_posterior.coef", 1)
+        if coef.numel() != 2:
+            raise DsEngineError("vae_posterior: coef must hold 2 floats")
+        want_out = True
+    new = lambda n: torch.empty(n, 4, h, w_, dtype=f32, device=x.device)
+    mean = new(B) if want_mean else None
+    logvar = new(B) if want_logvar else None
+    out = new(B * repeat) if want_out else None
+    if mean is None and logvar is None and out is None:
+        raise DsEngineError("vae_posterior: nothing to compute")
+    check(lib.ds_vae_posterior(x.data_ptr(), w.data_ptr(), bias.data_ptr(), _ptr(eps), float(scale), _ptr(noise),
+                               _ptr(coef) if noise is not None else None, repeat, _ptr(mean), _ptr(logvar), _ptr(out),
+                               B, h * w_, _stream()), "ds_vae_posterior")
+    return mean, logvar, out
+
+
 # ---------------------------------------------------------------------------------------------- image processors
 IMG_MODES = {"clip": 0, "vit": 1}     # DS_IMG_CLIP / DS_IMG_VIT
 IMG_SIZE = 224
@@ -984,6 +1035,45 @@ def image_preprocess(src: torch.Tensor, sizes, mode: str, offsets=None, out: Opt
     check(lib.ds_image_preprocess(src.data_ptr(), (C.c_int64 * n)(*offsets), _img_sizes(sizes), n, IMG_MODES[mode],
                                   out.data_ptr(), scratch.data_ptr(), scratch.numel(), _stream()), "ds_image_preprocess")
     return out
+
+
+def vae_image_preprocess(img: torch.Tensor, out_h: int, out_w: int, want_nchw: bool = True, want_nhwc4: bool = True):
+    """diffusers ``VaeImageProcessor.preprocess`` of one uint8 RGB HWC image ``img`` [H, W, 3] (CUDA): Pillow LANCZOS
+    resize to (out_h, out_w) (none when the size is unchanged), ``float32(u8) / 255``, ``2x - 1``.  Returns
+    (fp32 NCHW [1, 3, out_h, out_w], bf16 NHWC [1, out_h, out_w, 4] with a zero 4th channel), None where not asked."""
+    _req(img, torch.uint8, "vae_image_preprocess.img", 3)
+    H, W, c = img.shape
+    if c != 3:
+        raise DsEngineError("vae_image_preprocess: img must be uint8 RGB [H, W, 3]")
+    out_h, out_w = int(out_h), int(out_w)
+    need = int(lib.ds_vae_image_preprocess_scratch_bytes(H, W, out_h, out_w))
+    if need < 0:
+        raise DsEngineError(f"vae_image_preprocess: unsupported sizes {H} x {W} -> {out_h} x {out_w} "
+                            "(sides must be in [1, 65535])")
+    if not (want_nchw or want_nhwc4):
+        raise DsEngineError("vae_image_preprocess: nothing to compute")
+    scratch = torch.empty(max(need, 16), dtype=torch.uint8, device=img.device)
+    nchw = torch.empty(1, 3, out_h, out_w, dtype=f32, device=img.device) if want_nchw else None
+    nhwc4 = torch.empty(1, out_h, out_w, 4, dtype=bf16, device=img.device) if want_nhwc4 else None
+    check(lib.ds_vae_image_preprocess(img.data_ptr(), H, W, out_h, out_w, _ptr(nchw), _ptr(nhwc4), scratch.data_ptr(),
+                                      scratch.numel(), _stream()), "ds_vae_image_preprocess")
+    return nchw, nhwc4
+
+
+def vae_image_pack(x: torch.Tensor, normalize: bool, want_nchw: bool = True, want_nhwc4: bool = True):
+    """A float image batch already at its size, fp32 NCHW [B, 3, H, W] (CUDA) -> (``2x - 1`` if ``normalize`` else x)
+    as (fp32 NCHW [B, 3, H, W], bf16 NHWC [B, H, W, 4] with a zero 4th channel), None where not asked."""
+    _req(x, f32, "vae_image_pack.x", 4)
+    B, c, H, W = x.shape
+    if c != 3:
+        raise DsEngineError("vae_image_pack: x must have 3 channels")
+    if not (want_nchw or want_nhwc4):
+        raise DsEngineError("vae_image_pack: nothing to compute")
+    nchw = torch.empty_like(x) if want_nchw else None
+    nhwc4 = torch.empty(B, H, W, 4, dtype=bf16, device=x.device) if want_nhwc4 else None
+    check(lib.ds_vae_image_pack(x.data_ptr(), _ptr(nchw), _ptr(nhwc4), B, H * W, int(bool(normalize)), _stream()),
+          "ds_vae_image_pack")
+    return nchw, nhwc4
 
 
 launch_count = _lib.launch_count

@@ -13,6 +13,8 @@ engines and run through the two image processors on the GPU (image_processor.py)
 (token ids, pixel values) or outputs (``prompt_embeds`` ..., ``clip_image_embeds`` / ``magi_image_embeds``) can be
 passed instead; a raw prompt or image without what it needs raises, it does not fall back to anything.
 ``generate_page`` runs the panels of a page together (one front-end pass, one denoise per group of same-size panels).
+``image=`` / ``strength=`` start a panel from an image as diffusers' ``StableDiffusionXLImg2ImgPipeline`` does (needs
+``vae_encoder=``): the image is encoded, noised to the schedule's step ``t_start`` and denoised from there.
 
 Loop structure on the GPU (one process per GPU, one stream):
   once per panel : K|V projections of text and IP tokens for all cross-attention layers, time-embedding
@@ -32,35 +34,36 @@ from typing import List, Optional, Union
 import torch
 
 from . import ops
-from .image_processor import CLIPImageProcessor, ViTImageProcessor
-from .scheduler import DDIMScheduler, EulerDiscreteScheduler
+from .image_processor import CLIPImageProcessor, VaeImageProcessor, ViTImageProcessor
+from .scheduler import DDIMScheduler, EulerDiscreteScheduler, get_timesteps
 from .unet import UNetMangaEngine
 
 bf16, f32 = torch.bfloat16, torch.float32
 
 # generate_page: what a captured stepper bakes in is the same for the whole page; everything else is per panel
 PAGE_KEYS = frozenset({"num_inference_steps", "guidance_scale", "ip_scale", "output_type", "use_graph",
-                       "max_batch_panels"})
+                       "max_batch_panels", "strength"})
 PANEL_KEYS = frozenset({
     "prompt", "prompt_2", "negative_prompt", "negative_prompt_2", "height", "width", "num_samples", "generator",
     "latents", "original_size", "crops_coords_top_left", "target_size", "min_size_step", "ip_images",
     "ip_image_embeds", "clip_image_embeds", "magi_image_embeds", "clip_pixel_values", "magi_pixel_values", "ip_bbox",
     "dialog_bbox", "prompt_embeds", "negative_prompt_embeds", "pooled_prompt_embeds", "negative_pooled_prompt_embeds",
-    "prompt_input_ids", "prompt_input_ids_2", "negative_prompt_input_ids", "negative_prompt_input_ids_2"})
+    "prompt_input_ids", "prompt_input_ids_2", "negative_prompt_input_ids", "negative_prompt_input_ids_2", "image"})
 PAGE_MAX_ROWS = 8       # samples per page denoise: a UNet batch of 16 rows, as __call__(num_samples=8)
 
 
 def plan_page(shapes, max_batch_panels: int = PAGE_MAX_ROWS) -> List[List[int]]:
-    """The denoise chunks of a page.  ``shapes`` holds one (num_samples, h, w) per panel, h x w its latent size.
-    Panels of one latent size form a group, groups in order of first appearance; a group splits into consecutive
-    chunks of at most ``max_batch_panels`` samples, and a panel's samples are never split (a panel with more samples
-    than the cap is a chunk of its own).  Returns the panel indices of every chunk."""
+    """The denoise chunks of a page.  ``shapes`` holds one (num_samples, h, w) per panel, h x w its latent size, with
+    optional further entries that must also match for two panels to share a denoise (an img2img panel adds one: it
+    runs a different slice of the schedule).  Panels of one key form a group, groups in order of first appearance; a
+    group splits into consecutive chunks of at most ``max_batch_panels`` samples, and a panel's samples are never split
+    (a panel with more samples than the cap is a chunk of its own).  Returns the panel indices of every chunk."""
     cap = int(max_batch_panels)
     if cap < 1:
         raise ValueError(f"max_batch_panels must be >= 1, got {max_batch_panels}")
     groups = {}
-    for i, (_, h, w) in enumerate(shapes):
-        groups.setdefault((int(h), int(w)), []).append(i)
+    for i, shp in enumerate(shapes):
+        groups.setdefault((int(shp[1]), int(shp[2])) + tuple(shp[3:]), []).append(i)
     chunks = []
     for idx in groups.values():
         cur, rows = [], 0
@@ -109,9 +112,11 @@ class DiffSenseiPipeline:
     def __init__(self, unet: UNetMangaEngine,
                  scheduler: Optional[Union[DDIMScheduler, EulerDiscreteScheduler]] = None, vae_scale_factor: int = 8,
                  default_sample_size: int = 128, vae=None, text_encoder=None, text_encoder_2=None, image_encoder=None,
-                 tokenizer=None, tokenizer_2=None):
+                 tokenizer=None, tokenizer_2=None, vae_encoder=None):
         self.unet = unet
         self.vae = vae                      # VaeDecoderEngine (or None: latents out only)
+        self.vae_encoder = vae_encoder      # VaeEncoderEngine (or None: no image= / img2img)
+        self.vae_image_processor = VaeImageProcessor()
         self.text_encoder = text_encoder    # ClipTextEncoderEngine (CLIP-L) / (OpenCLIP bigG, with projection)
         self.text_encoder_2 = text_encoder_2
         self.image_encoder = image_encoder  # ClipVisionEncoderEngine (ViT-H/14)
@@ -279,22 +284,23 @@ class DiffSenseiPipeline:
     def make_stepper(self, latents: torch.Tensor, prompt_embeds: torch.Tensor, add_text_embeds: torch.Tensor,
                      add_time_ids: torch.Tensor, bbox: torch.Tensor, aspect_ratio: float,
                      dialog_bbox: Optional[torch.Tensor], num_inference_steps: int, guidance_scale: float,
-                     use_graph: bool = True, chains: Optional[int] = None) -> "DenoiseStepper":
+                     use_graph: bool = True, chains: Optional[int] = None, start_index: int = 0) -> "DenoiseStepper":
         return DenoiseStepper(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
-                              dialog_bbox, num_inference_steps, guidance_scale, use_graph, chains)
+                              dialog_bbox, num_inference_steps, guidance_scale, use_graph, chains, start_index)
 
     def stepper_for(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio, dialog_bbox,
-                    num_inference_steps, guidance_scale, chains=None) -> "DenoiseStepper":
+                    num_inference_steps, guidance_scale, chains=None, start_index: int = 0) -> "DenoiseStepper":
         """A graph-captured stepper loaded with this panel: a cached one of the same key is refilled in place
-        (no re-capture), otherwise a new one is built and cached."""
+        (no re-capture), otherwise a new one is built and cached.  The start index is part of the key: the stepper
+        bakes in its slice of the schedule (``set_timesteps`` would reset any scheduler state)."""
         key = (tuple(latents.shape), tuple(prompt_embeds.shape), None if dialog_bbox is None else
                (tuple(dialog_bbox.shape), dialog_bbox.dtype == bf16), float(aspect_ratio), int(num_inference_steps),
                float(guidance_scale), self.unet.scales_key(), chains, self.unet._ip_weights_version(),
-               type(self.scheduler).__name__, tuple(sorted(self.scheduler.config.items())))
+               type(self.scheduler).__name__, tuple(sorted(self.scheduler.config.items())), int(start_index))
         st = self._steppers.get(key)
         if st is None:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
-                                   dialog_bbox, num_inference_steps, guidance_scale, True, chains)
+                                   dialog_bbox, num_inference_steps, guidance_scale, True, chains, start_index)
             while len(self._steppers) >= self.max_cached_steppers:
                 self._steppers.pop(next(iter(self._steppers)))
             self._steppers[key] = st
@@ -306,15 +312,17 @@ class DiffSenseiPipeline:
     def denoise(self, latents: torch.Tensor, prompt_embeds: torch.Tensor, add_text_embeds: torch.Tensor,
                 add_time_ids: torch.Tensor, bbox: torch.Tensor, aspect_ratio: float,
                 dialog_bbox: Optional[torch.Tensor], num_inference_steps: int, guidance_scale: float,
-                use_graph: bool = True, on_step=None) -> torch.Tensor:
+                use_graph: bool = True, on_step=None, start_index: int = 0) -> torch.Tensor:
         """pipeline_diffsensei.py:306-337.  ``latents`` NCHW fp32 (bs,4,h,w); conditions already concatenated
-        [negative ; positive] along batch (:293-304).  Returns the final latents, NCHW fp32."""
+        [negative ; positive] along batch (:293-304).  ``start_index``: run steps start_index .. T-1 of the
+        ``num_inference_steps`` schedule (img2img; ``on_step`` then counts from 0).  Returns the final latents, NCHW
+        fp32."""
         if use_graph:
             st = self.stepper_for(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
-                                  dialog_bbox, num_inference_steps, guidance_scale)
+                                  dialog_bbox, num_inference_steps, guidance_scale, start_index=start_index)
         else:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
-                                   dialog_bbox, num_inference_steps, guidance_scale, False)
+                                   dialog_bbox, num_inference_steps, guidance_scale, False, start_index=start_index)
         for i, t in enumerate(st.timesteps):
             st.step(i)
             if on_step is not None:
@@ -337,7 +345,12 @@ class DiffSenseiPipeline:
                  latents: Optional[torch.Tensor] = None, output_type: str = "latent", use_graph: bool = True,
                  # ... or the INPUTS of those encoders, when the engines are registered (token ids / pixel values):
                  prompt_input_ids=None, prompt_input_ids_2=None, negative_prompt_input_ids=None,
-                 negative_prompt_input_ids_2=None, clip_pixel_values=None, magi_pixel_values=None):
+                 negative_prompt_input_ids_2=None, clip_pixel_values=None, magi_pixel_values=None,
+                 # img2img (diffusers' StableDiffusionXLImg2ImgPipeline): start from this image at `strength`
+                 image=None, strength: float = 0.3):
+        t_start = 0
+        if image is not None:
+            t_start, height, width = self._check_image(image, latents, strength, num_inference_steps, height, width)
         height = height or self.default_sample_size * self.vae_scale_factor
         width = width or self.default_sample_size * self.vae_scale_factor
         original_size = original_size or (height, width)
@@ -393,7 +406,11 @@ class DiffSenseiPipeline:
         self.set_ip_scale(ip_scale)
         dev = self.unet.device
         self.scheduler.set_timesteps(num_inference_steps, device=dev)    # :248 (init_noise_sigma depends on it)
-        if latents is None:
+        if image is not None:                                            # img2img prepare_latents (add_noise=True)
+            latents = self.vae_encoder.encode_latents(self.vae_image_processor.preprocess_nhwc4(image, height, width),
+                                                      generator, num_samples,
+                                                      self.scheduler.add_noise_coefficients(t_start, dev))
+        elif latents is None:
             latents = self.prepare_latents(num_samples, self.unet.config.in_channels, height, width, generator)
         else:
             latents = latents * self.scheduler.init_noise_sigma          # diffusers' prepare_latents
@@ -409,19 +426,39 @@ class DiffSenseiPipeline:
         ti = time_ids.repeat(2 * num_samples, 1)                                                   # :296,302
         pe = torch.cat([pe, torch.cat([neg_img, img], dim=0)], dim=1)                              # :297,303
         final = self.denoise(latents, pe, te, ti, torch.cat([neg_bbox, bbox], dim=0), aspect_ratio,
-                             torch.cat([neg_db, db], dim=0), num_inference_steps, guidance_scale, use_graph=use_graph)
+                             torch.cat([neg_db, db], dim=0), num_inference_steps, guidance_scale, use_graph=use_graph,
+                             start_index=t_start)
         if output_type == "latent":
             return SimpleNamespace(images=final, latents=final)
         # pipeline_diffsensei.py:339-363: latents / scaling_factor -> vae.decode -> image_processor.postprocess
         image = self.vae.decode_image(final)                                            # fp32 NCHW in [0, 1]
         return SimpleNamespace(images=_postprocess(image, output_type), latents=final)
 
+    def _check_image(self, image, latents, strength, num_inference_steps, height, width):
+        """The host-only checks of ``image=`` (before any GPU work).  Returns (t_start, height, width): the first step
+        of the schedule the loop runs, and the panel size the image is processed to."""
+        if self.vae_encoder is None:
+            raise ValueError("image= needs a VAE encoder: DiffSenseiPipeline(..., vae_encoder=VaeEncoderEngine)")
+        if latents is not None:
+            raise ValueError("`image` and `latents` can not be input together")
+        t_start, _ = get_timesteps(num_inference_steps, strength)
+        height, width = self.vae_image_processor.get_default_height_width(image, height, width)
+        if isinstance(image, torch.Tensor) and image.is_floating_point():
+            if image.dim() not in (3, 4) or (image.dim() == 4 and image.shape[0] != 1) or image.shape[-3] != 3:
+                raise ValueError(f"a float image must be an NCHW tensor of batch 1 with 3 channels, got "
+                                 f"{tuple(image.shape)}")
+            if tuple(image.shape[-2:]) != (height, width):
+                raise ValueError(f"a float image tensor is not resized: it must already be {height} x {width}, got "
+                                 f"{tuple(image.shape[-2:])}")
+        return t_start, height, width
+
     # ------------------------------------------------------------------------------ a page of panels
     @torch.no_grad()
     def generate_page(self, panels: List[dict], *, num_inference_steps: int = 40, guidance_scale: float = 5.0,
                       ip_scale: float = 1.0, output_type: str = "latent", use_graph: bool = True,
                       max_batch_panels: int = PAGE_MAX_ROWS, agent=None, tokenizer_mllm=None,
-                      mllm_scale: float = 0.4, max_new_tokens: int = 500) -> List[SimpleNamespace]:
+                      mllm_scale: float = 0.4, max_new_tokens: int = 500,
+                      strength: float = 0.3) -> List[SimpleNamespace]:
         """Several panels of a page in one call.  ``panels`` holds one dict per panel with the per-panel keywords of
         ``__call__`` (``PANEL_KEYS``); the keywords here are the same for the whole page.  Returns one
         ``SimpleNamespace(images=..., latents=...)`` per panel, in panel order, each ``torch.equal`` to
@@ -445,7 +482,11 @@ class DiffSenseiPipeline:
         224² images (encoded, not zeroed) and truncated to it, go through the encoders and the Resampler; the agent
         decodes every panel's ``mllm_inputs(prompt)`` with those embeddings (``generate_batch``, ``max_new_tokens``);
         its image features are blended as ``feat * mllm_scale + embeds * (1 - mllm_scale)``, and the blend is
-        denoised as ``ip_image_embeds`` with ``ip_images=[]`` and ``ip_bbox`` padded with zero boxes."""
+        denoised as ``ip_image_embeds`` with ``ip_images=[]`` and ``ip_bbox`` padded with zero boxes.
+
+        A panel with ``image`` starts from that image at the page's ``strength``, as ``__call__(image=...)`` does: it
+        draws the posterior sample's noise, then the latent noise, at its turn in panel order; same-size images are
+        encoded in one batch; img2img panels never share a denoise with text-to-image panels."""
         if not isinstance(panels, (list, tuple)) or len(panels) == 0:
             raise ValueError("generate_page needs a non-empty list of panel dicts")
         panels = [dict(p) for p in panels]
@@ -464,6 +505,9 @@ class DiffSenseiPipeline:
                              "fused CFG + scheduler update and does not implement the guidance-free variant")
         if int(max_batch_panels) < 1:
             raise ValueError(f"max_batch_panels must be >= 1, got {max_batch_panels}")
+        t_start = 0
+        if any(p.get("image") is not None for p in panels):
+            t_start, _ = get_timesteps(num_inference_steps, strength)
         if agent is not None:
             self._check_agent_panels(panels, tokenizer_mllm)
             for i, p in enumerate(panels):          # the panels' own checks too, before the agent's decode
@@ -502,17 +546,23 @@ class DiffSenseiPipeline:
         self.set_ip_scale(ip_scale)
         self.scheduler.set_timesteps(num_inference_steps, device=dev)
         for j in jobs:                                                     # panel order: the global RNG's order
-            if j.latents is None:
+            if j.image is not None:
+                j.eps, j.noise = self.vae_encoder.draw_noise(j.height // self.vae_scale_factor,
+                                                             j.width // self.vae_scale_factor, j.ns, j.generator)
+            elif j.latents is None:
                 j.latents = self.prepare_latents(j.ns, self.unet.config.in_channels, j.height, j.width, j.generator)
             else:
                 j.latents = j.latents * self.scheduler.init_noise_sigma
+        self._encode_page_latents([j for j in jobs if j.image is not None], t_start)
         results = [None] * len(jobs)
-        for chunk in plan_page([(j.ns,) + tuple(j.latents.shape[-2:]) for j in jobs], max_batch_panels):
+        shapes = [(j.ns,) + tuple(j.latents.shape[-2:]) + (("image",) if j.image is not None else ()) for j in jobs]
+        for chunk in plan_page(shapes, max_batch_panels):
             rows = [self._panel_rows(jobs[i]) for i in chunk]
             cat = lambda k: torch.cat([r[0][k] for r in rows] + [r[1][k] for r in rows], dim=0)
             lat = torch.cat([jobs[i].latents for i in chunk], dim=0)
             final = self.denoise(lat, cat("pe"), cat("te"), cat("ti"), cat("bbox"), lat.shape[-2] / lat.shape[-1],
-                                 cat("db"), num_inference_steps, guidance_scale, use_graph=use_graph)
+                                 cat("db"), num_inference_steps, guidance_scale, use_graph=use_graph,
+                                 start_index=t_start if jobs[chunk[0]].image is not None else 0)
             image = self.vae.decode_image(final) if output_type != "latent" else final
             r0 = 0
             for i in chunk:
@@ -521,13 +571,28 @@ class DiffSenseiPipeline:
                 r0 = r1
         return results
 
+    def _encode_page_latents(self, jobs, t_start: int) -> None:
+        """The img2img panels' initial latents: every image processed to its panel size, same-size images through
+        the encoder in one batch, then each panel's posterior sample + add_noise from the noise it drew."""
+        if not jobs:
+            return
+        for j in jobs:
+            j.x4 = self.vae_image_processor.preprocess_nhwc4(j.image, j.height, j.width)
+        coef = self.scheduler.add_noise_coefficients(t_start, self.unet.device)
+        for j, (m,) in zip(jobs, _stacked(lambda x4: (self.vae_encoder.moments_nhwc(x4),), [j.x4 for j in jobs])):
+            j.latents = self.vae_encoder.latents_from_moments(m, j.eps, j.ns, j.noise, coef)
+
     def _panel_job(self, i: int, p: dict) -> SimpleNamespace:
         """One panel's arguments resolved as ``__call__`` resolves them, with its ValueErrors prefixed by the panel
         index; runs on the host only (tokenization included), so a bad panel fails before any GPU work."""
         g = lambda k, d=None: p.get(k, d)
         try:
-            height = g("height") or self.default_sample_size * self.vae_scale_factor
-            width = g("width") or self.default_sample_size * self.vae_scale_factor
+            height, width = g("height"), g("width")
+            if g("image") is not None:
+                # the page's strength was checked already: only the panel's own image checks can fail here
+                _, height, width = self._check_image(g("image"), g("latents"), 1.0, 1, height, width)
+            height = height or self.default_sample_size * self.vae_scale_factor
+            width = width or self.default_sample_size * self.vae_scale_factor
             ip_images, ip_bbox = list(g("ip_images", ())), list(g("ip_bbox", ()))
             ip_image_embeds = g("ip_image_embeds")
             if len(ip_images) > 0:
@@ -585,6 +650,7 @@ class DiffSenseiPipeline:
         ns = int(g("num_samples", 1))
         return SimpleNamespace(
             index=i, ns=ns, height=height, width=width, generator=g("generator"), latents=g("latents"), ids=ids,
+            image=g("image"),
             pe=g("prompt_embeds"), npe=g("negative_prompt_embeds"), pp=g("pooled_prompt_embeds"),
             npp=g("negative_pooled_prompt_embeds"), ip_images=ip_images, clip_pv=clip_pv, magi_pv=magi_pv,
             clip=g("clip_image_embeds"), magi=g("magi_image_embeds"), ip_image_embeds=ip_image_embeds,
@@ -733,16 +799,21 @@ class DenoiseStepper:
 
     @torch.no_grad()
     def __init__(self, pipe: DiffSenseiPipeline, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox,
-                 aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale, use_graph=True, chains=None):
+                 aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale, use_graph=True, chains=None,
+                 start_index: int = 0):
         unet, dev = pipe.unet, pipe.unet.device
         self.unet, self.dev, self.guidance = unet, dev, float(guidance_scale)
         self.scheduler = pipe.scheduler
         self.num_inference_steps = int(num_inference_steps)
         self.aspect_ratio = float(aspect_ratio)
-        self.timesteps = pipe.scheduler.set_timesteps(num_inference_steps, device=dev)
-        self.coef_table = pipe.scheduler.coefficient_table(dev)                         # [T, 2] DDIM, [T, 3] Euler
+        # img2img runs steps start_index .. T-1 of the full schedule, with the full schedule's coefficients
+        self.start_index = s0 = int(start_index)
+        if not 0 <= s0 < self.num_inference_steps:
+            raise ValueError(f"start_index must be in [0, {self.num_inference_steps}), got {start_index}")
+        self.timesteps = pipe.scheduler.set_timesteps(num_inference_steps, device=dev)[s0:]
+        self.coef_table = pipe.scheduler.coefficient_table(dev)[s0:]                    # [T, 2] DDIM, [T, 3] Euler
         # scale_model_input's divisor per step; dividing by a device element is a true division, as in the kernels
-        self.in_div = torch.tensor(pipe.scheduler.model_input_divisors(), dtype=f32, device=dev)
+        self.in_div = torch.tensor(pipe.scheduler.model_input_divisors()[s0:], dtype=f32, device=dev)
         self.cond = None
         self.lat = self.model_in = self.db = self.temb_table = None
         self.round_bf16 = True

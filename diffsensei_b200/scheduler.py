@@ -8,6 +8,9 @@ stable-diffusion-xl-base-1.0 (scaled_linear betas 0.00085..0.012 over 1000 train
 * ``EulerDiscreteScheduler`` mirrors diffusers' ``EulerDiscreteScheduler`` with ``interpolation_type="linear"``,
   ``use_karras_sigmas=False`` and ``s_churn=0`` (no noise injection), the scheduler SDXL-base ships.
 
+For img2img both add ``add_noise`` (diffusers' API, torch fp32), ``add_noise_coefficients`` (the same arithmetic as the
+two fp32 factors ``ds_vae_posterior`` reads) and ``set_begin_index``; ``get_timesteps`` is the strength rule.
+
 ``scheduler_from_config`` picks one from a checkpoint's ``scheduler/scheduler_config.json``, the way diffusers does,
 and rejects any class or value whose arithmetic is not implemented here.
 
@@ -43,6 +46,7 @@ class DDIMScheduler:
         self.num_inference_steps = 0
         self.config = dict(_SDXL, num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
                            steps_offset=steps_offset, set_alpha_to_one=False, clip_sample=False)
+        self.begin_index = None
 
     def set_timesteps(self, num_inference_steps: int, device=None) -> List[int]:
         ratio = self.num_train_timesteps // num_inference_steps
@@ -70,6 +74,23 @@ class DDIMScheduler:
     def fused_step_(self, noise_pred, latents, model_in, coef, guidance: float) -> None:
         ops.cfg_ddim_step_(noise_pred, latents, model_in, coef, guidance)
 
+    def set_begin_index(self, begin_index: int = 0) -> None:
+        """The loop's first step (img2img); DDIM's arithmetic does not depend on it, only add_noise's timestep."""
+        self.begin_index = int(begin_index)
+
+    def add_noise_coefficients(self, start_index: int, device=None) -> torch.Tensor:
+        """fp32 [2] {sqrt(alpha_bar_t), sqrt(1 - alpha_bar_t)} at t = timesteps[start_index], each computed in fp32
+        as diffusers' add_noise does: ``add_noise(x, n, t) == c[0] * x + c[1] * n``."""
+        a = self.alphas_cumprod[self.timesteps[start_index]]
+        return torch.stack([a ** 0.5, (1 - a) ** 0.5]).to(device=device, dtype=torch.float32)
+
+    def add_noise(self, original_samples: torch.Tensor, noise: torch.Tensor, timesteps) -> torch.Tensor:
+        """diffusers' ``DDIMScheduler.add_noise``: sqrt(alpha_bar_t) x + sqrt(1 - alpha_bar_t) n in fp32."""
+        t = torch.as_tensor(timesteps).reshape(-1).long().cpu()
+        a = self.alphas_cumprod.to(original_samples.dtype)[t].to(original_samples.device)
+        shape = (-1,) + (1,) * (original_samples.dim() - 1)
+        return (a ** 0.5).reshape(shape) * original_samples + ((1 - a) ** 0.5).reshape(shape) * noise
+
 
 class EulerDiscreteScheduler:
     """diffusers' ``EulerDiscreteScheduler`` under the SDXL-base config, all schedule arithmetic in fp32:
@@ -89,6 +110,7 @@ class EulerDiscreteScheduler:
         self.sigmas = torch.cat([self.train_sigmas.flip(0), torch.zeros(1)])        # before set_timesteps
         self.config = dict(_SDXL, num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
                            steps_offset=steps_offset, interpolation_type="linear", use_karras_sigmas=False)
+        self.begin_index = None
 
     @property
     def init_noise_sigma(self) -> float:
@@ -120,6 +142,43 @@ class EulerDiscreteScheduler:
 
     def fused_step_(self, noise_pred, latents, model_in, coef, guidance: float) -> None:
         ops.cfg_euler_step_(noise_pred, latents, model_in, coef, guidance)
+
+    def set_begin_index(self, begin_index: int = 0) -> None:
+        """diffusers' ``set_begin_index``: the loop starts at sigma_{begin_index} (img2img)."""
+        self.begin_index = int(begin_index)
+
+    def add_noise_coefficients(self, start_index: int, device=None) -> torch.Tensor:
+        """fp32 [2] {1, sigma_{start_index}}: ``add_noise(x, n, .) == x + n * sigma == c[0] * x + c[1] * n`` bit for
+        bit (the product with 1 is exact)."""
+        return torch.stack([torch.ones((), dtype=torch.float32), self.sigmas[start_index]]).to(device=device)
+
+    def add_noise(self, original_samples: torch.Tensor, noise: torch.Tensor, timesteps) -> torch.Tensor:
+        """diffusers' ``EulerDiscreteScheduler.add_noise``: x + n * sigma in fp32, sigma at ``begin_index`` when set
+        (img2img), else at the index of each timestep in the schedule."""
+        t = torch.as_tensor(timesteps).reshape(-1)
+        if getattr(self, "begin_index", None) is not None:
+            idx = [self.begin_index] * t.numel()
+        else:
+            idx = [self.timesteps.index(int(v)) for v in t]
+        sigma = self.sigmas.to(original_samples.dtype)[idx].to(original_samples.device)
+        return original_samples + noise * sigma.reshape((-1,) + (1,) * (original_samples.dim() - 1))
+
+
+def get_timesteps(num_inference_steps: int, strength: float) -> Tuple[int, int]:
+    """diffusers' img2img ``get_timesteps``: (t_start, steps run).  The loop runs steps t_start .. T-1 of the full
+    ``set_timesteps(num_inference_steps)`` schedule with its coefficients; ``int(T * strength)`` truncates the float64
+    product as Python does (50 * 0.58 == 28.999999999999996 -> 28 steps).  A ``strength`` outside [0, 1] and a step
+    count below 1 after it raise ``ValueError``."""
+    strength = float(strength)
+    if not 0.0 <= strength <= 1.0:
+        raise ValueError(f"The value of strength should in [0.0, 1.0] but is {strength}")
+    n = int(num_inference_steps)
+    init = min(int(n * strength), n)
+    t_start = max(n - init, 0)
+    if n - t_start < 1:
+        raise ValueError(f"After adjusting the num_inference_steps by strength parameter: {strength}, the number of "
+                         f"pipeline steps is {n - t_start} which is < 1 and not appropriate for this pipeline.")
+    return t_start, n - t_start
 
 
 # (key, value implemented here, diffusers' default when the config omits the key) for every key that changes the

@@ -191,6 +191,51 @@ def vae_decoder_param_shapes(vc: VaeConfig) -> Dict[str, Shape]:
     return sh
 
 
+def vae_encoder_param_shapes(vc: VaeConfig) -> Dict[str, Shape]:
+    """diffusers AutoencoderKL keys the encode path reads: ``encoder.*`` + ``quant_conv`` (the mid-block attention
+    under the same ``to_q`` / ``to_k`` / ``to_v`` / ``to_out.0`` names as the decoder's)."""
+    sh: Dict[str, Shape] = {}
+    ch = vc.block_out_channels
+    L = vc.latent_channels
+
+    def conv(p, o, i, k):
+        sh[p + ".weight"] = (o, i, k, k)
+        sh[p + ".bias"] = (o,)
+
+    def norm(p, c):
+        sh[p + ".weight"] = (c,)
+        sh[p + ".bias"] = (c,)
+
+    def resnet(p, cin, cout):
+        norm(p + ".norm1", cin)
+        conv(p + ".conv1", cout, cin, 3)
+        norm(p + ".norm2", cout)
+        conv(p + ".conv2", cout, cout, 3)
+        if cin != cout:
+            conv(p + ".conv_shortcut", cout, cin, 1)
+
+    conv("encoder.conv_in", ch[0], vc.out_channels, 3)          # in_channels == out_channels (RGB) in AutoencoderKL
+    prev = ch[0]
+    for i, co in enumerate(ch):
+        for j in range(vc.layers_per_block):
+            resnet(f"encoder.down_blocks.{i}.resnets.{j}", prev if j == 0 else co, co)
+        if i < len(ch) - 1:
+            conv(f"encoder.down_blocks.{i}.downsamplers.0.conv", co, co, 3)
+        prev = co
+    c = ch[-1]
+    resnet("encoder.mid_block.resnets.0", c, c)
+    resnet("encoder.mid_block.resnets.1", c, c)
+    a = "encoder.mid_block.attentions.0"
+    norm(a + ".group_norm", c)
+    for nm in ("to_q", "to_k", "to_v", "to_out.0"):
+        sh[f"{a}.{nm}.weight"] = (c, c)
+        sh[f"{a}.{nm}.bias"] = (c,)
+    norm("encoder.conv_norm_out", c)
+    conv("encoder.conv_out", 2 * L, c, 3)
+    conv("quant_conv", 2 * L, 2 * L, 1)
+    return sh
+
+
 def agent_param_shapes(ac: AgentConfig) -> Dict[str, Shape]:
     """transformers ``LlamaForCausalLM`` keys (no biases)."""
     C, I, V = ac.hidden_size, ac.intermediate_size, ac.vocab_size

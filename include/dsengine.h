@@ -227,6 +227,10 @@ typedef struct {
    * 36 MACs per input pixel).  x: [B][H][W][Cin], out: [B][2H][2W][Cout] bf16, w: [4][Cout][2][2][Cin] bf16 from
    * weights.pack_conv3x3_up2 (phase = 2*row_parity + col_parity).  stride 1, no residual / rowbias. */
   int32_t upsample2;
+  /* 1: padding (left 0, right 1, top 0, bottom 1) instead of 1 on every side, stride 2 only — diffusers Downsample2D
+   * of the AutoencoderKL encoder (F.pad(x, (0, 1, 0, 1)) + Conv2d(stride=2, padding=0)): out [B][H/2][W/2][Cout],
+   * output pixel i reads input pixels 2i .. 2i+2.  0: the convolution described above. */
+  int32_t pad_bottom_right;
 } ds_conv3x3_args;
 
 int ds_conv3x3_nhwc(const ds_conv3x3_args* args, void* stream);
@@ -346,6 +350,18 @@ int ds_latent_pointwise(const float* latents, const float* w, const float* bias,
                         int HW, void* stream);
 int ds_softmax_rows(const float* S, void* P, int rows, int n, int64_t lds, int64_t ldp, float scale, void* stream);
 int ds_image_postprocess(const void* x, float* out, int B, int HW, int C, void* stream);
+/* The AutoencoderKL encoder's posterior, from its conv_out output x fp32 NHWC [B][HW][8] (diffusers
+ * AutoencoderKL.encode -> DiagonalGaussianDistribution, then StableDiffusionXLImg2ImgPipeline.prepare_latents):
+ *   moments = quant_conv(x) (w fp32 [8][8] (out, in), bias fp32 [8]);  mean = moments[:4],
+ *   logvar = clamp(moments[4:], -30, 20);  z = mean + exp(0.5 logvar) * eps  (eps NULL: z = mean, i.e. mode());
+ *   z = scale * z;  out[b * repeat + r] = c0 * z + c1 * noise[b * repeat + r] for r < repeat, with {c0, c1} = coef, a
+ *   DEVICE pointer: {sqrt(alpha_bar_t), sqrt(1 - alpha_bar_t)} for DDIM's add_noise, {1, sigma} for Euler's (noise NULL:
+ *   out = z repeated).  fp32 throughout, each operation rounded on its own.
+ *   mean / logvar / eps: fp32 NCHW [B][4][HW], each optional output may be NULL;  noise / out: fp32 NCHW
+ *   [B * repeat][4][HW].  x 16-byte aligned. */
+int ds_vae_posterior(const float* x, const float* w, const float* bias, const float* eps, float scale,
+                     const float* noise, const float* coef, int repeat, float* mean, float* logvar, float* out, int B,
+                     int HW, void* stream);
 
 /* The decoder's mid-block attention (diffusers Attention(heads=1, dim_head=D)) in ONE launch for the whole batch:
  *   out[b] = softmax(q[b] k[b]^T / sqrt(D)) v[b]                                                     [compute-bound]
@@ -397,6 +413,23 @@ int ds_embed_tokens(const int* ids, const void* tok_emb, const void* pos_emb, vo
 int64_t ds_image_preprocess_scratch_bytes(const int* sizes, int n, int mode);
 int ds_image_preprocess(const uint8_t* src, const int64_t* offsets, const int* sizes, int n, int mode, float* out,
                         void* scratch, int64_t scratch_bytes, void* stream);
+
+/* Image preprocessing of the AutoencoderKL encoder (diffusers VaeImageProcessor.preprocess, default config:
+ * do_resize with Pillow LANCZOS, do_normalize), bit-exact with Pillow + numpy / torch fp32:
+ *   ds_vae_image_preprocess : one uint8 RGB HWC image [H][W][3] -> Image.resize((out_w, out_h), LANCZOS) (skipped when
+ *                             the size does not change), then x = float32(u8) / 255, 2x - 1.  Writes `out` fp32 NCHW
+ *                             [3][out_h][out_w] and / or `out_nhwc4` bf16 NHWC [out_h][out_w][4] with a zero 4th
+ *                             channel (the input of the encoder's conv_in); either may be NULL.  Same 8-bit fixed-point
+ *                             resampler as ds_image_preprocess; the Lanczos tap tables are built on the host (with the
+ *                             host libm's sin, as Pillow does) and copied into the scratch, so the call is not
+ *                             graph-capturable.  scratch: ds_vae_image_preprocess_scratch_bytes(...) bytes, 16-byte
+ *                             aligned (-1: sizes the entry point rejects; sides in [1, 65535]).
+ *   ds_vae_image_pack       : a float NCHW [B][3][HW] image that is already at its size -> (normalize ? 2x - 1 : x) as
+ *                             fp32 NCHW `out` (may alias x) and / or bf16 NHWC `out_nhwc4` [B][HW][4], 4th channel 0. */
+int64_t ds_vae_image_preprocess_scratch_bytes(int H, int W, int out_h, int out_w);
+int ds_vae_image_preprocess(const uint8_t* src, int H, int W, int out_h, int out_w, float* out, void* out_nhwc4,
+                            void* scratch, int64_t scratch_bytes, void* stream);
+int ds_vae_image_pack(const float* x, float* out, void* out_nhwc4, int B, int HW, int normalize, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * LLaMA decoder of the MLLM agent (SURVEY.md §8f-4: ContinuousLVLM.generate, src/models/mllm/seed_x.py:90-171, over
