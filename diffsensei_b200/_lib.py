@@ -79,6 +79,8 @@ SIGNATURES = {
     "ds_timestep_embedding": [_vp, _vp, _i, _i, _vp],
     "ds_cfg_ddim_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp],
     "ds_cfg_euler_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp],
+    "ds_cfg_ddim_inpaint_step": [_vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _vp],
+    "ds_cfg_euler_inpaint_step": [_vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _vp],
     "ds_resampler_attn": [_vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "ds_attention_small": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i64, _i64, _i64, _i64, _f, _i, _vp],
     "ds_embed_tokens": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],
@@ -89,6 +91,8 @@ SIGNATURES = {
     "ds_image_preprocess": [_vp, _vp, _vp, _i, _i, _vp, _vp, _i64, _vp],
     "ds_vae_image_preprocess": [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _i64, _vp],
     "ds_vae_image_pack": [_vp, _vp, _vp, _i, _i, _i, _vp],
+    "ds_vae_mask_preprocess": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i64, _vp],
+    "ds_vae_mask_pack": [_vp, _i, _i, _vp, _vp, _vp],
     "ds_vae_posterior": [_vp, _vp, _vp, _vp, _f, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _vp],
     "ds_gemv_bf16": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "ds_rmsnorm": [_vp, _vp, _vp, _i, _i, _f, _vp],
@@ -102,7 +106,7 @@ SIGNATURES = {
 }
 OTHER_EXPORTS = ("ds_version", "ds_last_error", "ds_launch_count", "ds_groupnorm_scratch_floats",
                  "ds_gemm_splitk_ws_bytes", "ds_image_preprocess_scratch_bytes",
-                 "ds_vae_image_preprocess_scratch_bytes")
+                 "ds_vae_image_preprocess_scratch_bytes", "ds_vae_mask_preprocess_scratch_bytes")
 
 
 def _load() -> C.CDLL:
@@ -126,6 +130,8 @@ def _load() -> C.CDLL:
     lib.ds_image_preprocess_scratch_bytes.restype = C.c_int64
     lib.ds_vae_image_preprocess_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
     lib.ds_vae_image_preprocess_scratch_bytes.restype = C.c_int64
+    lib.ds_vae_mask_preprocess_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
+    lib.ds_vae_mask_preprocess_scratch_bytes.restype = C.c_int64
     return lib
 
 

@@ -1,6 +1,7 @@
 // glue_kernels.cu — small HBM-bound kernels around the tensor-core ops: conv_in (Cin = 4), layout changes at
 // the diffusers-facing boundary, nearest upsample, channel concat, SiLU, sinusoidal timestep features, and the
-// fused CFG + DDIM and CFG + Euler updates.  All vectorised to 16-byte accesses where the shape allows.
+// fused CFG + DDIM and CFG + Euler updates (plain and
+// inpaint).  All vectorised to 16-byte accesses where the shape allows.
 #include "ds_common.cuh"
 #include "ds_host.h"
 
@@ -164,32 +165,87 @@ __global__ void timestep_embedding_kernel(const float* __restrict__ t, __nv_bflo
 
 // ------------------------------------------------------------------------------------------------
 // CFG blend + DDIM step (eta = 0, epsilon prediction), src/pipelines/pipeline_diffsensei.py:315,332-337.
-// C == 4: one thread per pixel (8-byte bf16 vectors, 16-byte fp32 vector).
+// C == 4: one thread per pixel (8-byte bf16 vectors, 16-byte fp32 vector).  The per-pixel arithmetic lives in
+// __device__ functions that the plain and the inpaint kernels share, so a masked-in pixel of the inpaint kernel is
+// the plain kernel's result bit for bit.
 // ------------------------------------------------------------------------------------------------
-__global__ void cfg_ddim_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
-                                uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
-                                long long n_pix /* bs*HW */) {
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= n_pix) return;
+__device__ __forceinline__ void load_cfg_halves(const uint2* __restrict__ noise_pred, long long i, long long n_pix,
+                                                float u[4], float tt[4]) {
+  const uint2 eu = __ldg(noise_pred + i);          // uncond half
+  const uint2 et = __ldg(noise_pred + n_pix + i);  // text half
+  u[0] = bf16_lo(eu.x), u[1] = bf16_hi(eu.x), u[2] = bf16_lo(eu.y), u[3] = bf16_hi(eu.y);
+  tt[0] = bf16_lo(et.x), tt[1] = bf16_hi(et.x), tt[2] = bf16_lo(et.y), tt[3] = bf16_hi(et.y);
+}
+
+// xv <- DDIM(CFG(u, tt)) in place; coef = {alpha_prod_t, alpha_prod_t_prev}
+__device__ __forceinline__ void cfg_ddim_pixel(const float u[4], const float tt[4], float xv[4],
+                                               const float* __restrict__ coef, float guidance) {
   const float a_t = coef[0], a_prev = coef[1];
   const float sqrt_at = sqrtf(a_t), sqrt_1mat = sqrtf(1.0f - a_t);
   const float sqrt_ap = sqrtf(a_prev), sqrt_1map = sqrtf(1.0f - a_prev);
-  const uint2 eu = __ldg(noise_pred + i);          // uncond half
-  const uint2 et = __ldg(noise_pred + n_pix + i);  // text half
-  const float u[4] = {bf16_lo(eu.x), bf16_hi(eu.x), bf16_lo(eu.y), bf16_hi(eu.y)};
-  const float tt[4] = {bf16_lo(et.x), bf16_hi(et.x), bf16_lo(et.y), bf16_hi(et.y)};
-  float4 x = latents[i];
-  float xv[4] = {x.x, x.y, x.z, x.w};
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const float eps = u[j] + guidance * (tt[j] - u[j]);
     const float x0 = (xv[j] - sqrt_1mat * eps) / sqrt_at;
     xv[j] = sqrt_ap * x0 + sqrt_1map * eps;
   }
+}
+
+// xv <- Euler(CFG(u, tt)) in place; coef = {sigma_i, sigma_{i+1}, ...}
+__device__ __forceinline__ void cfg_euler_pixel(const float u[4], const float tt[4], float xv[4],
+                                                const float* __restrict__ coef, float guidance) {
+  const float sigma = coef[0], sigma_next = coef[1];
+  const float dt = __fsub_rn(sigma_next, sigma);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float eps = __fadd_rn(u[j], __fmul_rn(guidance, __fsub_rn(tt[j], u[j])));
+    const float x0 = __fsub_rn(xv[j], __fmul_rn(sigma, eps));
+    const float d = __fdiv_rn(__fsub_rn(xv[j], x0), sigma);
+    xv[j] = __fadd_rn(xv[j], __fmul_rn(d, dt));
+  }
+}
+
+// the fp32 master and both CFG halves of the next UNet input: bf16(xv / in_div), or bf16(xv) when in_div is NULL
+__device__ __forceinline__ void store_step(float4* __restrict__ latents, uint2* __restrict__ model_in, long long i,
+                                           long long n_pix, const float xv[4], const float* in_div) {
   latents[i] = make_float4(xv[0], xv[1], xv[2], xv[3]);
-  const uint2 o = make_uint2(pack_bf16(xv[0], xv[1]), pack_bf16(xv[2], xv[3]));
+  uint2 o;
+  if (in_div) {
+    const float d = *in_div;
+    o = make_uint2(pack_bf16(__fdiv_rn(xv[0], d), __fdiv_rn(xv[1], d)),
+                   pack_bf16(__fdiv_rn(xv[2], d), __fdiv_rn(xv[3], d)));
+  } else {
+    o = make_uint2(pack_bf16(xv[0], xv[1]), pack_bf16(xv[2], xv[3]));
+  }
   model_in[i] = o;
   model_in[n_pix + i] = o;
+}
+
+// diffusers' 4-channel inpaint blend after the scheduler step: where mask == 0 the pixel becomes init_proper =
+// c0 * z + c1 * n (add_noise of the image latents z at the next timestep, each product and the sum rounded on its
+// own as torch eager does; {c0, c1} = {1, 0} on the last step gives z); where mask == 1 it keeps the update.
+__device__ __forceinline__ void inpaint_blend(float xv[4], long long i, const float4* __restrict__ image_latents,
+                                              const float4* __restrict__ noise, const unsigned char* __restrict__ mask,
+                                              float c0, float c1) {
+  if (__ldg(mask + i)) return;
+  const float4 z = __ldg(image_latents + i), n = __ldg(noise + i);
+  xv[0] = __fadd_rn(__fmul_rn(c0, z.x), __fmul_rn(c1, n.x));
+  xv[1] = __fadd_rn(__fmul_rn(c0, z.y), __fmul_rn(c1, n.y));
+  xv[2] = __fadd_rn(__fmul_rn(c0, z.z), __fmul_rn(c1, n.z));
+  xv[3] = __fadd_rn(__fmul_rn(c0, z.w), __fmul_rn(c1, n.w));
+}
+
+__global__ void cfg_ddim_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
+                                uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
+                                long long n_pix /* bs*HW */) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n_pix) return;
+  float u[4], tt[4];
+  load_cfg_halves(noise_pred, i, n_pix, u, tt);
+  const float4 x = latents[i];
+  float xv[4] = {x.x, x.y, x.z, x.w};
+  cfg_ddim_pixel(u, tt, xv, coef, guidance);
+  store_step(latents, model_in, i, n_pix, xv, nullptr);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -203,27 +259,48 @@ __global__ void cfg_euler_kernel(const uint2* __restrict__ noise_pred, float4* _
                                  long long n_pix /* bs*HW */) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= n_pix) return;
-  const float sigma = coef[0], sigma_next = coef[1], in_div = coef[2];
-  const float dt = __fsub_rn(sigma_next, sigma);
-  const uint2 eu = __ldg(noise_pred + i);          // uncond half
-  const uint2 et = __ldg(noise_pred + n_pix + i);  // text half
-  const float u[4] = {bf16_lo(eu.x), bf16_hi(eu.x), bf16_lo(eu.y), bf16_hi(eu.y)};
-  const float tt[4] = {bf16_lo(et.x), bf16_hi(et.x), bf16_lo(et.y), bf16_hi(et.y)};
-  float4 x = latents[i];
+  float u[4], tt[4];
+  load_cfg_halves(noise_pred, i, n_pix, u, tt);
+  const float4 x = latents[i];
   float xv[4] = {x.x, x.y, x.z, x.w};
-  float sv[4];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float eps = __fadd_rn(u[j], __fmul_rn(guidance, __fsub_rn(tt[j], u[j])));
-    const float x0 = __fsub_rn(xv[j], __fmul_rn(sigma, eps));
-    const float d = __fdiv_rn(__fsub_rn(xv[j], x0), sigma);
-    xv[j] = __fadd_rn(xv[j], __fmul_rn(d, dt));
-    sv[j] = __fdiv_rn(xv[j], in_div);
-  }
-  latents[i] = make_float4(xv[0], xv[1], xv[2], xv[3]);
-  const uint2 o = make_uint2(pack_bf16(sv[0], sv[1]), pack_bf16(sv[2], sv[3]));
-  model_in[i] = o;
-  model_in[n_pix + i] = o;
+  cfg_euler_pixel(u, tt, xv, coef, guidance);
+  store_step(latents, model_in, i, n_pix, xv, coef + 2);
+}
+
+// ------------------------------------------------------------------------------------------------
+// The same two steps followed by the inpaint blend (diffusers' StableDiffusionXLInpaintPipeline, 4-channel UNet).
+// coef: DDIM {alpha_prod_t, alpha_prod_t_prev, c0, c1}, Euler {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1), c0,
+// c1}.  image_latents / noise fp32 NHWC [bs][HW][4], mask uint8 [bs][HW] (1: regenerate, 0: keep the image).
+// The next UNet input is computed from the blended latents.
+// ------------------------------------------------------------------------------------------------
+__global__ void cfg_ddim_inpaint_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
+                                        uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
+                                        const float4* __restrict__ image_latents, const float4* __restrict__ noise,
+                                        const unsigned char* __restrict__ mask, long long n_pix /* bs*HW */) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n_pix) return;
+  float u[4], tt[4];
+  load_cfg_halves(noise_pred, i, n_pix, u, tt);
+  const float4 x = latents[i];
+  float xv[4] = {x.x, x.y, x.z, x.w};
+  cfg_ddim_pixel(u, tt, xv, coef, guidance);
+  inpaint_blend(xv, i, image_latents, noise, mask, coef[2], coef[3]);
+  store_step(latents, model_in, i, n_pix, xv, nullptr);
+}
+
+__global__ void cfg_euler_inpaint_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
+                                         uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
+                                         const float4* __restrict__ image_latents, const float4* __restrict__ noise,
+                                         const unsigned char* __restrict__ mask, long long n_pix /* bs*HW */) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n_pix) return;
+  float u[4], tt[4];
+  load_cfg_halves(noise_pred, i, n_pix, u, tt);
+  const float4 x = latents[i];
+  float xv[4] = {x.x, x.y, x.z, x.w};
+  cfg_euler_pixel(u, tt, xv, coef, guidance);
+  inpaint_blend(xv, i, image_latents, noise, mask, coef[3], coef[4]);
+  store_step(latents, model_in, i, n_pix, xv, coef + 2);
 }
 
 }  // namespace ds
@@ -393,5 +470,41 @@ extern "C" int ds_cfg_euler_step(const void* noise_pred, float* latents, void* m
       static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
       guidance, n_pix);
   DS_LAUNCH_OK("cfg_euler_kernel");
+  return DS_OK;
+}
+
+extern "C" int ds_cfg_ddim_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
+                                        float guidance, const float* image_latents, const float* noise,
+                                        const uint8_t* mask, int bs, int HW, int C, void* stream) {
+  DS_REQUIRE(noise_pred && latents && model_in && coef && image_latents && noise && mask,
+             "ds_cfg_ddim_inpaint_step: NULL pointer");
+  DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "ds_cfg_ddim_inpaint_step: only C == 4 latents are supported (got C=%d)", C);
+  DS_REQUIRE((reinterpret_cast<uintptr_t>(image_latents) & 15) == 0 && (reinterpret_cast<uintptr_t>(noise) & 15) == 0,
+             "ds_cfg_ddim_inpaint_step: image_latents / noise must be 16-byte aligned");
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  const long long n_pix = static_cast<long long>(bs) * HW;
+  cfg_ddim_inpaint_kernel<<<static_cast<unsigned>((n_pix + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
+      guidance, reinterpret_cast<const float4*>(image_latents), reinterpret_cast<const float4*>(noise), mask, n_pix);
+  DS_LAUNCH_OK("cfg_ddim_inpaint_kernel");
+  return DS_OK;
+}
+
+extern "C" int ds_cfg_euler_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
+                                         float guidance, const float* image_latents, const float* noise,
+                                         const uint8_t* mask, int bs, int HW, int C, void* stream) {
+  DS_REQUIRE(noise_pred && latents && model_in && coef && image_latents && noise && mask,
+             "ds_cfg_euler_inpaint_step: NULL pointer");
+  DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "ds_cfg_euler_inpaint_step: only C == 4 latents are supported (got C=%d)", C);
+  DS_REQUIRE((reinterpret_cast<uintptr_t>(image_latents) & 15) == 0 && (reinterpret_cast<uintptr_t>(noise) & 15) == 0,
+             "ds_cfg_euler_inpaint_step: image_latents / noise must be 16-byte aligned");
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  const long long n_pix = static_cast<long long>(bs) * HW;
+  cfg_euler_inpaint_kernel<<<static_cast<unsigned>((n_pix + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
+      guidance, reinterpret_cast<const float4*>(image_latents), reinterpret_cast<const float4*>(noise), mask, n_pix);
+  DS_LAUNCH_OK("cfg_euler_inpaint_kernel");
   return DS_OK;
 }

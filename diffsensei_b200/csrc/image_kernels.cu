@@ -21,7 +21,8 @@
 // index is not bounded by anything but the image size.
 //
 // The same resampler also serves the AutoencoderKL encoder's preprocessing (ds_vae_image_preprocess: Pillow LANCZOS
-// to any size, then 2 * u8 / 255 - 1), with host-built tap tables; see the section below plan_images.
+// to any size, then 2 * u8 / 255 - 1) and the inpaint mask's (ds_vae_mask_preprocess: LANCZOS on the mask's own 1 or
+// 3 channels, RGB -> L, threshold), with host-built tap tables; see the section below plan_images.
 #include <cuda_bf16.h>
 
 #include <cmath>
@@ -278,7 +279,7 @@ struct VaePlan {
   long long coef_h, coef_v, inter, total;
 };
 
-static VaePlan plan_vae(int H, int W, int oh, int ow) {
+static VaePlan plan_vae(int H, int W, int oh, int ow, int C) {
   VaePlan p{};
   long long cur = 0;
   auto take = [&cur](long long bytes) {
@@ -290,12 +291,13 @@ static VaePlan plan_vae(int H, int W, int oh, int ow) {
   p.kv = oh != H ? lanczos_taps(H, oh) : 0;
   p.coef_h = p.kh ? take(4LL * ow * (2 + p.kh)) : 0;
   p.coef_v = p.kv ? take(4LL * oh * (2 + p.kv)) : 0;
-  p.inter = p.kh ? take(3LL * ow * H) : 0;
+  p.inter = p.kh ? take(static_cast<long long>(C) * ow * H) : 0;
   p.total = cur;
   return p;
 }
 
-// every source row, the ow output columns, 3 channels -> uint8 intermediate [H][ow][3]
+// every source row, the ow output columns, C channels -> uint8 intermediate [H][ow][C]
+template <int C>
 __global__ void vae_image_hpass_kernel(const unsigned char* __restrict__ img, const int* __restrict__ coef,
                                        unsigned char* __restrict__ inter, int W, int ow, int kh, long long total) {
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
@@ -304,18 +306,43 @@ __global__ void vae_image_hpass_kernel(const unsigned char* __restrict__ img, co
     const int x = static_cast<int>(i - y * ow);
     const int* k = coef + static_cast<size_t>(x) * (2 + kh);
     const int xmin = k[0], xmax = k[1];
-    const unsigned char* p = img + (y * W + xmin) * 3;
-    int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
+    const unsigned char* p = img + (y * W + xmin) * C;
+    int a[C];
+#pragma unroll
+    for (int c = 0; c < C; ++c) a[c] = 1 << (kPrecisionBits - 1);
     for (int t = 0; t < xmax; ++t) {
       const int w = k[2 + t];
-      a0 += p[3 * t] * w;
-      a1 += p[3 * t + 1] * w;
-      a2 += p[3 * t + 2] * w;
+#pragma unroll
+      for (int c = 0; c < C; ++c) a[c] += p[C * t + c] * w;
     }
-    unsigned char* o = inter + i * 3;
-    o[0] = static_cast<unsigned char>(clip8(a0));
-    o[1] = static_cast<unsigned char>(clip8(a1));
-    o[2] = static_cast<unsigned char>(clip8(a2));
+    unsigned char* o = inter + i * C;
+#pragma unroll
+    for (int c = 0; c < C; ++c) o[c] = static_cast<unsigned char>(clip8(a[c]));
+  }
+}
+
+// output pixel (y, x) of the vertical pass (or a copy when kv == 0) over C-channel uint8 rows of `pitch` bytes
+template <int C>
+__device__ __forceinline__ void vae_vpass_pixel(const unsigned char* __restrict__ base, long long pitch,
+                                                const int* __restrict__ coef, int kv, int y, int x, int v[C]) {
+  const unsigned char* col = base + static_cast<long long>(x) * C;
+  if (kv) {
+    const int* k = coef + static_cast<size_t>(y) * (2 + kv);
+    const int ymin = k[0], ymax = k[1];
+#pragma unroll
+    for (int c = 0; c < C; ++c) v[c] = 1 << (kPrecisionBits - 1);
+    for (int t = 0; t < ymax; ++t) {
+      const unsigned char* p = col + (ymin + t) * pitch;
+      const int w = k[2 + t];
+#pragma unroll
+      for (int c = 0; c < C; ++c) v[c] += p[c] * w;
+    }
+#pragma unroll
+    for (int c = 0; c < C; ++c) v[c] = clip8(v[c]);
+  } else {
+    const unsigned char* p = col + y * pitch;
+#pragma unroll
+    for (int c = 0; c < C; ++c) v[c] = p[c];
   }
 }
 
@@ -328,28 +355,8 @@ __global__ void vae_image_vpass_kernel(const unsigned char* __restrict__ base, l
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= hw) return;
   const int y = static_cast<int>(i / ow), x = static_cast<int>(i - static_cast<long long>(y) * ow);
-  const unsigned char* col = base + static_cast<long long>(x) * 3;
   int v[3];
-  if (kv) {
-    const int* k = coef + static_cast<size_t>(y) * (2 + kv);
-    const int ymin = k[0], ymax = k[1];
-    int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
-    for (int t = 0; t < ymax; ++t) {
-      const unsigned char* p = col + (ymin + t) * pitch;
-      const int w = k[2 + t];
-      a0 += p[0] * w;
-      a1 += p[1] * w;
-      a2 += p[2] * w;
-    }
-    v[0] = clip8(a0);
-    v[1] = clip8(a1);
-    v[2] = clip8(a2);
-  } else {
-    const unsigned char* p = col + y * pitch;
-    v[0] = p[0];
-    v[1] = p[1];
-    v[2] = p[2];
-  }
+  vae_vpass_pixel<3>(base, pitch, coef, kv, y, x, v);
   float o[3];
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
@@ -380,6 +387,71 @@ __global__ void vae_image_pack_kernel(const float* x, float* out, uint2* __restr
     __nv_bfloat162 lo = __floats2bfloat162_rn(o[0], o[1]), hi = __floats2bfloat162_rn(o[2], 0.0f);
     out4[i] = make_uint2(*reinterpret_cast<uint32_t*>(&lo), *reinterpret_cast<uint32_t*>(&hi));
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Inpaint mask preprocessing (diffusers VaeImageProcessor(do_normalize=False, do_binarize=True,
+// do_convert_grayscale=True).preprocess + prepare_mask_latents' nearest downsample): the same resampler on the mask's
+// own channels (1: "L", 3: "RGB"), then for RGB Pillow's RGB -> L conversion of the resized pixels,
+// L = (19595 R + 38470 G + 7471 B + 0x8000) >> 16, then float32(L) / 255 >= 0.5, i.e. L >= 128.  One output pixel per
+// thread; the pixel at (8i, 8j) also writes latent pixel (i, j) (F.interpolate nearest to H/8 x W/8).
+template <int C>
+__global__ void vae_mask_vpass_kernel(const unsigned char* __restrict__ base, long long pitch,
+                                      const int* __restrict__ coef, int kv, int oh, int ow, float* __restrict__ out,
+                                      unsigned char* __restrict__ out_latent) {
+  const long long hw = static_cast<long long>(oh) * ow;
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= hw) return;
+  const int y = static_cast<int>(i / ow), x = static_cast<int>(i - static_cast<long long>(y) * ow);
+  int v[C];
+  vae_vpass_pixel<C>(base, pitch, coef, kv, y, x, v);
+  const int l = C == 3 ? (v[0] * 19595 + v[1] * 38470 + v[2] * 7471 + 0x8000) >> 16 : v[0];
+  const bool keep = l >= 128;
+  if (out) out[i] = keep ? 1.0f : 0.0f;
+  if (out_latent && (y & 7) == 0 && (x & 7) == 0) out_latent[(y >> 3) * (ow >> 3) + (x >> 3)] = keep;
+}
+
+// a float mask already at its size [H][W] -> (x >= 0.5) as fp32 and / or the uint8 latent mask [H/8][W/8]
+__global__ void vae_mask_pack_kernel(const float* __restrict__ x, float* __restrict__ out,
+                                     unsigned char* __restrict__ out_latent, int H, int W) {
+  const long long hw = static_cast<long long>(H) * W;
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= hw) return;
+  const int y = static_cast<int>(i / W), xx = static_cast<int>(i - static_cast<long long>(y) * W);
+  const bool keep = x[i] >= 0.5f;
+  if (out) out[i] = keep ? 1.0f : 0.0f;
+  if (out_latent && (y & 7) == 0 && (xx & 7) == 0) out_latent[(y >> 3) * (W >> 3) + (xx >> 3)] = keep;
+}
+
+// The host half of the VAE resampler: the Lanczos tap tables into the scratch and the horizontal pass.  Returns the
+// rows the vertical pass reads (the source, or the intermediate) and their pitch.
+template <int C>
+static int vae_resample_begin(const uint8_t* src, int H, int W, int out_h, int out_w, const VaePlan& p,
+                              unsigned char* scr, cudaStream_t st, const unsigned char** base, long long* pitch) {
+  // host-built tap tables (pageable source: the copy is staged before the call returns)
+  std::vector<int> table;
+  if (p.kh) {
+    table.assign(static_cast<size_t>(out_w) * (2 + p.kh), 0);
+    lanczos_coeffs(W, out_w, p.kh, table.data());
+    DS_CUDA_OK(cudaMemcpyAsync(scr + p.coef_h, table.data(), table.size() * 4, cudaMemcpyHostToDevice, st));
+  }
+  if (p.kv) {
+    table.assign(static_cast<size_t>(out_h) * (2 + p.kv), 0);
+    lanczos_coeffs(H, out_h, p.kv, table.data());
+    DS_CUDA_OK(cudaMemcpyAsync(scr + p.coef_v, table.data(), table.size() * 4, cudaMemcpyHostToDevice, st));
+  }
+  *base = src;
+  *pitch = static_cast<long long>(C) * W;
+  if (p.kh) {
+    const long long total = static_cast<long long>(H) * out_w;
+    const long long blocks = (total + 255) / 256;
+    vae_image_hpass_kernel<C><<<static_cast<unsigned>(blocks < 4096 ? blocks : 4096), 256, 0, st>>>(
+        src, reinterpret_cast<const int*>(scr + p.coef_h), scr + p.inter, W, out_w, p.kh, total);
+    DS_LAUNCH_OK("vae_image_hpass_kernel");
+    *base = scr + p.inter;
+    *pitch = static_cast<long long>(C) * out_w;
+  }
+  return DS_OK;
 }
 
 }  // namespace ds
@@ -445,7 +517,7 @@ extern "C" int64_t ds_vae_image_preprocess_scratch_bytes(int H, int W, int out_h
   if (H < 1 || W < 1 || H > ds::kMaxSide || W > ds::kMaxSide || out_h < 1 || out_w < 1 || out_h > ds::kMaxSide ||
       out_w > ds::kMaxSide)
     return -1;
-  return ds::plan_vae(H, W, out_h, out_w).total;
+  return ds::plan_vae(H, W, out_h, out_w, 3).total;
 }
 
 extern "C" int ds_vae_image_preprocess(const uint8_t* src, int H, int W, int out_h, int out_w, float* out,
@@ -457,7 +529,7 @@ extern "C" int ds_vae_image_preprocess(const uint8_t* src, int H, int W, int out
              "ds_vae_image_preprocess: %d x %d -> %d x %d; sides must be in [1, %d]", H, W, out_h, out_w, kMaxSide);
   DS_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3) == 0 && (reinterpret_cast<uintptr_t>(out_nhwc4) & 7) == 0,
              "ds_vae_image_preprocess: out must be 4-byte and out_nhwc4 8-byte aligned");
-  const VaePlan p = plan_vae(H, W, out_h, out_w);
+  const VaePlan p = plan_vae(H, W, out_h, out_w, 3);
   DS_REQUIRE(p.total == 0 || (scratch && scratch_bytes >= p.total && (reinterpret_cast<uintptr_t>(scratch) & 15) == 0),
              "ds_vae_image_preprocess: needs %lld bytes of 16-byte aligned scratch "
              "(ds_vae_image_preprocess_scratch_bytes), got %lld", p.total, static_cast<long long>(scratch_bytes));
@@ -465,29 +537,10 @@ extern "C" int ds_vae_image_preprocess(const uint8_t* src, int H, int W, int out
   if (!get_device(&dev)) return DS_ERR_CUDA;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   unsigned char* scr = static_cast<unsigned char*>(scratch);
-  // host-built tap tables (pageable source: the copy is staged before the call returns)
-  std::vector<int> table;
-  if (p.kh) {
-    table.assign(static_cast<size_t>(out_w) * (2 + p.kh), 0);
-    lanczos_coeffs(W, out_w, p.kh, table.data());
-    DS_CUDA_OK(cudaMemcpyAsync(scr + p.coef_h, table.data(), table.size() * 4, cudaMemcpyHostToDevice, st));
-  }
-  if (p.kv) {
-    table.assign(static_cast<size_t>(out_h) * (2 + p.kv), 0);
-    lanczos_coeffs(H, out_h, p.kv, table.data());
-    DS_CUDA_OK(cudaMemcpyAsync(scr + p.coef_v, table.data(), table.size() * 4, cudaMemcpyHostToDevice, st));
-  }
-  const unsigned char* base = src;
-  long long pitch = 3LL * W;
-  if (p.kh) {
-    const long long total = static_cast<long long>(H) * out_w;
-    const long long blocks = (total + 255) / 256;
-    vae_image_hpass_kernel<<<static_cast<unsigned>(blocks < 4096 ? blocks : 4096), 256, 0, st>>>(
-        src, reinterpret_cast<const int*>(scr + p.coef_h), scr + p.inter, W, out_w, p.kh, total);
-    DS_LAUNCH_OK("vae_image_hpass_kernel");
-    base = scr + p.inter;
-    pitch = 3LL * out_w;
-  }
+  const unsigned char* base;
+  long long pitch;
+  const int rc = vae_resample_begin<3>(src, H, W, out_h, out_w, p, scr, st, &base, &pitch);
+  if (rc != DS_OK) return rc;
   const long long hw = static_cast<long long>(out_h) * out_w;
   vae_image_vpass_kernel<<<static_cast<unsigned>((hw + 255) / 256), 256, 0, st>>>(
       base, pitch, reinterpret_cast<const int*>(scr + p.coef_v), p.kv, out_h, out_w, out,
@@ -507,5 +560,62 @@ extern "C" int ds_vae_image_pack(const float* x, float* out, void* out_nhwc4, in
   vae_image_pack_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       x, out, static_cast<uint2*>(out_nhwc4), HW, normalize, total);
   DS_LAUNCH_OK("vae_image_pack_kernel");
+  return DS_OK;
+}
+
+extern "C" int64_t ds_vae_mask_preprocess_scratch_bytes(int H, int W, int C, int out_h, int out_w) {
+  if (H < 1 || W < 1 || H > ds::kMaxSide || W > ds::kMaxSide || out_h < 1 || out_w < 1 || out_h > ds::kMaxSide ||
+      out_w > ds::kMaxSide || (C != 1 && C != 3))
+    return -1;
+  return ds::plan_vae(H, W, out_h, out_w, C).total;
+}
+
+extern "C" int ds_vae_mask_preprocess(const uint8_t* src, int H, int W, int C, int out_h, int out_w, float* out,
+                                      uint8_t* out_latent, void* scratch, int64_t scratch_bytes, void* stream) {
+  using namespace ds;
+  DS_REQUIRE(src && (out || out_latent), "ds_vae_mask_preprocess: bad arguments");
+  DS_REQUIRE(C == 1 || C == 3, "ds_vae_mask_preprocess: C must be 1 (L) or 3 (RGB), got %d", C);
+  DS_REQUIRE(H >= 1 && W >= 1 && H <= kMaxSide && W <= kMaxSide && out_h >= 1 && out_w >= 1 && out_h <= kMaxSide &&
+                 out_w <= kMaxSide,
+             "ds_vae_mask_preprocess: %d x %d -> %d x %d; sides must be in [1, %d]", H, W, out_h, out_w, kMaxSide);
+  DS_REQUIRE(!out_latent || (out_h % 8 == 0 && out_w % 8 == 0),
+             "ds_vae_mask_preprocess: the latent mask needs an output size that is a multiple of 8, got %d x %d", out_h,
+             out_w);
+  DS_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3) == 0, "ds_vae_mask_preprocess: out must be 4-byte aligned");
+  const VaePlan p = plan_vae(H, W, out_h, out_w, C);
+  DS_REQUIRE(p.total == 0 || (scratch && scratch_bytes >= p.total && (reinterpret_cast<uintptr_t>(scratch) & 15) == 0),
+             "ds_vae_mask_preprocess: needs %lld bytes of 16-byte aligned scratch "
+             "(ds_vae_mask_preprocess_scratch_bytes), got %lld", p.total, static_cast<long long>(scratch_bytes));
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  unsigned char* scr = static_cast<unsigned char*>(scratch);
+  const unsigned char* base;
+  long long pitch;
+  const int rc = C == 3 ? vae_resample_begin<3>(src, H, W, out_h, out_w, p, scr, st, &base, &pitch)
+                        : vae_resample_begin<1>(src, H, W, out_h, out_w, p, scr, st, &base, &pitch);
+  if (rc != DS_OK) return rc;
+  const long long hw = static_cast<long long>(out_h) * out_w;
+  const unsigned blocks = static_cast<unsigned>((hw + 255) / 256);
+  const int* coef_v = reinterpret_cast<const int*>(scr + p.coef_v);
+  if (C == 3)
+    vae_mask_vpass_kernel<3><<<blocks, 256, 0, st>>>(base, pitch, coef_v, p.kv, out_h, out_w, out, out_latent);
+  else
+    vae_mask_vpass_kernel<1><<<blocks, 256, 0, st>>>(base, pitch, coef_v, p.kv, out_h, out_w, out, out_latent);
+  DS_LAUNCH_OK("vae_mask_vpass_kernel");
+  return DS_OK;
+}
+
+extern "C" int ds_vae_mask_pack(const float* x, int H, int W, float* out, uint8_t* out_latent, void* stream) {
+  using namespace ds;
+  DS_REQUIRE(x && (out || out_latent) && H > 0 && W > 0, "ds_vae_mask_pack: bad arguments");
+  DS_REQUIRE(!out_latent || (H % 8 == 0 && W % 8 == 0),
+             "ds_vae_mask_pack: the latent mask needs a size that is a multiple of 8, got %d x %d", H, W);
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  const long long hw = static_cast<long long>(H) * W;
+  vae_mask_pack_kernel<<<static_cast<unsigned>((hw + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      x, out, out_latent, H, W);
+  DS_LAUNCH_OK("vae_mask_pack_kernel");
   return DS_OK;
 }

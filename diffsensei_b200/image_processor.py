@@ -122,11 +122,34 @@ class VaeImageProcessor:
         ``float32(u8) / 255`` and ``2x - 1``;
       * a float NCHW tensor of batch 1 must already be at a multiple-of-8 size (float inputs are not resized); it is
         normalised with ``2x - 1`` only if its minimum is >= 0, diffusers' rule.
+
+    The one other configuration is the inpaint mask processor of diffusers' SDXL inpaint pipeline,
+    ``VaeImageProcessor(vae_scale_factor=8, do_normalize=False, do_binarize=True, do_convert_grayscale=True)``.
+    Its ``preprocess(mask, height, width)`` returns fp32 [1, 1, h, w] in {0, 1} and ``preprocess_latent_mask`` the
+    uint8 [1, h / 8, w / 8] latent mask (``F.interpolate`` nearest), both from ``ds_vae_mask_preprocess``:
+      * a PIL image of mode "L" or "RGB", or a uint8 [H, W] / [H, W, 3] array / tensor (taken as that mode), is resized
+        with Pillow's LANCZOS filter in its own mode, then converted to "L", then binarised at 0.5 (``L >= 128``);
+      * a float tensor / array [1, 1, H, W] or [H, W] must already be at the target size and is binarised at 0.5.
+    Other PIL modes ("1", "P", "RGBA", "LA", ...) raise ``ValueError``: Pillow resizes them differently (nearest,
+    premultiplied alpha).  Any other combination of options raises ``ValueError``.
     """
-    defaults = dict(do_resize=True, vae_scale_factor=8, resample="lanczos", do_normalize=True)
+    defaults = dict(do_resize=True, vae_scale_factor=8, resample="lanczos", do_normalize=True, do_binarize=False,
+                    do_convert_grayscale=False)
+    mask_config = dict(defaults, do_normalize=False, do_binarize=True, do_convert_grayscale=True)
 
     def __init__(self, device: Optional[torch.device] = None, **kwargs):
-        _DeviceImageProcessor._check(self, kwargs)
+        for key in kwargs:
+            if key not in self.defaults:
+                raise ValueError(f"VaeImageProcessor: option {key!r} is not supported "
+                                 f"(supported: {sorted(self.defaults)})")
+        config = {**self.defaults, **{k: _canon(v) for k, v in kwargs.items()}}
+        self.is_mask = all(_canon(config[k]) == _canon(v) for k, v in self.mask_config.items())
+        want = self.mask_config if self.is_mask else self.defaults
+        for key, value in config.items():
+            if _canon(value) != _canon(want[key]):
+                raise ValueError(f"VaeImageProcessor: only the default configuration and the inpaint mask "
+                                 f"configuration (do_normalize=False, do_binarize=True, do_convert_grayscale=True) are "
+                                 f"supported; got {key}={value!r}")
         self.vae_scale_factor = 8
         self.device = device
 
@@ -152,6 +175,9 @@ class VaeImageProcessor:
         return height, width
 
     def _prepare(self, image, height, width, want_nchw: bool, want_nhwc4: bool):
+        if self.is_mask:
+            raise ValueError("VaeImageProcessor: this is the mask configuration; use preprocess / "
+                             "preprocess_latent_mask")
         dev = self.device or torch.device("cuda", torch.cuda.current_device())
         h, w = self.get_default_height_width(image, height, width)
         if self._is_float_tensor(image):
@@ -168,8 +194,56 @@ class VaeImageProcessor:
         return ops.vae_image_preprocess(u8, h, w, want_nchw=want_nchw, want_nhwc4=want_nhwc4)
 
     def preprocess(self, image, height: Optional[int] = None, width: Optional[int] = None) -> torch.Tensor:
+        if self.is_mask:
+            return self._prepare_mask(image, height, width, True, False)[0]
         return self._prepare(image, height, width, True, False)[0]
 
     def preprocess_nhwc4(self, image, height: Optional[int] = None, width: Optional[int] = None) -> torch.Tensor:
         """The same image as bf16 NHWC [1, h, w, 4] with a zero 4th channel: the encoder's conv_in input."""
         return self._prepare(image, height, width, False, True)[1]
+
+    # ---------------------------------------------------------------------------------- the mask configuration
+    @staticmethod
+    def mask_host(mask, height: int, width: int):
+        """The host-only half of the mask processor (no GPU work): checks ``mask`` against the panel size
+        ``height`` x ``width`` and returns ("u8", uint8 [H, W] or [H, W, 3] tensor) or ("float", fp32 [H, W] tensor),
+        both on the host unless the mask was already a device tensor.  Raises ``ValueError`` for an unsupported PIL
+        mode, dtype or shape, and for a float mask that is not at the panel size."""
+        if isinstance(mask, np.ndarray):
+            mask = torch.from_numpy(np.ascontiguousarray(mask))
+        elif not isinstance(mask, torch.Tensor):
+            if not hasattr(mask, "convert") or not hasattr(mask, "mode"):
+                raise ValueError(f"mask_image must be a PIL image, an array or a tensor, got {type(mask)}")
+            if mask.mode not in ("L", "RGB"):
+                raise ValueError(f"mask_image: PIL mode {mask.mode!r} is not supported (use 'L' or 'RGB'; Pillow "
+                                 "resizes other modes with different arithmetic)")
+            mask = torch.from_numpy(np.array(mask, dtype=np.uint8))
+        if mask.is_floating_point():
+            if not (mask.dim() == 2 or (mask.dim() == 4 and mask.shape[:2] == (1, 1))):
+                raise ValueError(f"a float mask must be [1, 1, H, W] or [H, W], got {tuple(mask.shape)}")
+            if tuple(mask.shape[-2:]) != (int(height), int(width)):
+                raise ValueError(f"a float mask is not resized: it must already be {height} x {width}, got "
+                                 f"{tuple(mask.shape[-2:])}")
+            return "float", mask.reshape(mask.shape[-2:])
+        if mask.dtype != torch.uint8 or not (mask.dim() == 2 or (mask.dim() == 3 and mask.shape[2] == 3)):
+            raise ValueError(f"a mask array / tensor must be uint8 [H, W] ('L') or [H, W, 3] ('RGB'), or float, got "
+                             f"{mask.dtype} {tuple(mask.shape)}")
+        return "u8", mask
+
+    def _prepare_mask(self, mask, height, width, want_mask: bool, want_latent: bool):
+        if not self.is_mask:
+            raise ValueError("VaeImageProcessor: masks need the mask configuration (do_normalize=False, "
+                             "do_binarize=True, do_convert_grayscale=True)")
+        dev = self.device or torch.device("cuda", torch.cuda.current_device())
+        if isinstance(mask, np.ndarray):
+            mask = torch.from_numpy(np.ascontiguousarray(mask))
+        h, w = self.get_default_height_width(mask, height, width)
+        kind, t = self.mask_host(mask, h, w)
+        if kind == "float":
+            return ops.vae_mask_pack(t.to(device=dev, dtype=torch.float32).contiguous(), want_mask, want_latent)
+        return ops.vae_mask_preprocess(t.to(dev).contiguous(), h, w, want_mask, want_latent)
+
+    def preprocess_latent_mask(self, mask, height: Optional[int] = None, width: Optional[int] = None) -> torch.Tensor:
+        """The mask at latent resolution, uint8 [1, h / 8, w / 8] in {0, 1}: ``F.interpolate(preprocess(mask),
+        size=(h / 8, w / 8))`` (nearest), i.e. pixel (8i, 8j), as diffusers' ``prepare_mask_latents``."""
+        return self._prepare_mask(mask, height, width, False, True)[1]

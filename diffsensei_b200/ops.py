@@ -595,6 +595,41 @@ def cfg_euler_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: t
                                 float(guidance), bs, H * W, Cc, _stream()), "ds_cfg_euler_step")
 
 
+def _inpaint_step(fn, name: str, ncoef: int, noise_pred, latents, model_in, coef, guidance, image_latents, noise,
+                  mask) -> None:
+    _req(noise_pred, bf16, f"{name}.noise_pred", 4)
+    _req(latents, f32, f"{name}.latents", 4)
+    _req(model_in, bf16, f"{name}.model_in", 4)
+    _req(coef, f32, f"{name}.coef", 1)
+    _req(image_latents, f32, f"{name}.image_latents", 4)
+    _req(noise, f32, f"{name}.noise", 4)
+    _req(mask, torch.uint8, f"{name}.mask", 3)
+    bs, H, W, Cc = latents.shape
+    if noise_pred.shape != (2 * bs, H, W, Cc) or model_in.shape != (2 * bs, H, W, Cc) or coef.numel() < ncoef or \
+            image_latents.shape != latents.shape or noise.shape != latents.shape or mask.shape != (bs, H, W):
+        raise DsEngineError(f"{name}: shape mismatch")
+    check(fn(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(), float(guidance),
+             image_latents.data_ptr(), noise.data_ptr(), mask.data_ptr(), bs, H * W, Cc, _stream()), f"ds_{name}")
+
+
+def cfg_ddim_inpaint_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
+                           guidance: float, image_latents: torch.Tensor, noise: torch.Tensor, mask: torch.Tensor) -> None:
+    """``cfg_ddim_step_`` followed by the inpaint blend: where ``mask`` (uint8 [bs,H,W]) is 0 the latents become
+    ``coef[2] * image_latents + coef[3] * noise`` (both fp32 NHWC [bs,H,W,4]); model_in is made from the blend.
+    coef: fp32 {alpha_prod_t, alpha_prod_t_prev, c0, c1} on the device."""
+    _inpaint_step(lib.ds_cfg_ddim_inpaint_step, "cfg_ddim_inpaint_step", 4, noise_pred, latents, model_in, coef,
+                  guidance, image_latents, noise, mask)
+
+
+def cfg_euler_inpaint_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor,
+                            coef: torch.Tensor, guidance: float, image_latents: torch.Tensor, noise: torch.Tensor,
+                            mask: torch.Tensor) -> None:
+    """``cfg_euler_step_`` followed by the inpaint blend (see ``cfg_ddim_inpaint_step_``); model_in is the blend
+    divided by coef[2].  coef: fp32 {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1), c0, c1} on the device."""
+    _inpaint_step(lib.ds_cfg_euler_inpaint_step, "cfg_euler_inpaint_step", 5, noise_pred, latents, model_in, coef,
+                  guidance, image_latents, noise, mask)
+
+
 # ---------------------------------------------------------------------------------------------- encoder helpers
 def attention_small(qkv: torch.Tensor, heads: int, causal: bool = False, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """softmax(Q K^T / sqrt(d) [+ causal]) V from a fused projection ``qkv`` [B, N, 3*heads*d] (N <= 320, d % 8 == 0,
@@ -1074,6 +1109,49 @@ def vae_image_pack(x: torch.Tensor, normalize: bool, want_nchw: bool = True, wan
     check(lib.ds_vae_image_pack(x.data_ptr(), _ptr(nchw), _ptr(nhwc4), B, H * W, int(bool(normalize)), _stream()),
           "ds_vae_image_pack")
     return nchw, nhwc4
+
+
+def vae_mask_preprocess(img: torch.Tensor, out_h: int, out_w: int, want_mask: bool = True, want_latent: bool = True):
+    """The inpaint mask processor of one uint8 HWC image ``img`` (CUDA), [H, W] / [H, W, 1] ("L") or [H, W, 3] ("RGB"):
+    Pillow LANCZOS resize to (out_h, out_w) in its own mode, RGB -> L, ``>= 128``.  Returns (fp32 [1, 1, out_h, out_w]
+    in {0, 1}, uint8 [1, out_h / 8, out_w / 8] latent mask), None where not asked."""
+    _req(img, torch.uint8, "vae_mask_preprocess.img")
+    if img.dim() == 2:
+        img = img.unsqueeze(-1)
+    if img.dim() != 3 or img.shape[2] not in (1, 3):
+        raise DsEngineError(f"vae_mask_preprocess: img must be uint8 [H, W], [H, W, 1] or [H, W, 3], got "
+                            f"{tuple(img.shape)}")
+    H, W, c = img.shape
+    out_h, out_w = int(out_h), int(out_w)
+    need = int(lib.ds_vae_mask_preprocess_scratch_bytes(H, W, c, out_h, out_w))
+    if need < 0:
+        raise DsEngineError(f"vae_mask_preprocess: unsupported sizes {H} x {W} -> {out_h} x {out_w} "
+                            "(sides must be in [1, 65535])")
+    mask, lat = _mask_outputs("vae_mask_preprocess", out_h, out_w, want_mask, want_latent, img.device)
+    scratch = torch.empty(max(need, 16), dtype=torch.uint8, device=img.device)
+    check(lib.ds_vae_mask_preprocess(img.data_ptr(), H, W, c, out_h, out_w, _ptr(mask), _ptr(lat), scratch.data_ptr(),
+                                     scratch.numel(), _stream()), "ds_vae_mask_preprocess")
+    return mask, lat
+
+
+def vae_mask_pack(x: torch.Tensor, want_mask: bool = True, want_latent: bool = True):
+    """A float mask already at its size, fp32 [H, W] (CUDA) -> (``x >= 0.5`` as fp32 [1, 1, H, W], uint8
+    [1, H / 8, W / 8] latent mask), None where not asked."""
+    _req(x, f32, "vae_mask_pack.x", 2)
+    H, W = x.shape
+    mask, lat = _mask_outputs("vae_mask_pack", H, W, want_mask, want_latent, x.device)
+    check(lib.ds_vae_mask_pack(x.data_ptr(), H, W, _ptr(mask), _ptr(lat), _stream()), "ds_vae_mask_pack")
+    return mask, lat
+
+
+def _mask_outputs(name: str, H: int, W: int, want_mask: bool, want_latent: bool, dev):
+    if not (want_mask or want_latent):
+        raise DsEngineError(f"{name}: nothing to compute")
+    if want_latent and (H % 8 or W % 8):
+        raise DsEngineError(f"{name}: the latent mask needs a size that is a multiple of 8, got {H} x {W}")
+    mask = torch.empty(1, 1, H, W, dtype=f32, device=dev) if want_mask else None
+    lat = torch.empty(1, H // 8, W // 8, dtype=torch.uint8, device=dev) if want_latent else None
+    return mask, lat
 
 
 launch_count = _lib.launch_count

@@ -15,6 +15,11 @@ passed instead; a raw prompt or image without what it needs raises, it does not 
 ``generate_page`` runs the panels of a page together (one front-end pass, one denoise per group of same-size panels).
 ``image=`` / ``strength=`` start a panel from an image as diffusers' ``StableDiffusionXLImg2ImgPipeline`` does (needs
 ``vae_encoder=``): the image is encoded, noised to the schedule's step ``t_start`` and denoised from there.
+``mask_image=`` with ``image=`` redraws only the masked part, as diffusers' ``StableDiffusionXLInpaintPipeline`` does
+with a 4-channel UNet: after every step the unmasked latent pixels are reset to the image latents noised to the next
+timestep (fused into the step kernel, ``ds_cfg_*_inpaint_step``).  Departures from that pipeline's defaults: the
+panel size follows the img2img rule (the given ``height`` / ``width``, else the image's own; diffusers defaults to
+1024 x 1024), and ``strength`` keeps its 0.3 default (diffusers' inpaint default is 0.9999).
 
 Loop structure on the GPU (one process per GPU, one stream):
   once per panel : K|V projections of text and IP tokens for all cross-attention layers, time-embedding
@@ -48,14 +53,15 @@ PANEL_KEYS = frozenset({
     "latents", "original_size", "crops_coords_top_left", "target_size", "min_size_step", "ip_images",
     "ip_image_embeds", "clip_image_embeds", "magi_image_embeds", "clip_pixel_values", "magi_pixel_values", "ip_bbox",
     "dialog_bbox", "prompt_embeds", "negative_prompt_embeds", "pooled_prompt_embeds", "negative_pooled_prompt_embeds",
-    "prompt_input_ids", "prompt_input_ids_2", "negative_prompt_input_ids", "negative_prompt_input_ids_2", "image"})
+    "prompt_input_ids", "prompt_input_ids_2", "negative_prompt_input_ids", "negative_prompt_input_ids_2", "image",
+    "mask_image"})
 PAGE_MAX_ROWS = 8       # samples per page denoise: a UNet batch of 16 rows, as __call__(num_samples=8)
 
 
 def plan_page(shapes, max_batch_panels: int = PAGE_MAX_ROWS) -> List[List[int]]:
     """The denoise chunks of a page.  ``shapes`` holds one (num_samples, h, w) per panel, h x w its latent size, with
-    optional further entries that must also match for two panels to share a denoise (an img2img panel adds one: it
-    runs a different slice of the schedule).  Panels of one key form a group, groups in order of first appearance; a
+    optional further entries that must also match for two panels to share a denoise (an img2img or inpaint panel
+    adds one: it runs a different slice of the schedule, and an inpaint panel a different step kernel).  Panels of one key form a group, groups in order of first appearance; a
     group splits into consecutive chunks of at most ``max_batch_panels`` samples, and a panel's samples are never split
     (a panel with more samples than the cap is a chunk of its own).  Returns the panel indices of every chunk."""
     cap = int(max_batch_panels)
@@ -117,6 +123,8 @@ class DiffSenseiPipeline:
         self.vae = vae                      # VaeDecoderEngine (or None: latents out only)
         self.vae_encoder = vae_encoder      # VaeEncoderEngine (or None: no image= / img2img)
         self.vae_image_processor = VaeImageProcessor()
+        self.mask_processor = VaeImageProcessor(vae_scale_factor=8, do_normalize=False, do_binarize=True,
+                                                do_convert_grayscale=True)
         self.text_encoder = text_encoder    # ClipTextEncoderEngine (CLIP-L) / (OpenCLIP bigG, with projection)
         self.text_encoder_2 = text_encoder_2
         self.image_encoder = image_encoder  # ClipVisionEncoderEngine (ViT-H/14)
@@ -284,45 +292,55 @@ class DiffSenseiPipeline:
     def make_stepper(self, latents: torch.Tensor, prompt_embeds: torch.Tensor, add_text_embeds: torch.Tensor,
                      add_time_ids: torch.Tensor, bbox: torch.Tensor, aspect_ratio: float,
                      dialog_bbox: Optional[torch.Tensor], num_inference_steps: int, guidance_scale: float,
-                     use_graph: bool = True, chains: Optional[int] = None, start_index: int = 0) -> "DenoiseStepper":
+                     use_graph: bool = True, chains: Optional[int] = None, start_index: int = 0,
+                     inpaint=None) -> "DenoiseStepper":
         return DenoiseStepper(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
-                              dialog_bbox, num_inference_steps, guidance_scale, use_graph, chains, start_index)
+                              dialog_bbox, num_inference_steps, guidance_scale, use_graph, chains, start_index,
+                              inpaint)
 
     def stepper_for(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio, dialog_bbox,
-                    num_inference_steps, guidance_scale, chains=None, start_index: int = 0) -> "DenoiseStepper":
+                    num_inference_steps, guidance_scale, chains=None, start_index: int = 0,
+                    inpaint=None) -> "DenoiseStepper":
         """A graph-captured stepper loaded with this panel: a cached one of the same key is refilled in place
         (no re-capture), otherwise a new one is built and cached.  The start index is part of the key: the stepper
-        bakes in its slice of the schedule (``set_timesteps`` would reset any scheduler state)."""
+        bakes in its slice of the schedule (``set_timesteps`` would reset any scheduler state); so is whether it
+        inpaints, which selects the step kernel."""
         key = (tuple(latents.shape), tuple(prompt_embeds.shape), None if dialog_bbox is None else
                (tuple(dialog_bbox.shape), dialog_bbox.dtype == bf16), float(aspect_ratio), int(num_inference_steps),
                float(guidance_scale), self.unet.scales_key(), chains, self.unet._ip_weights_version(),
-               type(self.scheduler).__name__, tuple(sorted(self.scheduler.config.items())), int(start_index))
+               type(self.scheduler).__name__, tuple(sorted(self.scheduler.config.items())), int(start_index),
+               inpaint is not None)
         st = self._steppers.get(key)
         if st is None:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
-                                   dialog_bbox, num_inference_steps, guidance_scale, True, chains, start_index)
+                                   dialog_bbox, num_inference_steps, guidance_scale, True, chains, start_index,
+                                   inpaint)
             while len(self._steppers) >= self.max_cached_steppers:
                 self._steppers.pop(next(iter(self._steppers)))
             self._steppers[key] = st
         else:
-            st.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox)
+            st.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox, inpaint)
         return st
 
     @torch.no_grad()
     def denoise(self, latents: torch.Tensor, prompt_embeds: torch.Tensor, add_text_embeds: torch.Tensor,
                 add_time_ids: torch.Tensor, bbox: torch.Tensor, aspect_ratio: float,
                 dialog_bbox: Optional[torch.Tensor], num_inference_steps: int, guidance_scale: float,
-                use_graph: bool = True, on_step=None, start_index: int = 0) -> torch.Tensor:
+                use_graph: bool = True, on_step=None, start_index: int = 0, inpaint=None) -> torch.Tensor:
         """pipeline_diffsensei.py:306-337.  ``latents`` NCHW fp32 (bs,4,h,w); conditions already concatenated
         [negative ; positive] along batch (:293-304).  ``start_index``: run steps start_index .. T-1 of the
-        ``num_inference_steps`` schedule (img2img; ``on_step`` then counts from 0).  Returns the final latents, NCHW
-        fp32."""
+        ``num_inference_steps`` schedule (img2img; ``on_step`` then counts from 0).  ``inpaint``: (image_latents fp32
+        (bs,4,h,w), noise fp32 (bs,4,h,w), latent mask uint8 (bs,h,w)); after every step the pixels where the mask is
+        0 become the image latents noised to the next timestep (the image latents on the last step).  Returns the
+        final latents, NCHW fp32."""
         if use_graph:
             st = self.stepper_for(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
-                                  dialog_bbox, num_inference_steps, guidance_scale, start_index=start_index)
+                                  dialog_bbox, num_inference_steps, guidance_scale, start_index=start_index,
+                                  inpaint=inpaint)
         else:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
-                                   dialog_bbox, num_inference_steps, guidance_scale, False, start_index=start_index)
+                                   dialog_bbox, num_inference_steps, guidance_scale, False, start_index=start_index,
+                                   inpaint=inpaint)
         for i, t in enumerate(st.timesteps):
             st.step(i)
             if on_step is not None:
@@ -346,11 +364,16 @@ class DiffSenseiPipeline:
                  # ... or the INPUTS of those encoders, when the engines are registered (token ids / pixel values):
                  prompt_input_ids=None, prompt_input_ids_2=None, negative_prompt_input_ids=None,
                  negative_prompt_input_ids_2=None, clip_pixel_values=None, magi_pixel_values=None,
-                 # img2img (diffusers' StableDiffusionXLImg2ImgPipeline): start from this image at `strength`
-                 image=None, strength: float = 0.3):
+                 # img2img (diffusers' StableDiffusionXLImg2ImgPipeline): start from this image at `strength`;
+                 # with mask_image, inpaint (StableDiffusionXLInpaintPipeline): redraw only where the mask is white
+                 image=None, strength: float = 0.3, mask_image=None):
         t_start = 0
+        if mask_image is not None and image is None:
+            raise ValueError("`mask_image` needs `image`: inpainting redraws the masked part of that image")
         if image is not None:
             t_start, height, width = self._check_image(image, latents, strength, num_inference_steps, height, width)
+            if mask_image is not None:
+                self.mask_processor.mask_host(mask_image, height, width)
         height = height or self.default_sample_size * self.vae_scale_factor
         width = width or self.default_sample_size * self.vae_scale_factor
         original_size = original_size or (height, width)
@@ -406,7 +429,13 @@ class DiffSenseiPipeline:
         self.set_ip_scale(ip_scale)
         dev = self.unet.device
         self.scheduler.set_timesteps(num_inference_steps, device=dev)    # :248 (init_noise_sigma depends on it)
-        if image is not None:                                            # img2img prepare_latents (add_noise=True)
+        inpaint = None
+        if image is not None and mask_image is not None:                 # inpaint prepare_latents + mask latents
+            moments = self.vae_encoder.moments_nhwc(self.vae_image_processor.preprocess_nhwc4(image, height, width))
+            eps, noise = self._draw_inpaint_noise(moments.shape[1], moments.shape[2], num_samples, generator)
+            mask = self.mask_processor.preprocess_latent_mask(mask_image, height, width)
+            latents, inpaint = self._inpaint_start(moments, eps, noise, mask, num_samples, t_start, strength)
+        elif image is not None:                                          # img2img prepare_latents (add_noise=True)
             latents = self.vae_encoder.encode_latents(self.vae_image_processor.preprocess_nhwc4(image, height, width),
                                                       generator, num_samples,
                                                       self.scheduler.add_noise_coefficients(t_start, dev))
@@ -427,12 +456,35 @@ class DiffSenseiPipeline:
         pe = torch.cat([pe, torch.cat([neg_img, img], dim=0)], dim=1)                              # :297,303
         final = self.denoise(latents, pe, te, ti, torch.cat([neg_bbox, bbox], dim=0), aspect_ratio,
                              torch.cat([neg_db, db], dim=0), num_inference_steps, guidance_scale, use_graph=use_graph,
-                             start_index=t_start)
+                             start_index=t_start, inpaint=inpaint)
         if output_type == "latent":
             return SimpleNamespace(images=final, latents=final)
         # pipeline_diffsensei.py:339-363: latents / scaling_factor -> vae.decode -> image_processor.postprocess
         image = self.vae.decode_image(final)                                            # fp32 NCHW in [0, 1]
         return SimpleNamespace(images=_postprocess(image, output_type), latents=final)
+
+    def _draw_inpaint_noise(self, h: int, w: int, num_samples: int, generator):
+        """The generator draws of diffusers' 4-channel inpaint pipeline, in its order: the posterior sample's randn
+        [1, 4, h, w], the latent noise randn [num_samples, 4, h, w], then the masked image's posterior sample, which
+        diffusers draws and discards for a 4-channel UNet (drawn and dropped here, without running the encoder, so
+        the generator ends in the same state).  Returns (eps, noise)."""
+        eps, noise = self.vae_encoder.draw_noise(h, w, num_samples, generator)
+        self.vae_encoder.draw_noise(h, w, num_samples, generator, add_noise=False)
+        return eps, noise
+
+    def _inpaint_start(self, moments, eps, noise, mask, num_samples: int, t_start: int, strength: float):
+        """The start latents of one inpaint panel and the state its loop blends with: image_latents =
+        ``scaling_factor * sample`` repeated to ``num_samples``; latents = ``add_noise(image_latents, noise,
+        timesteps[t_start])``, or ``noise * init_noise_sigma`` (pure noise) at strength 1.  Returns (latents,
+        (image_latents, noise, mask repeated to num_samples))."""
+        enc = self.vae_encoder
+        z = enc.latents_from_moments(moments, eps, num_samples)
+        if float(strength) == 1.0:
+            latents = noise * self.scheduler.init_noise_sigma
+        else:
+            latents = enc.latents_from_moments(moments, eps, num_samples, noise,
+                                               self.scheduler.add_noise_coefficients(t_start, self.unet.device))
+        return latents, (z, noise, mask.repeat(num_samples, 1, 1))
 
     def _check_image(self, image, latents, strength, num_inference_steps, height, width):
         """The host-only checks of ``image=`` (before any GPU work).  Returns (t_start, height, width): the first step
@@ -486,7 +538,10 @@ class DiffSenseiPipeline:
 
         A panel with ``image`` starts from that image at the page's ``strength``, as ``__call__(image=...)`` does: it
         draws the posterior sample's noise, then the latent noise, at its turn in panel order; same-size images are
-        encoded in one batch; img2img panels never share a denoise with text-to-image panels."""
+        encoded in one batch; img2img panels never share a denoise with text-to-image panels.  A panel with ``image``
+        and ``mask_image`` inpaints, as ``__call__(image=..., mask_image=...)`` does: it draws the posterior sample's
+        noise, the latent noise and the discarded masked-image sample at its turn; inpaint panels share a denoise only
+        with inpaint panels of the same latent size."""
         if not isinstance(panels, (list, tuple)) or len(panels) == 0:
             raise ValueError("generate_page needs a non-empty list of panel dicts")
         panels = [dict(p) for p in panels]
@@ -547,22 +602,27 @@ class DiffSenseiPipeline:
         self.scheduler.set_timesteps(num_inference_steps, device=dev)
         for j in jobs:                                                     # panel order: the global RNG's order
             if j.image is not None:
-                j.eps, j.noise = self.vae_encoder.draw_noise(j.height // self.vae_scale_factor,
-                                                             j.width // self.vae_scale_factor, j.ns, j.generator)
+                draw = self._draw_inpaint_noise if j.mask_image is not None else self.vae_encoder.draw_noise
+                j.eps, j.noise = draw(j.height // self.vae_scale_factor, j.width // self.vae_scale_factor, j.ns,
+                                      j.generator)
             elif j.latents is None:
                 j.latents = self.prepare_latents(j.ns, self.unet.config.in_channels, j.height, j.width, j.generator)
             else:
                 j.latents = j.latents * self.scheduler.init_noise_sigma
-        self._encode_page_latents([j for j in jobs if j.image is not None], t_start)
+        self._encode_page_latents([j for j in jobs if j.image is not None], t_start, strength)
         results = [None] * len(jobs)
-        shapes = [(j.ns,) + tuple(j.latents.shape[-2:]) + (("image",) if j.image is not None else ()) for j in jobs]
+        kind = lambda j: () if j.image is None else ("inpaint",) if j.mask_image is not None else ("image",)
+        shapes = [(j.ns,) + tuple(j.latents.shape[-2:]) + kind(j) for j in jobs]
         for chunk in plan_page(shapes, max_batch_panels):
             rows = [self._panel_rows(jobs[i]) for i in chunk]
             cat = lambda k: torch.cat([r[0][k] for r in rows] + [r[1][k] for r in rows], dim=0)
             lat = torch.cat([jobs[i].latents for i in chunk], dim=0)
+            inpaint = None
+            if jobs[chunk[0]].inpaint is not None:
+                inpaint = tuple(torch.cat([jobs[i].inpaint[k] for i in chunk], dim=0) for k in range(3))
             final = self.denoise(lat, cat("pe"), cat("te"), cat("ti"), cat("bbox"), lat.shape[-2] / lat.shape[-1],
                                  cat("db"), num_inference_steps, guidance_scale, use_graph=use_graph,
-                                 start_index=t_start if jobs[chunk[0]].image is not None else 0)
+                                 start_index=t_start if jobs[chunk[0]].image is not None else 0, inpaint=inpaint)
             image = self.vae.decode_image(final) if output_type != "latent" else final
             r0 = 0
             for i in chunk:
@@ -571,16 +631,21 @@ class DiffSenseiPipeline:
                 r0 = r1
         return results
 
-    def _encode_page_latents(self, jobs, t_start: int) -> None:
-        """The img2img panels' initial latents: every image processed to its panel size, same-size images through
-        the encoder in one batch, then each panel's posterior sample + add_noise from the noise it drew."""
+    def _encode_page_latents(self, jobs, t_start: int, strength: float) -> None:
+        """The img2img and inpaint panels' initial latents: every image processed to its panel size, same-size images
+        through the encoder in one batch, then each panel's posterior sample + add_noise from the noise it drew (and,
+        for inpaint panels, the state the loop blends with)."""
         if not jobs:
             return
         for j in jobs:
             j.x4 = self.vae_image_processor.preprocess_nhwc4(j.image, j.height, j.width)
         coef = self.scheduler.add_noise_coefficients(t_start, self.unet.device)
         for j, (m,) in zip(jobs, _stacked(lambda x4: (self.vae_encoder.moments_nhwc(x4),), [j.x4 for j in jobs])):
-            j.latents = self.vae_encoder.latents_from_moments(m, j.eps, j.ns, j.noise, coef)
+            if j.mask_image is not None:
+                mask = self.mask_processor.preprocess_latent_mask(j.mask_image, j.height, j.width)
+                j.latents, j.inpaint = self._inpaint_start(m, j.eps, j.noise, mask, j.ns, t_start, strength)
+            else:
+                j.latents = self.vae_encoder.latents_from_moments(m, j.eps, j.ns, j.noise, coef)
 
     def _panel_job(self, i: int, p: dict) -> SimpleNamespace:
         """One panel's arguments resolved as ``__call__`` resolves them, with its ValueErrors prefixed by the panel
@@ -588,9 +653,13 @@ class DiffSenseiPipeline:
         g = lambda k, d=None: p.get(k, d)
         try:
             height, width = g("height"), g("width")
+            if g("mask_image") is not None and g("image") is None:
+                raise ValueError("`mask_image` needs `image`: inpainting redraws the masked part of that image")
             if g("image") is not None:
                 # the page's strength was checked already: only the panel's own image checks can fail here
                 _, height, width = self._check_image(g("image"), g("latents"), 1.0, 1, height, width)
+                if g("mask_image") is not None:
+                    self.mask_processor.mask_host(g("mask_image"), height, width)
             height = height or self.default_sample_size * self.vae_scale_factor
             width = width or self.default_sample_size * self.vae_scale_factor
             ip_images, ip_bbox = list(g("ip_images", ())), list(g("ip_bbox", ()))
@@ -650,7 +719,7 @@ class DiffSenseiPipeline:
         ns = int(g("num_samples", 1))
         return SimpleNamespace(
             index=i, ns=ns, height=height, width=width, generator=g("generator"), latents=g("latents"), ids=ids,
-            image=g("image"),
+            image=g("image"), mask_image=g("mask_image"), inpaint=None,
             pe=g("prompt_embeds"), npe=g("negative_prompt_embeds"), pp=g("pooled_prompt_embeds"),
             npp=g("negative_pooled_prompt_embeds"), ip_images=ip_images, clip_pv=clip_pv, magi_pv=magi_pv,
             clip=g("clip_image_embeds"), magi=g("magi_image_embeds"), ip_image_embeds=ip_image_embeds,
@@ -795,12 +864,14 @@ class DenoiseStepper:
     ``step(i)`` runs iteration i on device-resident latents; ``step_host(i, x)`` is the same call with HOST
     buffers (pinned fp32 NCHW latents in, updated latents out), i.e. what a caller on the other side of the
     plugin boundary sees.
+    With ``inpaint`` = (image_latents, noise, latent mask) the step is the scheduler's ``fused_inpaint_step_``, which
+    reads those three per-panel buffers and the inpaint coefficient table.
     """
 
     @torch.no_grad()
     def __init__(self, pipe: DiffSenseiPipeline, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox,
                  aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale, use_graph=True, chains=None,
-                 start_index: int = 0):
+                 start_index: int = 0, inpaint=None):
         unet, dev = pipe.unet, pipe.unet.device
         self.unet, self.dev, self.guidance = unet, dev, float(guidance_scale)
         self.scheduler = pipe.scheduler
@@ -811,14 +882,19 @@ class DenoiseStepper:
         if not 0 <= s0 < self.num_inference_steps:
             raise ValueError(f"start_index must be in [0, {self.num_inference_steps}), got {start_index}")
         self.timesteps = pipe.scheduler.set_timesteps(num_inference_steps, device=dev)[s0:]
-        self.coef_table = pipe.scheduler.coefficient_table(dev)[s0:]                    # [T, 2] DDIM, [T, 3] Euler
+        self.inpaint = inpaint is not None
+        if self.inpaint:                                                                # [T, 4] DDIM, [T, 5] Euler
+            self.coef_table = pipe.scheduler.inpaint_coefficient_table(s0, dev)
+        else:
+            self.coef_table = pipe.scheduler.coefficient_table(dev)[s0:]                # [T, 2] DDIM, [T, 3] Euler
         # scale_model_input's divisor per step; dividing by a device element is a true division, as in the kernels
         self.in_div = torch.tensor(pipe.scheduler.model_input_divisors()[s0:], dtype=f32, device=dev)
         self.cond = None
         self.lat = self.model_in = self.db = self.temb_table = None
+        self.inp_z = self.inp_n = self.inp_m = None
         self.round_bf16 = True
         self.graph = None
-        self.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox)
+        self.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox, inpaint)
         self.temb_cur = self.temb_table[0].clone()
         self.coef_cur = self.coef_table[0].clone()
         self._host_in = None
@@ -853,14 +929,32 @@ class DenoiseStepper:
             self.model_in.copy_(min0)
 
     @torch.no_grad()
-    def load_panel(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox) -> None:
+    def load_panel(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox,
+                   inpaint=None) -> None:
         """Everything that is per panel and timestep-invariant, written INTO the buffers the captured graph reads:
         K|V of the text / IP tokens for all cross-attention layers, the time-embedding row-bias table for all T
-        steps, the bbox tables, the initial latents.  First call allocates; later calls (same shapes) refill."""
+        steps, the bbox tables, the initial latents, and the inpaint state.  First call allocates; later calls (same
+        shapes) refill."""
         unet, dev = self.unet, self.dev
         bs = latents.shape[0]
         if prompt_embeds.shape[0] != 2 * bs:
             raise ValueError("denoise expects CFG-concatenated conditions: prompt_embeds.shape[0] == 2 * num_samples")
+        if (inpaint is not None) != self.inpaint:
+            raise ValueError("load_panel: inpaint state presence differs from the stepper's")
+        if inpaint is not None:
+            z, n, m = inpaint
+            if tuple(z.shape) != tuple(latents.shape) or tuple(n.shape) != tuple(latents.shape) or \
+                    tuple(m.shape) != (bs,) + tuple(latents.shape[-2:]):
+                raise ValueError("inpaint: image_latents / noise must have the latents' shape and the mask "
+                                 "(num_samples, h, w)")
+            nhwc = lambda t: t.to(device=dev, dtype=f32).permute(0, 2, 3, 1).contiguous()
+            z, n, m = nhwc(z), nhwc(n), m.to(device=dev, dtype=torch.uint8).contiguous()
+            if self.inp_z is None:
+                self.inp_z, self.inp_n, self.inp_m = z, n, m
+            else:
+                self.inp_z.copy_(z)
+                self.inp_n.copy_(n)
+                self.inp_m.copy_(m)
         self.cond = unet.prepare_conditions(prompt_embeds.to(dev), bbox, self.aspect_ratio, out=self.cond)
         self.temb_table = unet.time_rowbias_table(self.timesteps, add_text_embeds, add_time_ids)   # [T, 2bs, sumC]
         lat = latents.to(device=dev, dtype=f32).permute(0, 2, 3, 1).contiguous()         # fp32 NHWC master copy
@@ -909,7 +1003,11 @@ class DenoiseStepper:
             finally:
                 ops.SPLITK = prev_splitk
                 ops.GEMM_CHAINS = prev_chains
-        self.scheduler.fused_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance)  # :332-337, :315-317
+        if self.inpaint:
+            self.scheduler.fused_inpaint_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance, self.inp_z,
+                                               self.inp_n, self.inp_m)
+        else:
+            self.scheduler.fused_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance)  # :332-337,:315-317
 
     @torch.no_grad()
     def step(self, i: int) -> None:

@@ -10,6 +10,8 @@ stable-diffusion-xl-base-1.0 (scaled_linear betas 0.00085..0.012 over 1000 train
 
 For img2img both add ``add_noise`` (diffusers' API, torch fp32), ``add_noise_coefficients`` (the same arithmetic as the
 two fp32 factors ``ds_vae_posterior`` reads) and ``set_begin_index``; ``get_timesteps`` is the strength rule.
+For inpainting, ``inpaint_coefficient_table`` adds each step's ``add_noise`` factors at the next timestep to the
+coefficient table, and ``fused_inpaint_step_`` runs the update with the blend (``ds_cfg_*_inpaint_step``).
 
 ``scheduler_from_config`` picks one from a checkpoint's ``scheduler/scheduler_config.json``, the way diffusers does,
 and rejects any class or value whose arithmetic is not implemented here.
@@ -25,6 +27,19 @@ from typing import List, Tuple
 import torch
 
 from . import ops
+
+def _inpaint_table(sched, start_index: int, device) -> torch.Tensor:
+    """``coefficient_table`` rows start_index .. T-1 with two more columns: the {c0, c1} of
+    ``add_noise(image_latents, noise, timesteps[i + 1])`` (``add_noise_coefficients(i + 1)``), and {1, 0} on the last
+    step, where diffusers' inpaint loop keeps the image latents themselves."""
+    n = len(sched.timesteps)
+    s0 = int(start_index)
+    if not 0 <= s0 < n:
+        raise ValueError(f"start_index must be in [0, {n}), got {start_index}")
+    last = torch.tensor([1.0, 0.0], dtype=torch.float32)
+    c = torch.stack([sched.add_noise_coefficients(i + 1) if i + 1 < n else last for i in range(s0, n)])
+    return torch.cat([sched.coefficient_table("cpu")[s0:], c], dim=1).to(device)
+
 
 # stable-diffusion-xl-base-1.0 scheduler/scheduler_config.json, the values both classes implement
 _SDXL = {"num_train_timesteps": 1000, "beta_start": 0.00085, "beta_end": 0.012, "beta_schedule": "scaled_linear",
@@ -73,6 +88,15 @@ class DDIMScheduler:
 
     def fused_step_(self, noise_pred, latents, model_in, coef, guidance: float) -> None:
         ops.cfg_ddim_step_(noise_pred, latents, model_in, coef, guidance)
+
+    def inpaint_coefficient_table(self, start_index: int, device) -> torch.Tensor:
+        """fp32 [T - start_index, 4] device tensor of (alpha_prod_t, alpha_prod_t_prev, c0, c1) for the inpaint loop
+        (``fused_inpaint_step_``): c0 / c1 as ``add_noise_coefficients`` at the next step, {1, 0} on the last."""
+        return _inpaint_table(self, start_index, device)
+
+    def fused_inpaint_step_(self, noise_pred, latents, model_in, coef, guidance: float, image_latents, noise,
+                            mask) -> None:
+        ops.cfg_ddim_inpaint_step_(noise_pred, latents, model_in, coef, guidance, image_latents, noise, mask)
 
     def set_begin_index(self, begin_index: int = 0) -> None:
         """The loop's first step (img2img); DDIM's arithmetic does not depend on it, only add_noise's timestep."""
@@ -142,6 +166,16 @@ class EulerDiscreteScheduler:
 
     def fused_step_(self, noise_pred, latents, model_in, coef, guidance: float) -> None:
         ops.cfg_euler_step_(noise_pred, latents, model_in, coef, guidance)
+
+    def inpaint_coefficient_table(self, start_index: int, device) -> torch.Tensor:
+        """fp32 [T - start_index, 5] device tensor of (sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1), c0, c1) for the
+        inpaint loop: {c0, c1} = {1, sigma_{i+1}}, the sigma diffusers' ``add_noise`` reads through the step index
+        that ``step`` has already advanced, and {1, 0} on the last step."""
+        return _inpaint_table(self, start_index, device)
+
+    def fused_inpaint_step_(self, noise_pred, latents, model_in, coef, guidance: float, image_latents, noise,
+                            mask) -> None:
+        ops.cfg_euler_inpaint_step_(noise_pred, latents, model_in, coef, guidance, image_latents, noise, mask)
 
     def set_begin_index(self, begin_index: int = 0) -> None:
         """diffusers' ``set_begin_index``: the loop starts at sigma_{begin_index} (img2img)."""

@@ -329,6 +329,27 @@ int ds_cfg_ddim_step(const void* noise_pred, float* latents, void* model_in, con
 int ds_cfg_euler_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
                       int bs, int HW, int C, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * The two updates above followed by the inpaint blend of diffusers' StableDiffusionXLInpaintPipeline with a
+ * 4-channel UNet, fused.                                                           [HBM-bound]
+ *   init  = c0 * z + c1 * n        (add_noise of the image latents at the next timestep; {1, 0} on the last step;
+ *                                   each product and the sum rounded on its own)
+ *   x_new = mask ? x_new : init    ((1 - m) * init + m * x_new with a binary m)
+ * and the next UNet input is computed from the blended x_new.  A pixel with mask != 0 is the plain kernel's result
+ * bit for bit.
+ *   coef          : DDIM {alpha_prod_t, alpha_prod_t_prev, c0, c1}; Euler {sigma, sigma_next,
+ *                   sqrt(sigma_next^2 + 1), c0, c1} (device pointer)
+ *   image_latents : fp32 NHWC [bs][H][W][4] (z, scaling_factor * posterior sample), 16-byte aligned
+ *   noise         : fp32 NHWC [bs][H][W][4] (n, the noise the start latents were drawn with), 16-byte aligned
+ *   mask          : uint8 [bs][H][W], 1 = regenerate, 0 = keep the image
+ * --------------------------------------------------------------------------------------------- */
+int ds_cfg_ddim_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
+                             const float* image_latents, const float* noise, const uint8_t* mask, int bs, int HW,
+                             int C, void* stream);
+int ds_cfg_euler_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
+                              float guidance, const float* image_latents, const float* noise, const uint8_t* mask,
+                              int bs, int HW, int C, void* stream);
+
 /* Perceiver attention of the character Resampler: 16 latent queries x (n_kv) keys per (character, head),
  * q and k each pre-scaled by dim_head^-0.25, fp32 softmax (src/models/resampler.py:64-74).
  *   q: bf16 [Bc][nq][C], kv: bf16 [Bc][n_kv][2*C] (k | v), out: bf16 [Bc][nq][C]; C = heads*64 */
@@ -430,6 +451,23 @@ int64_t ds_vae_image_preprocess_scratch_bytes(int H, int W, int out_h, int out_w
 int ds_vae_image_preprocess(const uint8_t* src, int H, int W, int out_h, int out_w, float* out, void* out_nhwc4,
                             void* scratch, int64_t scratch_bytes, void* stream);
 int ds_vae_image_pack(const float* x, float* out, void* out_nhwc4, int B, int HW, int normalize, void* stream);
+
+/* Inpaint mask preprocessing (diffusers VaeImageProcessor(do_normalize=False, do_binarize=True,
+ * do_convert_grayscale=True).preprocess, then prepare_mask_latents' F.interpolate(nearest) to H/8 x W/8):
+ *   ds_vae_mask_preprocess : one uint8 HWC image with C = 1 ("L") or C = 3 ("RGB") channels -> Image.resize((out_w,
+ *                            out_h), LANCZOS) in its own mode (same resampler and host-built tap tables as
+ *                            ds_vae_image_preprocess) -> for RGB, Pillow's convert("L") of the resized pixels,
+ *                            (19595 R + 38470 G + 7471 B + 0x8000) >> 16 -> binarize float32(L) / 255 at 0.5, i.e.
+ *                            L >= 128.  Writes `out` fp32 [out_h][out_w] in {0, 1} and / or `out_latent` uint8
+ *                            [out_h/8][out_w/8] = the mask at (8i, 8j); either may be NULL (out_latent needs sizes that
+ *                            are multiples of 8).  Not graph-capturable (host tables).  scratch:
+ *                            ds_vae_mask_preprocess_scratch_bytes(...) bytes, 16-byte aligned (-1: rejected sizes).
+ *   ds_vae_mask_pack       : a float mask already at its size [H][W] -> (x >= 0.5) as `out` fp32 and / or
+ *                            `out_latent` uint8 [H/8][W/8]. */
+int64_t ds_vae_mask_preprocess_scratch_bytes(int H, int W, int C, int out_h, int out_w);
+int ds_vae_mask_preprocess(const uint8_t* src, int H, int W, int C, int out_h, int out_w, float* out,
+                           uint8_t* out_latent, void* scratch, int64_t scratch_bytes, void* stream);
+int ds_vae_mask_pack(const float* x, int H, int W, float* out, uint8_t* out_latent, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * LLaMA decoder of the MLLM agent (SURVEY.md §8f-4: ContinuousLVLM.generate, src/models/mllm/seed_x.py:90-171, over
