@@ -143,20 +143,108 @@ __device__ __forceinline__ int ld_acquire_gpu(const int* ptr) {
   return v;
 }
 
-template <int BN>
-__device__ __forceinline__ void wgmma_tile(float* acc, uint64_t adesc, uint64_t bdesc, int scale_d, bool narrow) {
-  if constexpr (BN > kNarrowBN) {
-    if (narrow) {
-      wgmma_m64n128_ss(acc, adesc, bdesc, scale_d);
-      return;
-    }
-  }
-  if constexpr (BN == 256)
+// Register budgets after setmaxnreg (the launch gives every thread 168): the producer warpgroup needs a handful for
+// one lane's TMA loop, the consumers hold a 64 x 256 fp32 accumulator (128 registers) beside the epilogue state.
+// 128 * 40 + 256 * 232 = 64512 <= 65536.
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
+
+template <int W>
+__device__ __forceinline__ void wgmma_tile(float* acc, uint64_t adesc, uint64_t bdesc, int scale_d) {
+  if constexpr (W == 256)
     wgmma_m64n256_ss(acc, adesc, bdesc, scale_d);
-  else if constexpr (BN == 192)
+  else if constexpr (W == 192)
     wgmma_m64n192_ss(acc, adesc, bdesc, scale_d);
   else
     wgmma_m64n128_ss(acc, adesc, bdesc, scale_d);
+}
+
+// One item's main loop, 4 x wgmma (64 x W x 16) per 64-wide k-block; kb + 1 is issued before the MMAs of kb are
+// waited for, and kb's stage is freed once they retired.  `narrow` (CTA-uniform) runs a 128-column unit of a wider
+// tile; callers that never have one pass a constant false, so their kernel has only the W-wide wgmma (the chain: a
+// data-dependent wgmma shape there made ptxas serialise its MMAs).
+template <int W, int STAGES, int BBYTES>
+__device__ __forceinline__ void mma_mainloop(float* acc, uint32_t a_base, uint32_t b_base, uint64_t* full_bar,
+                                             uint64_t* empty_bar, int& stage, uint32_t& phase, int k0, int k1,
+                                             bool narrow) {
+  int prev = -1;
+  for (int kb = k0; kb < k1; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t a_addr = a_base + stage * kABytes;
+    const uint32_t b_addr = b_base + stage * BBYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kBK / 16; ++k)
+      if (W > kNarrowBN && narrow)
+        wgmma_tile<kNarrowBN>(acc, make_wgmma_desc(a_addr + k * 32, 1024, 16),
+                              make_wgmma_desc(b_addr + k * 32, 1024, 16), (kb != k0 || k != 0) ? 1 : 0);
+      else
+        wgmma_tile<W>(acc, make_wgmma_desc(a_addr + k * 32, 1024, 16), make_wgmma_desc(b_addr + k * 32, 1024, 16),
+                      (kb != k0 || k != 0) ? 1 : 0);
+    wgmma_commit();
+    wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage may be refilled
+    if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+    prev = stage;
+    if (++stage == STAGES) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+  wgmma_wait<0>();
+  fence_regs<W / 2>(acc);
+  if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+}
+
+// item -> (unit, k-block range [k0, k1), index of the unit among the tail units or -1)
+__device__ __forceinline__ void decode_item(const GemmParams& p, int item, int& unit, int& k0, int& k1, int& tail_idx) {
+  if (item < p.tail_start) {
+    unit = item;
+    k0 = 0;
+    k1 = p.num_k_iters;
+    tail_idx = -1;
+  } else {
+    const int s = item - p.tail_start;
+    tail_idx = s / p.tail_parts;
+    const int part = s - tail_idx * p.tail_parts;
+    unit = p.tail_start + tail_idx;
+    k0 = part * p.num_k_iters / p.tail_parts;
+    k1 = (part + 1) * p.num_k_iters / p.tail_parts;
+  }
+}
+
+// unit -> (m-tile, first weight row of its columns, tile width)
+template <int BN>
+__device__ __forceinline__ void unit_geom(const GemmParams& p, int unit, int& m_tile, int& n_org, int& bn) {
+  if (unit < p.wide_units) {
+    m_tile = unit / p.num_n_tiles;
+    const int k = unit - m_tile * p.num_n_tiles;
+    n_org = k * BN;
+    bn = (p.last_narrow && k == p.num_n_tiles - 1) ? kNarrowBN : BN;
+  } else {
+    const int j = unit - p.wide_units;
+    const int mt = j / p.nt_narrow;
+    m_tile = p.wide_m_tiles + mt;
+    n_org = (j - mt * p.nt_narrow) * kNarrowBN;
+    bn = kNarrowBN;
+  }
+}
+
+// this CTA's items of problem q: round-robin over the grid, or — chain — its row of the host-built schedule
+// (item i of [beg, end) is sched_items[i] then)
+template <int MAXQ>
+__device__ __forceinline__ void item_range(const GemmLaunch<MAXQ>& L, int q, int& beg, int& end, int& step,
+                                           const int*& sched_items) {
+  beg = blockIdx.x;
+  end = L.p[q].total_items;
+  step = gridDim.x;
+  sched_items = nullptr;
+  if (MAXQ > 1) {
+    const int* hdr = L.sched + blockIdx.x * (kMaxChain + 1);
+    beg = __ldg(hdr + q);
+    end = __ldg(hdr + q + 1);
+    step = 1;
+    sched_items = L.sched + L.sched_items;
+  }
 }
 
 template <int BN, bool STATS, int MAXQ>
@@ -166,7 +254,6 @@ gemm_bf16_wgmma(const __grid_constant__ GemmLaunch<MAXQ> L) {
   constexpr int STAGES = Cfg::kStages;
   constexpr int ACC = BN / 2;  // fp32 accumulator registers per consumer thread (64 rows x BN per warpgroup)
   const int unit0 = blockIdx.x;
-  const int unit_step = gridDim.x;
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -210,86 +297,44 @@ gemm_bf16_wgmma(const __grid_constant__ GemmLaunch<MAXQ> L) {
   // Everything above overlapped the previous kernel's tail; from here on we touch its outputs.  The TMA producer lane
   // may wait later: it first requests the WEIGHT tiles of its first pipeline stages when they are constant data.
   const bool is_producer_lane = (warp == 0) && (lane == 0);
-  if (!is_producer_lane) pdl_wait();
-
-  // pipeline state carried from one problem of a chain to the next (each thread plays one role)
-  int st_stage = 0, st_iter = 0;
-  uint32_t st_phase = 0, st_res_phase = 0;
   const int nq = MAXQ == 1 ? 1 : L.nq;
-  for (int q = 0; q < nq; ++q) {
-  const GemmParams& p = L.p[q];
-  const CUtensorMap& tmA = L.tm[q][0];
-  const CUtensorMap& tmB = L.tm[q][1];
-  const CUtensorMap& tmC = L.tm[q][2];
-  const CUtensorMap& tmR = L.tm[q][3];
-  const CUtensorMap& tmA2 = L.tm[q][4];
-  const CUtensorMap& tmB2 = L.tm[q][5];
-  const int total_tiles = p.total_items;  // work items: whole units, then the K-slices of the tail units
-  // this CTA's items of the problem: round-robin over the grid, or — chain — its row of the host-built schedule
-  int it_beg = unit0, it_end = total_tiles, it_step = unit_step;
-  const int* sched_items = nullptr;
-  if (MAXQ > 1) {
-    const int* hdr = L.sched + unit0 * (kMaxChain + 1);
-    it_beg = __ldg(hdr + q);
-    it_end = __ldg(hdr + q + 1);
-    it_step = 1;
-    sched_items = L.sched + L.sched_items;
-  }
-  // item -> (unit, k-block range [k0, k1), index of the unit among the tail units or -1)
-  auto decode = [&](int item, int& unit, int& k0, int& k1, int& tail_idx) {
-    if (item < p.tail_start) {
-      unit = item;
-      k0 = 0;
-      k1 = p.num_k_iters;
-      tail_idx = -1;
-    } else {
-      const int s = item - p.tail_start;
-      tail_idx = s / p.tail_parts;
-      const int part = s - tail_idx * p.tail_parts;
-      unit = p.tail_start + tail_idx;
-      k0 = part * p.num_k_iters / p.tail_parts;
-      k1 = (part + 1) * p.num_k_iters / p.tail_parts;
-    }
-  };
 
-  // unit -> (m-tile, first weight row of its columns, tile width)
-  auto unit_geom = [&](int unit, int& m_tile, int& n_org, int& bn) {
-    if (unit < p.wide_units) {
-      m_tile = unit / p.num_n_tiles;
-      const int k = unit - m_tile * p.num_n_tiles;
-      n_org = k * BN;
-      bn = (p.last_narrow && k == p.num_n_tiles - 1) ? kNarrowBN : BN;
-    } else {
-      const int j = unit - p.wide_units;
-      const int mt = j / p.nt_narrow;
-      m_tile = p.wide_m_tiles + mt;
-      n_org = (j - mt * p.nt_narrow) * kNarrowBN;
-      bn = kNarrowBN;
-    }
-  };
-  // chain dependency: the A rows of row block m_blk are the output rows of ALL n-tiles of the previous problem
-  auto wait_chain_dep = [&](int m_blk) {
-    const int* cnt = L.dep + (q - 1) * L.dep_stride + m_blk;
-    const int need = L.p[q - 1].num_n_tiles;
-    if (ld_acquire_gpu(cnt) < need) {
-      const long long t0 = clock64();
-      while (ld_acquire_gpu(cnt) < need) {
-        if (clock64() - t0 > 4000000000LL) __trap();  // a protocol bug becomes a launch error, not a hang
-      }
-    }
-    asm volatile("fence.proxy.async;" ::: "memory");  // generic-proxy acquire -> async-proxy (TMA) reads
-  };
-
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
-      int& stage = st_stage;
-      uint32_t& phase = st_phase;
+  // Each role walks all problems of the chain inside its own branch, so that the register budget set by setmaxnreg at
+  // the head of the branch holds for all of the role's code.  The pipeline state (ring slot, barrier phases) carries
+  // from one problem to the next.
+  if (warp < 4) {
+    // ------------------------------------------------------------------ TMA producer (warpgroup 0, one lane)
+    setmaxnreg_dec<kProducerRegs>();
+    if (!is_producer_lane) pdl_wait();
+    if (is_producer_lane) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int q = 0; q < nq; ++q) {
+      const GemmParams& p = L.p[q];
+      const CUtensorMap& tmA = L.tm[q][0];
+      const CUtensorMap& tmB = L.tm[q][1];
+      const CUtensorMap& tmA2 = L.tm[q][4];
+      const CUtensorMap& tmB2 = L.tm[q][5];
+      int it_beg, it_end, it_step;
+      const int* sched_items;
+      item_range(L, q, it_beg, it_end, it_step, sched_items);
+      // chain dependency: the A rows of row block m_blk are the output rows of ALL n-tiles of the previous problem
+      auto wait_chain_dep = [&](int m_blk) {
+        const int* cnt = L.dep + (q - 1) * L.dep_stride + m_blk;
+        const int need = L.p[q - 1].num_n_tiles;
+        if (ld_acquire_gpu(cnt) < need) {
+          const long long t0 = clock64();
+          while (ld_acquire_gpu(cnt) < need) {
+            if (clock64() - t0 > 4000000000LL) __trap();  // a protocol bug becomes a launch error, not a hang
+          }
+        }
+        asm volatile("fence.proxy.async;" ::: "memory");  // generic-proxy acquire -> async-proxy (TMA) reads
+      };
       int pre_b = 0;  // k-blocks of the FIRST item whose weight tile was requested before griddepcontrol.wait
-      if (MAXQ == 1 && p.w_const && unit0 < total_tiles) {
+      if (MAXQ == 1 && p.w_const && unit0 < p.total_items) {
         int unit, k0, k1, tail_idx, m_tile, n_org, bn;
-        decode(unit0, unit, k0, k1, tail_idx);
-        unit_geom(unit, m_tile, n_org, bn);
+        decode_item(p, unit0, unit, k0, k1, tail_idx);
+        unit_geom<BN>(p, unit, m_tile, n_org, bn);
         const CUtensorMap* bm = (bn != BN) ? &tmB2 : &tmB;
         pre_b = (k1 - k0) < STAGES ? (k1 - k0) : STAGES;
         for (int i = 0; i < pre_b; ++i)  // stage i, first pass: the slot is free, its barrier is in phase 0
@@ -299,9 +344,9 @@ gemm_bf16_wgmma(const __grid_constant__ GemmLaunch<MAXQ> L) {
       for (int it = it_beg; it < it_end; it += it_step) {
         const int tile = MAXQ > 1 ? __ldg(sched_items + it) : it;
         int unit, k0, k1, tail_idx;
-        decode(tile, unit, k0, k1, tail_idx);
+        decode_item(p, tile, unit, k0, k1, tail_idx);
         int m_blk, n_org, bn;
-        unit_geom(unit, m_blk, n_org, bn);
+        unit_geom<BN>(p, unit, m_blk, n_org, bn);
         const bool narrow = bn != BN;
         if (MAXQ > 1 && q > 0 && L.dep != nullptr) wait_chain_dep(m_blk);
         const uint32_t stage_bytes = kABytes + bn * kBK * 2;
@@ -341,9 +386,12 @@ gemm_bf16_wgmma(const __grid_constant__ GemmLaunch<MAXQ> L) {
           }
         }
       }
+      }  // problems of the chain
     }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------------ consumers: MMA + epilogue
+  } else {
+    // ------------------------------------------------------------------ consumers (warpgroups 1-2): MMA + epilogue
+    setmaxnreg_inc<kConsumerRegs>();
+    pdl_wait();
     const int ct = threadIdx.x - 128;     // consumer thread 0..255
     const int wg = ct >> 7;               // consumer warpgroup: rows [64 wg, +64) of the tile
     const int cw = ct >> 5;               // consumer warp 0..7: rows [16 cw, +16)
@@ -352,13 +400,20 @@ gemm_bf16_wgmma(const __grid_constant__ GemmLaunch<MAXQ> L) {
     r_loc[0] = cw * 16 + (lane >> 2);
     r_loc[1] = r_loc[0] + 8;
     const bool issuer = ct == 0;          // drives the TMA engine for the epilogue
-    const bool geglu = p.epilogue == DS_EPI_GEGLU;
+    const uint32_t a_base = smem_u32(sA) + static_cast<uint32_t>(wg) * 64 * 128;  // this warpgroup's 64 A rows
+    const uint32_t b_base = smem_u32(sB);
     float acc[ACC];
 
-    int& stage = st_stage;
-    uint32_t& phase = st_phase;
-    int& iter = st_iter;
-    uint32_t& res_phase = st_res_phase;
+    int stage = 0, iter = 0;
+    uint32_t phase = 0, res_phase = 0;
+    for (int q = 0; q < nq; ++q) {
+    const GemmParams& p = L.p[q];
+    const CUtensorMap& tmC = L.tm[q][2];
+    const CUtensorMap& tmR = L.tm[q][3];
+    int it_beg, it_end, it_step;
+    const int* sched_items;
+    item_range(L, q, it_beg, it_end, it_step, sched_items);
+    const bool geglu = p.epilogue == DS_EPI_GEGLU;
     // chain: "this n-tile of row block m is written" is published one tile LATE: after the main loop of the CTA's
     // next tile (or at the end of the problem).  By then the tile's bulk stores have long completed (the wait is
     // free), and every consumer is past its trailing statistics atomics (the barrier at the head of the next tile).
@@ -373,10 +428,9 @@ gemm_bf16_wgmma(const __grid_constant__ GemmLaunch<MAXQ> L) {
     for (int it = it_beg; it < it_end; it += it_step, ++iter) {
       const int tile = MAXQ > 1 ? __ldg(sched_items + it) : it;
       int unit, k0, k1, tail_idx;
-      decode(tile, unit, k0, k1, tail_idx);
+      decode_item(p, tile, unit, k0, k1, tail_idx);
       int m_blk, n_org, bn_cur;  // n_org: first weight row of the tile's columns; bn_cur: BN, or 128 (narrow unit)
-      unit_geom(unit, m_blk, n_org, bn_cur);
-      const bool narrow = bn_cur != BN;
+      unit_geom<BN>(p, unit, m_blk, n_org, bn_cur);
       const int bn_out = geglu ? bn_cur / 2 : bn_cur;  // output columns of this item
       const int no_org = geglu ? n_org / 2 : n_org;    // first output column
 
@@ -453,32 +507,11 @@ gemm_bf16_wgmma(const __grid_constant__ GemmLaunch<MAXQ> L) {
       // tile's operands have arrived, i.e. after the producer saw the row block's dependency counter complete.
       if (MAXQ == 1) row_stats_io();
 
-      // ---------------- main loop: 4 x wgmma (64 x bn x 16) per 64-wide k-block
-      {
-        const uint32_t a_off = static_cast<uint32_t>(wg) * 64 * 128;  // this warpgroup's 64 rows of the A tile
-        int prev = -1;
-        for (int kb = k0; kb < k1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          const uint32_t a_addr = smem_u32(sA + stage * kABytes) + a_off;
-          const uint32_t b_addr = smem_u32(sB + stage * Cfg::kBBytes);
-          wgmma_fence();
-#pragma unroll
-          for (int k = 0; k < kBK / 16; ++k)
-            wgmma_tile<BN>(acc, make_wgmma_desc(a_addr + k * 32, 1024, 16), make_wgmma_desc(b_addr + k * 32, 1024, 16),
-                           (kb != k0 || k != 0) ? 1 : 0, narrow);
-          wgmma_commit();
-          wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage may be refilled
-          if (prev >= 0) mbar_arrive(&empty_bar[prev]);
-          prev = stage;
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        wgmma_wait<0>();
-        fence_regs<ACC>(acc);
-        if (prev >= 0) mbar_arrive(&empty_bar[prev]);
-      }
+      // ---------------- main loop.  Narrow (128-column) units only exist in single-problem launches of the wider
+      // tiles (last_narrow, mixed-width tail): prepare_gemm sets neither for a chain link, so the chain kernel has only
+      // the BN-wide loop.
+      mma_mainloop<BN, STAGES, Cfg::kBBytes>(acc, a_base, b_base, full_bar, empty_bar, stage, phase, k0, k1,
+                                             MAXQ == 1 && bn_cur != BN);
       if (MAXQ > 1) row_stats_io();
       if (chain_sig && pend_blk >= 0) {  // the previous item: see post_signal
         if (issuer) post_signal();
@@ -525,53 +558,69 @@ gemm_bf16_wgmma(const __grid_constant__ GemmLaunch<MAXQ> L) {
         }
       }
 
-      // accumulator -> fp32 values with LayerNorm / bias / row-bias / GEGLU / activation applied (no residual yet);
-      // GEGLU: value columns [0, bn/2) of the tile, gates [bn/2, bn) — the same thread holds both
+      // accumulator -> fp32 values with LayerNorm / bias / row-bias / GEGLU / activation applied (no residual yet).
+      // The GEGLU pass is a loop of its own: in one loop with the other epilogues, the value | gate pairs of every
+      // column block stay live across all branches and the accumulator no longer fits the register budget.
+      auto ln_bias = [&](float& v0, float& v1, int h, int c) {  // tile column c (value or gate)
+        if (p.ln_stats) {
+          const float nm = -ln_mean[h] * ln_rstd[h];
+          v0 = fmaf(v0, ln_rstd[h], nm * vec[BN + c]);
+          v1 = fmaf(v1, ln_rstd[h], nm * vec[BN + c + 1]);
+        }
+        v0 += vec[c];
+        v1 += vec[c + 1];
+      };
+      auto add_rowbias = [&](float& v0, float& v1, int h, int c) {
+        if (gemm_rowbias && row_ok[h]) {
+          const float* rb = p.rowbias + static_cast<long long>(batch[h]) * p.ldrb + n_org + c;
+          if (n_org + c < p.N) v0 += __ldg(rb);
+          if (n_org + c + 1 < p.N) v1 += __ldg(rb + 1);
+        }
+      };
+      if (geglu) {
+        // value columns [0, bn/2) of the tile, gates [bn/2, bn) — the same thread holds both.  GEGLU only runs on
+        // 256-column tiles (prepare_gemm refuses anything else), so narrower instantiations leave this pass out.
+        if constexpr (BN >= 256) {
+          constexpr int G = BN / 16;  // first gate block
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        if (j * 8 >= bn_out) continue;
-        const int c = j * 8 + cq;
+          for (int j = 0; j < BN / 16; ++j) {
+            if (j * 8 >= bn_out) continue;
+            const int c = j * 8 + cq;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-          if (p.ln_stats) {
-            const float nm = -ln_mean[h] * ln_rstd[h];
-            v0 = fmaf(v0, ln_rstd[h], nm * vec[BN + c]);
-            v1 = fmaf(v1, ln_rstd[h], nm * vec[BN + c + 1]);
-          }
-          v0 += vec[c];
-          v1 += vec[c + 1];
-          if (gemm_rowbias && row_ok[h]) {
-            const float* rb = p.rowbias + static_cast<long long>(batch[h]) * p.ldrb + n_org + c;
-            if (n_org + c < p.N) v0 += __ldg(rb);
-            if (n_org + c + 1 < p.N) v1 += __ldg(rb + 1);
-          }
-          if (geglu) {
-            if constexpr (BN >= 256) {
-              constexpr int G = BN / 16;  // first gate block
+            for (int h = 0; h < 2; ++h) {
+              float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+              ln_bias(v0, v1, h, c);
+              add_rowbias(v0, v1, h, c);
               float g0 = acc[4 * (j + G) + 2 * h], g1 = acc[4 * (j + G) + 2 * h + 1];
-              if (p.ln_stats) {
-                const float nm = -ln_mean[h] * ln_rstd[h];
-                g0 = fmaf(g0, ln_rstd[h], nm * vec[BN + BN / 2 + c]);
-                g1 = fmaf(g1, ln_rstd[h], nm * vec[BN + BN / 2 + c + 1]);
-              }
-              g0 += vec[BN / 2 + c];
-              g1 += vec[BN / 2 + c + 1];
-              v0 *= gelu_sig5(g0);
-              v1 *= gelu_sig5(g1);
+              ln_bias(g0, g1, h, BN / 2 + c);
+              acc[4 * j + 2 * h] = v0 * gelu_sig5(g0);
+              acc[4 * j + 2 * h + 1] = v1 * gelu_sig5(g1);
             }
-          } else if (p.epilogue == DS_EPI_GELU) {
-            v0 = gelu_sig5(v0);
-            v1 = gelu_sig5(v1);
-          } else if (p.epilogue == DS_EPI_SILU) {
-            v0 = silu_f(v0);
-            v1 = silu_f(v1);
-          } else if (p.epilogue == DS_EPI_QUICKGELU) {  // CLIP "quick_gelu": x * sigmoid(1.702 x)
-            v0 = __fdividef(v0, 1.0f + __expf(-1.702f * v0));
-            v1 = __fdividef(v1, 1.0f + __expf(-1.702f * v1));
           }
-          acc[4 * j + 2 * h] = v0;
-          acc[4 * j + 2 * h + 1] = v1;
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          if (j * 8 >= bn_out) continue;
+          const int c = j * 8 + cq;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            ln_bias(v0, v1, h, c);
+            add_rowbias(v0, v1, h, c);
+            if (p.epilogue == DS_EPI_GELU) {
+              v0 = gelu_sig5(v0);
+              v1 = gelu_sig5(v1);
+            } else if (p.epilogue == DS_EPI_SILU) {
+              v0 = silu_f(v0);
+              v1 = silu_f(v1);
+            } else if (p.epilogue == DS_EPI_QUICKGELU) {  // CLIP "quick_gelu": x * sigmoid(1.702 x)
+              v0 = __fdividef(v0, 1.0f + __expf(-1.702f * v0));
+              v1 = __fdividef(v1, 1.0f + __expf(-1.702f * v1));
+            }
+            acc[4 * j + 2 * h] = v0;
+            acc[4 * j + 2 * h + 1] = v1;
+          }
         }
       }
 
@@ -737,8 +786,8 @@ gemm_bf16_wgmma(const __grid_constant__ GemmLaunch<MAXQ> L) {
     // the staging tile must outlive the store's READ of it; global visibility of the bulk stores is the grid's
     // completion (what griddepcontrol.wait / stream order of the consumer waits for)
     if (p.tma_epilogue && issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    }  // problems of the chain
   }
-  }  // problems of the chain
 
   // ---------------------------------------------------------------------- teardown
   __syncthreads();
@@ -1006,6 +1055,8 @@ static int prepare_gemm(const CUtensorMap& tmA, const CUtensorMap& tmA2, const v
                         int conv_B, cudaStream_t stream, bool row_stats_zeroed, bool chain, const DeviceInfo& dev,
                         PreparedGemm* out) {
   const int bn = chain ? 256 : pick_bn(p.N, p.epilogue);
+  // the kernel's GEGLU pass pairs value | gate columns of a 256-wide tile; narrower instantiations do not compile it
+  DS_REQUIRE(p.epilogue != DS_EPI_GEGLU || bn == 256, "ds_gemm_bf16: GEGLU needs 256-column tiles (got %d)", bn);
   // coalesced TMA epilogue whenever the bf16 output (and residual) rows are 16-byte addressable
   auto aligned16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   p.tma_epilogue = !p.out_fp32 && p.n_out % 8 == 0 && p.ldo % 8 == 0 && aligned16(p.out) &&
@@ -1041,9 +1092,12 @@ static int prepare_gemm(const CUtensorMap& tmA, const CUtensorMap& tmA2, const v
   p.wide_m_tiles = 0;
   p.nt_narrow = 0;
   // narrow last n-tile: when the last BN-wide tile of a row would hold <= 128 real columns (N = 640 -> 256|256|128,
-  // N = 320 -> 192|128, N = 1920 -> 7 x 256|128) it runs as a 128-column unit: same unit count, no padded MMAs
+  // N = 320 -> 192|128, N = 1920 -> 7 x 256|128) it runs as a 128-column unit: same unit count, no padded MMAs.
+  // Not in a chain: the chain kernel has only the 256-wide wgmma (a data-dependent wgmma width there makes ptxas
+  // serialise its MMAs), so its last tile is a full 256-row weight box whose rows beyond N are TMA zero fill; the
+  // epilogue stops at n_out, so the outputs are the same.
   p.last_narrow = 0;
-  if (bn > kNarrowBN && p.epilogue != DS_EPI_GEGLU) {
+  if (!chain && bn > kNarrowBN && p.epilogue != DS_EPI_GEGLU) {
     const int last_cols = p.N - (p.num_n_tiles - 1) * bn;
     if (last_cols <= kNarrowBN) p.last_narrow = 1;
   }

@@ -36,6 +36,13 @@ __device__ __forceinline__ void fence_regs(float* d) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// Per-warpgroup register reallocation: every thread of the warpgroup executes the same instruction.  dec hands
+// registers back to the SM's pool, inc blocks until the pool can supply them; N is a multiple of 8 in [24, 256].
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // D[64 x 32] (+)= A(smem) * B(smem), both K-major; scale_d = 0 overwrites D
 __device__ __forceinline__ void wgmma_m64n32_ss(float* d, uint64_t adesc, uint64_t bdesc, int scale_d) {
   asm volatile(
