@@ -62,4 +62,25 @@ __device__ __forceinline__ bool ip_key_open(uint32_t bits, int key, int tokens_p
   return (bits >> ((key - num_dummy) / tokens_per_ip)) & 1u;
 }
 
+// bits [lo, hi) of a 64-bit word, the range clipped to [0, 64)
+__device__ __forceinline__ uint64_t bit_range64(int lo, int hi) {
+  lo = max(lo, 0);
+  hi = min(hi, 64);
+  if (lo >= hi) return 0ull;
+  const uint64_t below_hi = hi == 64 ? ~0ull : (1ull << hi) - 1ull;
+  return below_hi & ~((1ull << lo) - 1ull);
+}
+
+// ip_key_open for the 64 keys [key0, key0 + 64) at once: bit k set <=> key key0 + k is open.  Keys past the last IP
+// token are closed, as ip_key_open has them (their box index is >= num_ips).  A few range operations per open box
+// instead of an integer division per key.
+__device__ __forceinline__ uint64_t ip_open_keys64(uint32_t bits, int key0, int tokens_per_ip, int num_dummy) {
+  uint64_t m = bits == 0 ? bit_range64(-key0, num_dummy - key0) : 0ull;
+  for (uint32_t r = bits; r != 0; r &= r - 1) {
+    const int lo = num_dummy + (__ffs(r) - 1) * tokens_per_ip - key0;
+    m |= bit_range64(lo, lo + tokens_per_ip);
+  }
+  return m;
+}
+
 }  // namespace ds
