@@ -45,6 +45,17 @@ def _unsupported(attn, hidden_states, attention_mask):
         raise ops.DsEngineError("engine processors need bf16 CUDA hidden states (no CPU / fp32 fallback)")
 
 
+def _no_peft_lora(attn, names):
+    """The processors read ``.weight`` of the projections, which on a PEFT-wrapped layer is the base weight only: a
+    LoRA there would be dropped.  Merge it into the weights instead (``DiffSenseiPipeline.load_lora_weights``)."""
+    for n in names:
+        lin = attn.to_out[0] if n == "to_out.0" else getattr(attn, n)
+        if hasattr(lin, "lora_A"):
+            raise NotImplementedError(f"attn.{n} carries PEFT LoRA layers, which the engine processors do not run; "
+                                      "load the LoRA with DiffSenseiPipeline.load_lora_weights (merged into the "
+                                      "engine's weights)")
+
+
 class _PackCache:
     """Derived tensors (packed weights, projected K|V) keyed on the IDENTITY and version of their source tensors.
 
@@ -87,6 +98,7 @@ class AttnProcessor2_0(nn.Module):
         if encoder_hidden_states is not None:
             raise NotImplementedError("AttnProcessor2_0 is installed on attn1 (self-attention) sites only "
                                       "(src/models/unet.py:68-69)")
+        _no_peft_lora(attn, ("to_q", "to_k", "to_v", "to_out.0"))
         hs = hidden_states.contiguous()
         ws = (attn.to_q.weight, attn.to_k.weight, attn.to_v.weight)
         wqkv = self._cache.get(ws, lambda: torch.cat([w.detach() for w in ws], 0).to(bf16).contiguous())
@@ -114,6 +126,7 @@ class MaskedIPAttnProcessor2_0(nn.Module):
         if encoder_hidden_states is None or bbox is None or aspect_ratio is None:
             raise ValueError("MaskedIPAttnProcessor2_0 needs encoder_hidden_states, bbox and aspect_ratio "
                              "(cross_attention_kwargs, src/pipelines/pipeline_diffsensei.py:270-273)")
+        _no_peft_lora(attn, ("to_q", "to_k", "to_v", "to_out.0"))
         hs = hidden_states.contiguous()
         ehs = encoder_hidden_states
         end = ehs.shape[1] - (self.num_ip_tokens + self.num_dummy_tokens)        # reference :213

@@ -140,12 +140,36 @@ class ClipTextEncoderEngine(_EncoderBase):
             self.stack.add_layer(W, {k: f"{p}encoder.layers.{i}.{v}" for k, v in _CLIP_LAYER.items()})
         self.final_ln = (fp(W(p + "final_layer_norm.weight")), fp(W(p + "final_layer_norm.bias")))
         self.proj = bf(W("text_projection.weight")) if cfg.projection_dim > 0 else None
+        self._lora = None                  # new packed tensors: adapters and base copies of the old ones are gone
         if strict:
             used = 2 + 16 * cfg.num_hidden_layers + 2 + (1 if self.proj is not None else 0)
             extra = [k for k in sd if not k.endswith("position_ids")]
             if len(extra) != used:
                 raise KeyError(f"ClipTextEncoderEngine.load_state_dict: expected {used} tensors, got {len(extra)}")
         self._loaded = True
+
+    @property
+    def lora(self):
+        """The LoRA adapters merged into this engine's packed weights (``lora.LoraMerger``)."""
+        if getattr(self, "_lora", None) is None:
+            from .lora import LoraMerger
+            self._check()
+            self._lora = LoraMerger(self.lora_slots(), self.device)
+        return self._lora
+
+    def lora_slots(self):
+        """``text_model.encoder.layers.<i>.{self_attn.{q,k,v,out}_proj, mlp.fc1, mlp.fc2}`` -> where that linear lives
+        in the packed weights (``lora.Slot``; no LayerNorm is folded here)."""
+        from .lora import Slot
+        C, slots = self.cfg.hidden_size, {}
+        for i, L in enumerate(self.stack.layers):
+            p = f"text_model.encoder.layers.{i}"
+            for j, n in enumerate("qkv"):
+                slots[f"{p}.self_attn.{n}_proj"] = Slot(L.wqkv, j * C, C)
+            slots[f"{p}.self_attn.out_proj"] = Slot(L.wo, 0, C)
+            slots[f"{p}.mlp.fc1"] = Slot(L.w1, 0, L.w1.shape[0])
+            slots[f"{p}.mlp.fc2"] = Slot(L.w2, 0, C)
+        return slots
 
     @torch.no_grad()
     def forward(self, input_ids: torch.Tensor, output_hidden_states: bool = True):

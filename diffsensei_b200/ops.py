@@ -291,7 +291,7 @@ def _gemm_args(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = 
          row_stats_out: Optional[torch.Tensor] = None, zero_rows: Optional[torch.Tensor] = None,
          row_stats_zeroed: bool = False, a2: Optional[torch.Tensor] = None,
          chan_stats: Optional[torch.Tensor] = None, stats_rows_per_sample: int = 0,
-         w_const: bool = True):
+         w_const: bool = True, splitk: bool = True):
     """Validated ds_gemm_args + the output tensor of out[..., Nout] = epilogue(a[..., K] @ w[N, K]^T); ``a`` may have
     any leading dims.
 
@@ -299,7 +299,8 @@ def _gemm_args(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = 
     turn the call into LayerNorm(a) @ w_orig^T for weights folded by ``weights.fold_layernorm``; ``row_stats_out``
     [2*M] fp64 receives {sum, sumsq} of every (bf16-rounded) output row.
     ``w_const=False`` when ``w`` is not a parameter but the output of a preceding kernel (it is then fetched only after
-    the programmatic-dependent-launch wait)."""
+    the programmatic-dependent-launch wait).  ``splitk=False`` never splits K across CTAs, so the output bits depend
+    only on the operands (split-K otherwise depends on how many tiles the shape leaves for the last wave)."""
     _req(a, bf16, "gemm.a")
     _req(w, bf16, "gemm.w", 2)
     K1 = a.shape[-1]
@@ -354,7 +355,7 @@ def _gemm_args(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = 
         _req(row_stats_out, torch.float64, "gemm.row_stats_out", 1)
         if row_stats_out.numel() < 2 * M or out_fp32:
             raise DsEngineError("gemm: row_stats_out must hold 2*M doubles and needs a bf16 output")
-    ws = _splitk_ws()
+    ws = _splitk_ws() if splitk else None
     args = GemmArgs(a=a.data_ptr(), w=w.data_ptr(), out=out.data_ptr(), bias=_ptr(bias), rowbias=_ptr(rowbias),
                     residual=_ptr(residual), M=M, N=N, K=K, lda=K1, ldw=K, ldo=n_out, ldres=n_out,
                     rows_per_batch=rows_per_batch, rowbias_ld=rowbias_ld, epilogue=epilogue, out_fp32=int(out_fp32),

@@ -40,6 +40,7 @@ import torch
 
 from . import ops
 from .image_processor import CLIPImageProcessor, VaeImageProcessor, ViTImageProcessor
+from .lora import AdapterRegistry, lora_targets, normalize_lora, split_components
 from .scheduler import DDIMScheduler, EulerDiscreteScheduler, get_timesteps
 from .unet import UNetMangaEngine
 
@@ -143,6 +144,7 @@ class DiffSenseiPipeline:
         # panels of one shape re-use the graph and only refill its static buffers (DenoiseStepper.load_panel)
         self._steppers = {}
         self.max_cached_steppers = 8
+        self._lora = AdapterRegistry()
 
     # ------------------------------------------------------------------------------ reference surface
     def register_manga_modules(self, magi_image_encoder=None, image_proj_model=None):
@@ -173,6 +175,55 @@ class DiffSenseiPipeline:
 
     def set_ip_scale(self, scale):
         self.unet.set_ip_scale(scale)
+
+    # ------------------------------------------------------------------------------ LoRA (diffusers' surface)
+    def _lora_engines(self) -> dict:
+        return {"unet": self.unet, "text_encoder": self.text_encoder, "text_encoder_2": self.text_encoder_2}
+
+    def load_lora_weights(self, pretrained_model_name_or_path_or_dict, adapter_name: Optional[str] = None, *,
+                          alpha: Optional[float] = None, rank: Optional[int] = None) -> str:
+        """Load a LoRA (state dict or local ``.safetensors`` path; PEFT, diffusers or kohya keys, see
+        ``lora.normalize_lora``) as adapter ``adapter_name`` (default ``default_<n>``) and make it the only active
+        adapter, at weight 1.0.  Its UNet part goes to ``unet``, its text-encoder parts to ``text_encoder`` /
+        ``text_encoder_2``; they are merged into the engines' packed weights.  ``alpha`` / ``rank``: for PEFT keys,
+        which carry no alpha (default ``alpha = r``).  Every key and shape is checked before any weight is touched.
+        Returns the adapter name."""
+        name = self._lora.new_name(adapter_name)
+        eng = self._lora_engines()
+        cfg = lambda e: None if e is None else e.cfg
+        targets = lora_targets(cfg(self.unet), cfg(self.text_encoder), cfg(self.text_encoder_2))
+        parts = split_components(normalize_lora(pretrained_model_name_or_path_or_dict, targets, self.unet.cfg,
+                                                alpha=alpha, rank=rank))
+        for comp, loras in parts.items():
+            eng[comp].lora.add(name, loras)
+        self._lora.add(name)
+        self.set_adapters([name])
+        return name
+
+    def set_adapters(self, adapter_names, adapter_weights=None) -> None:
+        """Make exactly ``adapter_names`` active, at ``adapter_weights`` (default 1.0 each), and re-merge: the packed
+        weights become base + sum of weight * scale * B A over them, always from the pre-LoRA copies.  An empty list
+        restores the pre-LoRA weights bit for bit."""
+        active = self._lora.resolve(adapter_names, adapter_weights)
+        for e in self._lora_engines().values():
+            if e is not None and getattr(e, "_lora", None) is not None:
+                e.lora.set_active(active)
+        self._lora.active = active
+
+    def get_active_adapters(self) -> List[str]:
+        return list(self._lora.active)
+
+    def get_list_adapters(self) -> dict:
+        """Component -> the loaded adapters that have weights in it."""
+        return {c: list(e.lora.adapters) for c, e in self._lora_engines().items()
+                if e is not None and getattr(e, "_lora", None) is not None and e.lora.adapters}
+
+    def unload_lora_weights(self) -> None:
+        """Drop every adapter: the packed weights get their pre-LoRA bits back and the base copies are freed."""
+        for e in self._lora_engines().values():
+            if e is not None and getattr(e, "_lora", None) is not None:
+                e.lora.unload()
+        self._lora.clear()
 
     def tokenize_prompt(self, prompt: str, prompt_2=None, negative_prompt=None, negative_prompt_2=None):
         """The tokenizer half of diffusers' SDXL ``encode_prompt`` (pipeline_diffsensei.py:232-245): each prompt padded
@@ -333,6 +384,7 @@ class DiffSenseiPipeline:
         (bs,4,h,w), noise fp32 (bs,4,h,w), latent mask uint8 (bs,h,w)); after every step the pixels where the mask is
         0 become the image latents noised to the next timestep (the image latents on the last step).  Returns the
         final latents, NCHW fp32."""
+        self.unet.set_lora_scale(1.0)            # a direct unet(..., cross_attention_kwargs={"scale": s}) call may have left s
         if use_graph:
             st = self.stepper_for(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                   dialog_bbox, num_inference_steps, guidance_scale, start_index=start_index,

@@ -91,6 +91,7 @@ class UNetMangaEngine:
         self._loaded = False
         self._cond_cache: Optional[Conditions] = None
         self._processors = None
+        self._lora = None              # lora.LoraMerger, made by the first load_lora
         self.num_upsamplers = len(cfg.block_out_channels) - 1
         if self.device.type == "cuda":
             with torch.cuda.device(self.device):
@@ -139,6 +140,52 @@ class UNetMangaEngine:
     def _ip_weights_version(self) -> int:
         """Moves when a checkpoint is loaded INTO the processors (their Parameters alias the packed IP weights)."""
         return sum(blk.wkv_ip._version for t in self.transformers.values() for blk in t.blocks)
+
+    # ------------------------------------------------------------------------------------------ LoRA
+    @property
+    def lora(self):
+        """The LoRA adapters merged into this engine's packed weights (``lora.LoraMerger``)."""
+        if self._lora is None:
+            from .lora import LoraMerger
+            self._lora = LoraMerger(self.lora_slots(), self.device)
+        return self._lora
+
+    def lora_version(self) -> int:
+        """Moves whenever a LoRA merge or restore rewrites the packed weights (through raw pointers: ``_version``
+        does not see those writes)."""
+        return 0 if self._lora is None else self._lora.version
+
+    def set_lora_scale(self, scale: float) -> None:
+        """``cross_attention_kwargs["scale"]``: a factor on the active adapters' weights (re-merges when it changes;
+        nothing to do without an active adapter)."""
+        if self._lora is not None:
+            self._lora.set_multiplier(scale)
+
+    def lora_slots(self):
+        """diffusers module name -> where that linear lives in the packed weights (``lora.Slot``), for every linear
+        of every Transformer2DModel."""
+        from .lora import Slot, packed_row_order
+        if not self._loaded:
+            raise RuntimeError("LoRA: load_state_dict first")
+        slots = {}
+        for p, t in self.transformers.items():
+            c = t.c
+            slots[f"{p}.proj_in"] = Slot(t.w_in, 0, c)
+            slots[f"{p}.proj_out"] = Slot(t.w_out, 0, c)
+            perm = packed_row_order(pack_geglu, 8 * c, self.device)
+            for k, blk in enumerate(t.blocks):
+                b = f"{p}.transformer_blocks.{k}"
+                for j, n in enumerate("qkv"):
+                    slots[f"{b}.attn1.to_{n}"] = Slot(blk.wqkv, j * c, c, ln=blk.n1, bias=blk.bqkv, colsum=blk.cs_qkv)
+                slots[f"{b}.attn1.to_out.0"] = Slot(blk.wo1, 0, c)
+                slots[f"{b}.attn2.to_q"] = Slot(blk.wq2, 0, c, ln=blk.n2, bias=blk.bq2, colsum=blk.cs_q2)
+                slots[f"{b}.attn2.to_k"] = Slot(blk.wkv_t, 0, c)
+                slots[f"{b}.attn2.to_v"] = Slot(blk.wkv_t, c, c)
+                slots[f"{b}.attn2.to_out.0"] = Slot(blk.wo2, 0, c)
+                slots[f"{b}.ff.net.0.proj"] = Slot(blk.wff1, 0, 8 * c, perm=perm, ln=blk.n3, bias=blk.bff1,
+                                                   colsum=blk.cs_ff1)
+                slots[f"{b}.ff.net.2"] = Slot(blk.wff2, 0, c)
+        return slots
 
     def state_dict_keys(self):
         return list(unet_param_shapes(self.cfg).keys())
@@ -238,6 +285,7 @@ class UNetMangaEngine:
         self._loaded = True
         self._cond_cache = None
         self._processors = None
+        self._lora = None                  # new packed tensors: adapters and base copies of the old ones are gone
         return SimpleNamespace(missing_keys=missing, unexpected_keys=unexpected)
 
     # ------------------------------------------------------------------------------------------ hoisted work
@@ -474,7 +522,8 @@ class UNetMangaEngine:
         """Hoisted K|V for (ehs, bbox): reused across the steps of one panel.  The key holds the tensors THEMSELVES
         (identity + version counter) — never addresses, which the caching allocator recycles between panels."""
         c = self._cond_cache
-        key = (ehs, ehs._version, bbox, bbox._version, float(aspect_ratio), self._ip_weights_version())
+        key = (ehs, ehs._version, bbox, bbox._version, float(aspect_ratio), self._ip_weights_version(),
+               self.lora_version())
         hit = (c is not None and len(c.key) == len(key) and c.key[0] is ehs and c.key[2] is bbox and
                c.key[1] == key[1] and c.key[3] == key[3] and c.key[4:] == key[4:])
         if not hit:
@@ -504,6 +553,9 @@ class UNetMangaEngine:
                              "(src/pipelines/pipeline_diffsensei.py:270-273)")
         if added_cond_kwargs is None or "text_embeds" not in added_cond_kwargs or "time_ids" not in added_cond_kwargs:
             raise ValueError("added_cond_kwargs must carry `text_embeds` and `time_ids` (text_time conditioning)")
+        # the reference scales its PEFT LoRA layers by `scale` for this call (unet.py:213-223): here the merged
+        # weights are re-merged when it changes
+        self.set_lora_scale(float(cross_attention_kwargs.get("scale", 1.0)))
         out_dtype = sample.dtype
         if sample.dtype not in (f32, bf16):
             sample = sample.float()                       # fp16 pipelines: cast at the boundary
