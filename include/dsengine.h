@@ -265,7 +265,8 @@ int ds_attention_self(const void* qkv, void* out, int B, int N, int heads, void*
  *   kv_ip: bf16 [B][n_ip][2*C]    (to_k_ip | to_v_ip of the image tokens, n_ip = num_dummy + num_ips*tokens_per_ip)
  *   bbox : fp32 [B][num_ips][4];  the additive mask is evaluated in registers with the reference's
  *          closed-interval linspace membership and derived (H', W') (:131-163); masked keys get -10000.
- * n_text, n_ip <= 128. */
+ * n_text, n_ip: any positive lengths; both key sets stay resident in shared memory when they take <= 4 64-key tiles
+ * together, and stream otherwise.  num_ips <= 16. */
 typedef struct {
   const void* q;
   const void* kv_text;

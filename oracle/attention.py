@@ -95,6 +95,50 @@ def self_attention(hs, wq, wk, wv, wo, bo, heads: int):
     return F.linear(o, wo, bo)
 
 
+def attention_heads(q, k, v, heads: int, open_mask=None, dtype=torch.float64):
+    """softmax(Q K^T / sqrt(d) + M) V per head, on the attention kernels' token-major layout: q [B, Nq, heads*d],
+    k / v [B, Nk, heads*d] (head h at columns [h*d, (h+1)*d)) -> [B, Nq, heads*d] in ``dtype`` on q's device.
+
+    open_mask: bool [B, Nq, Nk], True where the key is attendable; closed keys get MASK_VALUE added, as in
+    ip_additive_mask.  One (batch, head) at a time, so a single [Nq, Nk] score matrix is live (512 MiB in fp64 at
+    Nq = Nk = 8192)."""
+    B, n, c = q.shape
+    d = c // heads
+    out = torch.empty(B, n, c, dtype=dtype, device=q.device)
+    for b in range(B):
+        mask = None
+        if open_mask is not None:
+            mask = torch.where(open_mask[b].to(q.device), 0.0, MASK_VALUE).to(dtype)
+        for h in range(heads):
+            cols = slice(h * d, (h + 1) * d)
+            out[b, :, cols] = sdpa(q[b, :, cols].to(dtype), k[b, :, cols].to(dtype), v[b, :, cols].to(dtype), mask)
+    return out
+
+
+def self_attention_abi(qkv, heads: int, dtype=torch.float64):
+    """ds_attention_self's operation on its fused projection qkv [B, N, 3C] (q | k | v column blocks)."""
+    c = qkv.shape[-1] // 3
+    return attention_heads(qkv[..., :c], qkv[..., c:2 * c], qkv[..., 2 * c:], heads, dtype=dtype)
+
+
+def resampler_attention_abi(q, kv, heads: int, dtype=torch.float64):
+    """ds_resampler_attn's operation: q [B, nq, C] against kv [B, n_kv, 2C] (k | v column blocks)."""
+    c = q.shape[-1]
+    return attention_heads(q, kv[..., :c], kv[..., c:], heads, dtype=dtype)
+
+
+def cross_ip_attention_abi(q, kv_text, kv_ip, bbox, heads: int, aspect_ratio: float, ip_scale: float,
+                           tokens_per_ip: int, num_dummy: int, dtype=torch.float64):
+    """ds_attention_cross_ip's operation: text attention + ip_scale * bbox-masked IP attention, on the projections
+    q [B, N, C], kv_text [B, n_text, 2C], kv_ip [B, n_ip, 2C] and bbox [B, num_ips, 4] (cross_ip_attention before its
+    output projection).  The mask is built on the CPU, whose linspace the kernels reproduce bit for bit."""
+    c = q.shape[-1]
+    open_ = ip_open_mask(bbox.cpu(), q.shape[1], aspect_ratio, tokens_per_ip, num_dummy)
+    text = attention_heads(q, kv_text[..., :c], kv_text[..., c:], heads, dtype=dtype)
+    ip = attention_heads(q, kv_ip[..., :c], kv_ip[..., c:], heads, open_, dtype=dtype)
+    return text + ip_scale * ip
+
+
 def cross_ip_attention(hs, ehs, bbox, aspect_ratio, wq, wk, wv, wk_ip, wv_ip, wo, bo, heads: int, scale: float,
                        num_ip_tokens: int, num_dummy: int):
     """MaskedIPAttnProcessor2_0 (:207-263): text cross-attention + scale * bbox-masked IP cross-attention,

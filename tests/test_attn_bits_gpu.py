@@ -124,6 +124,29 @@ def test_cross_attention_batch_invariant(ops):
     assert torch.equal(full[s], part)
 
 
+def test_cross_attention_streaming_batch_invariant(ops):
+    """300 text keys + 80 IP keys take 7 key tiles, more than stay resident: the streaming kernel."""
+    B, N, h = 4, 1000, 4
+    C = 64 * h
+    q = _randn(25, B, N, C).to(DEV)
+    kv_t = _randn(26, B, 300, 2 * C).to(DEV)
+    kv_i = _randn(27, B, 80, 2 * C).to(DEV)
+    bbox = torch.tensor([BENCH_BOXES, [[0.0] * 4] * 4] * (B // 2), device=DEV)
+    full = ops.attention_cross_ip(q, kv_t, kv_i, bbox, h, 0.625, 0.6, 16, 16)
+    s = slice(1, 3)
+    part = ops.attention_cross_ip(q[s].contiguous(), kv_t[s].contiguous(), kv_i[s].contiguous(),
+                                  bbox[s].contiguous(), h, 0.625, 0.6, 16, 16)
+    assert torch.equal(full[s], part)
+
+
+def test_resampler_batch_invariant(ops):
+    q = _randn(28, 8, 16, 64 * 20).to(DEV)
+    kv = _randn(29, 8, 274, 2 * 64 * 20).to(DEV)
+    full = ops.resampler_attn(q, kv, 20)
+    part = ops.resampler_attn(q[2:4].contiguous(), kv[2:4].contiguous(), 20)
+    assert torch.equal(full[2:4], part)
+
+
 if __name__ == "__main__":
     sys.path.insert(0, ROOT)
     from diffsensei_b200 import ops as o
