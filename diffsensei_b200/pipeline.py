@@ -7,12 +7,13 @@ Mirrors ``src/pipelines/pipeline_diffsensei.py``:
     repeat to ``num_samples``; ``prepare_dialog_bbox`` (:156-170)
   * the CFG denoise loop (:293-337) — ``denoise``: the hot path.
   * VAE decode + image post-process (:339-363) — ``VaeDecoderEngine`` (vae.py), ``output_type`` "pt" / "np" / "pil".
-``__call__`` keeps the reference's keyword surface.  A raw ``prompt`` string needs the two CLIP tokenizers
-(``tokenizer=`` / ``tokenizer_2=``, host objects) and the text-encoder engines; ``ip_images`` need the image-encoder
-engines and run through the two image processors on the GPU (image_processor.py).  Without them the encoders' inputs
-(token ids, pixel values) or outputs (``prompt_embeds`` ..., ``clip_image_embeds`` / ``magi_image_embeds``) can be
-passed instead; a raw prompt or image without what it needs raises, it does not fall back to anything.
-``generate_page`` runs the panels of a page together (one front-end pass, one denoise per group of same-size panels).
+``__call__`` keeps the reference's keyword surface and runs as a page of one panel: ``generate_page`` is the one
+implementation, and it runs the panels of a page together (one front-end pass, one denoise per group of same-size
+panels).  A raw ``prompt`` string needs the two CLIP tokenizers (``tokenizer=`` / ``tokenizer_2=``, host objects) and
+the text-encoder engines; ``ip_images`` need the image-encoder engines and run through the two image processors on the
+GPU (image_processor.py).  Without them the encoders' inputs (token ids, pixel values) or outputs (``prompt_embeds``
+..., ``clip_image_embeds`` / ``magi_image_embeds``) can be passed instead; a raw prompt or image without what it needs
+raises, it does not fall back to anything.
 ``image=`` / ``strength=`` start a panel from an image as diffusers' ``StableDiffusionXLImg2ImgPipeline`` does (needs
 ``vae_encoder=``): the image is encoded, noised to the schedule's step ``t_start`` and denoised from there.
 ``mask_image=`` with ``image=`` redraws only the masked part, as diffusers' ``StableDiffusionXLInpaintPipeline`` does
@@ -99,6 +100,12 @@ def _stacked(fn, xs):
             out[i] = tuple(t[r0:r1] for t in res)
             r0 = r1
     return out
+
+
+def _pad_boxes(boxes, m: int) -> List[List[float]]:
+    """The first ``m`` boxes, then zero boxes up to ``m`` (pipeline_diffsensei.py:121-122, :161-163)."""
+    boxes = [list(b) for b in list(boxes)[:m]]
+    return boxes + [[0.0, 0.0, 0.0, 0.0] for _ in range(m - len(boxes))]
 
 
 def _postprocess(image: torch.Tensor, output_type: str):
@@ -289,46 +296,22 @@ class DiffSenseiPipeline:
 
     def prepare_ip_image_embeds(self, clip_image_embeds: torch.Tensor, magi_image_embeds: torch.Tensor,
                                 ip_image_embeds: Optional[torch.Tensor], ip_bbox: List[List[float]], num_samples: int):
-        """clip_image_embeds (1, n, S, D) / magi_image_embeds (1, n, Dm) for the n <= max_num_ips real characters."""
-        cfg = self.unet.cfg
-        dev = self.unet.device
-        m = cfg.max_num_ips
-        ip_bbox = [list(b) for b in ip_bbox[:m]]
-        rc = getattr(self.image_proj_model, "rc", None)
-        if clip_image_embeds is None or magi_image_embeds is None:
-            # a panel without characters: the reference pads with black images and then zeroes every padded
-            # character's embeddings (:118-132), i.e. the Resampler sees all-zero inputs on both branches
-            if rc is None:
-                raise ValueError("a panel without character references needs an image_proj_model that exposes its "
-                                 "ResamplerConfig (`.rc`) to size the zero embeddings")
-            clip_image_embeds = torch.zeros(1, 0, 257, rc.embedding_dim, dtype=bf16, device=dev)
-            magi_image_embeds = torch.zeros(1, 0, rc.magi_embedding_dim, dtype=bf16, device=dev)
-        num_ips = min(clip_image_embeds.shape[1], m)
-        clip = torch.zeros(1, m, *clip_image_embeds.shape[2:], dtype=clip_image_embeds.dtype, device=dev)
-        magi = torch.zeros(1, m, magi_image_embeds.shape[-1], dtype=magi_image_embeds.dtype, device=dev)
-        if num_ips:
-            clip[0, :num_ips] = clip_image_embeds[0, :num_ips].to(dev)  # padded characters stay zero (:131-132)
-            magi[0, :num_ips] = magi_image_embeds[0, :num_ips].to(dev)
-        while len(ip_bbox) < m:
-            ip_bbox.append([0.0, 0.0, 0.0, 0.0])                        # :121-122
-        image_embeds = self.image_proj_model(clip, magi)                               # :133
-        negative_image_embeds = self.image_proj_model(torch.zeros_like(clip), torch.zeros_like(magi))   # :135
-        bbox = torch.tensor(ip_bbox, dtype=f32).unsqueeze(0).to(dev)                   # :137 (stays fp32)
-        neg_bbox = torch.zeros_like(bbox)
-        nv = cfg.num_vision_tokens
-        if ip_image_embeds is not None:                                                # :143-145
-            ip_image_embeds = ip_image_embeds[:m]
-            n, _, dim = ip_image_embeds.shape
-            image_embeds[0, nv:(1 + n) * nv, :] = ip_image_embeds.reshape(1, -1, dim).to(image_embeds)
+        """clip_image_embeds (1, n, S, D) / magi_image_embeds (1, n, Dm) for the n <= max_num_ips real characters, or
+        None for a panel without characters.  Returns (negative_image_embeds, image_embeds, negative_ip_bbox,
+        ip_bbox), each repeated to ``num_samples``."""
+        (img, neg), = self._character_embeds([(clip_image_embeds, magi_image_embeds, ip_image_embeds)])
+        return self._ip_rows(img, neg, ip_bbox, num_samples)
+
+    def _ip_rows(self, image_embeds, negative_image_embeds, ip_bbox, num_samples: int):
+        """The tail of ``prepare_ip_image_embeds`` (:137-152) for one panel's Resampler rows: the boxes padded to
+        ``max_num_ips`` (fp32), everything repeated to ``num_samples``."""
+        bbox = torch.tensor(_pad_boxes(ip_bbox, self.unet.cfg.max_num_ips), dtype=f32).unsqueeze(0).to(self.unet.device)
         rep = lambda t: t.repeat(num_samples, 1, 1)
-        return rep(negative_image_embeds).to(bf16), rep(image_embeds).to(bf16), rep(neg_bbox), rep(bbox)
+        return rep(negative_image_embeds).to(bf16), rep(image_embeds).to(bf16), rep(torch.zeros_like(bbox)), rep(bbox)
 
     def prepare_dialog_bbox(self, dialog_bbox: List[List[float]], num_samples: int):
-        m = self.unet.cfg.max_num_dialogs
-        dialog_bbox = [list(b) for b in dialog_bbox[:m]]
-        while len(dialog_bbox) < m:
-            dialog_bbox.append([0.0, 0.0, 0.0, 0.0])
-        db = torch.tensor(dialog_bbox, dtype=f32).unsqueeze(0).to(device=self.unet.device, dtype=self.unet.dtype)
+        db = torch.tensor(_pad_boxes(dialog_bbox, self.unet.cfg.max_num_dialogs), dtype=f32).unsqueeze(0).to(
+            device=self.unet.device, dtype=self.unet.dtype)
         db = db.repeat(num_samples, 1, 1)                                              # :166-167
         return torch.zeros_like(db), db
 
@@ -419,101 +402,14 @@ class DiffSenseiPipeline:
                  # img2img (diffusers' StableDiffusionXLImg2ImgPipeline): start from this image at `strength`;
                  # with mask_image, inpaint (StableDiffusionXLInpaintPipeline): redraw only where the mask is white
                  image=None, strength: float = 0.3, mask_image=None):
-        t_start = 0
-        if mask_image is not None and image is None:
-            raise ValueError("`mask_image` needs `image`: inpainting redraws the masked part of that image")
-        if image is not None:
-            t_start, height, width = self._check_image(image, latents, strength, num_inference_steps, height, width)
-            if mask_image is not None:
-                self.mask_processor.mask_host(mask_image, height, width)
-        height = height or self.default_sample_size * self.vae_scale_factor
-        width = width or self.default_sample_size * self.vae_scale_factor
-        original_size = original_size or (height, width)
-        target_size = target_size or (height, width)
-        if len(ip_images) > 0:
-            if ip_image_embeds is not None:
-                raise ValueError("`ip_images` and `ip_image_embeds` can not be input together!")
-            if clip_pixel_values is not None or magi_pixel_values is not None or clip_image_embeds is not None or \
-                    magi_image_embeds is not None:
-                raise ValueError("`ip_images` and pixel values / image embeddings can not be input together!")
-        if prompt_embeds is None and prompt_input_ids is None and isinstance(prompt, str) and \
-                self.tokenizer is not None and self.tokenizer_2 is not None:
-            prompt_input_ids, prompt_input_ids_2, negative_prompt_input_ids, negative_prompt_input_ids_2 = \
-                self.tokenize_prompt(prompt, prompt_2, negative_prompt, negative_prompt_2)
-        if prompt_embeds is None and prompt_input_ids is not None:
-            prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds, negative_pooled_prompt_embeds = \
-                self.encode_prompt_ids(prompt_input_ids, prompt_input_ids_2 if prompt_input_ids_2 is not None
-                                       else prompt_input_ids, negative_prompt_input_ids, negative_prompt_input_ids_2)
-        if clip_image_embeds is None and clip_pixel_values is not None:
-            clip_image_embeds, magi_image_embeds = self.encode_ip_images(clip_pixel_values, magi_pixel_values)
-        if prompt_embeds is None:
-            self.check_inputs(prompt, prompt_2, list(ip_images), ip_image_embeds, list(ip_bbox))
-            raise NotImplementedError(
-                "raw prompt strings need the CLIP tokenizers' vocabulary files (host-side assets, not part of the engine): "
-                "pass prompt_input_ids (+ prompt_input_ids_2) with the text-encoder engines registered, or "
-                "prompt_embeds / negative_prompt_embeds / pooled_prompt_embeds / negative_pooled_prompt_embeds")
-        if len(ip_images) > 0:
-            if len(ip_images) != len(ip_bbox):
-                raise ValueError(f"`ip_images` must have the same length as `ip_bbox`. But they are in length "
-                                 f"{len(ip_images)} and {len(ip_bbox)}!")
-            if self.image_encoder is None or self.magi_image_encoder is None:
-                raise NotImplementedError("ip_images need the image-encoder engines: DiffSenseiPipeline(..., "
-                                          "image_encoder=ClipVisionEncoderEngine) and register_manga_modules("
-                                          "magi_image_encoder=VitMaeEncoderEngine, ...); or pass clip_image_embeds / "
-                                          "magi_image_embeds")
-            m = self.unet.cfg.max_num_ips                                  # :112-114
-            ip_bbox = list(ip_bbox)[:m]
-            clip_image_embeds, magi_image_embeds = self.encode_ip_images(*self.preprocess_ip_images(list(ip_images)[:m]))
-        if output_type not in ("latent", "pt", "np", "pil"):
-            raise ValueError(f"output_type must be one of latent / pt / np / pil, got {output_type!r}")
-        if output_type != "latent" and self.vae is None:
-            raise ValueError("output_type other than 'latent' needs a VAE decoder: DiffSenseiPipeline(..., vae=...)")
-        n_real = clip_image_embeds.shape[1] if clip_image_embeds is not None else 0
-        num_ips = len(ip_image_embeds) if ip_image_embeds is not None else n_real
-        if num_ips != len(ip_bbox):
-            raise ValueError(f"`ip_images` must have the same length as `ip_bbox`. But they are in length {num_ips} "
-                             f"and {len(ip_bbox)}!")
-        if guidance_scale <= 1.0:
-            raise ValueError("guidance_scale <= 1 disables classifier-free guidance on the reference "
-                             "(pipeline_diffsensei.py:315-334: text-only batch, no blend); the engine's denoise step is "
-                             "the fused CFG + scheduler update and does not implement the guidance-free variant")
-        self._guidance_scale = guidance_scale
-        self.set_ip_scale(ip_scale)
-        dev = self.unet.device
-        self.scheduler.set_timesteps(num_inference_steps, device=dev)    # :248 (init_noise_sigma depends on it)
-        inpaint = None
-        if image is not None and mask_image is not None:                 # inpaint prepare_latents + mask latents
-            moments = self.vae_encoder.moments_nhwc(self.vae_image_processor.preprocess_nhwc4(image, height, width))
-            eps, noise = self._draw_inpaint_noise(moments.shape[1], moments.shape[2], num_samples, generator)
-            mask = self.mask_processor.preprocess_latent_mask(mask_image, height, width)
-            latents, inpaint = self._inpaint_start(moments, eps, noise, mask, num_samples, t_start, strength)
-        elif image is not None:                                          # img2img prepare_latents (add_noise=True)
-            latents = self.vae_encoder.encode_latents(self.vae_image_processor.preprocess_nhwc4(image, height, width),
-                                                      generator, num_samples,
-                                                      self.scheduler.add_noise_coefficients(t_start, dev))
-        elif latents is None:
-            latents = self.prepare_latents(num_samples, self.unet.config.in_channels, height, width, generator)
-        else:
-            latents = latents * self.scheduler.init_noise_sigma          # diffusers' prepare_latents
-        neg_img, img, neg_bbox, bbox = self.prepare_ip_image_embeds(clip_image_embeds, magi_image_embeds,
-                                                                    ip_image_embeds, list(ip_bbox), num_samples)
-        aspect_ratio = latents.shape[-2] / latents.shape[-1]                            # :272
-        time_ids = torch.tensor([list(original_size) + list(crops_coords_top_left) + list(target_size)],
-                                dtype=f32, device=dev)                                  # _get_add_time_ids
-        neg_db, db = self.prepare_dialog_bbox(list(dialog_bbox), num_samples)
-        rep = lambda t: t.to(dev).repeat(num_samples, 1, 1) if t.dim() == 3 else t.to(dev).repeat(num_samples, 1)
-        pe = torch.cat([rep(negative_prompt_embeds), rep(prompt_embeds)], dim=0).to(bf16)          # :294
-        te = torch.cat([rep(negative_pooled_prompt_embeds), rep(pooled_prompt_embeds)], dim=0)     # :295
-        ti = time_ids.repeat(2 * num_samples, 1)                                                   # :296,302
-        pe = torch.cat([pe, torch.cat([neg_img, img], dim=0)], dim=1)                              # :297,303
-        final = self.denoise(latents, pe, te, ti, torch.cat([neg_bbox, bbox], dim=0), aspect_ratio,
-                             torch.cat([neg_db, db], dim=0), num_inference_steps, guidance_scale, use_graph=use_graph,
-                             start_index=t_start, inpaint=inpaint)
-        if output_type == "latent":
-            return SimpleNamespace(images=final, latents=final)
-        # pipeline_diffsensei.py:339-363: latents / scaling_factor -> vae.decode -> image_processor.postprocess
-        image = self.vae.decode_image(final)                                            # fp32 NCHW in [0, 1]
-        return SimpleNamespace(images=_postprocess(image, output_type), latents=final)
+        """A page of one panel: ``generate_page([panel], ...)[0]``, the panel holding this call's per-panel keywords
+        (``PANEL_KEYS``) and the page the others.  Its input errors carry no panel index."""
+        args = locals()
+        panel = {k: args[k] for k in PANEL_KEYS}                    # as given, defaults included
+        page = dict(num_inference_steps=num_inference_steps, guidance_scale=guidance_scale, output_type=output_type,
+                    max_batch_panels=PAGE_MAX_ROWS, strength=strength)
+        t_start = self._check_page([panel], **page)
+        return self._run_page([self._panel_job(panel)], t_start, ip_scale=ip_scale, use_graph=use_graph, **page)[0]
 
     def _draw_inpaint_noise(self, h: int, w: int, num_samples: int, generator):
         """The generator draws of diffusers' 4-channel inpaint pipeline, in its order: the posterior sample's randn
@@ -538,14 +434,13 @@ class DiffSenseiPipeline:
                                                self.scheduler.add_noise_coefficients(t_start, self.unet.device))
         return latents, (z, noise, mask.repeat(num_samples, 1, 1))
 
-    def _check_image(self, image, latents, strength, num_inference_steps, height, width):
-        """The host-only checks of ``image=`` (before any GPU work).  Returns (t_start, height, width): the first step
-        of the schedule the loop runs, and the panel size the image is processed to."""
+    def _check_image(self, image, latents, height, width):
+        """The host-only checks of one panel's ``image=`` (its ``strength`` is the page's, checked by ``_check_page``).
+        Returns the panel size the image is processed to."""
         if self.vae_encoder is None:
             raise ValueError("image= needs a VAE encoder: DiffSenseiPipeline(..., vae_encoder=VaeEncoderEngine)")
         if latents is not None:
             raise ValueError("`image` and `latents` can not be input together")
-        t_start, _ = get_timesteps(num_inference_steps, strength)
         height, width = self.vae_image_processor.get_default_height_width(image, height, width)
         if isinstance(image, torch.Tensor) and image.is_floating_point():
             if image.dim() not in (3, 4) or (image.dim() == 4 and image.shape[0] != 1) or image.shape[-3] != 3:
@@ -554,7 +449,25 @@ class DiffSenseiPipeline:
             if tuple(image.shape[-2:]) != (height, width):
                 raise ValueError(f"a float image tensor is not resized: it must already be {height} x {width}, got "
                                  f"{tuple(image.shape[-2:])}")
-        return t_start, height, width
+        return height, width
+
+    def _check_page(self, panels, num_inference_steps, guidance_scale, output_type, max_batch_panels,
+                    strength) -> int:
+        """The host-only checks of the page keywords.  Returns the first step of the schedule that image panels run
+        (0 on a page without them, where ``strength`` is not used)."""
+        if output_type not in ("latent", "pt", "np", "pil"):
+            raise ValueError(f"output_type must be one of latent / pt / np / pil, got {output_type!r}")
+        if output_type != "latent" and self.vae is None:
+            raise ValueError("output_type other than 'latent' needs a VAE decoder: DiffSenseiPipeline(..., vae=...)")
+        if guidance_scale <= 1.0:
+            raise ValueError("guidance_scale <= 1 disables classifier-free guidance on the reference "
+                             "(pipeline_diffsensei.py:315-334: text-only batch, no blend); the engine's denoise step is "
+                             "the fused CFG + scheduler update and does not implement the guidance-free variant")
+        if int(max_batch_panels) < 1:
+            raise ValueError(f"max_batch_panels must be >= 1, got {max_batch_panels}")
+        if any(p.get("image") is not None for p in panels):
+            return get_timesteps(num_inference_steps, strength)[0]
+        return 0
 
     # ------------------------------------------------------------------------------ a page of panels
     @torch.no_grad()
@@ -566,8 +479,9 @@ class DiffSenseiPipeline:
         """Several panels of a page in one call.  ``panels`` holds one dict per panel with the per-panel keywords of
         ``__call__`` (``PANEL_KEYS``); the keywords here are the same for the whole page.  Returns one
         ``SimpleNamespace(images=..., latents=...)`` per panel, in panel order, each ``torch.equal`` to
-        ``pipe(**panel, <the page keywords>)`` run alone: every kernel on the path gives a row the same bits whatever
-        the batch around it.
+        ``pipe(**panel, <the page keywords>)``, which is this call on a page of that one panel: every kernel on the
+        path gives a row the same bits whatever the batch around it.  A panel's input errors are ``pipe(...)``'s with
+        ``panel i: `` in front.
 
         The front end runs once per page: each text encoder on the stacked token ids of every panel (positives and
         string negatives), the two image processors and each image encoder on every panel's character images, and the
@@ -578,8 +492,8 @@ class DiffSenseiPipeline:
         at the 16 rows of ``__call__(num_samples=8)``.  Each chunk is one ``denoise`` (a cached stepper is refilled
         when the chunk's shapes repeat) and one batched VAE decode.
 
-        Initial noise: each panel draws its latents from its own ``generator``, with the solo call's shape; panels
-        without a generator draw from the global RNG in panel order, as the same calls made one after another would.
+        Initial noise: each panel draws its latents from its own ``generator``; panels without a generator draw from
+        the global RNG in panel order, as the same calls made one after another would.
 
         ``agent=`` (an ``AgentEngine``, with ``tokenizer_mllm``) runs the demo's MLLM composition
         (scripts/demo/gradio.py:85-129) for every panel: the character images, padded to ``max_num_ips`` with black
@@ -588,12 +502,11 @@ class DiffSenseiPipeline:
         its image features are blended as ``feat * mllm_scale + embeds * (1 - mllm_scale)``, and the blend is
         denoised as ``ip_image_embeds`` with ``ip_images=[]`` and ``ip_bbox`` padded with zero boxes.
 
-        A panel with ``image`` starts from that image at the page's ``strength``, as ``__call__(image=...)`` does: it
-        draws the posterior sample's noise, then the latent noise, at its turn in panel order; same-size images are
-        encoded in one batch; img2img panels never share a denoise with text-to-image panels.  A panel with ``image``
-        and ``mask_image`` inpaints, as ``__call__(image=..., mask_image=...)`` does: it draws the posterior sample's
-        noise, the latent noise and the discarded masked-image sample at its turn; inpaint panels share a denoise only
-        with inpaint panels of the same latent size."""
+        A panel with ``image`` starts from that image at the page's ``strength``: it draws the posterior sample's
+        noise, then the latent noise, at its turn in panel order; same-size images are encoded in one batch; img2img
+        panels never share a denoise with text-to-image panels.  A panel with ``image`` and ``mask_image`` inpaints:
+        it draws the posterior sample's noise, the latent noise and the discarded masked-image sample at its turn;
+        inpaint panels share a denoise only with inpaint panels of the same latent size."""
         if not isinstance(panels, (list, tuple)) or len(panels) == 0:
             raise ValueError("generate_page needs a non-empty list of panel dicts")
         panels = [dict(p) for p in panels]
@@ -603,25 +516,28 @@ class DiffSenseiPipeline:
                     raise ValueError(f"panel {i}: `{k}` is the same for the whole page; pass it to generate_page")
                 if k not in PANEL_KEYS:
                     raise ValueError(f"panel {i}: unknown key `{k}`")
-        if output_type not in ("latent", "pt", "np", "pil"):
-            raise ValueError(f"output_type must be one of latent / pt / np / pil, got {output_type!r}")
-        if output_type != "latent" and self.vae is None:
-            raise ValueError("output_type other than 'latent' needs a VAE decoder: DiffSenseiPipeline(..., vae=...)")
-        if guidance_scale <= 1.0:
-            raise ValueError("guidance_scale <= 1 disables classifier-free guidance; the engine's denoise step is the "
-                             "fused CFG + scheduler update and does not implement the guidance-free variant")
-        if int(max_batch_panels) < 1:
-            raise ValueError(f"max_batch_panels must be >= 1, got {max_batch_panels}")
-        t_start = 0
-        if any(p.get("image") is not None for p in panels):
-            t_start, _ = get_timesteps(num_inference_steps, strength)
+        page = dict(num_inference_steps=num_inference_steps, guidance_scale=guidance_scale, output_type=output_type,
+                    max_batch_panels=max_batch_panels, strength=strength)
+        t_start = self._check_page(panels, **page)
         if agent is not None:
             self._check_agent_panels(panels, tokenizer_mllm)
-            for i, p in enumerate(panels):          # the panels' own checks too, before the agent's decode
-                self._panel_job(i, p)
+            self._panel_jobs(panels)                # the panels' own checks too, before the agent's decode
             panels = self._agent_panels(panels, agent, tokenizer_mllm, mllm_scale, max_new_tokens)
-        jobs = [self._panel_job(i, p) for i, p in enumerate(panels)]        # host checks and tokenization only
+        return self._run_page(self._panel_jobs(panels), t_start, ip_scale=ip_scale, use_graph=use_graph, **page)
 
+    def _panel_jobs(self, panels) -> List[SimpleNamespace]:
+        """``_panel_job`` of every panel, its errors prefixed with the panel index."""
+        jobs = []
+        for i, p in enumerate(panels):
+            try:
+                jobs.append(self._panel_job(p))
+            except (ValueError, NotImplementedError) as e:
+                raise type(e)(f"panel {i}: {e}") from e
+        return jobs
+
+    def _run_page(self, jobs, t_start: int, *, num_inference_steps, guidance_scale, ip_scale, output_type, use_graph,
+                  max_batch_panels, strength) -> List[SimpleNamespace]:
+        """The GPU half of a page whose panels (``_panel_job``) and keywords (``_check_page``) passed their checks."""
         # ---- front end, once per page
         dev = self.unet.device
         text = _stacked(lambda ids: (self.text_encoder(ids, output_hidden_states=True).hidden_states[-2],),
@@ -640,18 +556,13 @@ class DiffSenseiPipeline:
                 (h1,), (h2, pooled) = text.pop(0), text_2.pop(0)
                 j.npe, j.npp = torch.cat([h1, h2], dim=-1), pooled
         self._encode_page_images(jobs)
-        m, nv = self.unet.cfg.max_num_ips, self.unet.cfg.num_vision_tokens
-        for j, (img, neg) in zip(jobs, self._character_embeds([(j.clip, j.magi) for j in jobs])):
-            if j.ip_image_embeds is not None:                                          # :143-145
-                e = j.ip_image_embeds[:m]
-                img = img.clone()
-                img[0, nv:(1 + e.shape[0]) * nv, :] = e.reshape(1, -1, e.shape[-1]).to(img)
+        for j, (img, neg) in zip(jobs, self._character_embeds([(j.clip, j.magi, j.ip_image_embeds) for j in jobs])):
             j.img, j.neg_img = img, neg
 
         # ---- noise and per-panel condition rows, then one denoise + one decode per chunk
         self._guidance_scale = guidance_scale
         self.set_ip_scale(ip_scale)
-        self.scheduler.set_timesteps(num_inference_steps, device=dev)
+        self.scheduler.set_timesteps(num_inference_steps, device=dev)    # :248 (init_noise_sigma depends on it)
         for j in jobs:                                                     # panel order: the global RNG's order
             if j.image is not None:
                 draw = self._draw_inpaint_noise if j.mask_image is not None else self.vae_encoder.draw_noise
@@ -660,7 +571,7 @@ class DiffSenseiPipeline:
             elif j.latents is None:
                 j.latents = self.prepare_latents(j.ns, self.unet.config.in_channels, j.height, j.width, j.generator)
             else:
-                j.latents = j.latents * self.scheduler.init_noise_sigma
+                j.latents = j.latents * self.scheduler.init_noise_sigma    # diffusers' prepare_latents
         self._encode_page_latents([j for j in jobs if j.image is not None], t_start, strength)
         results = [None] * len(jobs)
         kind = lambda j: () if j.image is None else ("inpaint",) if j.mask_image is not None else ("image",)
@@ -675,6 +586,7 @@ class DiffSenseiPipeline:
             final = self.denoise(lat, cat("pe"), cat("te"), cat("ti"), cat("bbox"), lat.shape[-2] / lat.shape[-1],
                                  cat("db"), num_inference_steps, guidance_scale, use_graph=use_graph,
                                  start_index=t_start if jobs[chunk[0]].image is not None else 0, inpaint=inpaint)
+            # pipeline_diffsensei.py:339-363: latents / scaling_factor -> vae.decode -> image_processor.postprocess
             image = self.vae.decode_image(final) if output_type != "latent" else final
             r0 = 0
             for i in chunk:
@@ -699,85 +611,79 @@ class DiffSenseiPipeline:
             else:
                 j.latents = self.vae_encoder.latents_from_moments(m, j.eps, j.ns, j.noise, coef)
 
-    def _panel_job(self, i: int, p: dict) -> SimpleNamespace:
-        """One panel's arguments resolved as ``__call__`` resolves them, with its ValueErrors prefixed by the panel
-        index; runs on the host only (tokenization included), so a bad panel fails before any GPU work."""
+    def _panel_job(self, p: dict) -> SimpleNamespace:
+        """One panel's keywords (``PANEL_KEYS``, with ``__call__``'s defaults) checked and resolved; runs on the host
+        only (tokenization included), so a bad panel fails before any GPU work."""
         g = lambda k, d=None: p.get(k, d)
-        try:
-            height, width = g("height"), g("width")
-            if g("mask_image") is not None and g("image") is None:
-                raise ValueError("`mask_image` needs `image`: inpainting redraws the masked part of that image")
-            if g("image") is not None:
-                # the page's strength was checked already: only the panel's own image checks can fail here
-                _, height, width = self._check_image(g("image"), g("latents"), 1.0, 1, height, width)
-                if g("mask_image") is not None:
-                    self.mask_processor.mask_host(g("mask_image"), height, width)
-            height = height or self.default_sample_size * self.vae_scale_factor
-            width = width or self.default_sample_size * self.vae_scale_factor
-            ip_images, ip_bbox = list(g("ip_images", ())), list(g("ip_bbox", ()))
-            ip_image_embeds = g("ip_image_embeds")
-            if len(ip_images) > 0:
-                if ip_image_embeds is not None:
-                    raise ValueError("`ip_images` and `ip_image_embeds` can not be input together!")
-                if any(g(k) is not None for k in ("clip_pixel_values", "magi_pixel_values", "clip_image_embeds",
-                                                  "magi_image_embeds")):
-                    raise ValueError("`ip_images` and pixel values / image embeddings can not be input together!")
-            ids = None
-            if g("prompt_embeds") is None:
-                if g("prompt_input_ids") is None and isinstance(g("prompt"), str) and \
-                        self.tokenizer is not None and self.tokenizer_2 is not None:
-                    ids = self.tokenize_prompt(g("prompt"), g("prompt_2"), g("negative_prompt"),
-                                               g("negative_prompt_2"))
-                elif g("prompt_input_ids") is not None:
-                    ids = (g("prompt_input_ids"), g("prompt_input_ids_2"), g("negative_prompt_input_ids"),
-                           g("negative_prompt_input_ids_2"))
-                if ids is None:
-                    self.check_inputs(g("prompt"), g("prompt_2"), ip_images, ip_image_embeds, ip_bbox)
-                    raise NotImplementedError(
-                        "raw prompt strings need the CLIP tokenizers (tokenizer= / tokenizer_2=): pass "
-                        "prompt_input_ids with the text-encoder engines registered, or the prompt embeddings")
-                if self.text_encoder is None or self.text_encoder_2 is None:
-                    raise ValueError("encode_prompt_ids needs text_encoder and text_encoder_2 engines")
-                as_ids = lambda t: None if t is None else torch.as_tensor(t)
-                # negative_prompt_input_ids_2 without negative_prompt_input_ids: zero negatives, as in __call__
-                ids = (as_ids(ids[0]), as_ids(ids[1] if ids[1] is not None else ids[0]), as_ids(ids[2]),
-                       None if ids[2] is None else as_ids(ids[3] if ids[3] is not None else ids[2]))
-            m = self.unet.cfg.max_num_ips
-            clip_pv = magi_pv = None
-            n_real = 0
-            if len(ip_images) > 0:
-                if len(ip_images) != len(ip_bbox):
-                    raise ValueError(f"`ip_images` must have the same length as `ip_bbox`. But they are in length "
-                                     f"{len(ip_images)} and {len(ip_bbox)}!")
-                if self.image_encoder is None or self.magi_image_encoder is None:
-                    raise NotImplementedError("ip_images need the image-encoder engines (image_encoder= and "
-                                              "register_manga_modules(magi_image_encoder=...)); or pass "
-                                              "clip_image_embeds / magi_image_embeds")
-                ip_images, ip_bbox = ip_images[:m], ip_bbox[:m]
-                n_real = len(ip_images)
-            elif g("clip_image_embeds") is None and g("clip_pixel_values") is not None:
-                if self.image_encoder is None or self.magi_image_encoder is None:
-                    raise ValueError("encode_ip_images needs image_encoder and magi_image_encoder engines")
-                clip_pv, magi_pv = torch.as_tensor(g("clip_pixel_values")), torch.as_tensor(g("magi_pixel_values"))
-                n_real = clip_pv.shape[0]
-            elif g("clip_image_embeds") is not None:
-                n_real = g("clip_image_embeds").shape[1]
-            num_ips = len(ip_image_embeds) if ip_image_embeds is not None else n_real
-            if num_ips != len(ip_bbox):
+        height, width = g("height"), g("width")
+        if g("mask_image") is not None and g("image") is None:
+            raise ValueError("`mask_image` needs `image`: inpainting redraws the masked part of that image")
+        if g("image") is not None:
+            height, width = self._check_image(g("image"), g("latents"), height, width)
+            if g("mask_image") is not None:
+                self.mask_processor.mask_host(g("mask_image"), height, width)
+        height = height or self.default_sample_size * self.vae_scale_factor
+        width = width or self.default_sample_size * self.vae_scale_factor
+        ip_images, ip_bbox = list(g("ip_images", ())), list(g("ip_bbox", ()))
+        ip_image_embeds = g("ip_image_embeds")
+        if len(ip_images) > 0:
+            if ip_image_embeds is not None:
+                raise ValueError("`ip_images` and `ip_image_embeds` can not be input together!")
+            if any(g(k) is not None for k in ("clip_pixel_values", "magi_pixel_values", "clip_image_embeds",
+                                              "magi_image_embeds")):
+                raise ValueError("`ip_images` and pixel values / image embeddings can not be input together!")
+        ids = None
+        if g("prompt_embeds") is None:
+            if g("prompt_input_ids") is None and isinstance(g("prompt"), str) and \
+                    self.tokenizer is not None and self.tokenizer_2 is not None:
+                ids = self.tokenize_prompt(g("prompt"), g("prompt_2"), g("negative_prompt"), g("negative_prompt_2"))
+            elif g("prompt_input_ids") is not None:
+                ids = (g("prompt_input_ids"), g("prompt_input_ids_2"), g("negative_prompt_input_ids"),
+                       g("negative_prompt_input_ids_2"))
+            if ids is None:
+                self.check_inputs(g("prompt"), g("prompt_2"), ip_images, ip_image_embeds, ip_bbox)
+                raise NotImplementedError(
+                    "raw prompt strings need the CLIP tokenizers (tokenizer= / tokenizer_2=): pass "
+                    "prompt_input_ids with the text-encoder engines registered, or the prompt embeddings")
+            if self.text_encoder is None or self.text_encoder_2 is None:
+                raise ValueError("encode_prompt_ids needs text_encoder and text_encoder_2 engines")
+            as_ids = lambda t: None if t is None else torch.as_tensor(t)
+            # negative_prompt_input_ids_2 without negative_prompt_input_ids: zero negatives, as encode_prompt_ids
+            ids = (as_ids(ids[0]), as_ids(ids[1] if ids[1] is not None else ids[0]), as_ids(ids[2]),
+                   None if ids[2] is None else as_ids(ids[3] if ids[3] is not None else ids[2]))
+        m = self.unet.cfg.max_num_ips
+        clip_pv = magi_pv = None
+        n_real = 0
+        if len(ip_images) > 0:
+            if len(ip_images) != len(ip_bbox):
                 raise ValueError(f"`ip_images` must have the same length as `ip_bbox`. But they are in length "
-                                 f"{num_ips} and {len(ip_bbox)}!")
-        except (ValueError, NotImplementedError) as e:
-            raise type(e)(f"panel {i}: {e}") from e
-        ns = int(g("num_samples", 1))
+                                 f"{len(ip_images)} and {len(ip_bbox)}!")
+            if self.image_encoder is None or self.magi_image_encoder is None:
+                raise NotImplementedError("ip_images need the image-encoder engines (image_encoder= and "
+                                          "register_manga_modules(magi_image_encoder=...)); or pass "
+                                          "clip_image_embeds / magi_image_embeds")
+            ip_images, ip_bbox = ip_images[:m], ip_bbox[:m]                 # :112-114
+            n_real = len(ip_images)
+        elif g("clip_image_embeds") is None and g("clip_pixel_values") is not None:
+            if self.image_encoder is None or self.magi_image_encoder is None:
+                raise ValueError("encode_ip_images needs image_encoder and magi_image_encoder engines")
+            clip_pv, magi_pv = torch.as_tensor(g("clip_pixel_values")), torch.as_tensor(g("magi_pixel_values"))
+            n_real = clip_pv.shape[0]
+        elif g("clip_image_embeds") is not None:
+            n_real = g("clip_image_embeds").shape[1]
+        num_ips = len(ip_image_embeds) if ip_image_embeds is not None else n_real
+        if num_ips != len(ip_bbox):
+            raise ValueError(f"`ip_images` must have the same length as `ip_bbox`. But they are in length "
+                             f"{num_ips} and {len(ip_bbox)}!")
         return SimpleNamespace(
-            index=i, ns=ns, height=height, width=width, generator=g("generator"), latents=g("latents"), ids=ids,
-            image=g("image"), mask_image=g("mask_image"), inpaint=None,
+            ns=int(g("num_samples", 1)), height=height, width=width, generator=g("generator"), latents=g("latents"),
+            ids=ids, image=g("image"), mask_image=g("mask_image"), inpaint=None,
             pe=g("prompt_embeds"), npe=g("negative_prompt_embeds"), pp=g("pooled_prompt_embeds"),
             npp=g("negative_pooled_prompt_embeds"), ip_images=ip_images, clip_pv=clip_pv, magi_pv=magi_pv,
             clip=g("clip_image_embeds"), magi=g("magi_image_embeds"), ip_image_embeds=ip_image_embeds,
             ip_bbox=ip_bbox, dialog_bbox=list(g("dialog_bbox", ())),
             time_ids=list(g("original_size") or (height, width)) + list(g("crops_coords_top_left", (0, 0))) +
-            list(g("target_size") or (height, width)))
+            list(g("target_size") or (height, width)))                   # _get_add_time_ids
 
     def _encode_page_images(self, jobs) -> None:
         """Every panel's character images through the two processors and each image encoder once; panels given
@@ -804,20 +710,23 @@ class DiffSenseiPipeline:
             j.clip, j.magi = c.unsqueeze(0), mg.unsqueeze(0)
 
     def _character_embeds(self, chars):
-        """``prepare_ip_image_embeds``' Resampler passes (:118-135) for a page: ``chars`` holds one (clip (1, n, S, D),
-        magi (1, n, Dm)) per panel, or (None, None) for a panel without characters.  Each panel's characters are
-        truncated / zero-padded to ``max_num_ips`` and all panels of one sequence length S go through the Resampler in
-        one call, together with the all-zero row that is every such panel's negative (a panel without characters is
-        all zeros on both branches, with S = 257).  Returns one (image_embeds, negative_image_embeds) pair per panel,
-        (1, T, D) bf16 rows of the shared output: clone before writing."""
-        m, dev = self.unet.cfg.max_num_ips, self.unet.device
+        """``prepare_ip_image_embeds``' Resampler passes (:118-135) and paste (:143-145) for a page: ``chars`` holds one
+        (clip (1, n, S, D), magi (1, n, Dm), ip_image_embeds (k, T, D) or None) per panel, clip and magi None for a
+        panel without characters.  Each panel's characters are truncated / zero-padded to ``max_num_ips`` and all
+        panels of one sequence length S go through the Resampler in one call, together with the all-zero row that is
+        every such panel's negative (a panel without characters is all zeros on both branches, with S = 257).  A
+        panel's ``ip_image_embeds`` (the first ``max_num_ips``) then replace its image tokens after the dummy tokens.
+        Returns one (image_embeds, negative_image_embeds) pair per panel, (1, T, D) bf16 rows of the shared output
+        (a pasted row is a copy): clone before writing."""
+        m, nv, dev = self.unet.cfg.max_num_ips, self.unet.cfg.num_vision_tokens, self.unet.device
         rc = getattr(self.image_proj_model, "rc", None)
         groups = {}
-        for i, (clip, magi) in enumerate(chars):
+        for i, (clip, magi, _) in enumerate(chars):
             if clip is None or magi is None:
+                # the reference pads with black images and then zeroes every padded character's embeddings (:118-132)
                 if rc is None:
-                    raise ValueError(f"panel {i}: a panel without character references needs an image_proj_model "
-                                     "that exposes its ResamplerConfig (`.rc`) to size the zero embeddings")
+                    raise ValueError("a panel without character references needs an image_proj_model that exposes "
+                                     "its ResamplerConfig (`.rc`) to size the zero embeddings")
                 key = (257, rc.embedding_dim, rc.magi_embedding_dim)
             else:
                 key = (clip.shape[2], clip.shape[3], magi.shape[-1])
@@ -828,7 +737,7 @@ class DiffSenseiPipeline:
             clip = torch.zeros(len(real) + 1, m, S, D, dtype=bf16, device=dev)
             magi = torch.zeros(len(real) + 1, m, Dm, dtype=bf16, device=dev)
             for r, i in enumerate(real):
-                c, mg = chars[i]
+                c, mg, _ = chars[i]
                 n = min(c.shape[1], m)
                 clip[r, :n] = c[0, :n].to(dev).to(bf16)       # the dtype cast the Resampler applies, element by element
                 magi[r, :n] = mg[0, :n].to(dev).to(bf16)
@@ -836,25 +745,26 @@ class DiffSenseiPipeline:
             neg = emb[-1:]
             for i in idx:
                 out[i] = (emb[real.index(i):real.index(i) + 1] if i in real else neg, neg)
+        for i, (_, _, e) in enumerate(chars):
+            if e is not None:
+                img, e = out[i][0].clone(), e[:m]
+                img[0, nv:(1 + e.shape[0]) * nv, :] = e.reshape(1, -1, e.shape[-1]).to(img)
+                out[i] = (img, out[i][1])
         return out
 
     def _panel_rows(self, j):
         """One panel's [negative, positive] condition rows, each repeated to its ``num_samples`` (:293-304)."""
         dev, ns = self.unet.device, j.ns
-        m = self.unet.cfg.max_num_ips
-        ip_bbox = [list(b) for b in j.ip_bbox[:m]]
-        while len(ip_bbox) < m:
-            ip_bbox.append([0.0, 0.0, 0.0, 0.0])                                       # :121-122
-        bbox = torch.tensor(ip_bbox, dtype=f32).unsqueeze(0).to(dev)
+        neg_img, img, neg_bbox, bbox = self._ip_rows(j.img, j.neg_img, j.ip_bbox, ns)
         neg_db, db = self.prepare_dialog_bbox(j.dialog_bbox, ns)
         rep = lambda t: t.to(dev).repeat(ns, 1, 1) if t.dim() == 3 else t.to(dev).repeat(ns, 1)
         ti = torch.tensor([j.time_ids], dtype=f32, device=dev).repeat(ns, 1)
-        side = lambda pe, pp, img, bb, d: dict(pe=torch.cat([rep(pe).to(bf16), rep(img).to(bf16)], dim=1),
-                                               te=rep(pp), ti=ti, bbox=rep(bb), db=d)
-        return (side(j.npe, j.npp, j.neg_img, torch.zeros_like(bbox), neg_db), side(j.pe, j.pp, j.img, bbox, db))
+        side = lambda pe, pp, im, bb, d: dict(pe=torch.cat([rep(pe).to(bf16), im], dim=1), te=rep(pp), ti=ti, bbox=bb,
+                                              db=d)
+        return side(j.npe, j.npp, neg_img, neg_bbox, neg_db), side(j.pe, j.pp, img, bbox, db)
 
     def _check_agent_panels(self, panels, tokenizer_mllm) -> None:
-        """The host-only checks of the ``agent=`` path."""
+        """The host-only checks of the ``agent=`` path (each panel's own checks follow: ``_panel_job``)."""
         if tokenizer_mllm is None:
             raise ValueError("agent= needs tokenizer_mllm")
         if self.image_encoder is None or self.magi_image_encoder is None or self.image_proj_model is None:
@@ -866,9 +776,6 @@ class DiffSenseiPipeline:
                       "magi_pixel_values", "prompt_embeds", "prompt_input_ids"):
                 if p.get(k) is not None:
                     raise ValueError(f"panel {i}: agent= takes `prompt` and `ip_images`, not `{k}`")
-            if len(p.get("ip_images", ())) != len(p.get("ip_bbox", ())):
-                raise ValueError(f"panel {i}: `ip_images` must have the same length as `ip_bbox`. But they are in "
-                                 f"length {len(p.get('ip_images', ()))} and {len(p.get('ip_bbox', ()))}!")
 
     def _agent_panels(self, panels, agent, tokenizer_mllm, mllm_scale, max_new_tokens):
         """The demo's MLLM composition (scripts/demo/gradio.py:85-129) for every panel at once; returns the panels as
@@ -885,7 +792,7 @@ class DiffSenseiPipeline:
         magi_pv = self.magi_image_processor(images=flat, return_tensors="pt").pixel_values
         clip = self.image_encoder(clip_pv, output_hidden_states=True).hidden_states[-2]
         magi = self.magi_image_encoder(magi_pv).last_hidden_state[:, 0]
-        chars = [(clip[k * m:(k + 1) * m].unsqueeze(0), magi[k * m:(k + 1) * m].unsqueeze(0))
+        chars = [(clip[k * m:(k + 1) * m].unsqueeze(0), magi[k * m:(k + 1) * m].unsqueeze(0), None)
                  for k in range(len(panels))]
         embeds = [img[:, nv:, :] for img, _ in self._character_embeds(chars)]         # gradio.py:96-97
         prompts = [mllm_inputs(p["prompt"], tokenizer_mllm) for p in panels]
@@ -899,9 +806,8 @@ class DiffSenseiPipeline:
                 raise ValueError(f"panel {i}: the agent generated {o['num_gen_imgs']} images (num_gen_imgs); the "
                                  "mllm_scale blend needs exactly one")
             blend = o["img_gen_feat"].view(m, nv, -1) * mllm_scale + e.view(m, nv, -1) * (1 - mllm_scale)  # :108-109
-            bbox = [list(b) for b in list(p.get("ip_bbox", ()))[:m]]
-            bbox += [[0.0, 0.0, 0.0, 0.0]] * (m - len(bbox))
-            out_panels.append({**p, "ip_images": [], "ip_image_embeds": blend, "ip_bbox": bbox})
+            out_panels.append({**p, "ip_images": [], "ip_image_embeds": blend,
+                               "ip_bbox": _pad_boxes(p.get("ip_bbox", ()), m)})
         return out_panels
 
 

@@ -287,10 +287,11 @@ def test_agent_engine_matches_executed_reference(ops, name):
             assert rel_l2(o["img_gen_feat"].float(), case["img_gen_feat"]) < 2e-2
 
 
-def test_agent_feeds_the_pipeline_end_to_end(ops):
+def test_agent_feeds_the_unet_end_to_end(ops):
     """character ResamplerEngine -> AgentEngine.generate -> the demo's mllm_scale blend (gradio.py:108-109) ->
     DiffSenseiPipeline(ip_image_embeds=...) at TINY sizes; the blend is checked against the same composition built
-    from the fp32 oracle (transformers LLaMA + restated resamplers) and the pasted IP tokens against the blend."""
+    from the fp32 oracle (transformers LLaMA + restated resamplers), and the IP tokens in the conditions the denoise
+    loop receives against the blend."""
     import dataclasses
     import diffsensei_b200 as ds
     from diffsensei_b200.weights import random_state_dict, resampler_param_shapes, unet_param_shapes
@@ -336,12 +337,12 @@ def test_agent_feeds_the_pipeline_end_to_end(ops):
     pipe = ds.DiffSenseiPipeline(unet)
     pipe.register_manga_modules(None, res)
     seen = {}
-    inner = pipe.prepare_ip_image_embeds
+    inner = pipe.denoise
 
-    def spy(*a, **k):
-        seen["out"] = inner(*a, **k)
-        return seen["out"]
-    pipe.prepare_ip_image_embeds = spy
+    def spy(latents, prompt_embeds, *a, **k):
+        seen["pe"] = prompt_embeds.clone()
+        return inner(latents, prompt_embeds, *a, **k)
+    pipe.denoise = spy
     gp = torch.Generator().manual_seed(4)
     out = pipe(prompt="p", height=128, width=192, num_inference_steps=2, guidance_scale=7.5,
                generator=torch.Generator().manual_seed(0), ip_image_embeds=got, ip_scale=0.6,
@@ -353,6 +354,9 @@ def test_agent_feeds_the_pipeline_end_to_end(ops):
                clip_image_embeds=torch.randn(1, 4, 33, rc.embedding_dim, generator=gp),
                magi_image_embeds=torch.randn(1, 4, rc.magi_embedding_dim, generator=gp))
     assert out.latents.shape == (1, 4, 16, 24) and bool(torch.isfinite(out.latents).all())
-    pasted = seen["out"][1][0, ds.TINY.num_vision_tokens:5 * ds.TINY.num_vision_tokens].float().cpu()
+    # the UNet's conditions are [negative ; positive] rows of 77 text tokens + the image tokens, whose first
+    # num_vision_tokens are the Resampler's dummy tokens: the four pasted characters follow them in the positive row
+    nv = ds.TINY.num_vision_tokens
+    pasted = seen["pe"][1, 77 + nv:77 + 5 * nv].float().cpu()
     assert torch.equal(pasted, got.reshape(64, D).to(torch.bfloat16).float().cpu())
     assert rel_l2(pasted, want.reshape(64, D)) < 2e-2
