@@ -70,6 +70,7 @@ SIGNATURES = {
     "ds_conv_in_3x3": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "ds_im2col_latent": [_vp, _vp, _i, _i, _i, _vp],
     "ds_attention_self": [_vp, _vp, _i, _i, _i, _vp],
+    "ds_attention_self_pag": [_vp, _vp, _i, _i, _i, _i, _vp],
     "ds_attention_cross_ip": [C.POINTER(CrossIpArgs), _vp],
     "ds_nchw_to_nhwc": [_vp, _i, _vp, _i, _i, _i, _i, _vp],
     "ds_nhwc_to_nchw": [_vp, _vp, _i, _i, _i, _i, _i, _vp],
@@ -81,6 +82,10 @@ SIGNATURES = {
     "ds_cfg_euler_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp],
     "ds_cfg_ddim_inpaint_step": [_vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _vp],
     "ds_cfg_euler_inpaint_step": [_vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _vp],
+    "ds_cfg_pag_ddim_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp],
+    "ds_cfg_pag_euler_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp],
+    "ds_cfg_pag_ddim_inpaint_step": [_vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _vp],
+    "ds_cfg_pag_euler_inpaint_step": [_vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _vp],
     "ds_resampler_attn": [_vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "ds_attention_small": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i64, _i64, _i64, _i64, _f, _i, _vp],
     "ds_embed_tokens": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],

@@ -1,8 +1,11 @@
 // attn_wgmma.cu — fused attention for head_dim 64 on sm_90a warpgroup tensor cores.
 //
-// Three entry points:
+// Four entry points:
 //   ds_attention_self      self-attention (AttnProcessor2_0, src/models/attention_processor.py:69-81):
 //                          softmax(Q K^T / 8) V over the fused [B][N][3C] projection, no mask;
+//   ds_attention_self_pag  the same launch for perturbed-attention guidance: batch rows from first_perturbed_row on
+//                          take the identity attention map (out = V, diffusers' PAGCFGIdentitySelfAttnProcessor2_0),
+//                          their CTAs copy V instead of running the flash pipeline;
 //   ds_resampler_attn      the Resampler's perceiver attention (src/models/resampler.py:64-74), same math;
 //   ds_attention_cross_ip  out = softmax(Q Kt^T/8) Vt + scale * softmax(Q Kip^T/8 + M(bbox)) Vip
 //                          (MaskedIPAttnProcessor2_0, :231-258) in ONE pass over both key sets; the additive bbox mask
@@ -61,7 +64,24 @@ struct AttnParams {
   float ip_scale;
   // attn_cross_kernel: items are (batch, head, query tile) in that nesting; CTA c walks [c * items / ctas, ...)
   int heads, q_tiles, items;
+  // attn_stream_kernel, perturbed-attention guidance: when v_src is set, the CTAs of batch rows >= pag_b0 copy their
+  // rows of V (v_src [B][Nq][ld_src], head h at columns [64 h, +64)) to out instead of attending (identity map)
+  const __nv_bfloat16* v_src;
+  int ld_src, pag_b0;
 };
+
+// The identity-attention rows of one CTA: out rows [q0, q0 + 128) of (b, head) = V, 16-byte vectors.  Every thread of
+// the CTA takes part; no shared memory, no barrier.
+__device__ __forceinline__ void copy_v_rows(const AttnParams& p, int b, int head, int q0) {
+  const int rows = min(kQTile, p.Nq - q0);
+  const size_t src0 = (static_cast<size_t>(b) * p.Nq + q0) * p.ld_src + head * kHd;
+  const size_t dst0 = (static_cast<size_t>(b) * p.Nq + q0) * p.ldo + head * kHd;
+  for (int i = threadIdx.x; i < rows * (kHd / 8); i += kAttnThreads) {
+    const int r = i >> 3, c = (i & 7) * 8;
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>(p.v_src + src0 + static_cast<size_t>(r) * p.ld_src + c));
+    *reinterpret_cast<uint4*>(p.out + dst0 + static_cast<size_t>(r) * p.ldo + c) = v;
+  }
+}
 
 __device__ __forceinline__ float ex2(float x) {
   float y;
@@ -297,6 +317,13 @@ attn_stream_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const int tiles0 = (p.n_keys[0] + kKTile - 1) / kKTile;
   const int tiles1 = (p.n_keys[1] + kKTile - 1) / kKTile;
 
+  if (p.v_src != nullptr && b >= p.pag_b0) {  // a perturbed row (uniform per CTA): identity attention, out = V
+    pdl_launch_dependents();
+    pdl_wait();
+    copy_v_rows(p, b, head, q0);
+    return;
+  }
+
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK0);
@@ -522,7 +549,8 @@ static int launch_stream(const CUtensorMap& tmQ, const CUtensorMap& tmK0, const 
 
 // Q [B][Nq][ldq] (head h at column q_col0 + 64 h) against K / V [B][Nkv][ldkv] at columns k_col0 / v_col0 + 64 h
 static int launch_flash(const void* q, int ldq, int q_cols, const void* kv, int ldkv, int kv_cols, int k_col0,
-                        int v_col0, void* out, int ldo, int B, int Nq, int Nkv, int heads, float scale, cudaStream_t st) {
+                        int v_col0, void* out, int ldo, int B, int Nq, int Nkv, int heads, float scale, cudaStream_t st,
+                        const void* v_src = nullptr, int pag_b0 = 0) {
   DeviceInfo dev;
   if (!get_device(&dev)) return DS_ERR_CUDA;
   CUtensorMap tmQ, tmK;
@@ -537,6 +565,9 @@ static int launch_flash(const void* q, int ldq, int q_cols, const void* kv, int 
   p.k_col0 = k_col0;
   p.v_col0 = v_col0;
   p.scale_log2 = scale * kLog2e;
+  p.v_src = static_cast<const __nv_bfloat16*>(v_src);
+  p.ld_src = ldkv;
+  p.pag_b0 = pag_b0;
   return launch_stream(tmQ, tmK, tmK, p, B, heads, st);
 }
 
@@ -553,6 +584,21 @@ extern "C" int ds_attention_self(const void* qkv, void* out, int B, int N, int h
   // tensor maps over the fused [B][N][3C] projection; K and V are column offsets C and 2C
   return launch_flash(qkv, 3 * C, 3 * C, qkv, 3 * C, 3 * C, C, 2 * C, out, C, B, N, N, heads, 0.125f,
                       static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int ds_attention_self_pag(const void* qkv, void* out, int B, int N, int heads, int first_perturbed_row,
+                                     void* stream) {
+  DS_REQUIRE(qkv && out, "ds_attention_self_pag: NULL pointer");
+  DS_REQUIRE(B > 0 && N > 0 && heads > 0, "ds_attention_self_pag: bad shape");
+  DS_REQUIRE(first_perturbed_row >= 0 && first_perturbed_row <= B,
+             "ds_attention_self_pag: first_perturbed_row (%d) must be in [0, B = %d]", first_perturbed_row, B);
+  DS_REQUIRE((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
+             "ds_attention_self_pag: pointers must be 16-byte aligned");
+  const int C = heads * kHd;
+  // ds_attention_self's launch; the CTAs of rows >= first_perturbed_row copy the V third instead of attending
+  return launch_flash(qkv, 3 * C, 3 * C, qkv, 3 * C, 3 * C, C, 2 * C, out, C, B, N, N, heads, 0.125f,
+                      static_cast<cudaStream_t>(stream), static_cast<const __nv_bfloat16*>(qkv) + 2 * C,
+                      first_perturbed_row);
 }
 
 extern "C" int ds_resampler_attn(const void* q, const void* kv, void* out, int Bc, int nq, int n_kv, int heads,

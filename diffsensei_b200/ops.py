@@ -471,6 +471,27 @@ def attention_self(qkv: torch.Tensor, heads: int, out: Optional[torch.Tensor] = 
     return out
 
 
+def attention_self_pag(qkv: torch.Tensor, heads: int, first_perturbed_row: int,
+                       out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``attention_self`` on batch rows [0, first_perturbed_row) and the identity attention map of perturbed-attention
+    guidance on the rest: those rows of the output are the V columns [2C, 3C) of ``qkv``, copied.  One launch."""
+    _req(qkv, bf16, "attention_self_pag.qkv", 3)
+    B, N, C3 = qkv.shape
+    if C3 != 3 * heads * 64:
+        raise DsEngineError(f"attention_self_pag: last dim {C3} != 3*heads*64")
+    if not 0 <= int(first_perturbed_row) <= B:
+        raise DsEngineError(f"attention_self_pag: first_perturbed_row {first_perturbed_row} not in [0, {B}]")
+    if out is None:
+        out = torch.empty(B, N, heads * 64, dtype=bf16, device=qkv.device)
+    else:
+        _req(out, bf16, "attention_self_pag.out")
+        if out.shape != (B, N, heads * 64):
+            raise DsEngineError("attention_self_pag: out shape mismatch")
+    check(lib.ds_attention_self_pag(qkv.data_ptr(), out.data_ptr(), B, N, heads, int(first_perturbed_row), _stream()),
+          "ds_attention_self_pag")
+    return out
+
+
 def attention_cross_ip(q: torch.Tensor, kv_text: torch.Tensor, kv_ip: torch.Tensor, bbox: torch.Tensor, heads: int,
                        aspect_ratio: float, ip_scale: float, tokens_per_ip: int, num_dummy: int,
                        out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -629,6 +650,59 @@ def cfg_euler_inpaint_step_(noise_pred: torch.Tensor, latents: torch.Tensor, mod
     divided by coef[2].  coef: fp32 {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1), c0, c1} on the device."""
     _inpaint_step(lib.ds_cfg_euler_inpaint_step, "cfg_euler_inpaint_step", 5, noise_pred, latents, model_in, coef,
                   guidance, image_latents, noise, mask)
+
+
+def _pag_step(fn, name: str, ncoef: int, noise_pred, latents, model_in, coef, guidance, inpaint=None) -> None:
+    _req(noise_pred, bf16, f"{name}.noise_pred", 4)
+    _req(latents, f32, f"{name}.latents", 4)
+    _req(model_in, bf16, f"{name}.model_in", 4)
+    _req(coef, f32, f"{name}.coef", 1)
+    bs, H, W, Cc = latents.shape
+    if noise_pred.shape != (3 * bs, H, W, Cc) or model_in.shape != (3 * bs, H, W, Cc) or coef.numel() != ncoef:
+        raise DsEngineError(f"{name}: shape mismatch")
+    args = [noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(), float(guidance)]
+    if inpaint is not None:
+        image_latents, noise, mask = inpaint
+        _req(image_latents, f32, f"{name}.image_latents", 4)
+        _req(noise, f32, f"{name}.noise", 4)
+        _req(mask, torch.uint8, f"{name}.mask", 3)
+        if image_latents.shape != latents.shape or noise.shape != latents.shape or mask.shape != (bs, H, W):
+            raise DsEngineError(f"{name}: shape mismatch")
+        args += [image_latents.data_ptr(), noise.data_ptr(), mask.data_ptr()]
+    check(fn(*args, bs, H * W, Cc, _stream()), f"ds_{name}")
+
+
+def cfg_pag_ddim_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
+                       guidance: float) -> None:
+    """CFG + perturbed-attention guidance + DDIM, in place: noise_pred bf16 [3bs,H,W,4] = [uncond ; text ;
+    perturbed], eps = u + guidance (t - u) + s (t - p); latents fp32 [bs,H,W,4]; model_in bf16 [3bs,H,W,4] <- cat[x]*3.
+    coef: fp32 {alpha_prod_t, alpha_prod_t_prev, s} on the device (exactly 3 entries: s is the last)."""
+    _pag_step(lib.ds_cfg_pag_ddim_step, "cfg_pag_ddim_step", 3, noise_pred, latents, model_in, coef, guidance)
+
+
+def cfg_pag_euler_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
+                        guidance: float) -> None:
+    """``cfg_pag_ddim_step_`` with the Euler update; model_in <- cat[x / coef[2]]*3.  coef: fp32 {sigma_i,
+    sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1), s} on the device."""
+    _pag_step(lib.ds_cfg_pag_euler_step, "cfg_pag_euler_step", 4, noise_pred, latents, model_in, coef, guidance)
+
+
+def cfg_pag_ddim_inpaint_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor,
+                               coef: torch.Tensor, guidance: float, image_latents: torch.Tensor, noise: torch.Tensor,
+                               mask: torch.Tensor) -> None:
+    """``cfg_pag_ddim_step_`` followed by the inpaint blend of ``cfg_ddim_inpaint_step_``.  coef: fp32
+    {alpha_prod_t, alpha_prod_t_prev, c0, c1, s} on the device."""
+    _pag_step(lib.ds_cfg_pag_ddim_inpaint_step, "cfg_pag_ddim_inpaint_step", 5, noise_pred, latents, model_in, coef,
+              guidance, (image_latents, noise, mask))
+
+
+def cfg_pag_euler_inpaint_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor,
+                                coef: torch.Tensor, guidance: float, image_latents: torch.Tensor, noise: torch.Tensor,
+                                mask: torch.Tensor) -> None:
+    """``cfg_pag_euler_step_`` followed by the inpaint blend.  coef: fp32 {sigma_i, sigma_{i+1},
+    sqrt(sigma_{i+1}^2 + 1), c0, c1, s} on the device."""
+    _pag_step(lib.ds_cfg_pag_euler_inpaint_step, "cfg_pag_euler_inpaint_step", 6, noise_pred, latents, model_in,
+              coef, guidance, (image_latents, noise, mask))
 
 
 # ---------------------------------------------------------------------------------------------- encoder helpers

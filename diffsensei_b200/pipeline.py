@@ -42,14 +42,14 @@ import torch
 from . import ops
 from .image_processor import CLIPImageProcessor, VaeImageProcessor, ViTImageProcessor
 from .lora import AdapterRegistry, lora_targets, normalize_lora, split_components
-from .scheduler import DDIMScheduler, EulerDiscreteScheduler, get_timesteps
-from .unet import UNetMangaEngine
+from .scheduler import DDIMScheduler, EulerDiscreteScheduler, get_timesteps, pag_scales, with_pag_column
+from .unet import UNetMangaEngine, resolve_pag_layers
 
 bf16, f32 = torch.bfloat16, torch.float32
 
 # generate_page: what a captured stepper bakes in is the same for the whole page; everything else is per panel
 PAGE_KEYS = frozenset({"num_inference_steps", "guidance_scale", "ip_scale", "output_type", "use_graph",
-                       "max_batch_panels", "strength"})
+                       "max_batch_panels", "strength", "pag_scale", "pag_adaptive_scale"})
 PANEL_KEYS = frozenset({
     "prompt", "prompt_2", "negative_prompt", "negative_prompt_2", "height", "width", "num_samples", "generator",
     "latents", "original_size", "crops_coords_top_left", "target_size", "min_size_step", "ip_images",
@@ -126,7 +126,7 @@ class DiffSenseiPipeline:
     def __init__(self, unet: UNetMangaEngine,
                  scheduler: Optional[Union[DDIMScheduler, EulerDiscreteScheduler]] = None, vae_scale_factor: int = 8,
                  default_sample_size: int = 128, vae=None, text_encoder=None, text_encoder_2=None, image_encoder=None,
-                 tokenizer=None, tokenizer_2=None, vae_encoder=None):
+                 tokenizer=None, tokenizer_2=None, vae_encoder=None, pag_applied_layers="mid"):
         self.unet = unet
         self.vae = vae                      # VaeDecoderEngine (or None: latents out only)
         self.vae_encoder = vae_encoder      # VaeEncoderEngine (or None: no image= / img2img)
@@ -152,6 +152,8 @@ class DiffSenseiPipeline:
         self._steppers = {}
         self.max_cached_steppers = 8
         self._lora = AdapterRegistry()
+        self._pag_scale = 0.0
+        self.set_pag_applied_layers(pag_applied_layers)
 
     # ------------------------------------------------------------------------------ reference surface
     def register_manga_modules(self, magi_image_encoder=None, image_proj_model=None):
@@ -165,6 +167,41 @@ class DiffSenseiPipeline:
     @property
     def do_classifier_free_guidance(self):
         return self._guidance_scale > 1
+
+    # ------------------------------------------------------------------------------ perturbed-attention guidance
+    def set_pag_applied_layers(self, pag_applied_layers) -> None:
+        """diffusers' ``PAGMixin.set_pag_applied_layers``: the self-attention sites perturbed-attention guidance
+        perturbs, a string or a list of regular expressions matched with ``re.search`` against the module names
+        (``mid_block.attentions.0.transformer_blocks.3.attn1``; see ``unet.resolve_pag_layers``).  An identifier
+        that matches no site raises ``ValueError`` here (on first use when the pipeline has no UNet yet)."""
+        layers = [pag_applied_layers] if isinstance(pag_applied_layers, str) else list(pag_applied_layers)
+        cfg = getattr(self.unet, "cfg", None)
+        self._pag_sites = None if cfg is None else resolve_pag_layers(cfg, layers)
+        self._pag_applied_layers = layers
+
+    def _pag_site_set(self) -> frozenset:
+        if self._pag_sites is None:
+            self._pag_sites = resolve_pag_layers(self.unet.cfg, self._pag_applied_layers)
+        return self._pag_sites
+
+    @property
+    def pag_applied_layers(self) -> List[str]:
+        return list(self._pag_applied_layers)
+
+    @property
+    def pag_scale(self) -> float:
+        return self._pag_scale
+
+    @property
+    def do_perturbed_attention_guidance(self) -> bool:
+        """As diffusers: on when the last call's ``pag_scale > 0`` and at least one layer is selected."""
+        return self._pag_scale > 0 and len(self._pag_site_set()) > 0
+
+    def _pag(self, pag_scale: float, pag_adaptive_scale: float):
+        """What the stepper needs for a denoise at these scales: None when PAG is off, else (sites, scale, adaptive)."""
+        if float(pag_scale) > 0 and self._pag_site_set():
+            return self._pag_site_set(), float(pag_scale), float(pag_adaptive_scale)
+        return None
 
     def check_inputs(self, prompt, prompt_2, ip_images, ip_image_embeds, ip_bbox):
         if prompt is None:
@@ -327,55 +364,60 @@ class DiffSenseiPipeline:
                      add_time_ids: torch.Tensor, bbox: torch.Tensor, aspect_ratio: float,
                      dialog_bbox: Optional[torch.Tensor], num_inference_steps: int, guidance_scale: float,
                      use_graph: bool = True, chains: Optional[int] = None, start_index: int = 0,
-                     inpaint=None) -> "DenoiseStepper":
+                     inpaint=None, pag=None) -> "DenoiseStepper":
         return DenoiseStepper(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                               dialog_bbox, num_inference_steps, guidance_scale, use_graph, chains, start_index,
-                              inpaint)
+                              inpaint, pag)
 
     def stepper_for(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio, dialog_bbox,
                     num_inference_steps, guidance_scale, chains=None, start_index: int = 0,
-                    inpaint=None) -> "DenoiseStepper":
+                    inpaint=None, pag=None) -> "DenoiseStepper":
         """A graph-captured stepper loaded with this panel: a cached one of the same key is refilled in place
         (no re-capture), otherwise a new one is built and cached.  The start index is part of the key: the stepper
         bakes in its slice of the schedule (``set_timesteps`` would reset any scheduler state); so is whether it
-        inpaints, which selects the step kernel."""
+        inpaints, which selects the step kernel, and the perturbed-attention sites (``pag``: None when off).  The
+        PAG scales are not: they live in the coefficient table, which ``load_panel`` rewrites."""
         key = (tuple(latents.shape), tuple(prompt_embeds.shape), None if dialog_bbox is None else
                (tuple(dialog_bbox.shape), dialog_bbox.dtype == bf16), float(aspect_ratio), int(num_inference_steps),
                float(guidance_scale), self.unet.scales_key(), chains, self.unet._ip_weights_version(),
                type(self.scheduler).__name__, tuple(sorted(self.scheduler.config.items())), int(start_index),
-               inpaint is not None)
+               inpaint is not None, None if pag is None else tuple(sorted(pag[0])))
         st = self._steppers.get(key)
         if st is None:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                    dialog_bbox, num_inference_steps, guidance_scale, True, chains, start_index,
-                                   inpaint)
+                                   inpaint, pag)
             while len(self._steppers) >= self.max_cached_steppers:
                 self._steppers.pop(next(iter(self._steppers)))
             self._steppers[key] = st
         else:
-            st.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox, inpaint)
+            st.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox, inpaint, pag)
         return st
 
     @torch.no_grad()
     def denoise(self, latents: torch.Tensor, prompt_embeds: torch.Tensor, add_text_embeds: torch.Tensor,
                 add_time_ids: torch.Tensor, bbox: torch.Tensor, aspect_ratio: float,
                 dialog_bbox: Optional[torch.Tensor], num_inference_steps: int, guidance_scale: float,
-                use_graph: bool = True, on_step=None, start_index: int = 0, inpaint=None) -> torch.Tensor:
+                use_graph: bool = True, on_step=None, start_index: int = 0, inpaint=None, pag_scale: float = 0.0,
+                pag_adaptive_scale: float = 0.0) -> torch.Tensor:
         """pipeline_diffsensei.py:306-337.  ``latents`` NCHW fp32 (bs,4,h,w); conditions already concatenated
-        [negative ; positive] along batch (:293-304).  ``start_index``: run steps start_index .. T-1 of the
+        [negative ; positive] along batch (:293-304), or [negative ; positive ; positive] with perturbed-attention
+        guidance (``pag_scale > 0``: diffusers' PAGMixin; the third chunk takes the identity attention map at the
+        ``pag_applied_layers`` sites and eps = u + g (t - u) + s_i (t - p), s_i per ``scheduler.pag_scales``).  ``start_index``: run steps start_index .. T-1 of the
         ``num_inference_steps`` schedule (img2img; ``on_step`` then counts from 0).  ``inpaint``: (image_latents fp32
         (bs,4,h,w), noise fp32 (bs,4,h,w), latent mask uint8 (bs,h,w)); after every step the pixels where the mask is
         0 become the image latents noised to the next timestep (the image latents on the last step).  Returns the
         final latents, NCHW fp32."""
         self.unet.set_lora_scale(1.0)            # a direct unet(..., cross_attention_kwargs={"scale": s}) call may have left s
+        pag = self._pag(pag_scale, pag_adaptive_scale)
         if use_graph:
             st = self.stepper_for(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                   dialog_bbox, num_inference_steps, guidance_scale, start_index=start_index,
-                                  inpaint=inpaint)
+                                  inpaint=inpaint, pag=pag)
         else:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                    dialog_bbox, num_inference_steps, guidance_scale, False, start_index=start_index,
-                                   inpaint=inpaint)
+                                   inpaint=inpaint, pag=pag)
         for i, t in enumerate(st.timesteps):
             st.step(i)
             if on_step is not None:
@@ -401,13 +443,16 @@ class DiffSenseiPipeline:
                  negative_prompt_input_ids_2=None, clip_pixel_values=None, magi_pixel_values=None,
                  # img2img (diffusers' StableDiffusionXLImg2ImgPipeline): start from this image at `strength`;
                  # with mask_image, inpaint (StableDiffusionXLInpaintPipeline): redraw only where the mask is white
-                 image=None, strength: float = 0.3, mask_image=None):
+                 image=None, strength: float = 0.3, mask_image=None,
+                 # perturbed-attention guidance (diffusers' StableDiffusionXLPAGPipeline): on when pag_scale > 0
+                 pag_scale: float = 0.0, pag_adaptive_scale: float = 0.0):
         """A page of one panel: ``generate_page([panel], ...)[0]``, the panel holding this call's per-panel keywords
         (``PANEL_KEYS``) and the page the others.  Its input errors carry no panel index."""
         args = locals()
         panel = {k: args[k] for k in PANEL_KEYS}                    # as given, defaults included
         page = dict(num_inference_steps=num_inference_steps, guidance_scale=guidance_scale, output_type=output_type,
-                    max_batch_panels=PAGE_MAX_ROWS, strength=strength)
+                    max_batch_panels=PAGE_MAX_ROWS, strength=strength, pag_scale=pag_scale,
+                    pag_adaptive_scale=pag_adaptive_scale)
         t_start = self._check_page([panel], **page)
         return self._run_page([self._panel_job(panel)], t_start, ip_scale=ip_scale, use_graph=use_graph, **page)[0]
 
@@ -452,7 +497,7 @@ class DiffSenseiPipeline:
         return height, width
 
     def _check_page(self, panels, num_inference_steps, guidance_scale, output_type, max_batch_panels,
-                    strength) -> int:
+                    strength, pag_scale, pag_adaptive_scale) -> int:
         """The host-only checks of the page keywords.  Returns the first step of the schedule that image panels run
         (0 on a page without them, where ``strength`` is not used)."""
         if output_type not in ("latent", "pt", "np", "pil"):
@@ -465,6 +510,9 @@ class DiffSenseiPipeline:
                              "the fused CFG + scheduler update and does not implement the guidance-free variant")
         if int(max_batch_panels) < 1:
             raise ValueError(f"max_batch_panels must be >= 1, got {max_batch_panels}")
+        for name, v in (("pag_scale", pag_scale), ("pag_adaptive_scale", pag_adaptive_scale)):
+            if isinstance(v, bool) or not isinstance(v, (int, float)) or v != v or abs(v) == float("inf"):
+                raise ValueError(f"`{name}` must be a finite number, got {v!r}")
         if any(p.get("image") is not None for p in panels):
             return get_timesteps(num_inference_steps, strength)[0]
         return 0
@@ -475,7 +523,8 @@ class DiffSenseiPipeline:
                       ip_scale: float = 1.0, output_type: str = "latent", use_graph: bool = True,
                       max_batch_panels: int = PAGE_MAX_ROWS, agent=None, tokenizer_mllm=None,
                       mllm_scale: float = 0.4, max_new_tokens: int = 500,
-                      strength: float = 0.3) -> List[SimpleNamespace]:
+                      strength: float = 0.3, pag_scale: float = 0.0,
+                      pag_adaptive_scale: float = 0.0) -> List[SimpleNamespace]:
         """Several panels of a page in one call.  ``panels`` holds one dict per panel with the per-panel keywords of
         ``__call__`` (``PANEL_KEYS``); the keywords here are the same for the whole page.  Returns one
         ``SimpleNamespace(images=..., latents=...)`` per panel, in panel order, each ``torch.equal`` to
@@ -506,7 +555,13 @@ class DiffSenseiPipeline:
         noise, then the latent noise, at its turn in panel order; same-size images are encoded in one batch; img2img
         panels never share a denoise with text-to-image panels.  A panel with ``image`` and ``mask_image`` inpaints:
         it draws the posterior sample's noise, the latent noise and the discarded masked-image sample at its turn;
-        inpaint panels share a denoise only with inpaint panels of the same latent size."""
+        inpaint panels share a denoise only with inpaint panels of the same latent size.
+
+        ``pag_scale > 0`` adds perturbed-attention guidance (diffusers' SDXL PAG pipelines) at the
+        ``pag_applied_layers`` sites: every denoise runs [all negatives ; all positives ; all positives again], the
+        third block with the identity self-attention map, and guides with ``u + g (t - u) + s_i (t - p)``;
+        ``pag_adaptive_scale > 0`` lowers s_i with the timestep as diffusers does.  Departure: ``pag_scale`` defaults
+        to 0 (off), not diffusers' 3.0."""
         if not isinstance(panels, (list, tuple)) or len(panels) == 0:
             raise ValueError("generate_page needs a non-empty list of panel dicts")
         panels = [dict(p) for p in panels]
@@ -517,7 +572,8 @@ class DiffSenseiPipeline:
                 if k not in PANEL_KEYS:
                     raise ValueError(f"panel {i}: unknown key `{k}`")
         page = dict(num_inference_steps=num_inference_steps, guidance_scale=guidance_scale, output_type=output_type,
-                    max_batch_panels=max_batch_panels, strength=strength)
+                    max_batch_panels=max_batch_panels, strength=strength, pag_scale=pag_scale,
+                    pag_adaptive_scale=pag_adaptive_scale)
         t_start = self._check_page(panels, **page)
         if agent is not None:
             self._check_agent_panels(panels, tokenizer_mllm)
@@ -536,7 +592,7 @@ class DiffSenseiPipeline:
         return jobs
 
     def _run_page(self, jobs, t_start: int, *, num_inference_steps, guidance_scale, ip_scale, output_type, use_graph,
-                  max_batch_panels, strength) -> List[SimpleNamespace]:
+                  max_batch_panels, strength, pag_scale, pag_adaptive_scale) -> List[SimpleNamespace]:
         """The GPU half of a page whose panels (``_panel_job``) and keywords (``_check_page``) passed their checks."""
         # ---- front end, once per page
         dev = self.unet.device
@@ -561,6 +617,7 @@ class DiffSenseiPipeline:
 
         # ---- noise and per-panel condition rows, then one denoise + one decode per chunk
         self._guidance_scale = guidance_scale
+        self._pag_scale = float(pag_scale)
         self.set_ip_scale(ip_scale)
         self.scheduler.set_timesteps(num_inference_steps, device=dev)    # :248 (init_noise_sigma depends on it)
         for j in jobs:                                                     # panel order: the global RNG's order
@@ -578,14 +635,17 @@ class DiffSenseiPipeline:
         shapes = [(j.ns,) + tuple(j.latents.shape[-2:]) + kind(j) for j in jobs]
         for chunk in plan_page(shapes, max_batch_panels):
             rows = [self._panel_rows(jobs[i]) for i in chunk]
-            cat = lambda k: torch.cat([r[0][k] for r in rows] + [r[1][k] for r in rows], dim=0)
+            # [negatives ; positives], and the positives again as the perturbed block with PAG (diffusers' PAGMixin)
+            sides = (0, 1, 1) if self.do_perturbed_attention_guidance else (0, 1)
+            cat = lambda k: torch.cat([r[side][k] for side in sides for r in rows], dim=0)
             lat = torch.cat([jobs[i].latents for i in chunk], dim=0)
             inpaint = None
             if jobs[chunk[0]].inpaint is not None:
                 inpaint = tuple(torch.cat([jobs[i].inpaint[k] for i in chunk], dim=0) for k in range(3))
             final = self.denoise(lat, cat("pe"), cat("te"), cat("ti"), cat("bbox"), lat.shape[-2] / lat.shape[-1],
                                  cat("db"), num_inference_steps, guidance_scale, use_graph=use_graph,
-                                 start_index=t_start if jobs[chunk[0]].image is not None else 0, inpaint=inpaint)
+                                 start_index=t_start if jobs[chunk[0]].image is not None else 0, inpaint=inpaint,
+                                 pag_scale=pag_scale, pag_adaptive_scale=pag_adaptive_scale)
             # pipeline_diffsensei.py:339-363: latents / scaling_factor -> vae.decode -> image_processor.postprocess
             image = self.vae.decode_image(final) if output_type != "latent" else final
             r0 = 0
@@ -824,12 +884,15 @@ class DenoiseStepper:
     plugin boundary sees.
     With ``inpaint`` = (image_latents, noise, latent mask) the step is the scheduler's ``fused_inpaint_step_``, which
     reads those three per-panel buffers and the inpaint coefficient table.
+    With ``pag`` = (sites, pag_scale, pag_adaptive_scale) the batch is [uncond ; text ; perturbed] (3 bs rows), the
+    UNet perturbs the self-attention ``sites`` of the third chunk, and the step is ``fused_pag_step_`` over the
+    coefficient table with each step's PAG scale appended (``with_pag_column``).
     """
 
     @torch.no_grad()
     def __init__(self, pipe: DiffSenseiPipeline, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox,
                  aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale, use_graph=True, chains=None,
-                 start_index: int = 0, inpaint=None):
+                 start_index: int = 0, inpaint=None, pag=None):
         unet, dev = pipe.unet, pipe.unet.device
         self.unet, self.dev, self.guidance = unet, dev, float(guidance_scale)
         self.scheduler = pipe.scheduler
@@ -842,9 +905,13 @@ class DenoiseStepper:
         self.timesteps = pipe.scheduler.set_timesteps(num_inference_steps, device=dev)[s0:]
         self.inpaint = inpaint is not None
         if self.inpaint:                                                                # [T, 4] DDIM, [T, 5] Euler
-            self.coef_table = pipe.scheduler.inpaint_coefficient_table(s0, dev)
+            self.base_coef_table = pipe.scheduler.inpaint_coefficient_table(s0, dev)
         else:
-            self.coef_table = pipe.scheduler.coefficient_table(dev)[s0:]                # [T, 2] DDIM, [T, 3] Euler
+            self.base_coef_table = pipe.scheduler.coefficient_table(dev)[s0:]           # [T, 2] DDIM, [T, 3] Euler
+        self.coef_table = self.base_coef_table
+        # perturbed-attention guidance: the sites are baked into the graph, the scales live in the coefficient table
+        self.pag_sites = None if pag is None else frozenset(pag[0])
+        self.n_chunks = 2 if pag is None else 3
         # scale_model_input's divisor per step; dividing by a device element is a true division, as in the kernels
         self.in_div = torch.tensor(pipe.scheduler.model_input_divisors()[s0:], dtype=f32, device=dev)
         self.cond = None
@@ -852,7 +919,7 @@ class DenoiseStepper:
         self.inp_z = self.inp_n = self.inp_m = None
         self.round_bf16 = True
         self.graph = None
-        self.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox, inpaint)
+        self.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox, inpaint, pag)
         self.temb_cur = self.temb_table[0].clone()
         self.coef_cur = self.coef_table[0].clone()
         self._host_in = None
@@ -865,6 +932,8 @@ class DenoiseStepper:
         want = int(os.environ.get("DS_CHAINS", "1")) if chains is None else int(chains)
         self.chains = max(1, min(want, B2))
         self._parts, self._side = [(0, B2)], []
+        # first perturbed row of the whole batch (None: no PAG); each part gets it relative to its own slice
+        self._pag_row0 = None if pag is None else 2 * self.lat.shape[0]
         if self.chains > 1:
             cuts = [round(k * B2 / self.chains) for k in range(self.chains + 1)]
             self._parts = [(cuts[k], cuts[k + 1]) for k in range(self.chains) if cuts[k + 1] > cuts[k]]
@@ -888,17 +957,26 @@ class DenoiseStepper:
 
     @torch.no_grad()
     def load_panel(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox,
-                   inpaint=None) -> None:
+                   inpaint=None, pag=None) -> None:
         """Everything that is per panel and timestep-invariant, written INTO the buffers the captured graph reads:
         K|V of the text / IP tokens for all cross-attention layers, the time-embedding row-bias table for all T
-        steps, the bbox tables, the initial latents, and the inpaint state.  First call allocates; later calls (same
-        shapes) refill."""
+        steps, the bbox tables, the initial latents, the inpaint state, and the PAG scale of every step.  First call
+        allocates; later calls (same shapes) refill."""
         unet, dev = self.unet, self.dev
         bs = latents.shape[0]
-        if prompt_embeds.shape[0] != 2 * bs:
-            raise ValueError("denoise expects CFG-concatenated conditions: prompt_embeds.shape[0] == 2 * num_samples")
+        k = self.n_chunks
+        if (pag is None) != (self.pag_sites is None) or (pag is not None and frozenset(pag[0]) != self.pag_sites):
+            raise ValueError("load_panel: perturbed-attention sites differ from the stepper's")
+        if prompt_embeds.shape[0] != k * bs:
+            if k == 2:
+                raise ValueError("denoise expects CFG-concatenated conditions: prompt_embeds.shape[0] == 2 * "
+                                 "num_samples")
+            raise ValueError("denoise with perturbed-attention guidance expects [negative ; positive ; positive] "
+                             "conditions: prompt_embeds.shape[0] == 3 * num_samples")
         if (inpaint is not None) != self.inpaint:
             raise ValueError("load_panel: inpaint state presence differs from the stepper's")
+        if pag is not None:                                             # s_i of every step as the table's last column
+            self.coef_table = with_pag_column(self.base_coef_table, pag_scales(self.timesteps, pag[1], pag[2]))
         if inpaint is not None:
             z, n, m = inpaint
             if tuple(z.shape) != tuple(latents.shape) or tuple(n.shape) != tuple(latents.shape) or \
@@ -920,13 +998,13 @@ class DenoiseStepper:
         first = self.lat is None
         if first:
             self.lat = lat
-            self.model_in = torch.cat([x, x]).to(bf16).contiguous()                     # :315 (first step only)
+            self.model_in = torch.cat([x] * k).to(bf16).contiguous()                   # :315 (first step only)
         else:
             if lat.shape != self.lat.shape or (dialog_bbox is None) != (self.db is None):
                 raise ValueError("load_panel: latent shape / dialog_bbox presence differs from the captured panel")
             self.lat.copy_(lat)
-            self.model_in[:bs].copy_(x)
-            self.model_in[bs:].copy_(x)
+            for c in range(k):
+                self.model_in[c * bs:(c + 1) * bs].copy_(x)
         if dialog_bbox is not None:
             rb = dialog_bbox.dtype == bf16
             db = dialog_bbox.to(device=dev, dtype=f32).contiguous()
@@ -937,9 +1015,16 @@ class DenoiseStepper:
                     raise ValueError("load_panel: dialog_bbox dtype / shape differs from the captured panel")
                 self.db.copy_(db)
 
+    def _pag_args(self, s: int, e: int) -> dict:
+        """forward_nhwc's PAG keywords for batch rows [s, e): the first perturbed row relative to the slice."""
+        if self.pag_sites is None:
+            return {}
+        return dict(pag_sites=self.pag_sites, pag_row0=min(max(self._pag_row0 - s, 0), e - s))
+
     def _launch(self):
         if len(self._parts) == 1:
-            eps = self.unet.forward_nhwc(self.model_in, self.temb_cur, self.cond, self.db, self.round_bf16)  # :322-329
+            eps = self.unet.forward_nhwc(self.model_in, self.temb_cur, self.cond, self.db, self.round_bf16,
+                                         **self._pag_args(0, self.model_in.shape[0]))                     # :322-329
         else:
             main = torch.cuda.current_stream(self.dev)
             eps = self._eps
@@ -955,13 +1040,16 @@ class DenoiseStepper:
                     with torch.cuda.stream(st):
                         self.unet.forward_nhwc(self.model_in[s:e], self.temb_cur[s:e], self._cond_parts[k],
                                                None if self.db is None else self.db[s:e], self.round_bf16,
-                                               out=eps[s:e])
+                                               out=eps[s:e], **self._pag_args(s, e))
                 for st in self._side:
                     main.wait_stream(st)                       # join before the CFG blend needs both halves
             finally:
                 ops.SPLITK = prev_splitk
                 ops.GEMM_CHAINS = prev_chains
-        if self.inpaint:
+        if self.pag_sites is not None:
+            self.scheduler.fused_pag_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance,
+                                           (self.inp_z, self.inp_n, self.inp_m) if self.inpaint else None)
+        elif self.inpaint:
             self.scheduler.fused_inpaint_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance, self.inp_z,
                                                self.inp_n, self.inp_m)
         else:
@@ -986,8 +1074,8 @@ class DenoiseStepper:
         self.lat.copy_(nhwc)
         bs = self.lat.shape[0]
         x = nhwc / self.in_div[i]                                                       # step i's scale_model_input
-        self.model_in[:bs].copy_(x)
-        self.model_in[bs:].copy_(x)
+        for c in range(self.n_chunks):
+            self.model_in[c * bs:(c + 1) * bs].copy_(x)
         self.step(i)
         out_host.copy_(self.lat.permute(0, 3, 1, 2), non_blocking=True)                 # D2H
         torch.cuda.current_stream(self.dev).synchronize()

@@ -12,6 +12,8 @@ For img2img both add ``add_noise`` (diffusers' API, torch fp32), ``add_noise_coe
 two fp32 factors ``ds_vae_posterior`` reads) and ``set_begin_index``; ``get_timesteps`` is the strength rule.
 For inpainting, ``inpaint_coefficient_table`` adds each step's ``add_noise`` factors at the next timestep to the
 coefficient table, and ``fused_inpaint_step_`` runs the update with the blend (``ds_cfg_*_inpaint_step``).
+With perturbed-attention guidance, ``with_pag_column`` appends each step's PAG scale (``pag_scales``) to either table
+and ``fused_pag_step_`` runs the three-chunk update (``ds_cfg_pag_*``).
 
 ``scheduler_from_config`` picks one from a checkpoint's ``scheduler/scheduler_config.json``, the way diffusers does,
 and rejects any class or value whose arithmetic is not implemented here.
@@ -39,6 +41,22 @@ def _inpaint_table(sched, start_index: int, device) -> torch.Tensor:
     last = torch.tensor([1.0, 0.0], dtype=torch.float32)
     c = torch.stack([sched.add_noise_coefficients(i + 1) if i + 1 < n else last for i in range(s0, n)])
     return torch.cat([sched.coefficient_table("cpu")[s0:], c], dim=1).to(device)
+
+
+def pag_scales(timesteps, pag_scale: float, pag_adaptive_scale: float = 0.0) -> torch.Tensor:
+    """The perturbed-attention guidance scale of every step, fp32 [T]: diffusers' ``PAGMixin._get_pag_scale``, i.e.
+    ``pag_scale`` or, with ``pag_adaptive_scale > 0``, ``max(pag_scale - pag_adaptive_scale * (1000 - t), 0)`` in
+    its tensor arithmetic (the constant is 1000 whatever the schedule's length; every operation rounded to fp32)."""
+    t = torch.as_tensor([int(x) for x in timesteps], dtype=torch.int64)
+    if float(pag_adaptive_scale) > 0:
+        s = float(pag_scale) - float(pag_adaptive_scale) * (1000 - t)
+        return torch.where(s < 0, torch.zeros_like(s), s).to(torch.float32)
+    return torch.full((t.numel(),), float(pag_scale), dtype=torch.float32)
+
+
+def with_pag_column(table: torch.Tensor, scales: torch.Tensor) -> torch.Tensor:
+    """A coefficient table with the per-step PAG scale appended as its last column (what ``ds_cfg_pag_*`` read)."""
+    return torch.cat([table, scales.to(device=table.device, dtype=torch.float32).reshape(-1, 1)], dim=1).contiguous()
 
 
 # stable-diffusion-xl-base-1.0 scheduler/scheduler_config.json, the values both classes implement
@@ -97,6 +115,14 @@ class DDIMScheduler:
     def fused_inpaint_step_(self, noise_pred, latents, model_in, coef, guidance: float, image_latents, noise,
                             mask) -> None:
         ops.cfg_ddim_inpaint_step_(noise_pred, latents, model_in, coef, guidance, image_latents, noise, mask)
+
+    def fused_pag_step_(self, noise_pred, latents, model_in, coef, guidance: float, inpaint=None) -> None:
+        """CFG + perturbed-attention guidance + DDIM (``ds_cfg_pag_ddim[_inpaint]_step``): ``coef`` is a row of
+        ``with_pag_column`` over the plain or inpaint table, ``inpaint`` None or (image_latents, noise, mask)."""
+        if inpaint is None:
+            ops.cfg_pag_ddim_step_(noise_pred, latents, model_in, coef, guidance)
+        else:
+            ops.cfg_pag_ddim_inpaint_step_(noise_pred, latents, model_in, coef, guidance, *inpaint)
 
     def set_begin_index(self, begin_index: int = 0) -> None:
         """The loop's first step (img2img); DDIM's arithmetic does not depend on it, only add_noise's timestep."""
@@ -176,6 +202,13 @@ class EulerDiscreteScheduler:
     def fused_inpaint_step_(self, noise_pred, latents, model_in, coef, guidance: float, image_latents, noise,
                             mask) -> None:
         ops.cfg_euler_inpaint_step_(noise_pred, latents, model_in, coef, guidance, image_latents, noise, mask)
+
+    def fused_pag_step_(self, noise_pred, latents, model_in, coef, guidance: float, inpaint=None) -> None:
+        """CFG + perturbed-attention guidance + Euler (``ds_cfg_pag_euler[_inpaint]_step``); see DDIM's."""
+        if inpaint is None:
+            ops.cfg_pag_euler_step_(noise_pred, latents, model_in, coef, guidance)
+        else:
+            ops.cfg_pag_euler_inpaint_step_(noise_pred, latents, model_in, coef, guidance, *inpaint)
 
     def set_begin_index(self, begin_index: int = 0) -> None:
         """diffusers' ``set_begin_index``: the loop starts at sigma_{begin_index} (img2img)."""

@@ -19,6 +19,7 @@ exposes one object per site (``attention_processor.py``) for API compatibility.
 from __future__ import annotations
 
 import os
+import re
 from dataclasses import dataclass
 from types import SimpleNamespace
 from typing import Dict, List, Optional, Tuple
@@ -42,6 +43,31 @@ _CHAIN_LONG_MIN_ROWS, _CHAIN_SHORT_MIN_ROWS, _CHAIN_SHORT_MIN_C, _CHAIN_LONG_MIN
 
 
 bf16, f32 = torch.bfloat16, torch.float32
+
+
+def self_attention_sites(cfg: UNetConfig) -> List[str]:
+    """diffusers module name of every self-attention (``...transformer_blocks.<k>.attn1``), in execution order."""
+    return [f"{p}.transformer_blocks.{k}.attn1" for p, _c, depth in transformer_sites(cfg) for k in range(depth)]
+
+
+def resolve_pag_layers(cfg: UNetConfig, pag_applied_layers) -> frozenset:
+    """The self-attention sites perturbed-attention guidance perturbs, as diffusers' ``PAGMixin`` selects them: a
+    site is taken when ``re.search(identifier, name)`` matches its module name for one of the identifiers (a string
+    or a list of regular expressions), except where both the identifier's and the name's last dotted component are
+    the same number.  An identifier that matches no site raises ``ValueError``."""
+    layers = [pag_applied_layers] if isinstance(pag_applied_layers, str) else list(pag_applied_layers)
+    names = self_attention_sites(cfg)
+    out = set()
+    for lid in layers:
+        if not isinstance(lid, str):
+            raise ValueError(f"pag_applied_layers: identifiers must be strings, got {type(lid)}")
+        last = lid.split(".")[-1]
+        hit = [n for n in names if re.search(lid, n) is not None and
+               not (last.isnumeric() and n.split(".")[-1].isnumeric() and last == n.split(".")[-1])]
+        if not hit:
+            raise ValueError(f"Cannot find PAG layer to set attention processor for: {lid}")
+        out.update(hit)
+    return frozenset(out)
 
 
 @dataclass
@@ -399,7 +425,8 @@ class UNetMangaEngine:
         st2 = pool.take(r.cout) if want_stats else None
         return ops.conv3x3(h, r.w2, r.b2, residual=sc, chan_stats=st2), st2
 
-    def _transformer(self, p: str, x, x_st, cond: Conditions, pool, want_stats: bool = True):
+    def _transformer(self, p: str, x, x_st, cond: Conditions, pool, want_stats: bool = True,
+                     pag_sites: frozenset = frozenset(), pag_row0: Optional[int] = None):
         t, cfg = self.transformers[p], self.cfg
         B, H, W, Cc = x.shape
         h = ops.groupnorm_apply(x, self._stats(x, x_st, pool), t.norm[0], t.norm[1], cfg.norm_num_groups, 1e-6, False)
@@ -432,7 +459,10 @@ class UNetMangaEngine:
         h, qkv = ops.gemm_chain([produce_args(h.view(B, H * W, Cc), t.w_in, t.b_in),
                                  consume_args(None, b0.wqkv, b0.bqkv, b0.cs_qkv)], enable=short_run)
         for bi, blk in enumerate(t.blocks):
-            a = ops.attention_self(qkv, t.heads)
+            if pag_row0 is not None and pag_row0 < B and f"{p}.transformer_blocks.{bi}.attn1" in pag_sites:
+                a = ops.attention_self_pag(qkv, t.heads, pag_row0)       # rows >= pag_row0: identity attention
+            else:
+                a = ops.attention_self(qkv, t.heads)
             _, q = ops.gemm_chain([produce_args(a, blk.wo1, blk.bo1, residual=h, out=h),
                                    consume_args(None, blk.wq2, blk.bq2, blk.cs_q2, out=a)], enable=short_run)
             a = ops.attention_cross_ip(q, cond.kv_text[blk.layer], cond.kv_ip[blk.layer], cond.bbox, t.heads,
@@ -455,10 +485,15 @@ class UNetMangaEngine:
     # ------------------------------------------------------------------------------------------ forward
     def forward_nhwc(self, x: torch.Tensor, temb: torch.Tensor, cond: Conditions,
                      dialog_bbox: Optional[torch.Tensor] = None, round_bf16: bool = True,
-                     out: Optional[torch.Tensor] = None) -> torch.Tensor:
+                     out: Optional[torch.Tensor] = None, pag_sites: frozenset = frozenset(),
+                     pag_row0: Optional[int] = None) -> torch.Tensor:
         """x: bf16 [B,H,W,4]; temb: fp32 [B, sum(Cout)] from ``time_rowbias``; returns eps bf16 [B,H,W,4]
-        (written into ``out`` when given — a contiguous batch slice of a larger buffer is fine)."""
+        (written into ``out`` when given — a contiguous batch slice of a larger buffer is fine).
+        Perturbed-attention guidance: at the self-attention sites named in ``pag_sites`` (``resolve_pag_layers``),
+        batch rows ``pag_row0`` .. B-1 take the identity attention map, ``to_out(to_v(x))``."""
         cfg = self.cfg
+        tr = lambda p, h, st, **kw: self._transformer(p, h, st, cond, pool, pag_sites=pag_sites, pag_row0=pag_row0,
+                                                      **kw)
         ch, depth = cfg.block_out_channels, cfg.transformer_layers_per_block
         nlev = len(ch)
         B, H, W, _ = x.shape
@@ -481,7 +516,7 @@ class UNetMangaEngine:
                     skips[-1] = (h, st)
                 h, st = self._resnet(f"down_blocks.{i}.resnets.{j}", h, st, temb, pool)
                 if depth[i] > 0:
-                    h, st = self._transformer(f"down_blocks.{i}.attentions.{j}", h, st, cond, pool)
+                    h, st = tr(f"down_blocks.{i}.attentions.{j}", h, st)
                 skips.append((h, st))
             if i < nlev - 1:
                 w, b = self.down_convs[i]
@@ -489,7 +524,7 @@ class UNetMangaEngine:
                 h = ops.conv3x3(h, w, b, stride=2, chan_stats=st)
                 skips.append((h, st))
         h, st = self._resnet("mid_block.resnets.0", h, st, temb, pool)
-        h, st = self._transformer("mid_block.attentions.0", h, st, cond, pool)
+        h, st = tr("mid_block.attentions.0", h, st)
         h, st = self._resnet("mid_block.resnets.1", h, st, temb, pool)
         rdepth = list(reversed(depth))
         rch = list(reversed(ch))
@@ -502,7 +537,7 @@ class UNetMangaEngine:
                 h, st = self._resnet(f"up_blocks.{i}.resnets.{j}", h, st, temb, pool, skip=sk, skip_st=sk_st,
                                      want_stats=feeds_gn or has_attn)
                 if has_attn:
-                    h, st = self._transformer(f"up_blocks.{i}.attentions.{j}", h, st, cond, pool, want_stats=feeds_gn)
+                    h, st = tr(f"up_blocks.{i}.attentions.{j}", h, st, want_stats=feeds_gn)
             if i < nlev - 1:
                 if need_size:
                     Ho, Wo = skips[-1][0].shape[1:3]                                  # unet.py:312-313

@@ -255,6 +255,12 @@ int ds_im2col_latent(const void* x, void* a, int B, int H, int W, void* stream);
  *   out : bf16 [B][N][C]
  * --------------------------------------------------------------------------------------------- */
 int ds_attention_self(const void* qkv, void* out, int B, int N, int heads, void* stream);
+/* Perturbed-attention guidance (diffusers' PAGCFGIdentitySelfAttnProcessor2_0): ds_attention_self on batch rows
+ * [0, first_perturbed_row), bit for bit, and the identity attention map on rows [first_perturbed_row, B): out = the V
+ * columns [2C, 3C) of qkv, copied exactly.  One launch; the CTAs of perturbed rows copy instead of attending.
+ * 0 <= first_perturbed_row <= B (B: no perturbed row). */
+int ds_attention_self_pag(const void* qkv, void* out, int B, int N, int heads, int first_perturbed_row,
+                          void* stream);
 
 /* Fused text + masked-IP cross-attention, head_dim 64:                              [HBM-bound]
  *   out = softmax(Q Kt^T/8) Vt + scale * softmax(Q Kip^T/8 + M(bbox)) Vip
@@ -350,6 +356,28 @@ int ds_cfg_ddim_inpaint_step(const void* noise_pred, float* latents, void* model
 int ds_cfg_euler_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
                               float guidance, const float* image_latents, const float* noise, const uint8_t* mask,
                               int bs, int HW, int C, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * CFG + perturbed-attention guidance (diffusers' PAGMixin, do_classifier_free_guidance) fused with the four updates
+ * above.                                                                           [HBM-bound]
+ *   noise_pred : bf16 NHWC [3*bs][H][W][4], chunks [uncond ; text ; perturbed]
+ *   eps        = (e_uncond + guidance * (e_text - e_uncond)) + s * (e_text - e_perturbed)
+ * then the DDIM / Euler update (and the inpaint blend) of the matching CFG kernel, every operation rounded on its
+ * own in diffusers' eager order (the DDIM update too); model_in : bf16 NHWC [3*bs][H][W][4], the next UNet input
+ * in all three chunks.  s is the LAST entry of the step's coefficient row, read on the device:
+ *   DDIM {a_t, a_prev, s}                 Euler {sigma, sigma_next, sqrt(sigma_next^2 + 1), s}
+ *   DDIM inpaint {a_t, a_prev, c0, c1, s} Euler inpaint {sigma, sigma_next, sqrt(sigma_next^2 + 1), c0, c1, s}
+ * --------------------------------------------------------------------------------------------- */
+int ds_cfg_pag_ddim_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
+                         int bs, int HW, int C, void* stream);
+int ds_cfg_pag_euler_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
+                          int bs, int HW, int C, void* stream);
+int ds_cfg_pag_ddim_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
+                                 float guidance, const float* image_latents, const float* noise, const uint8_t* mask,
+                                 int bs, int HW, int C, void* stream);
+int ds_cfg_pag_euler_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
+                                  float guidance, const float* image_latents, const float* noise, const uint8_t* mask,
+                                  int bs, int HW, int C, void* stream);
 
 /* Perceiver attention of the character Resampler: 16 latent queries x (n_kv) keys per (character, head),
  * q and k each pre-scaled by dim_head^-0.25, fp32 softmax (src/models/resampler.py:64-74).
