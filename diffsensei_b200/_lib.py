@@ -78,14 +78,7 @@ SIGNATURES = {
     "ds_concat_channels": [_vp, _vp, _vp, _i, _i, _i, _vp],
     "ds_silu": [_vp, _vp, _i64, _vp],
     "ds_timestep_embedding": [_vp, _vp, _i, _i, _vp],
-    "ds_cfg_ddim_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp],
-    "ds_cfg_euler_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp],
-    "ds_cfg_ddim_inpaint_step": [_vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _vp],
-    "ds_cfg_euler_inpaint_step": [_vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _vp],
-    "ds_cfg_pag_ddim_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp],
-    "ds_cfg_pag_euler_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp],
-    "ds_cfg_pag_ddim_inpaint_step": [_vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _vp],
-    "ds_cfg_pag_euler_inpaint_step": [_vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _vp],
+    "ds_cfg_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp],
     "ds_resampler_attn": [_vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "ds_attention_small": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i64, _i64, _i64, _i64, _f, _i, _vp],
     "ds_embed_tokens": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],

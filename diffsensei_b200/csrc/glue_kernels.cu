@@ -164,10 +164,10 @@ __global__ void timestep_embedding_kernel(const float* __restrict__ t, __nv_bflo
 }
 
 // ------------------------------------------------------------------------------------------------
-// CFG blend + DDIM step (eta = 0, epsilon prediction), src/pipelines/pipeline_diffsensei.py:315,332-337.
-// C == 4: one thread per pixel (8-byte bf16 vectors, 16-byte fp32 vector).  The per-pixel arithmetic lives in
-// __device__ functions that the plain and the inpaint kernels share, so a masked-in pixel of the inpaint kernel is
-// the plain kernel's result bit for bit.
+// The end of every denoise step, fused: the guidance blend of the UNet's eps chunks, the scheduler update
+// (src/pipelines/pipeline_diffsensei.py:315-317,332-337) and the next step's UNet input, optionally followed by the
+// inpaint blend.  C == 4: one thread per pixel (8-byte bf16 vectors, 16-byte fp32 vector).  See ds_cfg_step in
+// dsengine.h for the coefficient row and the formulas.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void load_cfg_halves(const uint2* __restrict__ noise_pred, long long i, long long n_pix,
                                                 float u[4], float tt[4]) {
@@ -177,7 +177,7 @@ __device__ __forceinline__ void load_cfg_halves(const uint2* __restrict__ noise_
   tt[0] = bf16_lo(et.x), tt[1] = bf16_hi(et.x), tt[2] = bf16_lo(et.y), tt[3] = bf16_hi(et.y);
 }
 
-// xv <- DDIM(CFG(u, tt)) in place; coef = {alpha_prod_t, alpha_prod_t_prev}
+// xv <- DDIM(CFG(u, tt)) in place, the compiler free to contract into FMAs; coef = {alpha_prod_t, alpha_prod_t_prev}
 __device__ __forceinline__ void cfg_ddim_pixel(const float u[4], const float tt[4], float xv[4],
                                                const float* __restrict__ coef, float guidance) {
   const float a_t = coef[0], a_prev = coef[1];
@@ -191,34 +191,29 @@ __device__ __forceinline__ void cfg_ddim_pixel(const float u[4], const float tt[
   }
 }
 
-// xv <- Euler(CFG(u, tt)) in place; coef = {sigma_i, sigma_{i+1}, ...}
-__device__ __forceinline__ void cfg_euler_pixel(const float u[4], const float tt[4], float xv[4],
-                                                const float* __restrict__ coef, float guidance) {
+// diffusers' DDIMScheduler.step (eta = 0) on a guided eps, each operation rounded on its own; coef = {a_t, a_prev}
+__device__ __forceinline__ void ddim_update_rn(const float eps[4], float xv[4], const float* __restrict__ coef) {
+  const float a_t = coef[0], a_prev = coef[1];
+  const float sqrt_at = __fsqrt_rn(a_t), sqrt_1mat = __fsqrt_rn(__fsub_rn(1.0f, a_t));
+  const float sqrt_ap = __fsqrt_rn(a_prev), sqrt_1map = __fsqrt_rn(__fsub_rn(1.0f, a_prev));
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float x0 = __fdiv_rn(__fsub_rn(xv[j], __fmul_rn(sqrt_1mat, eps[j])), sqrt_at);
+    xv[j] = __fadd_rn(__fmul_rn(sqrt_ap, x0), __fmul_rn(sqrt_1map, eps[j]));
+  }
+}
+
+// diffusers' EulerDiscreteScheduler.step (s_churn = 0) on a guided eps, each operation rounded on its own;
+// coef = {sigma_i, sigma_{i+1}, ...}
+__device__ __forceinline__ void euler_update_rn(const float eps[4], float xv[4], const float* __restrict__ coef) {
   const float sigma = coef[0], sigma_next = coef[1];
   const float dt = __fsub_rn(sigma_next, sigma);
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
-    const float eps = __fadd_rn(u[j], __fmul_rn(guidance, __fsub_rn(tt[j], u[j])));
-    const float x0 = __fsub_rn(xv[j], __fmul_rn(sigma, eps));
+    const float x0 = __fsub_rn(xv[j], __fmul_rn(sigma, eps[j]));
     const float d = __fdiv_rn(__fsub_rn(xv[j], x0), sigma);
     xv[j] = __fadd_rn(xv[j], __fmul_rn(d, dt));
   }
-}
-
-// the fp32 master and both CFG halves of the next UNet input: bf16(xv / in_div), or bf16(xv) when in_div is NULL
-__device__ __forceinline__ void store_step(float4* __restrict__ latents, uint2* __restrict__ model_in, long long i,
-                                           long long n_pix, const float xv[4], const float* in_div) {
-  latents[i] = make_float4(xv[0], xv[1], xv[2], xv[3]);
-  uint2 o;
-  if (in_div) {
-    const float d = *in_div;
-    o = make_uint2(pack_bf16(__fdiv_rn(xv[0], d), __fdiv_rn(xv[1], d)),
-                   pack_bf16(__fdiv_rn(xv[2], d), __fdiv_rn(xv[3], d)));
-  } else {
-    o = make_uint2(pack_bf16(xv[0], xv[1]), pack_bf16(xv[2], xv[3]));
-  }
-  model_in[i] = o;
-  model_in[n_pix + i] = o;
 }
 
 // diffusers' 4-channel inpaint blend after the scheduler step: where mask == 0 the pixel becomes init_proper =
@@ -235,122 +230,10 @@ __device__ __forceinline__ void inpaint_blend(float xv[4], long long i, const fl
   xv[3] = __fadd_rn(__fmul_rn(c0, z.w), __fmul_rn(c1, n.w));
 }
 
-__global__ void cfg_ddim_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
-                                uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
-                                long long n_pix /* bs*HW */) {
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= n_pix) return;
-  float u[4], tt[4];
-  load_cfg_halves(noise_pred, i, n_pix, u, tt);
-  const float4 x = latents[i];
-  float xv[4] = {x.x, x.y, x.z, x.w};
-  cfg_ddim_pixel(u, tt, xv, coef, guidance);
-  store_step(latents, model_in, i, n_pix, xv, nullptr);
-}
-
-// ------------------------------------------------------------------------------------------------
-// CFG blend + Euler step (s_churn = 0, epsilon prediction) + the next step's scale_model_input,
-// src/pipelines/pipeline_diffsensei.py:315-317,332-337.  coef = {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1)}.
-// Every operation is rounded on its own (no FMA contraction), in diffusers' order, so the update is the one its
-// fp32 eager ops compute.  C == 4: one thread per pixel (8-byte bf16 vectors, 16-byte fp32 vector).
-// ------------------------------------------------------------------------------------------------
-__global__ void cfg_euler_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
-                                 uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
-                                 long long n_pix /* bs*HW */) {
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= n_pix) return;
-  float u[4], tt[4];
-  load_cfg_halves(noise_pred, i, n_pix, u, tt);
-  const float4 x = latents[i];
-  float xv[4] = {x.x, x.y, x.z, x.w};
-  cfg_euler_pixel(u, tt, xv, coef, guidance);
-  store_step(latents, model_in, i, n_pix, xv, coef + 2);
-}
-
-// ------------------------------------------------------------------------------------------------
-// The same two steps followed by the inpaint blend (diffusers' StableDiffusionXLInpaintPipeline, 4-channel UNet).
-// coef: DDIM {alpha_prod_t, alpha_prod_t_prev, c0, c1}, Euler {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1), c0,
-// c1}.  image_latents / noise fp32 NHWC [bs][HW][4], mask uint8 [bs][HW] (1: regenerate, 0: keep the image).
-// The next UNet input is computed from the blended latents.
-// ------------------------------------------------------------------------------------------------
-__global__ void cfg_ddim_inpaint_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
-                                        uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
-                                        const float4* __restrict__ image_latents, const float4* __restrict__ noise,
-                                        const unsigned char* __restrict__ mask, long long n_pix /* bs*HW */) {
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= n_pix) return;
-  float u[4], tt[4];
-  load_cfg_halves(noise_pred, i, n_pix, u, tt);
-  const float4 x = latents[i];
-  float xv[4] = {x.x, x.y, x.z, x.w};
-  cfg_ddim_pixel(u, tt, xv, coef, guidance);
-  inpaint_blend(xv, i, image_latents, noise, mask, coef[2], coef[3]);
-  store_step(latents, model_in, i, n_pix, xv, nullptr);
-}
-
-__global__ void cfg_euler_inpaint_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
-                                         uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
-                                         const float4* __restrict__ image_latents, const float4* __restrict__ noise,
-                                         const unsigned char* __restrict__ mask, long long n_pix /* bs*HW */) {
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= n_pix) return;
-  float u[4], tt[4];
-  load_cfg_halves(noise_pred, i, n_pix, u, tt);
-  const float4 x = latents[i];
-  float xv[4] = {x.x, x.y, x.z, x.w};
-  cfg_euler_pixel(u, tt, xv, coef, guidance);
-  inpaint_blend(xv, i, image_latents, noise, mask, coef[3], coef[4]);
-  store_step(latents, model_in, i, n_pix, xv, coef + 2);
-}
-
-// ------------------------------------------------------------------------------------------------
-// CFG + perturbed-attention guidance (diffusers' PAGMixin with classifier-free guidance) fused with the same two
-// scheduler steps, plain and inpaint.  noise_pred holds three chunks of n_pix pixels, [uncond ; text ; perturbed]:
-//   eps = (u + g * (t - u)) + s_i * (t - p)
-// with s_i = the LAST entry of the step's coefficient row (so one captured graph serves every pag_scale and adaptive
-// schedule).  Every operation is rounded on its own in diffusers' eager order (no FMA contraction), the DDIM update
-// included; the next UNet input goes to all three chunks of model_in.
-//   coef: DDIM {a_t, a_prev, s}, Euler {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1), s}; inpaint DDIM {a_t, a_prev,
-//   c0, c1, s}, Euler {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1), c0, c1, s}.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void load_pag_eps(const uint2* __restrict__ noise_pred, long long i, long long n_pix,
-                                             float guidance, float s, float eps[4]) {
-  const uint2 eu = __ldg(noise_pred + i), et = __ldg(noise_pred + n_pix + i), ep = __ldg(noise_pred + 2 * n_pix + i);
-  const float u[4] = {bf16_lo(eu.x), bf16_hi(eu.x), bf16_lo(eu.y), bf16_hi(eu.y)};
-  const float t[4] = {bf16_lo(et.x), bf16_hi(et.x), bf16_lo(et.y), bf16_hi(et.y)};
-  const float pp[4] = {bf16_lo(ep.x), bf16_hi(ep.x), bf16_lo(ep.y), bf16_hi(ep.y)};
-#pragma unroll
-  for (int j = 0; j < 4; ++j)
-    eps[j] = __fadd_rn(__fadd_rn(u[j], __fmul_rn(guidance, __fsub_rn(t[j], u[j]))), __fmul_rn(s, __fsub_rn(t[j], pp[j])));
-}
-
-// diffusers' DDIMScheduler.step (eta = 0) on a guided eps, each operation rounded on its own; coef = {a_t, a_prev}
-__device__ __forceinline__ void ddim_update_rn(const float eps[4], float xv[4], const float* __restrict__ coef) {
-  const float a_t = coef[0], a_prev = coef[1];
-  const float sqrt_at = __fsqrt_rn(a_t), sqrt_1mat = __fsqrt_rn(__fsub_rn(1.0f, a_t));
-  const float sqrt_ap = __fsqrt_rn(a_prev), sqrt_1map = __fsqrt_rn(__fsub_rn(1.0f, a_prev));
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float x0 = __fdiv_rn(__fsub_rn(xv[j], __fmul_rn(sqrt_1mat, eps[j])), sqrt_at);
-    xv[j] = __fadd_rn(__fmul_rn(sqrt_ap, x0), __fmul_rn(sqrt_1map, eps[j]));
-  }
-}
-
-// the Euler update of cfg_euler_pixel on a guided eps; coef = {sigma_i, sigma_{i+1}, ...}
-__device__ __forceinline__ void euler_update_rn(const float eps[4], float xv[4], const float* __restrict__ coef) {
-  const float sigma = coef[0], sigma_next = coef[1];
-  const float dt = __fsub_rn(sigma_next, sigma);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float x0 = __fsub_rn(xv[j], __fmul_rn(sigma, eps[j]));
-    const float d = __fdiv_rn(__fsub_rn(xv[j], x0), sigma);
-    xv[j] = __fadd_rn(xv[j], __fmul_rn(d, dt));
-  }
-}
-
-// store_step for the three chunks of a CFG + PAG batch
-__device__ __forceinline__ void store_step3(float4* __restrict__ latents, uint2* __restrict__ model_in, long long i,
-                                            long long n_pix, const float xv[4], const float* in_div) {
+// the fp32 master and all kChunks chunks of the next UNet input: bf16(xv / in_div), or bf16(xv) when in_div is NULL
+template <int kChunks>
+__device__ __forceinline__ void store_step(float4* __restrict__ latents, uint2* __restrict__ model_in, long long i,
+                                           long long n_pix, const float xv[4], const float* in_div) {
   latents[i] = make_float4(xv[0], xv[1], xv[2], xv[3]);
   uint2 o;
   if (in_div) {
@@ -360,47 +243,47 @@ __device__ __forceinline__ void store_step3(float4* __restrict__ latents, uint2*
   } else {
     o = make_uint2(pack_bf16(xv[0], xv[1]), pack_bf16(xv[2], xv[3]));
   }
-  model_in[i] = o;
-  model_in[n_pix + i] = o;
-  model_in[2 * n_pix + i] = o;
+#pragma unroll
+  for (int c = 0; c < kChunks; ++c) model_in[c * n_pix + i] = o;
 }
 
-template <bool kEuler>
-__global__ void cfg_pag_step_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
-                                    uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
-                                    long long n_pix /* bs*HW */) {
+// noise_pred holds kChunks chunks of n_pix pixels, [uncond ; text (; perturbed)]; coef is the step's row
+// {update (2 DDIM, 3 Euler) | c0, c1 if kInpaint | s if kChunks == 3}.
+template <bool kEuler, int kChunks, bool kInpaint>
+__global__ void cfg_step_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
+                                uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
+                                long long n_pix /* bs*HW */, const float4* __restrict__ image_latents,
+                                const float4* __restrict__ noise, const unsigned char* __restrict__ mask) {
+  static_assert(kChunks == 2 || kChunks == 3, "CFG (2 chunks) or CFG + PAG (3 chunks)");
+  constexpr int kC0 = kEuler ? 3 : 2;                 // {c0, c1} follow the update's coefficients
+  constexpr int kS = kC0 + (kInpaint ? 2 : 0);         // then the PAG scale
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= n_pix) return;
-  float eps[4];
-  load_pag_eps(noise_pred, i, n_pix, guidance, coef[kEuler ? 3 : 2], eps);
+  float u[4], tt[4];
+  load_cfg_halves(noise_pred, i, n_pix, u, tt);
   const float4 x = latents[i];
   float xv[4] = {x.x, x.y, x.z, x.w};
-  if (kEuler)
-    euler_update_rn(eps, xv, coef);
-  else
-    ddim_update_rn(eps, xv, coef);
-  store_step3(latents, model_in, i, n_pix, xv, kEuler ? coef + 2 : nullptr);
-}
-
-template <bool kEuler>
-__global__ void cfg_pag_inpaint_step_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
-                                            uint2* __restrict__ model_in, const float* __restrict__ coef,
-                                            float guidance, const float4* __restrict__ image_latents,
-                                            const float4* __restrict__ noise, const unsigned char* __restrict__ mask,
-                                            long long n_pix /* bs*HW */) {
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= n_pix) return;
-  constexpr int kC0 = kEuler ? 3 : 2;  // {c0, c1, s} follow the plain step's coefficients
-  float eps[4];
-  load_pag_eps(noise_pred, i, n_pix, guidance, coef[kC0 + 2], eps);
-  const float4 x = latents[i];
-  float xv[4] = {x.x, x.y, x.z, x.w};
-  if (kEuler)
-    euler_update_rn(eps, xv, coef);
-  else
-    ddim_update_rn(eps, xv, coef);
-  inpaint_blend(xv, i, image_latents, noise, mask, coef[kC0], coef[kC0 + 1]);
-  store_step3(latents, model_in, i, n_pix, xv, kEuler ? coef + 2 : nullptr);
+  if constexpr (!kEuler && kChunks == 2) {
+    // the CFG-only DDIM step has always let the compiler contract into FMAs; rounding it op by op changes its bits
+    cfg_ddim_pixel(u, tt, xv, coef, guidance);
+  } else {
+    float eps[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) eps[j] = __fadd_rn(u[j], __fmul_rn(guidance, __fsub_rn(tt[j], u[j])));
+    if constexpr (kChunks == 3) {
+      const float s = coef[kS];
+      const uint2 ep = __ldg(noise_pred + 2 * n_pix + i);  // perturbed chunk
+      const float pp[4] = {bf16_lo(ep.x), bf16_hi(ep.x), bf16_lo(ep.y), bf16_hi(ep.y)};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) eps[j] = __fadd_rn(eps[j], __fmul_rn(s, __fsub_rn(tt[j], pp[j])));
+    }
+    if constexpr (kEuler)
+      euler_update_rn(eps, xv, coef);
+    else
+      ddim_update_rn(eps, xv, coef);
+  }
+  if constexpr (kInpaint) inpaint_blend(xv, i, image_latents, noise, mask, coef[kC0], coef[kC0 + 1]);
+  store_step<kChunks>(latents, model_in, i, n_pix, xv, kEuler ? coef + 2 : nullptr);
 }
 
 }  // namespace ds
@@ -545,121 +428,33 @@ extern "C" int ds_timestep_embedding(const float* t, void* out, int rows, int di
   return DS_OK;
 }
 
-extern "C" int ds_cfg_ddim_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
-                                float guidance, int bs, int HW, int C, void* stream) {
-  DS_REQUIRE(noise_pred && latents && model_in && coef, "ds_cfg_ddim_step: NULL pointer");
-  DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "ds_cfg_ddim_step: only C == 4 latents are supported (got C=%d)", C);
-  DeviceInfo dev;
-  if (!get_device(&dev)) return DS_ERR_CUDA;
-  const long long n_pix = static_cast<long long>(bs) * HW;
-  cfg_ddim_kernel<<<static_cast<unsigned>((n_pix + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
-      guidance, n_pix);
-  DS_LAUNCH_OK("cfg_ddim_kernel");
-  return DS_OK;
-}
-
-extern "C" int ds_cfg_euler_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
-                                 float guidance, int bs, int HW, int C, void* stream) {
-  DS_REQUIRE(noise_pred && latents && model_in && coef, "ds_cfg_euler_step: NULL pointer");
-  DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "ds_cfg_euler_step: only C == 4 latents are supported (got C=%d)", C);
-  DeviceInfo dev;
-  if (!get_device(&dev)) return DS_ERR_CUDA;
-  const long long n_pix = static_cast<long long>(bs) * HW;
-  cfg_euler_kernel<<<static_cast<unsigned>((n_pix + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
-      guidance, n_pix);
-  DS_LAUNCH_OK("cfg_euler_kernel");
-  return DS_OK;
-}
-
-extern "C" int ds_cfg_ddim_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
-                                        float guidance, const float* image_latents, const float* noise,
-                                        const uint8_t* mask, int bs, int HW, int C, void* stream) {
-  DS_REQUIRE(noise_pred && latents && model_in && coef && image_latents && noise && mask,
-             "ds_cfg_ddim_inpaint_step: NULL pointer");
-  DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "ds_cfg_ddim_inpaint_step: only C == 4 latents are supported (got C=%d)", C);
-  DS_REQUIRE((reinterpret_cast<uintptr_t>(image_latents) & 15) == 0 && (reinterpret_cast<uintptr_t>(noise) & 15) == 0,
-             "ds_cfg_ddim_inpaint_step: image_latents / noise must be 16-byte aligned");
-  DeviceInfo dev;
-  if (!get_device(&dev)) return DS_ERR_CUDA;
-  const long long n_pix = static_cast<long long>(bs) * HW;
-  cfg_ddim_inpaint_kernel<<<static_cast<unsigned>((n_pix + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
-      guidance, reinterpret_cast<const float4*>(image_latents), reinterpret_cast<const float4*>(noise), mask, n_pix);
-  DS_LAUNCH_OK("cfg_ddim_inpaint_kernel");
-  return DS_OK;
-}
-
-extern "C" int ds_cfg_euler_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
-                                         float guidance, const float* image_latents, const float* noise,
-                                         const uint8_t* mask, int bs, int HW, int C, void* stream) {
-  DS_REQUIRE(noise_pred && latents && model_in && coef && image_latents && noise && mask,
-             "ds_cfg_euler_inpaint_step: NULL pointer");
-  DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "ds_cfg_euler_inpaint_step: only C == 4 latents are supported (got C=%d)", C);
-  DS_REQUIRE((reinterpret_cast<uintptr_t>(image_latents) & 15) == 0 && (reinterpret_cast<uintptr_t>(noise) & 15) == 0,
-             "ds_cfg_euler_inpaint_step: image_latents / noise must be 16-byte aligned");
-  DeviceInfo dev;
-  if (!get_device(&dev)) return DS_ERR_CUDA;
-  const long long n_pix = static_cast<long long>(bs) * HW;
-  cfg_euler_inpaint_kernel<<<static_cast<unsigned>((n_pix + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
-      guidance, reinterpret_cast<const float4*>(image_latents), reinterpret_cast<const float4*>(noise), mask, n_pix);
-  DS_LAUNCH_OK("cfg_euler_inpaint_kernel");
-  return DS_OK;
-}
-
-static int cfg_pag_step(bool euler, const char* name, const void* noise_pred, float* latents, void* model_in,
-                        const float* coef, float guidance, const float* image_latents, const float* noise,
-                        const uint8_t* mask, bool inpaint, int bs, int HW, int C, void* stream) {
-  DS_REQUIRE(noise_pred && latents && model_in && coef, "%s: NULL pointer", name);
-  DS_REQUIRE(!inpaint || (image_latents && noise && mask), "%s: NULL pointer", name);
-  DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "%s: only C == 4 latents are supported (got C=%d)", name, C);
+extern "C" int ds_cfg_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
+                           int update, int chunks, const float* image_latents, const float* noise, const uint8_t* mask,
+                           int bs, int HW, int C, void* stream) {
+  const bool inpaint = image_latents || noise || mask;
+  DS_REQUIRE(noise_pred && latents && model_in && coef, "ds_cfg_step: NULL pointer");
+  DS_REQUIRE(!inpaint || (image_latents && noise && mask),
+             "ds_cfg_step: image_latents / noise / mask must all be given or all be NULL");
+  DS_REQUIRE(update == 0 || update == 1, "ds_cfg_step: update must be 0 (DDIM) or 1 (Euler), got %d", update);
+  DS_REQUIRE(chunks == 2 || chunks == 3, "ds_cfg_step: chunks must be 2 or 3, got %d", chunks);
+  DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "ds_cfg_step: only C == 4 latents are supported (got C=%d)", C);
   DS_REQUIRE(!inpaint || ((reinterpret_cast<uintptr_t>(image_latents) & 15) == 0 &&
                           (reinterpret_cast<uintptr_t>(noise) & 15) == 0),
-             "%s: image_latents / noise must be 16-byte aligned", name);
+             "ds_cfg_step: image_latents / noise must be 16-byte aligned");
   DeviceInfo dev;
   if (!get_device(&dev)) return DS_ERR_CUDA;
+  using StepKernel = void (*)(const uint2*, float4*, uint2*, const float*, float, long long, const float4*,
+                              const float4*, const unsigned char*);
+  static constexpr StepKernel kKernels[2][2][2] = {  // [update][chunks - 2][inpaint]
+      {{cfg_step_kernel<false, 2, false>, cfg_step_kernel<false, 2, true>},
+       {cfg_step_kernel<false, 3, false>, cfg_step_kernel<false, 3, true>}},
+      {{cfg_step_kernel<true, 2, false>, cfg_step_kernel<true, 2, true>},
+       {cfg_step_kernel<true, 3, false>, cfg_step_kernel<true, 3, true>}}};
   const long long n_pix = static_cast<long long>(bs) * HW;
-  const unsigned blocks = static_cast<unsigned>((n_pix + 255) / 256);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const uint2* np = static_cast<const uint2*>(noise_pred);
-  float4* lat = reinterpret_cast<float4*>(latents);
-  uint2* mi = static_cast<uint2*>(model_in);
-  if (inpaint) {
-    auto k = euler ? cfg_pag_inpaint_step_kernel<true> : cfg_pag_inpaint_step_kernel<false>;
-    k<<<blocks, 256, 0, st>>>(np, lat, mi, coef, guidance, reinterpret_cast<const float4*>(image_latents),
-                              reinterpret_cast<const float4*>(noise), mask, n_pix);
-  } else {
-    auto k = euler ? cfg_pag_step_kernel<true> : cfg_pag_step_kernel<false>;
-    k<<<blocks, 256, 0, st>>>(np, lat, mi, coef, guidance, n_pix);
-  }
-  DS_LAUNCH_OK(name);
+  kKernels[update][chunks - 2][inpaint]<<<static_cast<unsigned>((n_pix + 255) / 256), 256, 0,
+                                          static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
+      guidance, n_pix, reinterpret_cast<const float4*>(image_latents), reinterpret_cast<const float4*>(noise), mask);
+  DS_LAUNCH_OK("cfg_step_kernel");
   return DS_OK;
-}
-
-extern "C" int ds_cfg_pag_ddim_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
-                                    float guidance, int bs, int HW, int C, void* stream) {
-  return cfg_pag_step(false, "ds_cfg_pag_ddim_step", noise_pred, latents, model_in, coef, guidance, nullptr, nullptr,
-                      nullptr, false, bs, HW, C, stream);
-}
-
-extern "C" int ds_cfg_pag_euler_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
-                                     float guidance, int bs, int HW, int C, void* stream) {
-  return cfg_pag_step(true, "ds_cfg_pag_euler_step", noise_pred, latents, model_in, coef, guidance, nullptr, nullptr,
-                      nullptr, false, bs, HW, C, stream);
-}
-
-extern "C" int ds_cfg_pag_ddim_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
-                                            float guidance, const float* image_latents, const float* noise,
-                                            const uint8_t* mask, int bs, int HW, int C, void* stream) {
-  return cfg_pag_step(false, "ds_cfg_pag_ddim_inpaint_step", noise_pred, latents, model_in, coef, guidance,
-                      image_latents, noise, mask, true, bs, HW, C, stream);
-}
-
-extern "C" int ds_cfg_pag_euler_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
-                                             float guidance, const float* image_latents, const float* noise,
-                                             const uint8_t* mask, int bs, int HW, int C, void* stream) {
-  return cfg_pag_step(true, "ds_cfg_pag_euler_inpaint_step", noise_pred, latents, model_in, coef, guidance,
-                      image_latents, noise, mask, true, bs, HW, C, stream);
 }

@@ -588,121 +588,37 @@ def timestep_embedding(t: torch.Tensor, dim: int, out: Optional[torch.Tensor] = 
     return out
 
 
-def cfg_ddim_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
-                   guidance: float) -> None:
-    """In place: latents (fp32 NHWC [bs,H,W,4]) <- DDIM(CFG(noise_pred)); model_in (bf16 [2bs,H,W,4]) <- cat[x]*2."""
-    _req(noise_pred, bf16, "cfg_ddim_step.noise_pred", 4)
-    _req(latents, f32, "cfg_ddim_step.latents", 4)
-    _req(model_in, bf16, "cfg_ddim_step.model_in", 4)
-    _req(coef, f32, "cfg_ddim_step.coef", 1)
+def cfg_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
+              guidance: float, euler: bool, inpaint=None) -> None:
+    """The fused end of a denoise step (``ds_cfg_step``), in place.  noise_pred bf16 [k*bs,H,W,4] holds k = 2 chunks
+    [uncond ; text] (CFG) or k = 3 [uncond ; text ; perturbed] (CFG + perturbed-attention guidance):
+    eps = u + guidance (t - u) [+ s (t - p)].  latents fp32 NHWC [bs,H,W,4] <- DDIM or (``euler``) Euler update;
+    model_in bf16 [k*bs,H,W,4] <- cat[x]*k (DDIM) or cat[x / coef[2]]*k (Euler).  ``inpaint`` None or
+    (image_latents, noise, mask): fp32 NHWC [bs,H,W,4] twice and uint8 [bs,H,W]; where mask is 0 the latents become
+    c0 * image_latents + c1 * noise.  coef: the step's fp32 row on the device, exactly
+    DDIM {alpha_prod_t, alpha_prod_t_prev} / Euler {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1)},
+    then {c0, c1} with ``inpaint``, then s with 3 chunks."""
+    _req(noise_pred, bf16, "cfg_step.noise_pred", 4)
+    _req(latents, f32, "cfg_step.latents", 4)
+    _req(model_in, bf16, "cfg_step.model_in", 4)
+    _req(coef, f32, "cfg_step.coef", 1)
     bs, H, W, Cc = latents.shape
-    if noise_pred.shape != (2 * bs, H, W, Cc) or model_in.shape != (2 * bs, H, W, Cc) or coef.numel() < 2:
-        raise DsEngineError("cfg_ddim_step: shape mismatch")
-    check(lib.ds_cfg_ddim_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(),
-                               float(guidance), bs, H * W, Cc, _stream()), "ds_cfg_ddim_step")
-
-
-def cfg_euler_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
-                    guidance: float) -> None:
-    """In place: latents (fp32 NHWC [bs,H,W,4]) <- Euler(CFG(noise_pred)); model_in (bf16 [2bs,H,W,4]) <-
-    cat[x / coef[2]]*2.  coef: fp32 {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1)} on the device."""
-    _req(noise_pred, bf16, "cfg_euler_step.noise_pred", 4)
-    _req(latents, f32, "cfg_euler_step.latents", 4)
-    _req(model_in, bf16, "cfg_euler_step.model_in", 4)
-    _req(coef, f32, "cfg_euler_step.coef", 1)
-    bs, H, W, Cc = latents.shape
-    if noise_pred.shape != (2 * bs, H, W, Cc) or model_in.shape != (2 * bs, H, W, Cc) or coef.numel() < 3:
-        raise DsEngineError("cfg_euler_step: shape mismatch")
-    check(lib.ds_cfg_euler_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(),
-                                float(guidance), bs, H * W, Cc, _stream()), "ds_cfg_euler_step")
-
-
-def _inpaint_step(fn, name: str, ncoef: int, noise_pred, latents, model_in, coef, guidance, image_latents, noise,
-                  mask) -> None:
-    _req(noise_pred, bf16, f"{name}.noise_pred", 4)
-    _req(latents, f32, f"{name}.latents", 4)
-    _req(model_in, bf16, f"{name}.model_in", 4)
-    _req(coef, f32, f"{name}.coef", 1)
-    _req(image_latents, f32, f"{name}.image_latents", 4)
-    _req(noise, f32, f"{name}.noise", 4)
-    _req(mask, torch.uint8, f"{name}.mask", 3)
-    bs, H, W, Cc = latents.shape
-    if noise_pred.shape != (2 * bs, H, W, Cc) or model_in.shape != (2 * bs, H, W, Cc) or coef.numel() < ncoef or \
-            image_latents.shape != latents.shape or noise.shape != latents.shape or mask.shape != (bs, H, W):
-        raise DsEngineError(f"{name}: shape mismatch")
-    check(fn(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(), float(guidance),
-             image_latents.data_ptr(), noise.data_ptr(), mask.data_ptr(), bs, H * W, Cc, _stream()), f"ds_{name}")
-
-
-def cfg_ddim_inpaint_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
-                           guidance: float, image_latents: torch.Tensor, noise: torch.Tensor, mask: torch.Tensor) -> None:
-    """``cfg_ddim_step_`` followed by the inpaint blend: where ``mask`` (uint8 [bs,H,W]) is 0 the latents become
-    ``coef[2] * image_latents + coef[3] * noise`` (both fp32 NHWC [bs,H,W,4]); model_in is made from the blend.
-    coef: fp32 {alpha_prod_t, alpha_prod_t_prev, c0, c1} on the device."""
-    _inpaint_step(lib.ds_cfg_ddim_inpaint_step, "cfg_ddim_inpaint_step", 4, noise_pred, latents, model_in, coef,
-                  guidance, image_latents, noise, mask)
-
-
-def cfg_euler_inpaint_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor,
-                            coef: torch.Tensor, guidance: float, image_latents: torch.Tensor, noise: torch.Tensor,
-                            mask: torch.Tensor) -> None:
-    """``cfg_euler_step_`` followed by the inpaint blend (see ``cfg_ddim_inpaint_step_``); model_in is the blend
-    divided by coef[2].  coef: fp32 {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1), c0, c1} on the device."""
-    _inpaint_step(lib.ds_cfg_euler_inpaint_step, "cfg_euler_inpaint_step", 5, noise_pred, latents, model_in, coef,
-                  guidance, image_latents, noise, mask)
-
-
-def _pag_step(fn, name: str, ncoef: int, noise_pred, latents, model_in, coef, guidance, inpaint=None) -> None:
-    _req(noise_pred, bf16, f"{name}.noise_pred", 4)
-    _req(latents, f32, f"{name}.latents", 4)
-    _req(model_in, bf16, f"{name}.model_in", 4)
-    _req(coef, f32, f"{name}.coef", 1)
-    bs, H, W, Cc = latents.shape
-    if noise_pred.shape != (3 * bs, H, W, Cc) or model_in.shape != (3 * bs, H, W, Cc) or coef.numel() != ncoef:
-        raise DsEngineError(f"{name}: shape mismatch")
-    args = [noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(), float(guidance)]
+    chunks = noise_pred.shape[0] // bs if bs else 0
+    ncoef = (3 if euler else 2) + (0 if inpaint is None else 2) + (chunks == 3)
+    if chunks not in (2, 3) or noise_pred.shape != (chunks * bs, H, W, Cc) or model_in.shape != noise_pred.shape \
+            or coef.numel() != ncoef:
+        raise DsEngineError("cfg_step: shape mismatch")
+    ptrs = [None] * 3
     if inpaint is not None:
         image_latents, noise, mask = inpaint
-        _req(image_latents, f32, f"{name}.image_latents", 4)
-        _req(noise, f32, f"{name}.noise", 4)
-        _req(mask, torch.uint8, f"{name}.mask", 3)
+        _req(image_latents, f32, "cfg_step.image_latents", 4)
+        _req(noise, f32, "cfg_step.noise", 4)
+        _req(mask, torch.uint8, "cfg_step.mask", 3)
         if image_latents.shape != latents.shape or noise.shape != latents.shape or mask.shape != (bs, H, W):
-            raise DsEngineError(f"{name}: shape mismatch")
-        args += [image_latents.data_ptr(), noise.data_ptr(), mask.data_ptr()]
-    check(fn(*args, bs, H * W, Cc, _stream()), f"ds_{name}")
-
-
-def cfg_pag_ddim_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
-                       guidance: float) -> None:
-    """CFG + perturbed-attention guidance + DDIM, in place: noise_pred bf16 [3bs,H,W,4] = [uncond ; text ;
-    perturbed], eps = u + guidance (t - u) + s (t - p); latents fp32 [bs,H,W,4]; model_in bf16 [3bs,H,W,4] <- cat[x]*3.
-    coef: fp32 {alpha_prod_t, alpha_prod_t_prev, s} on the device (exactly 3 entries: s is the last)."""
-    _pag_step(lib.ds_cfg_pag_ddim_step, "cfg_pag_ddim_step", 3, noise_pred, latents, model_in, coef, guidance)
-
-
-def cfg_pag_euler_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
-                        guidance: float) -> None:
-    """``cfg_pag_ddim_step_`` with the Euler update; model_in <- cat[x / coef[2]]*3.  coef: fp32 {sigma_i,
-    sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1), s} on the device."""
-    _pag_step(lib.ds_cfg_pag_euler_step, "cfg_pag_euler_step", 4, noise_pred, latents, model_in, coef, guidance)
-
-
-def cfg_pag_ddim_inpaint_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor,
-                               coef: torch.Tensor, guidance: float, image_latents: torch.Tensor, noise: torch.Tensor,
-                               mask: torch.Tensor) -> None:
-    """``cfg_pag_ddim_step_`` followed by the inpaint blend of ``cfg_ddim_inpaint_step_``.  coef: fp32
-    {alpha_prod_t, alpha_prod_t_prev, c0, c1, s} on the device."""
-    _pag_step(lib.ds_cfg_pag_ddim_inpaint_step, "cfg_pag_ddim_inpaint_step", 5, noise_pred, latents, model_in, coef,
-              guidance, (image_latents, noise, mask))
-
-
-def cfg_pag_euler_inpaint_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor,
-                                coef: torch.Tensor, guidance: float, image_latents: torch.Tensor, noise: torch.Tensor,
-                                mask: torch.Tensor) -> None:
-    """``cfg_pag_euler_step_`` followed by the inpaint blend.  coef: fp32 {sigma_i, sigma_{i+1},
-    sqrt(sigma_{i+1}^2 + 1), c0, c1, s} on the device."""
-    _pag_step(lib.ds_cfg_pag_euler_inpaint_step, "cfg_pag_euler_inpaint_step", 6, noise_pred, latents, model_in,
-              coef, guidance, (image_latents, noise, mask))
+            raise DsEngineError("cfg_step: shape mismatch")
+        ptrs = [image_latents.data_ptr(), noise.data_ptr(), mask.data_ptr()]
+    check(lib.ds_cfg_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(),
+                          float(guidance), int(bool(euler)), chunks, *ptrs, bs, H * W, Cc, _stream()), "ds_cfg_step")
 
 
 # ---------------------------------------------------------------------------------------------- encoder helpers

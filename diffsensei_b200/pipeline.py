@@ -18,15 +18,15 @@ raises, it does not fall back to anything.
 ``vae_encoder=``): the image is encoded, noised to the schedule's step ``t_start`` and denoised from there.
 ``mask_image=`` with ``image=`` redraws only the masked part, as diffusers' ``StableDiffusionXLInpaintPipeline`` does
 with a 4-channel UNet: after every step the unmasked latent pixels are reset to the image latents noised to the next
-timestep (fused into the step kernel, ``ds_cfg_*_inpaint_step``).  Departures from that pipeline's defaults: the
+timestep (fused into the step kernel, ``ds_cfg_step``).  Departures from that pipeline's defaults: the
 panel size follows the img2img rule (the given ``height`` / ``width``, else the image's own; diffusers defaults to
 1024 x 1024), and ``strength`` keeps its 0.3 default (diffusers' inpaint default is 0.9999).
 
 Loop structure on the GPU (one process per GPU, one stream):
   once per panel : K|V projections of text and IP tokens for all cross-attention layers, time-embedding
                    row-bias table for all T steps, the scheduler's coefficient table
-  per step       : ONE CUDA-graph replay = UNet forward (NHWC bf16) + the scheduler's fused CFG update (DDIM or
-                   Euler), preceded by two tiny device-to-device copies that select this step's row of the two tables.
+  per step       : ONE CUDA-graph replay = UNet forward (NHWC bf16) + the scheduler's fused CFG update
+                   (``ds_cfg_step``, DDIM or Euler), preceded by two tiny device-to-device copies that select this step's row of the two tables.
 The scheduler is ``pipe.scheduler``: DDIM by default, or whichever ``scheduler_from_config`` returns for a
 checkpoint's scheduler config.
 """
@@ -42,7 +42,7 @@ import torch
 from . import ops
 from .image_processor import CLIPImageProcessor, VaeImageProcessor, ViTImageProcessor
 from .lora import AdapterRegistry, lora_targets, normalize_lora, split_components
-from .scheduler import DDIMScheduler, EulerDiscreteScheduler, get_timesteps, pag_scales, with_pag_column
+from .scheduler import DDIMScheduler, EulerDiscreteScheduler, get_timesteps, pag_scales, step_table, with_pag_column
 from .unet import UNetMangaEngine, resolve_pag_layers
 
 bf16, f32 = torch.bfloat16, torch.float32
@@ -63,8 +63,8 @@ PAGE_MAX_ROWS = 8       # samples per page denoise: a UNet batch of 16 rows, as 
 def plan_page(shapes, max_batch_panels: int = PAGE_MAX_ROWS) -> List[List[int]]:
     """The denoise chunks of a page.  ``shapes`` holds one (num_samples, h, w) per panel, h x w its latent size, with
     optional further entries that must also match for two panels to share a denoise (an img2img or inpaint panel
-    adds one: it runs a different slice of the schedule, and an inpaint panel a different step kernel).  Panels of one key form a group, groups in order of first appearance; a
-    group splits into consecutive chunks of at most ``max_batch_panels`` samples, and a panel's samples are never split
+    adds one: it runs a different slice of the schedule, and an inpaint panel the step with the inpaint blend).  Panels
+    of one key form a group, groups in order of first appearance; a group splits into consecutive chunks of at most ``max_batch_panels`` samples, and a panel's samples are never split
     (a panel with more samples than the cap is a chunk of its own).  Returns the panel indices of every chunk."""
     cap = int(max_batch_panels)
     if cap < 1:
@@ -882,11 +882,11 @@ class DenoiseStepper:
     ``step(i)`` runs iteration i on device-resident latents; ``step_host(i, x)`` is the same call with HOST
     buffers (pinned fp32 NCHW latents in, updated latents out), i.e. what a caller on the other side of the
     plugin boundary sees.
-    With ``inpaint`` = (image_latents, noise, latent mask) the step is the scheduler's ``fused_inpaint_step_``, which
-    reads those three per-panel buffers and the inpaint coefficient table.
+    The step is the scheduler's ``fused_step_`` over a row of ``step_table``.  With ``inpaint`` = (image_latents,
+    noise, latent mask) it also reads those three per-panel buffers and the table's {c0, c1} columns.
     With ``pag`` = (sites, pag_scale, pag_adaptive_scale) the batch is [uncond ; text ; perturbed] (3 bs rows), the
-    UNet perturbs the self-attention ``sites`` of the third chunk, and the step is ``fused_pag_step_`` over the
-    coefficient table with each step's PAG scale appended (``with_pag_column``).
+    UNet perturbs the self-attention ``sites`` of the third chunk, and the table has each step's PAG scale appended
+    (``with_pag_column``).
     """
 
     @torch.no_grad()
@@ -904,10 +904,7 @@ class DenoiseStepper:
             raise ValueError(f"start_index must be in [0, {self.num_inference_steps}), got {start_index}")
         self.timesteps = pipe.scheduler.set_timesteps(num_inference_steps, device=dev)[s0:]
         self.inpaint = inpaint is not None
-        if self.inpaint:                                                                # [T, 4] DDIM, [T, 5] Euler
-            self.base_coef_table = pipe.scheduler.inpaint_coefficient_table(s0, dev)
-        else:
-            self.base_coef_table = pipe.scheduler.coefficient_table(dev)[s0:]           # [T, 2] DDIM, [T, 3] Euler
+        self.base_coef_table = step_table(pipe.scheduler, s0, dev, self.inpaint)
         self.coef_table = self.base_coef_table
         # perturbed-attention guidance: the sites are baked into the graph, the scales live in the coefficient table
         self.pag_sites = None if pag is None else frozenset(pag[0])
@@ -1046,14 +1043,8 @@ class DenoiseStepper:
             finally:
                 ops.SPLITK = prev_splitk
                 ops.GEMM_CHAINS = prev_chains
-        if self.pag_sites is not None:
-            self.scheduler.fused_pag_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance,
-                                           (self.inp_z, self.inp_n, self.inp_m) if self.inpaint else None)
-        elif self.inpaint:
-            self.scheduler.fused_inpaint_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance, self.inp_z,
-                                               self.inp_n, self.inp_m)
-        else:
-            self.scheduler.fused_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance)  # :332-337,:315-317
+        self.scheduler.fused_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance,     # :332-337,:315-317
+                                   (self.inp_z, self.inp_n, self.inp_m) if self.inpaint else None)
 
     @torch.no_grad()
     def step(self, i: int) -> None:

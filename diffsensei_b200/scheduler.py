@@ -10,16 +10,15 @@ stable-diffusion-xl-base-1.0 (scaled_linear betas 0.00085..0.012 over 1000 train
 
 For img2img both add ``add_noise`` (diffusers' API, torch fp32), ``add_noise_coefficients`` (the same arithmetic as the
 two fp32 factors ``ds_vae_posterior`` reads) and ``set_begin_index``; ``get_timesteps`` is the strength rule.
-For inpainting, ``inpaint_coefficient_table`` adds each step's ``add_noise`` factors at the next timestep to the
-coefficient table, and ``fused_inpaint_step_`` runs the update with the blend (``ds_cfg_*_inpaint_step``).
-With perturbed-attention guidance, ``with_pag_column`` appends each step's PAG scale (``pag_scales``) to either table
-and ``fused_pag_step_`` runs the three-chunk update (``ds_cfg_pag_*``).
+``step_table`` gives the rows of the coefficient table a loop runs, and for inpainting adds each step's
+``add_noise`` factors at the next timestep.  With perturbed-attention guidance, ``with_pag_column`` appends each
+step's PAG scale (``pag_scales``) to that table.
 
 ``scheduler_from_config`` picks one from a checkpoint's ``scheduler/scheduler_config.json``, the way diffusers does,
 and rejects any class or value whose arithmetic is not implemented here.
 
-The per-step update itself runs on the GPU, fused with the CFG blend and the next step's input scaling
-(``ds_cfg_ddim_step`` / ``ds_cfg_euler_step``); these classes produce the timesteps, the per-step coefficient table
+The per-step update itself runs on the GPU, fused with the guidance blend, the inpaint blend and the next step's
+input scaling (``fused_step_``, ``ds_cfg_step``); these classes produce the timesteps, the per-step coefficient table
 the kernel reads (``coefficient_table``) and the divisor of the first step's UNet input (``model_input_divisors``).
 """
 from __future__ import annotations
@@ -30,17 +29,23 @@ import torch
 
 from . import ops
 
-def _inpaint_table(sched, start_index: int, device) -> torch.Tensor:
-    """``coefficient_table`` rows start_index .. T-1 with two more columns: the {c0, c1} of
-    ``add_noise(image_latents, noise, timesteps[i + 1])`` (``add_noise_coefficients(i + 1)``), and {1, 0} on the last
-    step, where diffusers' inpaint loop keeps the image latents themselves."""
+
+def step_table(sched, start_index: int, device, inpaint: bool) -> torch.Tensor:
+    """The fp32 rows ``fused_step_`` reads for steps start_index .. T-1: ``coefficient_table`` (DDIM [., 2], Euler
+    [., 3]), with ``inpaint`` two more columns: the {c0, c1} of ``add_noise(image_latents, noise, timesteps[i + 1])``
+    (``add_noise_coefficients(i + 1)``: DDIM's sqrt factors, Euler's {1, sigma_{i+1}}, the sigma diffusers'
+    ``add_noise`` reads through the step index ``step`` has already advanced), and {1, 0} on the last step, where
+    diffusers' inpaint loop keeps the image latents themselves."""
     n = len(sched.timesteps)
     s0 = int(start_index)
     if not 0 <= s0 < n:
         raise ValueError(f"start_index must be in [0, {n}), got {start_index}")
-    last = torch.tensor([1.0, 0.0], dtype=torch.float32)
-    c = torch.stack([sched.add_noise_coefficients(i + 1) if i + 1 < n else last for i in range(s0, n)])
-    return torch.cat([sched.coefficient_table("cpu")[s0:], c], dim=1).to(device)
+    table = sched.coefficient_table("cpu")[s0:]
+    if inpaint:
+        last = torch.tensor([1.0, 0.0], dtype=torch.float32)
+        c = torch.stack([sched.add_noise_coefficients(i + 1) if i + 1 < n else last for i in range(s0, n)])
+        table = torch.cat([table, c], dim=1)
+    return table.to(device)
 
 
 def pag_scales(timesteps, pag_scale: float, pag_adaptive_scale: float = 0.0) -> torch.Tensor:
@@ -55,7 +60,7 @@ def pag_scales(timesteps, pag_scale: float, pag_adaptive_scale: float = 0.0) -> 
 
 
 def with_pag_column(table: torch.Tensor, scales: torch.Tensor) -> torch.Tensor:
-    """A coefficient table with the per-step PAG scale appended as its last column (what ``ds_cfg_pag_*`` read)."""
+    """A coefficient table with the per-step PAG scale appended as its last column (what a 3-chunk step reads)."""
     return torch.cat([table, scales.to(device=table.device, dtype=torch.float32).reshape(-1, 1)], dim=1).contiguous()
 
 
@@ -104,25 +109,10 @@ class DDIMScheduler:
         """scale_model_input(x, timesteps[i]) == x / model_input_divisors()[i]: the identity for DDIM."""
         return [1.0] * len(self.timesteps)
 
-    def fused_step_(self, noise_pred, latents, model_in, coef, guidance: float) -> None:
-        ops.cfg_ddim_step_(noise_pred, latents, model_in, coef, guidance)
-
-    def inpaint_coefficient_table(self, start_index: int, device) -> torch.Tensor:
-        """fp32 [T - start_index, 4] device tensor of (alpha_prod_t, alpha_prod_t_prev, c0, c1) for the inpaint loop
-        (``fused_inpaint_step_``): c0 / c1 as ``add_noise_coefficients`` at the next step, {1, 0} on the last."""
-        return _inpaint_table(self, start_index, device)
-
-    def fused_inpaint_step_(self, noise_pred, latents, model_in, coef, guidance: float, image_latents, noise,
-                            mask) -> None:
-        ops.cfg_ddim_inpaint_step_(noise_pred, latents, model_in, coef, guidance, image_latents, noise, mask)
-
-    def fused_pag_step_(self, noise_pred, latents, model_in, coef, guidance: float, inpaint=None) -> None:
-        """CFG + perturbed-attention guidance + DDIM (``ds_cfg_pag_ddim[_inpaint]_step``): ``coef`` is a row of
-        ``with_pag_column`` over the plain or inpaint table, ``inpaint`` None or (image_latents, noise, mask)."""
-        if inpaint is None:
-            ops.cfg_pag_ddim_step_(noise_pred, latents, model_in, coef, guidance)
-        else:
-            ops.cfg_pag_ddim_inpaint_step_(noise_pred, latents, model_in, coef, guidance, *inpaint)
+    def fused_step_(self, noise_pred, latents, model_in, coef, guidance: float, inpaint=None) -> None:
+        """The guidance blend + DDIM update (``ops.cfg_step_``): ``coef`` is a row of ``step_table``, with the PAG
+        scale appended for a 3-chunk ``noise_pred``; ``inpaint`` None or (image_latents, noise, mask)."""
+        ops.cfg_step_(noise_pred, latents, model_in, coef, guidance, euler=False, inpaint=inpaint)
 
     def set_begin_index(self, begin_index: int = 0) -> None:
         """The loop's first step (img2img); DDIM's arithmetic does not depend on it, only add_noise's timestep."""
@@ -190,25 +180,9 @@ class EulerDiscreteScheduler:
         """scale_model_input(x, timesteps[i]) == x / model_input_divisors()[i] (fp32 values)."""
         return self._divisors()[:-1].tolist()
 
-    def fused_step_(self, noise_pred, latents, model_in, coef, guidance: float) -> None:
-        ops.cfg_euler_step_(noise_pred, latents, model_in, coef, guidance)
-
-    def inpaint_coefficient_table(self, start_index: int, device) -> torch.Tensor:
-        """fp32 [T - start_index, 5] device tensor of (sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1), c0, c1) for the
-        inpaint loop: {c0, c1} = {1, sigma_{i+1}}, the sigma diffusers' ``add_noise`` reads through the step index
-        that ``step`` has already advanced, and {1, 0} on the last step."""
-        return _inpaint_table(self, start_index, device)
-
-    def fused_inpaint_step_(self, noise_pred, latents, model_in, coef, guidance: float, image_latents, noise,
-                            mask) -> None:
-        ops.cfg_euler_inpaint_step_(noise_pred, latents, model_in, coef, guidance, image_latents, noise, mask)
-
-    def fused_pag_step_(self, noise_pred, latents, model_in, coef, guidance: float, inpaint=None) -> None:
-        """CFG + perturbed-attention guidance + Euler (``ds_cfg_pag_euler[_inpaint]_step``); see DDIM's."""
-        if inpaint is None:
-            ops.cfg_pag_euler_step_(noise_pred, latents, model_in, coef, guidance)
-        else:
-            ops.cfg_pag_euler_inpaint_step_(noise_pred, latents, model_in, coef, guidance, *inpaint)
+    def fused_step_(self, noise_pred, latents, model_in, coef, guidance: float, inpaint=None) -> None:
+        """The guidance blend + Euler update + the next step's scale_model_input (``ops.cfg_step_``); see DDIM's."""
+        ops.cfg_step_(noise_pred, latents, model_in, coef, guidance, euler=True, inpaint=inpaint)
 
     def set_begin_index(self, begin_index: int = 0) -> None:
         """diffusers' ``set_begin_index``: the loop starts at sigma_{begin_index} (img2img)."""

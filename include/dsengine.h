@@ -304,80 +304,37 @@ int ds_silu(const void* x, void* y, int64_t n, void* stream);
 int ds_timestep_embedding(const float* t, void* out, int rows, int dim, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * CFG blend + DDIM (eta = 0, epsilon-prediction) update, fused.                    [HBM-bound]
- * Replaces src/pipelines/pipeline_diffsensei.py:315,332-337 (chunk, u + g*(t-u), scheduler.step,
- * and the torch.cat([latents]*2) for the next step):
- *   eps   = e_uncond + guidance * (e_text - e_uncond)
- *   x0    = (x - sqrt(1-a_t) * eps) / sqrt(a_t)
- *   x_new = sqrt(a_prev) * x0 + sqrt(1-a_prev) * eps
- *   noise_pred : bf16 NHWC [2*bs][H][W][4] (uncond half first)
- *   latents    : fp32 [bs][H][W][4] updated in place (fp32 master copy)
- *   model_in   : bf16 NHWC [2*bs][H][W][4] — x_new duplicated for both CFG halves (next step's UNet input)
- *   coef       : device pointer to 2 floats {alpha_prod_t, alpha_prod_t_prev} for this step
- * --------------------------------------------------------------------------------------------- */
-int ds_cfg_ddim_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
-                     int bs, int HW, int C, void* stream);
-
-/* ---------------------------------------------------------------------------------------------
- * CFG blend + Euler (EulerDiscreteScheduler, s_churn = 0, epsilon-prediction) update + the next
- * step's scale_model_input, fused.                                                 [HBM-bound]
- * Replaces src/pipelines/pipeline_diffsensei.py:315-317,332-337 (chunk, u + g*(t-u), scheduler.step,
- * the torch.cat([latents]*2) and scheduler.scale_model_input for the next step), fp32, each operation
- * rounded separately in this order:
- *   eps     = e_uncond + guidance * (e_text - e_uncond)
- *   x0      = x - sigma * eps
- *   d       = (x - x0) / sigma
- *   x_new   = x + d * (sigma_next - sigma)
- *   noise_pred : bf16 NHWC [2*bs][H][W][4] (uncond half first)
- *   latents    : fp32 [bs][H][W][4] updated in place (fp32 master copy)
- *   model_in   : bf16 NHWC [2*bs][H][W][4] — x_new / sqrt(sigma_next^2 + 1) for both CFG halves
- *   coef       : device pointer to 3 floats {sigma, sigma_next, sqrt(sigma_next^2 + 1)} for this step
- * --------------------------------------------------------------------------------------------- */
-int ds_cfg_euler_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
-                      int bs, int HW, int C, void* stream);
-
-/* ---------------------------------------------------------------------------------------------
- * The two updates above followed by the inpaint blend of diffusers' StableDiffusionXLInpaintPipeline with a
- * 4-channel UNet, fused.                                                           [HBM-bound]
- *   init  = c0 * z + c1 * n        (add_noise of the image latents at the next timestep; {1, 0} on the last step;
- *                                   each product and the sum rounded on its own)
- *   x_new = mask ? x_new : init    ((1 - m) * init + m * x_new with a binary m)
- * and the next UNet input is computed from the blended x_new.  A pixel with mask != 0 is the plain kernel's result
- * bit for bit.
- *   coef          : DDIM {alpha_prod_t, alpha_prod_t_prev, c0, c1}; Euler {sigma, sigma_next,
- *                   sqrt(sigma_next^2 + 1), c0, c1} (device pointer)
+ * The end of every denoise step, fused: the guidance blend, the scheduler update and the next step's UNet input,
+ * optionally followed by the inpaint blend.                                        [HBM-bound]
+ * Replaces src/pipelines/pipeline_diffsensei.py:315-317,332-337 (chunk, the guidance blend, scheduler.step, the
+ * torch.cat([latents] * chunks) and scheduler.scale_model_input for the next step).
+ *   update        : 0 = DDIMScheduler (eta = 0), 1 = EulerDiscreteScheduler (s_churn = 0); epsilon prediction
+ *   chunks        : 2 = CFG, noise_pred [uncond ; text]; 3 = CFG + perturbed-attention guidance (diffusers' PAGMixin
+ *                   under classifier-free guidance), noise_pred [uncond ; text ; perturbed]
+ *   noise_pred    : bf16 NHWC [chunks*bs][H][W][4]
+ *   latents       : fp32 [bs][H][W][4] updated in place (fp32 master copy)
+ *   model_in      : bf16 NHWC [chunks*bs][H][W][4], the next UNet input in every chunk: x_new (DDIM),
+ *                   x_new / sqrt(sigma_next^2 + 1) (Euler)
  *   image_latents : fp32 NHWC [bs][H][W][4] (z, scaling_factor * posterior sample), 16-byte aligned
  *   noise         : fp32 NHWC [bs][H][W][4] (n, the noise the start latents were drawn with), 16-byte aligned
  *   mask          : uint8 [bs][H][W], 1 = regenerate, 0 = keep the image
+ *                   (all three NULL: no inpaint blend; all three or none must be given)
+ *   coef          : device pointer to this step's row, columns in this order:
+ *                   DDIM {alpha_prod_t, alpha_prod_t_prev} or Euler {sigma, sigma_next, sqrt(sigma_next^2 + 1)},
+ *                   then {c0, c1} when inpainting, then s when chunks == 3
+ * The arithmetic, per element:
+ *   eps   = e_uncond + guidance * (e_text - e_uncond)      [+ s * (e_text - e_perturbed) with 3 chunks]
+ *   DDIM  : x0 = (x - sqrt(1-a_t) * eps) / sqrt(a_t);  x_new = sqrt(a_prev) * x0 + sqrt(1-a_prev) * eps
+ *   Euler : x0 = x - sigma * eps;  d = (x - x0) / sigma;  x_new = x + d * (sigma_next - sigma)
+ *   inpaint: init = c0 * z + c1 * n (add_noise of the image latents at the next timestep; {1, 0} on the last step);
+ *            x_new = mask ? x_new : init, and the next UNet input is computed from the blended x_new
+ * Rounding: every operation is rounded on its own in diffusers' eager fp32 order, except DDIM with 2 chunks, where
+ * the compiler may contract multiply-adds into FMAs.  A pixel with mask != 0 is the result without inpaint bit for
+ * bit.
  * --------------------------------------------------------------------------------------------- */
-int ds_cfg_ddim_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
-                             const float* image_latents, const float* noise, const uint8_t* mask, int bs, int HW,
-                             int C, void* stream);
-int ds_cfg_euler_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
-                              float guidance, const float* image_latents, const float* noise, const uint8_t* mask,
-                              int bs, int HW, int C, void* stream);
-
-/* ---------------------------------------------------------------------------------------------
- * CFG + perturbed-attention guidance (diffusers' PAGMixin, do_classifier_free_guidance) fused with the four updates
- * above.                                                                           [HBM-bound]
- *   noise_pred : bf16 NHWC [3*bs][H][W][4], chunks [uncond ; text ; perturbed]
- *   eps        = (e_uncond + guidance * (e_text - e_uncond)) + s * (e_text - e_perturbed)
- * then the DDIM / Euler update (and the inpaint blend) of the matching CFG kernel, every operation rounded on its
- * own in diffusers' eager order (the DDIM update too); model_in : bf16 NHWC [3*bs][H][W][4], the next UNet input
- * in all three chunks.  s is the LAST entry of the step's coefficient row, read on the device:
- *   DDIM {a_t, a_prev, s}                 Euler {sigma, sigma_next, sqrt(sigma_next^2 + 1), s}
- *   DDIM inpaint {a_t, a_prev, c0, c1, s} Euler inpaint {sigma, sigma_next, sqrt(sigma_next^2 + 1), c0, c1, s}
- * --------------------------------------------------------------------------------------------- */
-int ds_cfg_pag_ddim_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
-                         int bs, int HW, int C, void* stream);
-int ds_cfg_pag_euler_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
-                          int bs, int HW, int C, void* stream);
-int ds_cfg_pag_ddim_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
-                                 float guidance, const float* image_latents, const float* noise, const uint8_t* mask,
-                                 int bs, int HW, int C, void* stream);
-int ds_cfg_pag_euler_inpaint_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
-                                  float guidance, const float* image_latents, const float* noise, const uint8_t* mask,
-                                  int bs, int HW, int C, void* stream);
+int ds_cfg_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance, int update,
+                int chunks, const float* image_latents, const float* noise, const uint8_t* mask, int bs, int HW, int C,
+                void* stream);
 
 /* Perceiver attention of the character Resampler: 16 latent queries x (n_kv) keys per (character, head),
  * q and k each pre-scaled by dim_head^-0.25, fp32 softmax (src/models/resampler.py:64-74).

@@ -1,4 +1,4 @@
-"""The Euler scheduler on the GPU: the fused ds_cfg_euler_step kernel against a torch fp32 restatement, the denoise
+"""The Euler scheduler on the GPU: the fused ds_cfg_step kernel's Euler update against a torch fp32 restatement, the denoise
 loop against the oracle (tiny model and full SDXL topology), scheduler switching on one pipeline, and __call__'s
 initial noise scaling."""
 import dataclasses
@@ -25,7 +25,7 @@ def _bf16_ulps(a: torch.Tensor, b: torch.Tensor) -> int:
 
 @pytest.mark.parametrize("bs,H,W,step", [(1, 16, 16, 0), (2, 17, 23, 7), (3, 6, 5, 12), (2, 9, 31, 29),
                                          (3, 20, 13, 29)])
-def test_cfg_euler_step_matches_torch(bs, H, W, step):
+def test_cfg_step_euler_matches_torch(bs, H, W, step):
     """HW = 391, 30, 279, 260 are not multiples of the 256-thread block; step 29 of 30 is the last (sigma_next = 0)."""
     from diffsensei_b200 import ops
     from diffsensei_b200.scheduler import EulerDiscreteScheduler
@@ -46,12 +46,12 @@ def test_cfg_euler_step_matches_torch(bs, H, W, step):
     want = lat + d * (s1 - s)
     want_in = (want / div).to(bf16)
     latd, mi = lat.clone(), torch.empty(2 * bs, H, W, 4, dtype=bf16, device=DEV)
-    ops.cfg_euler_step_(eps, latd, mi, coef, 7.5)
+    ops.cfg_step_(eps, latd, mi, coef, 7.5, euler=True)
     torch.testing.assert_close(latd, want, rtol=1e-6, atol=1e-6)
     assert torch.equal(mi[:bs], mi[bs:])
     assert _bf16_ulps(mi[:bs], want_in) <= 1
     with pytest.raises(ops.DsEngineError, match="shape mismatch"):
-        ops.cfg_euler_step_(eps, latd, mi, coef[:2].contiguous(), 7.5)
+        ops.cfg_step_(eps, latd, mi, coef[:2].contiguous(), 7.5, euler=True)
 
 
 def test_euler_denoise_loop_matches_oracle_and_graph_equals_eager(tiny):  # noqa: F811

@@ -64,11 +64,12 @@ def _step_inputs(bs, h, w, seed):
 
 @pytest.mark.parametrize("sched", ["ddim", "euler"])
 @pytest.mark.parametrize("bs,h,w", [(1, 9, 13), (2, 16, 19), (3, 40, 37)])
-def test_inpaint_step_kernels(sched, bs, h, w):
+def test_cfg_step_inpaint_blend(sched, bs, h, w):
     import diffsensei_b200 as ds
+    from diffsensei_b200.scheduler import step_table
     s = ds.EulerDiscreteScheduler() if sched == "euler" else ds.DDIMScheduler()
     s.set_timesteps(10)
-    tab = s.inpaint_coefficient_table(0, DEV)
+    tab = step_table(s, 0, DEV, inpaint=True)
     for i in (0, 6, 9):                                             # 9: the last step, {c0, c1} = {1, 0}
         coef = tab[i].contiguous()
         plain_coef = coef[:-2].contiguous()
@@ -82,7 +83,7 @@ def test_inpaint_step_kernels(sched, bs, h, w):
         mi_init = (init / div if div is not None else init).to(bf16)
         for name, m in (("ones", torch.ones_like(rnd)), ("zeros", torch.zeros_like(rnd)), ("random", rnd)):
             lat, mi = lat0.clone(), torch.zeros(2 * bs, h, w, 4, dtype=bf16, device=DEV)
-            s.fused_inpaint_step_(eps, lat, mi, coef, 7.5, z, n, m)
+            s.fused_step_(eps, lat, mi, coef, 7.5, (z, n, m))
             keep = m.bool()[..., None]
             want_lat = torch.where(keep, lat_p, init)
             want_mi = torch.where(keep, mi_p[:bs], mi_init)

@@ -66,14 +66,16 @@ def test_float_mask_binarise():
 
 
 @pytest.mark.parametrize("steps,start", [(5, 0), (5, 2), (30, 12), (4, 3)])
-def test_inpaint_coefficient_tables(steps, start):
+def test_inpaint_step_tables(steps, start):
     from diffsensei_b200 import DDIMScheduler, EulerDiscreteScheduler
+    from diffsensei_b200.scheduler import step_table
     g = torch.Generator().manual_seed(steps + start)
     x, n = torch.randn(2, 4, 5, 6, generator=g), torch.randn(2, 4, 5, 6, generator=g)
     for sched in (DDIMScheduler(), EulerDiscreteScheduler()):
         ts = sched.set_timesteps(steps)
-        tab = sched.inpaint_coefficient_table(start, "cpu")
+        tab = step_table(sched, start, "cpu", inpaint=True)
         base = sched.coefficient_table("cpu")[start:]
+        assert torch.equal(step_table(sched, start, "cpu", inpaint=False), base)
         assert tab.dtype == torch.float32 and tab.shape == (steps - start, base.shape[1] + 2)
         assert torch.equal(tab[:, :-2], base)
         for r, i in enumerate(range(start, steps)):
@@ -85,10 +87,11 @@ def test_inpaint_coefficient_tables(steps, start):
                 assert torch.equal(c0 * x + c1 * n, sched.add_noise(x, n, torch.tensor([ts[i + 1]] * 2))), (i, sched)
     eul = EulerDiscreteScheduler()
     eul.set_timesteps(30)
-    tab = eul.inpaint_coefficient_table(21, "cpu")
+    tab = step_table(eul, 21, "cpu", inpaint=True)
     assert abs(float(tab[0, 4]) - float(eul.sigmas[22])) == 0 and float(tab[0, 3]) == 1.0
-    with pytest.raises(ValueError):
-        eul.inpaint_coefficient_table(30, "cpu")
+    for inpaint in (True, False):
+        with pytest.raises(ValueError):
+            step_table(eul, 30, "cpu", inpaint)
 
 
 def test_mask_processor_configurations():

@@ -271,7 +271,7 @@ def test_layout_upsample_concat_silu_timestep(ops):
         assert (ops.timestep_embedding(t.to(DEV), dim).float().cpu() - timestep_sinusoid(t, dim)).abs().max() < 8e-3
 
 
-def test_cfg_ddim_step(ops):
+def test_cfg_step_ddim(ops):
     from oracle.ddim import DDIMSchedule
     sch = DDIMSchedule()
     t = sch.set_timesteps(50)[7]
@@ -281,7 +281,7 @@ def test_cfg_ddim_step(ops):
     eu, et = eps.float().chunk(2)
     want = sch.step(eu + 7.5 * (et - eu), t, lat)
     latd, mi = lat.to(DEV).clone(), torch.empty(2 * bs, H, W, 4, dtype=bf16, device=DEV)
-    ops.cfg_ddim_step_(eps.to(DEV), latd, mi, torch.tensor([a_t, a_prev], device=DEV), 7.5)
+    ops.cfg_step_(eps.to(DEV), latd, mi, torch.tensor([a_t, a_prev], device=DEV), 7.5, euler=False)
     assert rel_l2(latd, want) < 1e-5
     assert torch.equal(mi[:bs], mi[bs:]) and torch.equal(mi[:bs].cpu(), latd.cpu().to(bf16))
 

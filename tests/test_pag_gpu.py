@@ -1,6 +1,6 @@
-"""Perturbed-attention guidance on the H100: the identity self-attention entry point, the four fused CFG + PAG step
-kernels against a torch fp32 restatement, the UNet with the mid block perturbed and the denoise loop against the
-oracle (tests/pag_oracle.py), the stepper cache, unchanged behaviour at pag_scale = 0, and pages."""
+"""Perturbed-attention guidance on the H100: the identity self-attention entry point, the four fused CFG + PAG
+variants of the step kernel against a torch fp32 restatement, the UNet with the mid block perturbed and the denoise
+loop against the oracle (tests/pag_oracle.py), the stepper cache, unchanged behaviour at pag_scale = 0, and pages."""
 import pytest
 import torch
 
@@ -71,13 +71,13 @@ def _torch_pag_step(sched, eps, lat, coef, guidance, inpaint):
 @pytest.mark.parametrize("sched", ["ddim", "euler"])
 @pytest.mark.parametrize("inpaint", [False, True])
 @pytest.mark.parametrize("bs,H,W,step", [(1, 16, 16, 0), (2, 17, 23, 7), (3, 6, 5, 12), (2, 9, 31, 29)])
-def test_pag_step_kernels(sched, inpaint, bs, H, W, step):
+def test_cfg_step_pag_matches_torch(sched, inpaint, bs, H, W, step):
     """HW = 391, 30, 279 are not multiples of the 256-thread block; step 29 of 30 is the last."""
     from diffsensei_b200 import ops
-    from diffsensei_b200.scheduler import DDIMScheduler, EulerDiscreteScheduler, pag_scales, with_pag_column
+    from diffsensei_b200.scheduler import DDIMScheduler, EulerDiscreteScheduler, pag_scales, step_table, with_pag_column
     sch = DDIMScheduler() if sched == "ddim" else EulerDiscreteScheduler()
     ts = sch.set_timesteps(30)
-    table = sch.inpaint_coefficient_table(0, DEV) if inpaint else sch.coefficient_table(DEV)
+    table = step_table(sch, 0, DEV, inpaint)
     coef = with_pag_column(table, pag_scales(ts, 3.0, 0.003))[step].contiguous()
     g = torch.Generator().manual_seed(200 + step + 7 * bs)
     eps = torch.randn(3 * bs, H, W, 4, generator=g).to(bf16).to(DEV)
@@ -88,16 +88,15 @@ def test_pag_step_kernels(sched, inpaint, bs, H, W, step):
                (torch.rand(bs, H, W, generator=g) > 0.4).to(torch.uint8).to(DEV))
     want, want_in = _torch_pag_step(sched, eps, lat, coef, 7.5, inp)
     latd, mi = lat.clone(), torch.full((3 * bs, H, W, 4), float("nan"), dtype=bf16, device=DEV)
-    sch.fused_pag_step_(eps, latd, mi, coef, 7.5, inp)
+    sch.fused_step_(eps, latd, mi, coef, 7.5, inp)
     torch.testing.assert_close(latd, want, rtol=1e-6, atol=1e-6)
     assert torch.equal(mi[:bs], mi[bs:2 * bs]) and torch.equal(mi[:bs], mi[2 * bs:])
     assert _bf16_ulps(mi[:bs], want_in) <= 1
     if inpaint:                                     # kept pixels are exactly the noised image latents
         keep = ~inp[2].bool()
         assert torch.equal(latd[keep], (coef[-3] * inp[0] + coef[-2] * inp[1])[keep])
-    fn = ops.cfg_pag_ddim_step_ if sched == "ddim" else ops.cfg_pag_euler_step_
     with pytest.raises(ops.DsEngineError, match="shape mismatch"):
-        fn(eps[:2 * bs], latd, mi, coef, 7.5)
+        ops.cfg_step_(eps[:2 * bs], latd, mi, coef, 7.5, euler=sched == "euler", inpaint=inp)
 
 
 # ------------------------------------------------------------------------------------------------ UNet forward

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Inpainting on one GPU, one JSON object:
 
-* the fused step: ``ds_cfg_{ddim,euler}_inpaint_step`` against the plain ``ds_cfg_{ddim,euler}_step`` at the latent
+* the fused step: ``ds_cfg_step`` with the inpaint blend against the step without it, DDIM and Euler, at the latent
   shape of a 1024x1024 panel with 4 samples (128 x 128 latents, a UNet batch of 8), alternating, CUDA events around
   the replay of 200 launches captured in one graph (the 4-6 MB operands stay in the 50 MB L2), medians; the inpaint kernel with an all-zero mask (every pixel reads the image latents and the noise:
   97 B / pixel against 64) and with a half mask; bytes from shapes over kernel time;
@@ -53,6 +53,7 @@ def graphed(fn):
 
 
 def bench_step(ds, dev, rounds):
+    from diffsensei_b200.scheduler import step_table
     bs, h, w = 4, 128, 128
     g = torch.Generator().manual_seed(0)
     eps = torch.randn(2 * bs, h, w, 4, generator=g).to(bf16).to(dev)
@@ -65,12 +66,12 @@ def bench_step(ds, dev, rounds):
     px = bs * h * w
     for name, s in (("ddim", ds.DDIMScheduler()), ("euler", ds.EulerDiscreteScheduler())):
         s.set_timesteps(30)
-        coef = s.inpaint_coefficient_table(0, dev)[10].contiguous()
+        coef = step_table(s, 0, dev, inpaint=True)[10].contiguous()
         plain = coef[:-2].contiguous()
         lat.copy_(lat0)
         paths = {"plain": lambda: s.fused_step_(eps, lat, mi, plain, 5.0)}
         for mk, m in masks.items():
-            paths[f"inpaint_mask_{mk}"] = (lambda m=m: s.fused_inpaint_step_(eps, lat, mi, coef, 5.0, z, n, m))
+            paths[f"inpaint_mask_{mk}"] = (lambda m=m: s.fused_step_(eps, lat, mi, coef, 5.0, (z, n, m)))
         res = alternate({k: graphed(fn) for k, fn in paths.items()}, rounds, lambda fn: events_ms(fn) * 1e3 / LAUNCHES)
         nbytes = {"plain": 64 * px, "inpaint_mask_zeros": 97 * px,
                   "inpaint_mask_half": int(65 * px + 32 * int((masks["half"] == 0).sum()))}

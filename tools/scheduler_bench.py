@@ -2,7 +2,7 @@
 
 * the whole cfg2 step (UNet forward + the scheduler's fused CFG update), graph replay, alternating DDIM and Euler over
   several rounds so that both see the same machine state;
-* the two fused update kernels alone (ds_cfg_ddim_step / ds_cfg_euler_step) at the cfg2 latent shape: each op
+* the fused update kernel alone (ds_cfg_step, DDIM and Euler, 2 chunks) at the cfg2 latent shape: each op
   captured 100 times in a CUDA graph, rotating over buffer sets larger than the 50 MB L2, timed with CUDA events;
 * the GPU's name and power limit, read with `nvidia-smi --query-gpu=name,power.limit` (read only).
 

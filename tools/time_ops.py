@@ -84,7 +84,7 @@ def wrap(name):
 
 
 for n in ("groupnorm_silu", "groupnorm_apply", "channel_stats", "layernorm", "dialog_embed_add_", "gemm", "conv3x3", "conv_in", "attention_self",
-          "attention_cross_ip", "upsample_nearest", "concat_channels", "silu", "cfg_ddim_step_", "nchw_to_nhwc",
+          "attention_cross_ip", "upsample_nearest", "concat_channels", "silu", "cfg_step_", "nchw_to_nhwc",
           "nhwc_to_nchw", "timestep_embedding"):
     wrap(n)
 
