@@ -60,6 +60,8 @@ SIGNATURES = {
     "ds_channel_stats": [_vp, _vp, _i, _i, _i, _vp],
     "ds_groupnorm_apply": [_vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _f, _i, _vp],
     "ds_layernorm": [_vp, _vp, _vp, _vp, _i, _i, _f, _vp],
+    "ds_freeu_moments": [_vp, _vp, _i, _i, _i, _i, _vp],
+    "ds_freeu_apply": [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _f, _f, _i, _i, _i, _vp],
     "ds_dialog_embed_add": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp],
     "ds_ip_mask": [_vp, _vp, _i, _i, _d, _i, _i, _i, _vp],
     "ds_gemm_bf16": [C.POINTER(GemmArgs), _vp],

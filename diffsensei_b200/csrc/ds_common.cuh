@@ -46,6 +46,15 @@ __device__ __forceinline__ uint32_t pack_bf16_alu(float lo, float hi) {
   return __byte_perm(a, b, 0x7632);  // {b.hi16, a.hi16}
 }
 
+// Items of a per-(sample, channel) reduction (gn_plan, ds_host.h): a launch has exactly one resident wave of CTAs
+// (grid = SMs x occupancy) and CTA c owns the contiguous item range [c*I/G, (c+1)*I/G) — so no tail wave, and a CTA
+// touches at most a couple of samples.
+__device__ __forceinline__ void gn_item_range(int total_items, int& i0, int& i1) {
+  const long long g = gridDim.x, c = blockIdx.x;
+  i0 = static_cast<int>(c * total_items / g);
+  i1 = static_cast<int>((c + 1) * total_items / g);
+}
+
 // ----------------------------------------------------------------------------------------------
 // Programmatic dependent launch (PDL).  A kernel launched with programmaticStreamSerializationAllowed may start
 // (and run its prologue: barrier init, tensor-map prefetch) while its predecessor in the stream / graph

@@ -35,6 +35,32 @@ inline int device_slot() {
   return d & (kMaxDevices - 1);
 }
 
+// Work decomposition of the per-(sample, channel) reductions over channels-last [B][HW][C] bf16 tensors
+// (chan_stats_kernel, the GroupNorm apply, the FreeU kernels): the tensor is cut into ITEMS of `ipx` consecutive pixels
+// of one sample (item id = sample * items_per_sample + k).  blockDim = cv * rpb threads (cv = C/8 16-byte vectors per
+// pixel, rpb pixel rows per sweep, cv * rpb <= target), every thread pinned to the same 8 channels; an item is `sweeps`
+// sweeps of the CTA's pixel rows.  A kernel that emits GroupNorm statistics with ds_channel_stats' plan
+// (kGnStatsThreads, kGnStatsSweeps) and its per-item fp32 partials produces the same statistics bit for bit.
+constexpr int kGnStatsThreads = 512;
+constexpr int kGnStatsSweeps = 8;
+struct GnPlan {
+  int threads, rpb, ipx, items_per_sample, total_items;
+};
+inline bool gn_plan(int B, int HW, int C, int target_threads, int sweeps, GnPlan* pl) {
+  const int cv = C / 8;
+  if (cv > 1024) return false;
+  int rpb = target_threads / cv;
+  if (rpb < 1) rpb = 1;
+  pl->rpb = rpb;
+  pl->threads = cv * rpb;
+  pl->ipx = sweeps * rpb;
+  pl->items_per_sample = (HW + pl->ipx - 1) / pl->ipx;
+  const long long t = static_cast<long long>(B) * pl->items_per_sample;
+  if (t >= (1ll << 30)) return false;
+  pl->total_items = static_cast<int>(t);
+  return true;
+}
+
 #define DS_REQUIRE(cond, ...)        \
   do {                               \
     if (!(cond)) {                   \

@@ -21,10 +21,9 @@
 
 namespace ds {
 
-// Launch shape: threads per CTA of the apply and statistics kernels, the apply kernel's independent 16-byte loads in
-// flight per thread, and its cap on resident CTAs per SM.
+// Launch shape of the apply kernel (the statistics kernel's is kGnStatsThreads / kGnStatsSweeps, ds_host.h): threads
+// per CTA, independent 16-byte loads in flight per thread, and the cap on resident CTAs per SM.
 constexpr int kGnApplyThreads = 256;
-constexpr int kGnStatsThreads = 512;
 constexpr int kGnUnroll = 8;
 constexpr int kGnMaxOcc = 8;
 
@@ -48,16 +47,7 @@ __device__ __forceinline__ uint4 ldg_hint(const uint4* ptr, uint64_t pol) {
   return v;
 }
 
-// Work decomposition: the tensor is cut into ITEMS of `ipx` consecutive pixels of one sample (item id = sample *
-// items_per_sample + k); a launch has exactly one resident wave of CTAs (grid = SMs x occupancy) and CTA c owns the
-// contiguous item range [c*I/G, (c+1)*I/G) — so no tail wave, and a CTA touches at most a couple of samples.
-// blockDim.x = cv * rpb (cv = C/8 16-byte vectors per pixel, rpb pixel rows per sweep); every thread stays pinned to
-// the same 8 channels.
-__device__ __forceinline__ void gn_item_range(int total_items, int& i0, int& i1) {
-  const long long g = gridDim.x, c = blockIdx.x;
-  i0 = static_cast<int>(c * total_items / g);
-  i1 = static_cast<int>((c + 1) * total_items / g);
-}
+// Work decomposition: items of pixels, one resident wave of CTAs (gn_item_range and gn_plan, ds_common.cuh / ds_host.h).
 
 // Per-(sample, channel) {sum, sum of squares} of a [B][HW][C] bf16 tensor -> fp64 [B][C][2] (accumulated: the caller
 // zeroes it).  Threads keep fp32 partials over one item's pixels, the CTA's pixel rows are combined in a fixed order
@@ -315,27 +305,6 @@ __global__ void layernorm_kernel(const uint4* __restrict__ x, uint4* __restrict_
 
 }  // namespace ds
 
-namespace {
-struct GnPlan {
-  int threads, rpb, ipx, items_per_sample, total_items;
-};
-// blockDim = cv * rpb threads (<= target), items of `sweeps` sweeps of the CTA's pixel rows
-static bool gn_plan(int B, int HW, int C, int target_threads, int sweeps, GnPlan* pl) {
-  const int cv = C / 8;
-  if (cv > 1024) return false;
-  int rpb = target_threads / cv;
-  if (rpb < 1) rpb = 1;
-  pl->rpb = rpb;
-  pl->threads = cv * rpb;
-  pl->ipx = sweeps * rpb;
-  pl->items_per_sample = (HW + pl->ipx - 1) / pl->ipx;
-  const long long t = static_cast<long long>(B) * pl->items_per_sample;
-  if (t >= (1ll << 30)) return false;
-  pl->total_items = static_cast<int>(t);
-  return true;
-}
-}  // namespace
-
 extern "C" int ds_channel_stats(const void* x, double* stats, int B, int HW, int C, void* stream) {
   using namespace ds;
   DS_REQUIRE(x && stats, "ds_channel_stats: NULL pointer");
@@ -346,7 +315,7 @@ extern "C" int ds_channel_stats(const void* x, double* stats, int B, int HW, int
   if (!get_device(&dev)) return DS_ERR_CUDA;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   GnPlan pl;
-  DS_REQUIRE(gn_plan(B, HW, C, kGnStatsThreads, 8, &pl), "ds_channel_stats: tensor too large");
+  DS_REQUIRE(gn_plan(B, HW, C, kGnStatsThreads, kGnStatsSweeps, &pl), "ds_channel_stats: tensor too large");
   const size_t smem = static_cast<size_t>(pl.rpb) * C * 2 * sizeof(float);
   static size_t attr[kMaxDevices] = {};
   if (smem > 48 * 1024 && smem > attr[device_slot()]) {

@@ -117,6 +117,65 @@ def groupnorm_apply(x: torch.Tensor, stats: torch.Tensor, gamma: torch.Tensor, b
     return out
 
 
+def freeu_moments(skip: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp64 [B, C, 7] moments of FreeU's Fourier filter (``ds_freeu_moments``) of channels-last bf16 ``skip``
+    [B, H, W, C].  ``out`` is ACCUMULATED into (it must be zero); without it a zeroed buffer is allocated."""
+    _req(skip, bf16, "freeu_moments.skip", 4)
+    B, H, W, Cc = skip.shape
+    if out is None:
+        out = zero_(torch.empty(B, Cc, 7, dtype=torch.float64, device=skip.device))
+    else:
+        _req(out, torch.float64, "freeu_moments.out")
+        if out.numel() != 7 * B * Cc:
+            raise DsEngineError("freeu_moments: out must hold B*C*7 doubles")
+    check(lib.ds_freeu_moments(skip.data_ptr(), out.data_ptr(), B, H, W, Cc, _stream()), "ds_freeu_moments")
+    return out
+
+
+def freeu_apply(skip: torch.Tensor, hidden: torch.Tensor, moments: torch.Tensor, s: float, b: float,
+                skip_out: Optional[torch.Tensor] = None, hidden_out: Optional[torch.Tensor] = None,
+                skip_stats: Optional[torch.Tensor] = None, hidden_stats: Optional[torch.Tensor] = None):
+    """FreeU at one up-block resnet (``ds_freeu_apply``, one launch): ``skip`` [B, H, W, Cs] through the Fourier filter
+    of scale ``s`` (its ``freeu_moments`` given), ``hidden`` [B, H, W, Ch] with channels [0, Ch/2) times ``b``, plus the
+    GroupNorm statistics of both results (accumulated into ``*_stats``, which must be zero; allocated zeroed when
+    not given).  ``skip_out`` / ``hidden_out`` may be the inputs themselves (in place); new tensors when not given.
+    Returns (skip_out, hidden_out, skip_stats, hidden_stats)."""
+    _req(skip, bf16, "freeu_apply.skip", 4)
+    _req(hidden, bf16, "freeu_apply.hidden", 4)
+    B, H, W, Cs = skip.shape
+    Ch = hidden.shape[-1]
+    if tuple(hidden.shape[:3]) != (B, H, W):
+        raise DsEngineError("freeu_apply: skip and hidden must have the same batch and pixels")
+    _req(moments, torch.float64, "freeu_apply.moments")
+    if moments.numel() != 7 * B * Cs:
+        raise DsEngineError("freeu_apply: moments must hold B*C_skip*7 doubles")
+
+    def out_(t, like, name):
+        if t is None:
+            return torch.empty_like(like)
+        _req(t, bf16, name)
+        if t.shape != like.shape:
+            raise DsEngineError(f"{name}: shape mismatch")
+        return t
+
+    def stats_(t, Cc, name):
+        if t is None:
+            return zero_(torch.empty(B, Cc, 2, dtype=torch.float64, device=skip.device))
+        _req(t, torch.float64, name)
+        if t.numel() != 2 * B * Cc:
+            raise DsEngineError(f"{name}: must hold B*C*2 doubles")
+        return t
+
+    skip_out = out_(skip_out, skip, "freeu_apply.skip_out")
+    hidden_out = out_(hidden_out, hidden, "freeu_apply.hidden_out")
+    skip_stats = stats_(skip_stats, Cs, "freeu_apply.skip_stats")
+    hidden_stats = stats_(hidden_stats, Ch, "freeu_apply.hidden_stats")
+    check(lib.ds_freeu_apply(skip.data_ptr(), moments.data_ptr(), skip_out.data_ptr(), skip_stats.data_ptr(), Cs,
+                             hidden.data_ptr(), hidden_out.data_ptr(), hidden_stats.data_ptr(), Ch, float(s), float(b),
+                             B, H, W, _stream()), "ds_freeu_apply")
+    return skip_out, hidden_out, skip_stats, hidden_stats
+
+
 def groupnorm_silu(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, groups: int, eps: float,
                    silu: bool = True, out: Optional[torch.Tensor] = None,
                    stats: Optional[torch.Tensor] = None) -> torch.Tensor:

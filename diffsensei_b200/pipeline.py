@@ -203,6 +203,16 @@ class DiffSenseiPipeline:
             return self._pag_site_set(), float(pag_scale), float(pag_adaptive_scale)
         return None
 
+    # ------------------------------------------------------------------------------ FreeU
+    def enable_freeu(self, s1: float, s2: float, b1: float, b2: float) -> None:
+        """diffusers' ``StableDiffusionMixin.enable_freeu``, delegated to the UNet (``UNetMangaEngine.enable_freeu``):
+        every later denoise (``__call__``, ``generate_page``, all their modes) runs with FreeU while all four values are
+        truthy.  Pipeline state, not a call argument; the values are part of the captured stepper's key."""
+        self.unet.enable_freeu(s1, s2, b1, b2)
+
+    def disable_freeu(self) -> None:
+        self.unet.disable_freeu()
+
     def check_inputs(self, prompt, prompt_2, ip_images, ip_image_embeds, ip_bbox):
         if prompt is None:
             raise ValueError(f"`prompt` has to be of type `str` but is {type(prompt)}")
@@ -369,19 +379,26 @@ class DiffSenseiPipeline:
                               dialog_bbox, num_inference_steps, guidance_scale, use_graph, chains, start_index,
                               inpaint, pag)
 
+    def stepper_key(self, latents, prompt_embeds, aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale,
+                    chains=None, start_index: int = 0, inpaint=None, pag=None) -> tuple:
+        """Everything a captured stepper bakes in (``stepper_for``), FreeU's values (``unet.freeu``) included."""
+        return (tuple(latents.shape), tuple(prompt_embeds.shape), None if dialog_bbox is None else
+                (tuple(dialog_bbox.shape), dialog_bbox.dtype == bf16), float(aspect_ratio), int(num_inference_steps),
+                float(guidance_scale), self.unet.scales_key(), chains, self.unet._ip_weights_version(),
+                type(self.scheduler).__name__, tuple(sorted(self.scheduler.config.items())), int(start_index),
+                inpaint is not None, None if pag is None else tuple(sorted(pag[0])), self.unet.freeu)
+
     def stepper_for(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio, dialog_bbox,
                     num_inference_steps, guidance_scale, chains=None, start_index: int = 0,
                     inpaint=None, pag=None) -> "DenoiseStepper":
         """A graph-captured stepper loaded with this panel: a cached one of the same key is refilled in place
         (no re-capture), otherwise a new one is built and cached.  The start index is part of the key: the stepper
         bakes in its slice of the schedule (``set_timesteps`` would reset any scheduler state); so is whether it
-        inpaints, which selects the step kernel, and the perturbed-attention sites (``pag``: None when off).  The
-        PAG scales are not: they live in the coefficient table, which ``load_panel`` rewrites."""
-        key = (tuple(latents.shape), tuple(prompt_embeds.shape), None if dialog_bbox is None else
-               (tuple(dialog_bbox.shape), dialog_bbox.dtype == bf16), float(aspect_ratio), int(num_inference_steps),
-               float(guidance_scale), self.unet.scales_key(), chains, self.unet._ip_weights_version(),
-               type(self.scheduler).__name__, tuple(sorted(self.scheduler.config.items())), int(start_index),
-               inpaint is not None, None if pag is None else tuple(sorted(pag[0])))
+        inpaints, which selects the step kernel, the perturbed-attention sites (``pag``: None when off) and FreeU's
+        values, which the graph bakes in.  The PAG scales are not: they live in the coefficient table, which
+        ``load_panel`` rewrites."""
+        key = self.stepper_key(latents, prompt_embeds, aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale,
+                               chains, start_index, inpaint, pag)
         st = self._steppers.get(key)
         if st is None:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,

@@ -118,6 +118,7 @@ class UNetMangaEngine:
         self._cond_cache: Optional[Conditions] = None
         self._processors = None
         self._lora = None              # lora.LoraMerger, made by the first load_lora
+        self._freeu = None             # (s1, s2, b1, b2) as enable_freeu was given them
         self.num_upsamplers = len(cfg.block_out_channels) - 1
         if self.device.type == "cuda":
             with torch.cuda.device(self.device):
@@ -162,6 +163,34 @@ class UNetMangaEngine:
         if self._processors is None:
             return (self.ip_scale,)
         return tuple(float(p.scale) for p in self._processors.values() if hasattr(p, "scale"))
+
+    # ------------------------------------------------------------------------------------------ FreeU
+    def enable_freeu(self, s1, s2, b1, b2) -> None:
+        """diffusers' ``UNet2DConditionModel.enable_freeu``: up-blocks 0 and 1 scale the first half of the backbone
+        channels by ``b1`` / ``b2`` and the low frequencies of the skip connections by ``s1`` / ``s2`` in front of each
+        resnet.  As in diffusers, FreeU only acts while all four values are truthy (a 0 turns it off)."""
+        self._freeu = (s1, s2, b1, b2)
+
+    def disable_freeu(self) -> None:
+        self._freeu = None
+
+    @property
+    def freeu(self) -> Optional[Tuple[float, float, float, float]]:
+        """(s1, s2, b1, b2) as floats while FreeU acts, else None.  A captured CUDA graph bakes them in by value."""
+        f = self._freeu
+        return None if f is None or not all(f) else tuple(float(v) for v in f)
+
+    def _freeu_pool_slots(self) -> int:
+        """Statistics-pool slots (B * max(C) * 2 doubles each) FreeU takes per forward: at each of its sites the skip's
+        moments (7 per channel) and the new statistics of the skip and the hidden tensor (2 per channel each)."""
+        ch, nres = self.cfg.block_out_channels, self.cfg.layers_per_block + 1
+        rch, cmax, n = list(reversed(ch)), max(ch), 0
+        for i in range(min(2, len(ch))):
+            for j in range(nres):
+                c_hidden = (rch[i - 1] if i else rch[0]) if j == 0 else rch[i]
+                c_skip = rch[i] if j < nres - 1 else rch[min(i + 1, len(ch) - 1)]
+                n += -(-(9 * c_skip + 2 * c_hidden) // (2 * cmax))
+        return n
 
     def _ip_weights_version(self) -> int:
         """Moves when a checkpoint is loaded INTO the processors (their Parameters alias the packed IP weights)."""
@@ -401,11 +430,11 @@ class UNetMangaEngine:
             ops.zero_(self.buf)                                               # ONE memset node per forward
             self.off, self.B = 0, B
 
-        def take(self, C: int) -> torch.Tensor:
-            n = self.B * C * 2
+        def take(self, C: int, per_channel: int = 2) -> torch.Tensor:
+            n = self.B * C * per_channel
             if self.off + n > self.buf.numel():
                 raise RuntimeError("UNetMangaEngine: statistics pool exhausted")
-            v = self.buf[self.off:self.off + n].view(self.B, C, 2)
+            v = self.buf[self.off:self.off + n].view(self.B, C, per_channel)
             self.off += n
             return v
 
@@ -490,7 +519,8 @@ class UNetMangaEngine:
         """x: bf16 [B,H,W,4]; temb: fp32 [B, sum(Cout)] from ``time_rowbias``; returns eps bf16 [B,H,W,4]
         (written into ``out`` when given — a contiguous batch slice of a larger buffer is fine).
         Perturbed-attention guidance: at the self-attention sites named in ``pag_sites`` (``resolve_pag_layers``),
-        batch rows ``pag_row0`` .. B-1 take the identity attention map, ``to_out(to_v(x))``."""
+        batch rows ``pag_row0`` .. B-1 take the identity attention map, ``to_out(to_v(x))``.
+        FreeU (``enable_freeu``) acts on every row."""
         cfg = self.cfg
         tr = lambda p, h, st, **kw: self._transformer(p, h, st, cond, pool, pag_sites=pag_sites, pag_row0=pag_row0,
                                                       **kw)
@@ -498,7 +528,8 @@ class UNetMangaEngine:
         nlev = len(ch)
         B, H, W, _ = x.shape
         need_size = (H % (2 ** (nlev - 1)) != 0) or (W % (2 ** (nlev - 1)) != 0)       # unet.py:152-162
-        pool = self._Pool(B, max(ch), x.device)
+        freeu = self.freeu
+        pool = self._Pool(B, max(ch), x.device, 64 + (self._freeu_pool_slots() if freeu else 0))
         # conv_in on the tensor cores: im2col of the 4-channel latent (K = 36 -> 64) + one GEMM whose epilogue also
         # takes the GroupNorm statistics — unless the dialog embedding is added afterwards (it changes them)
         st = None
@@ -532,6 +563,13 @@ class UNetMangaEngine:
             nres = cfg.layers_per_block + 1
             for j in range(nres):
                 sk, sk_st = skips.pop()
+                if freeu is not None and i < 2:
+                    # diffusers' apply_freeu, in place: the popped skip and the hidden tensor have no other reader;
+                    # the statistics their producers emitted are stale, the kernel emits new ones
+                    mom = ops.freeu_moments(sk, out=pool.take(sk.shape[-1], 7))
+                    sk_st, st = pool.take(sk.shape[-1]), pool.take(h.shape[-1])
+                    ops.freeu_apply(sk, h, mom, freeu[i], freeu[2 + i], skip_out=sk, hidden_out=h, skip_stats=sk_st,
+                                    hidden_stats=st)
                 feeds_gn = not (j == nres - 1 and i < nlev - 1)       # the block's last output only feeds the upsampler
                 has_attn = rdepth[i] > 0
                 h, st = self._resnet(f"up_blocks.{i}.resnets.{j}", h, st, temb, pool, skip=sk, skip_st=sk_st,

@@ -65,6 +65,28 @@ int64_t ds_groupnorm_scratch_floats(int B, int C);
 int ds_groupnorm_silu(const void* x, void* y, const float* gamma, const float* beta, float* stats, int B, int HW,
                       int C, int groups, float eps, int apply_silu, void* stream);
 
+/* FreeU (diffusers' enable_freeu(s1, s2, b1, b2) / apply_freeu), in front of every resnet of up-blocks 0 and 1:
+ *   hidden[:, :C_hidden/2] *= b  and  skip = fourier_filter(skip, threshold=1, scale=s)      [HBM-bound]
+ * fourier_filter (diffusers.utils.torch_utils) scales the frequencies {0, -1 mod H} x {0, -1 mod W} (as sets: a size-1
+ * axis contributes {0} alone) of the 2-D DFT over (H, W) by s; with threshold 1 that is a closed form in 7 real moments
+ * per (sample, channel), so no FFT runs (freeu_kernels.cu).  NHWC bf16, per site:
+ *   ds_freeu_moments : moments fp64 [B][C][7] of skip [B][H][W][C] = {sum x, sum x cos th, sum x sin th, sum x cos ph,
+ *                      sum x sin ph, sum x cos(th + ph), sum x sin(th + ph)}, th = 2 pi h / H, ph = 2 pi w / W.
+ *                      ACCUMULATES into `moments` (caller zeroes): fp32 partials over runs of pixels that depend
+ *                      only on (H, W, C), combined with fp64 atomics, so a sample's moments do not depend on B.
+ *   ds_freeu_apply   : ONE launch writes the filtered skip to skip_out and hidden [B][H][W][C_hidden] with channels
+ *                      [0, C_hidden/2) multiplied by b to hidden_out (an fp32 multiply and one bf16 rounding, torch's
+ *                      bf16 `x * b`; the filter in fp32, one rounding), from the moments of ds_freeu_moments.  It also
+ *                      ACCUMULATES the GroupNorm statistics (ds_channel_stats' layout fp64 [B][C][2], caller zeroes)
+ *                      of both outputs into skip_stats / hidden_stats — the same bits ds_channel_stats gives for them.
+ *                      skip_out may be skip and hidden_out may be hidden (in place: the engine's up path does that; the
+ *                      hidden channels from C_hidden/2 on are then not written); otherwise no overlap.
+ * Pointers 16-byte aligned (moments 8-byte); C, C_skip, C_hidden multiples of 8, <= 4096; H, W <= 2048. */
+int ds_freeu_moments(const void* skip, double* moments, int B, int H, int W, int C, void* stream);
+int ds_freeu_apply(const void* skip, const double* moments, void* skip_out, double* skip_stats, int C_skip,
+                   const void* hidden, void* hidden_out, double* hidden_stats, int C_hidden, float s, float b, int B,
+                   int H, int W, void* stream);
+
 /* LayerNorm over the last dim, bf16 in/out, fp32 affine.     [HBM-bound]
  * Replaces BasicTransformerBlock.norm1/2/3 (eps 1e-5) and Resampler LayerNorms
  * (src/models/resampler.py:14,40-41,104). rows x C, C % 8 == 0, C <= 5120. */
