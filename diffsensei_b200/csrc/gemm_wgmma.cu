@@ -1180,8 +1180,12 @@ static int build_problem(const ds_gemm_args* a, CUtensorMap* tmA_out, CUtensorMa
   DS_REQUIRE((reinterpret_cast<uintptr_t>(a->a) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->w) & 15) == 0,
              "ds_gemm_bf16: a and w must be 16-byte aligned");
   DS_REQUIRE(a->epilogue >= DS_EPI_NONE && a->epilogue <= DS_EPI_QUICKGELU, "ds_gemm_bf16: bad epilogue %d", a->epilogue);
-  if (a->epilogue == DS_EPI_GEGLU)
+  if (a->epilogue == DS_EPI_GEGLU) {
     DS_REQUIRE(a->N % 256 == 0, "ds_gemm_bf16: GEGLU needs N %% 256 == 0 (128 value + 128 gate rows per block)");
+    // the GEGLU pass adds the row bias to the value columns only (one more per-element load for the gates spills
+    // the 256-wide accumulator): refuse the combination rather than return value * gelu(gate without row bias)
+    DS_REQUIRE(a->rowbias == nullptr, "ds_gemm_bf16: GEGLU takes no rowbias");
+  }
   if (a->rowbias) DS_REQUIRE(a->rows_per_batch > 0, "ds_gemm_bf16: rowbias needs rows_per_batch > 0");
   const int n_out = a->epilogue == DS_EPI_GEGLU ? a->N / 2 : a->N;
   DS_REQUIRE(a->ldo >= n_out, "ds_gemm_bf16: ldo (%d) smaller than output width (%d)", a->ldo, n_out);

@@ -123,8 +123,8 @@ int ds_ip_mask(const float* bbox, float* mask, int B, int N, double aspect_ratio
  *   v = acc + bias[n] + rowbias[row / rows_per_batch][n]
  *   DS_EPI_GEGLU: W/bias rows are packed in blocks of 128 "value" rows followed by their 128 "gate"
  *                 rows (see diffsensei_b200.weights.pack_geglu); out[:, j] = v_val * gelu_erf(v_gate),
- *                 Nout = N/2.  gelu_erf(x) = x * Phi(x) is evaluated as x * sigmoid(2k(x + a x^3 + b x^5)) with
- *                 (k, a, b) fitted to Phi: |abs err| <= 2.6e-5 for all x (the bf16 output rounding is >= 10x larger).
+ *                 Nout = N/2; no rowbias (refused).  gelu_erf(x) = x * Phi(x) is evaluated as x * sigmoid(2k(x + a x^3 + b x^5)) with
+ *                 (k, a, b) fitted to Phi: |abs err| <= 2.6e-5 for x >= -8900 (the bf16 output rounding is >= 10x larger).
  *   DS_EPI_GELU / DS_EPI_SILU / DS_EPI_QUICKGELU : v = act(v)
  *   then v += residual[row][n] (bf16) and v *= out_scale (if != 0).
  * LayerNorm fusion (diffusers BasicTransformerBlock.norm1/2/3 -> the linears on either side of them):
