@@ -89,11 +89,9 @@ SIGNATURES = {
     "ds_image_postprocess": [_vp, _vp, _i, _i, _i, _vp],
     "ds_attention_single_head": [_vp, _vp, _vp, _vp, _i, _i, _i, _i64, _vp],
     "ds_image_preprocess": [_vp, _vp, _vp, _i, _i, _vp, _vp, _i64, _vp],
-    "ds_vae_image_preprocess": [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _i64, _vp],
+    "ds_vae_preprocess": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i64, _vp],
     "ds_vae_image_pack": [_vp, _vp, _vp, _i, _i, _i, _vp],
-    "ds_vae_mask_preprocess": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i64, _vp],
     "ds_vae_mask_pack": [_vp, _i, _i, _vp, _vp, _vp],
-    "ds_vae_fill_preprocess": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i64, _vp],
     "ds_vae_overlay": [_vp, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i64, _vp],
     "ds_vae_posterior": [_vp, _vp, _vp, _vp, _f, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _vp],
     "ds_gemv_bf16": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],
@@ -107,9 +105,8 @@ SIGNATURES = {
     "ds_agent_next_token_rows": [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i64, _i, _i, _vp],
 }
 OTHER_EXPORTS = ("ds_version", "ds_last_error", "ds_launch_count", "ds_groupnorm_scratch_floats",
-                 "ds_gemm_splitk_ws_bytes", "ds_image_preprocess_scratch_bytes",
-                 "ds_vae_image_preprocess_scratch_bytes", "ds_vae_mask_preprocess_scratch_bytes",
-                 "ds_vae_fill_preprocess_scratch_bytes", "ds_vae_overlay_scratch_bytes")
+                 "ds_gemm_splitk_ws_bytes", "ds_image_preprocess_scratch_bytes", "ds_vae_preprocess_scratch_bytes",
+                 "ds_vae_overlay_scratch_bytes")
 
 
 def _load() -> C.CDLL:
@@ -131,12 +128,8 @@ def _load() -> C.CDLL:
     lib.ds_gemm_splitk_ws_bytes.restype = C.c_int64
     lib.ds_image_preprocess_scratch_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int]
     lib.ds_image_preprocess_scratch_bytes.restype = C.c_int64
-    lib.ds_vae_image_preprocess_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
-    lib.ds_vae_image_preprocess_scratch_bytes.restype = C.c_int64
-    lib.ds_vae_mask_preprocess_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
-    lib.ds_vae_mask_preprocess_scratch_bytes.restype = C.c_int64
-    lib.ds_vae_fill_preprocess_scratch_bytes.argtypes = [C.c_int] * 10
-    lib.ds_vae_fill_preprocess_scratch_bytes.restype = C.c_int64
+    lib.ds_vae_preprocess_scratch_bytes.argtypes = [C.c_int] * 10
+    lib.ds_vae_preprocess_scratch_bytes.restype = C.c_int64
     lib.ds_vae_overlay_scratch_bytes.argtypes = [C.c_int] * 9
     lib.ds_vae_overlay_scratch_bytes.restype = C.c_int64
     return lib

@@ -20,9 +20,10 @@
 // crop / rescale / normalise.  Tables and the intermediate live in the caller's scratch; the tap count per output
 // index is not bounded by anything but the image size.
 //
-// The same resampler also serves the AutoencoderKL encoder's preprocessing (ds_vae_image_preprocess: Pillow LANCZOS
-// to any size, then 2 * u8 / 255 - 1) and the inpaint mask's (ds_vae_mask_preprocess: LANCZOS on the mask's own 1 or
-// 3 channels, RGB -> L, threshold), with host-built tap tables; see the section below plan_images.
+// The same resampler also serves diffusers' VaeImageProcessor.preprocess (ds_vae_preprocess: an optional crop, Pillow
+// LANCZOS to any size or _resize_and_fill, then the AutoencoderKL encoder's 2 * u8 / 255 - 1 or the inpaint mask's
+// RGB -> L and threshold) and apply_overlay (ds_vae_overlay), with host-built tap tables; see the sections below
+// plan_images.
 #include <cuda_bf16.h>
 
 #include <cmath>
@@ -368,29 +369,6 @@ __device__ __forceinline__ void vae_vpass_pixel(const unsigned char* __restrict_
   }
 }
 
-// one output pixel per thread: vertical pass (or a copy), float32(u8) / 255, 2x - 1 -> fp32 NCHW and / or bf16 NHWC
-// with a zero 4th channel (the input of the encoder's conv_in)
-__global__ void vae_image_vpass_kernel(const unsigned char* __restrict__ base, long long pitch,
-                                       const int* __restrict__ coef, int kv, int oh, int ow, float* __restrict__ out,
-                                       uint2* __restrict__ out4) {
-  const long long hw = static_cast<long long>(oh) * ow;
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= hw) return;
-  const int y = static_cast<int>(i / ow), x = static_cast<int>(i - static_cast<long long>(y) * ow);
-  int v[3];
-  vae_vpass_pixel<3>(base, pitch, coef, kv, y, x, v);
-  float o[3];
-#pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    o[c] = __fsub_rn(__fmul_rn(2.0f, __fdiv_rn(static_cast<float>(v[c]), 255.0f)), 1.0f);
-    if (out) out[c * hw + i] = o[c];
-  }
-  if (out4) {
-    __nv_bfloat162 lo = __floats2bfloat162_rn(o[0], o[1]), hi = __floats2bfloat162_rn(o[2], 0.0f);
-    out4[i] = make_uint2(*reinterpret_cast<uint32_t*>(&lo), *reinterpret_cast<uint32_t*>(&hi));
-  }
-}
-
 // float NCHW [B][3][HW] -> (normalize ? 2x - 1 : x) as fp32 NCHW (may alias x) and / or bf16 NHWC with a zero 4th channel
 __global__ void vae_image_pack_kernel(const float* x, float* out, uint2* __restrict__ out4, int HW, int normalize,
                                       long long total) {
@@ -409,28 +387,6 @@ __global__ void vae_image_pack_kernel(const float* x, float* out, uint2* __restr
     __nv_bfloat162 lo = __floats2bfloat162_rn(o[0], o[1]), hi = __floats2bfloat162_rn(o[2], 0.0f);
     out4[i] = make_uint2(*reinterpret_cast<uint32_t*>(&lo), *reinterpret_cast<uint32_t*>(&hi));
   }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Inpaint mask preprocessing (diffusers VaeImageProcessor(do_normalize=False, do_binarize=True,
-// do_convert_grayscale=True).preprocess + prepare_mask_latents' nearest downsample): the same resampler on the mask's
-// own channels (1: "L", 3: "RGB"), then for RGB Pillow's RGB -> L conversion of the resized pixels,
-// L = (19595 R + 38470 G + 7471 B + 0x8000) >> 16, then float32(L) / 255 >= 0.5, i.e. L >= 128.  One output pixel per
-// thread; the pixel at (8i, 8j) also writes latent pixel (i, j) (F.interpolate nearest to H/8 x W/8).
-template <int C>
-__global__ void vae_mask_vpass_kernel(const unsigned char* __restrict__ base, long long pitch,
-                                      const int* __restrict__ coef, int kv, int oh, int ow, float* __restrict__ out,
-                                      unsigned char* __restrict__ out_latent) {
-  const long long hw = static_cast<long long>(oh) * ow;
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= hw) return;
-  const int y = static_cast<int>(i / ow), x = static_cast<int>(i - static_cast<long long>(y) * ow);
-  int v[C];
-  vae_vpass_pixel<C>(base, pitch, coef, kv, y, x, v);
-  const int l = C == 3 ? (v[0] * 19595 + v[1] * 38470 + v[2] * 7471 + 0x8000) >> 16 : v[0];
-  const bool keep = l >= 128;
-  if (out) out[i] = keep ? 1.0f : 0.0f;
-  if (out_latent && (y & 7) == 0 && (x & 7) == 0) out_latent[(y >> 3) * (ow >> 3) + (x >> 3)] = keep;
 }
 
 // a float mask already at its size [H][W] -> (x >= 0.5) as fp32 and / or the uint8 latent mask [H/8][W/8]
@@ -488,8 +444,9 @@ static int vae_resample_begin(const uint8_t* src, int H, int W, long long row_px
 }
 
 // ------------------------------------------------------------------------------------------------
-// diffusers VaeImageProcessor.preprocess(..., crops_coords, resize_mode) of the SDXL inpaint pipeline's
-// padding_mask_crop: Image.crop(crops_coords), then
+// diffusers VaeImageProcessor.preprocess(..., crops_coords, resize_mode) of one uint8 image or mask:
+// Image.crop(crops_coords) (the whole image without them; the SDXL inpaint pipeline's padding_mask_crop passes them),
+// then
 //   resize_mode "fill"    (_resize_and_fill): ratio = w / h, src_ratio = cw / ch (crop size), the crop resized with
 //                         LANCZOS to fit, rw = ratio < src_ratio ? w : cw * h // ch, rh = ratio >= src_ratio ? h :
 //                         ch * w // cw, pasted at (w // 2 - rw // 2, h // 2 - rh // 2) on a black w x h canvas; when
@@ -499,9 +456,16 @@ static int vae_resample_begin(const uint8_t* src, int H, int W, long long row_px
 //                         (zero-width) source box, every stripe row the same weighted mix of the resized image's
 //                         first (last) rows; a canvas row or column neither covers stays black;
 //   resize_mode "default" (Image.resize): the crop resized with LANCZOS to w x h.
-// One launch of the existing horizontal pass over the crop (the source rows keep the image's pitch), then one thread
-// per output pixel: the vertical pass of the resized pixel, or of the 2 resized rows (columns) a stripe pixel
-// mixes, then the image epilogue (float32(u8) / 255, 2x - 1) or the mask epilogue (RGB -> L, >= 128).
+// Then the epilogue of the processor's configuration:
+//   image (the default one, the AutoencoderKL encoder's input): float32(u8) / 255, 2x - 1 -> fp32 NCHW and / or bf16
+//         NHWC with a zero 4th channel (the input of the encoder's conv_in);
+//   mask  (do_normalize=False, do_binarize=True, do_convert_grayscale=True; resized in its own mode, C = 1 "L" or
+//         3 "RGB"): for RGB Pillow's RGB -> L conversion of the resized pixels, L = (19595 R + 38470 G + 7471 B +
+//         0x8000) >> 16, then float32(L) / 255 >= 0.5, i.e. L >= 128 -> fp32; the pixel at (8i, 8j) also writes
+//         latent pixel (i, j) (prepare_mask_latents' F.interpolate nearest to H/8 x W/8).
+// One launch of the horizontal pass over the crop (the source rows keep the image's pitch; skipped when the width
+// does not change), then one thread per output pixel: the vertical pass of the resized pixel (a copy when the height
+// does not change), or of the 2 resized rows (columns) a stripe pixel mixes, then the epilogue.
 struct FillPlan {
   VaePlan main;           // the crop (ch x cw) -> rh x rw resize
   int x1, y1, cw, ch;     // crop origin and size in the source
@@ -590,7 +554,7 @@ __device__ __forceinline__ void fill_stripe_pixel(const FillArgs& a, const int* 
 }
 
 template <int C, bool kMask>
-__global__ void vae_fill_kernel(FillArgs a) {
+__global__ void vae_preprocess_kernel(FillArgs a) {
   const long long hw = static_cast<long long>(a.oh) * a.ow;
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= hw) return;
@@ -828,42 +792,6 @@ extern "C" int ds_image_preprocess(const uint8_t* src, const int64_t* offsets, c
   return DS_OK;
 }
 
-extern "C" int64_t ds_vae_image_preprocess_scratch_bytes(int H, int W, int out_h, int out_w) {
-  if (H < 1 || W < 1 || H > ds::kMaxSide || W > ds::kMaxSide || out_h < 1 || out_w < 1 || out_h > ds::kMaxSide ||
-      out_w > ds::kMaxSide)
-    return -1;
-  return ds::plan_vae(H, W, out_h, out_w, 3).total;
-}
-
-extern "C" int ds_vae_image_preprocess(const uint8_t* src, int H, int W, int out_h, int out_w, float* out,
-                                       void* out_nhwc4, void* scratch, int64_t scratch_bytes, void* stream) {
-  using namespace ds;
-  DS_REQUIRE(src && (out || out_nhwc4), "ds_vae_image_preprocess: bad arguments");
-  DS_REQUIRE(H >= 1 && W >= 1 && H <= kMaxSide && W <= kMaxSide && out_h >= 1 && out_w >= 1 && out_h <= kMaxSide &&
-                 out_w <= kMaxSide,
-             "ds_vae_image_preprocess: %d x %d -> %d x %d; sides must be in [1, %d]", H, W, out_h, out_w, kMaxSide);
-  DS_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3) == 0 && (reinterpret_cast<uintptr_t>(out_nhwc4) & 7) == 0,
-             "ds_vae_image_preprocess: out must be 4-byte and out_nhwc4 8-byte aligned");
-  const VaePlan p = plan_vae(H, W, out_h, out_w, 3);
-  DS_REQUIRE(p.total == 0 || (scratch && scratch_bytes >= p.total && (reinterpret_cast<uintptr_t>(scratch) & 15) == 0),
-             "ds_vae_image_preprocess: needs %lld bytes of 16-byte aligned scratch "
-             "(ds_vae_image_preprocess_scratch_bytes), got %lld", p.total, static_cast<long long>(scratch_bytes));
-  DeviceInfo dev;
-  if (!get_device(&dev)) return DS_ERR_CUDA;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  unsigned char* scr = static_cast<unsigned char*>(scratch);
-  const unsigned char* base;
-  long long pitch;
-  const int rc = vae_resample_begin<3>(src, H, W, W, out_h, out_w, p, scr, st, &base, &pitch);
-  if (rc != DS_OK) return rc;
-  const long long hw = static_cast<long long>(out_h) * out_w;
-  vae_image_vpass_kernel<<<static_cast<unsigned>((hw + 255) / 256), 256, 0, st>>>(
-      base, pitch, reinterpret_cast<const int*>(scr + p.coef_v), p.kv, out_h, out_w, out,
-      static_cast<uint2*>(out_nhwc4));
-  DS_LAUNCH_OK("vae_image_vpass_kernel");
-  return DS_OK;
-}
-
 extern "C" int ds_vae_image_pack(const float* x, float* out, void* out_nhwc4, int B, int HW, int normalize,
                                  void* stream) {
   using namespace ds;
@@ -875,49 +803,6 @@ extern "C" int ds_vae_image_pack(const float* x, float* out, void* out_nhwc4, in
   vae_image_pack_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       x, out, static_cast<uint2*>(out_nhwc4), HW, normalize, total);
   DS_LAUNCH_OK("vae_image_pack_kernel");
-  return DS_OK;
-}
-
-extern "C" int64_t ds_vae_mask_preprocess_scratch_bytes(int H, int W, int C, int out_h, int out_w) {
-  if (H < 1 || W < 1 || H > ds::kMaxSide || W > ds::kMaxSide || out_h < 1 || out_w < 1 || out_h > ds::kMaxSide ||
-      out_w > ds::kMaxSide || (C != 1 && C != 3))
-    return -1;
-  return ds::plan_vae(H, W, out_h, out_w, C).total;
-}
-
-extern "C" int ds_vae_mask_preprocess(const uint8_t* src, int H, int W, int C, int out_h, int out_w, float* out,
-                                      uint8_t* out_latent, void* scratch, int64_t scratch_bytes, void* stream) {
-  using namespace ds;
-  DS_REQUIRE(src && (out || out_latent), "ds_vae_mask_preprocess: bad arguments");
-  DS_REQUIRE(C == 1 || C == 3, "ds_vae_mask_preprocess: C must be 1 (L) or 3 (RGB), got %d", C);
-  DS_REQUIRE(H >= 1 && W >= 1 && H <= kMaxSide && W <= kMaxSide && out_h >= 1 && out_w >= 1 && out_h <= kMaxSide &&
-                 out_w <= kMaxSide,
-             "ds_vae_mask_preprocess: %d x %d -> %d x %d; sides must be in [1, %d]", H, W, out_h, out_w, kMaxSide);
-  DS_REQUIRE(!out_latent || (out_h % 8 == 0 && out_w % 8 == 0),
-             "ds_vae_mask_preprocess: the latent mask needs an output size that is a multiple of 8, got %d x %d", out_h,
-             out_w);
-  DS_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3) == 0, "ds_vae_mask_preprocess: out must be 4-byte aligned");
-  const VaePlan p = plan_vae(H, W, out_h, out_w, C);
-  DS_REQUIRE(p.total == 0 || (scratch && scratch_bytes >= p.total && (reinterpret_cast<uintptr_t>(scratch) & 15) == 0),
-             "ds_vae_mask_preprocess: needs %lld bytes of 16-byte aligned scratch "
-             "(ds_vae_mask_preprocess_scratch_bytes), got %lld", p.total, static_cast<long long>(scratch_bytes));
-  DeviceInfo dev;
-  if (!get_device(&dev)) return DS_ERR_CUDA;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  unsigned char* scr = static_cast<unsigned char*>(scratch);
-  const unsigned char* base;
-  long long pitch;
-  const int rc = C == 3 ? vae_resample_begin<3>(src, H, W, W, out_h, out_w, p, scr, st, &base, &pitch)
-                        : vae_resample_begin<1>(src, H, W, W, out_h, out_w, p, scr, st, &base, &pitch);
-  if (rc != DS_OK) return rc;
-  const long long hw = static_cast<long long>(out_h) * out_w;
-  const unsigned blocks = static_cast<unsigned>((hw + 255) / 256);
-  const int* coef_v = reinterpret_cast<const int*>(scr + p.coef_v);
-  if (C == 3)
-    vae_mask_vpass_kernel<3><<<blocks, 256, 0, st>>>(base, pitch, coef_v, p.kv, out_h, out_w, out, out_latent);
-  else
-    vae_mask_vpass_kernel<1><<<blocks, 256, 0, st>>>(base, pitch, coef_v, p.kv, out_h, out_w, out, out_latent);
-  DS_LAUNCH_OK("vae_mask_vpass_kernel");
   return DS_OK;
 }
 
@@ -935,34 +820,34 @@ extern "C" int ds_vae_mask_pack(const float* x, int H, int W, float* out, uint8_
   return DS_OK;
 }
 
-extern "C" int64_t ds_vae_fill_preprocess_scratch_bytes(int H, int W, int C, int x1, int y1, int x2, int y2,
-                                                        int out_h, int out_w, int fill) {
+extern "C" int64_t ds_vae_preprocess_scratch_bytes(int H, int W, int C, int x1, int y1, int x2, int y2, int out_h,
+                                                   int out_w, int fill) {
   ds::FillPlan p;
   if (!ds::plan_fill(H, W, C, x1, y1, x2, y2, out_h, out_w, fill, &p)) return -1;
   return p.total;
 }
 
-extern "C" int ds_vae_fill_preprocess(const uint8_t* src, int H, int W, int C, int x1, int y1, int x2, int y2,
-                                      int out_h, int out_w, int fill, int mask, float* out, void* out2, void* scratch,
-                                      int64_t scratch_bytes, void* stream) {
+extern "C" int ds_vae_preprocess(const uint8_t* src, int H, int W, int C, int x1, int y1, int x2, int y2, int out_h,
+                                 int out_w, int fill, int mask, float* out, void* out2, void* scratch,
+                                 int64_t scratch_bytes, void* stream) {
   using namespace ds;
-  DS_REQUIRE(src && (out || out2), "ds_vae_fill_preprocess: bad arguments");
-  DS_REQUIRE(mask == 0 || mask == 1, "ds_vae_fill_preprocess: mask must be 0 (image) or 1 (mask), got %d", mask);
-  DS_REQUIRE(mask ? (C == 1 || C == 3) : C == 3, "ds_vae_fill_preprocess: C must be 3 for an image, 1 or 3 for a "
+  DS_REQUIRE(src && (out || out2), "ds_vae_preprocess: bad arguments");
+  DS_REQUIRE(mask == 0 || mask == 1, "ds_vae_preprocess: mask must be 0 (image) or 1 (mask), got %d", mask);
+  DS_REQUIRE(mask ? (C == 1 || C == 3) : C == 3, "ds_vae_preprocess: C must be 3 for an image, 1 or 3 for a "
              "mask, got %d", C);
   FillPlan p;
   DS_REQUIRE(plan_fill(H, W, C, x1, y1, x2, y2, out_h, out_w, fill, &p),
-             "ds_vae_fill_preprocess: crop (%d, %d, %d, %d) of a %d x %d image -> %d x %d (fill %d) is not supported: "
+             "ds_vae_preprocess: crop (%d, %d, %d, %d) of a %d x %d image -> %d x %d (fill %d) is not supported: "
              "the crop must lie inside the image, sides in [1, %d], and the resized crop must be at least 1 x 1",
              x1, y1, x2, y2, H, W, out_h, out_w, fill, kMaxSide);
   DS_REQUIRE(!(mask && out2) || (out_h % 8 == 0 && out_w % 8 == 0),
-             "ds_vae_fill_preprocess: the latent mask needs an output size that is a multiple of 8, got %d x %d", out_h,
+             "ds_vae_preprocess: the latent mask needs an output size that is a multiple of 8, got %d x %d", out_h,
              out_w);
   DS_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3) == 0 && (mask || (reinterpret_cast<uintptr_t>(out2) & 7) == 0),
-             "ds_vae_fill_preprocess: out must be 4-byte and an image's out2 8-byte aligned");
+             "ds_vae_preprocess: out must be 4-byte and an image's out2 8-byte aligned");
   DS_REQUIRE(p.total == 0 || (scratch && scratch_bytes >= p.total && (reinterpret_cast<uintptr_t>(scratch) & 15) == 0),
-             "ds_vae_fill_preprocess: needs %lld bytes of 16-byte aligned scratch "
-             "(ds_vae_fill_preprocess_scratch_bytes), got %lld", p.total, static_cast<long long>(scratch_bytes));
+             "ds_vae_preprocess: needs %lld bytes of 16-byte aligned scratch "
+             "(ds_vae_preprocess_scratch_bytes), got %lld", p.total, static_cast<long long>(scratch_bytes));
   DeviceInfo dev;
   if (!get_device(&dev)) return DS_ERR_CUDA;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -998,12 +883,12 @@ extern "C" int ds_vae_fill_preprocess(const uint8_t* src, int H, int W, int C, i
   a.out2 = out2;
   const unsigned blocks = static_cast<unsigned>((static_cast<long long>(out_h) * out_w + 255) / 256);
   if (!mask)
-    vae_fill_kernel<3, false><<<blocks, 256, 0, st>>>(a);
+    vae_preprocess_kernel<3, false><<<blocks, 256, 0, st>>>(a);
   else if (C == 3)
-    vae_fill_kernel<3, true><<<blocks, 256, 0, st>>>(a);
+    vae_preprocess_kernel<3, true><<<blocks, 256, 0, st>>>(a);
   else
-    vae_fill_kernel<1, true><<<blocks, 256, 0, st>>>(a);
-  DS_LAUNCH_OK("vae_fill_kernel");
+    vae_preprocess_kernel<1, true><<<blocks, 256, 0, st>>>(a);
+  DS_LAUNCH_OK("vae_preprocess_kernel");
   return DS_OK;
 }
 

@@ -114,19 +114,21 @@ class VaeImageProcessor:
     """diffusers ``VaeImageProcessor(vae_scale_factor=8)`` with its default configuration (``do_resize=True``,
     ``resample="lanczos"``, ``do_normalize=True``), the preprocessing of SDXL img2img, on the GPU.
 
+    Every uint8 / PIL input of either configuration goes through one kernel, ``ds_vae_preprocess`` (``crops_coords``
+    and ``resize_mode`` below; without them the whole image is resized), bit-exact with Pillow.
+
     ``preprocess(image, height=None, width=None)`` returns fp32 NCHW [1, 3, h, w] in [-1, 1]:
       * target size: ``height`` / ``width`` if given, else the image's own, each rounded down to a multiple of 8
         (``get_default_height_width``);
       * a PIL image or uint8 RGB HWC array / tensor is converted to RGB (as the character images are), resized with
-        Pillow's LANCZOS filter when its size differs (``ds_vae_image_preprocess``, bit-exact with Pillow), then
-        ``float32(u8) / 255`` and ``2x - 1``;
+        Pillow's LANCZOS filter along each side whose size differs, then ``float32(u8) / 255`` and ``2x - 1``;
       * a float NCHW tensor of batch 1 must already be at a multiple-of-8 size (float inputs are not resized); it is
         normalised with ``2x - 1`` only if its minimum is >= 0, diffusers' rule.
 
     The one other configuration is the inpaint mask processor of diffusers' SDXL inpaint pipeline,
     ``VaeImageProcessor(vae_scale_factor=8, do_normalize=False, do_binarize=True, do_convert_grayscale=True)``.
     Its ``preprocess(mask, height, width)`` returns fp32 [1, 1, h, w] in {0, 1} and ``preprocess_latent_mask`` the
-    uint8 [1, h / 8, w / 8] latent mask (``F.interpolate`` nearest), both from ``ds_vae_mask_preprocess``:
+    uint8 [1, h / 8, w / 8] latent mask (``F.interpolate`` nearest):
       * a PIL image of mode "L" or "RGB", or a uint8 [H, W] / [H, W, 3] array / tensor (taken as that mode), is resized
         with Pillow's LANCZOS filter in its own mode, then converted to "L", then binarised at 0.5 (``L >= 128``);
       * a float tensor / array [1, 1, H, W] or [H, W] must already be at the target size and is binarised at 0.5.
@@ -138,8 +140,8 @@ class VaeImageProcessor:
         ratio ``width / height`` and kept inside the image, as (x1, y1, x2, y2);
       * ``preprocess`` / ``preprocess_nhwc4`` / ``preprocess_latent_mask`` take ``crops_coords`` and ``resize_mode``:
         "default" resizes (the crop, when given) to the target size, "fill" is ``_resize_and_fill`` (fit, centre,
-        fill the margins from the edge rows / columns); ``ds_vae_fill_preprocess``, bit-exact with Pillow.  With
-        ``crops_coords`` the target size defaults to the crop's own.  Only uint8 / PIL inputs are cropped;
+        fill the margins from the edge rows / columns).  With ``crops_coords`` the target size defaults to the
+        crop's own.  Only uint8 / PIL inputs are cropped or filled;
       * ``apply_overlay(mask, init_image, image, crop_coords)``: the result resized back over the crop and composited
         with the original where the mask is not white (``ds_vae_overlay``, bit-exact with Pillow).
     """
@@ -185,15 +187,14 @@ class VaeImageProcessor:
         return height, width
 
     @staticmethod
-    def _check_resize(resize_mode: str, crops_coords, image) -> bool:
-        """True when the call goes through the crop / fill kernel."""
+    def _check_resize(resize_mode: str, crops_coords, image) -> None:
+        """Float inputs are not resized: they take neither ``crops_coords`` nor ``resize_mode="fill"``."""
         if resize_mode not in ("default", "fill"):
             raise ValueError(f"resize_mode must be 'default' or 'fill', got {resize_mode!r}")
         if crops_coords is None and resize_mode == "default":
-            return False
+            return
         if VaeImageProcessor._is_float_tensor(image) or (isinstance(image, np.ndarray) and image.dtype != np.uint8):
             raise ValueError("crops_coords / resize_mode='fill' need a uint8 or PIL image, got a float one")
-        return True
 
     @staticmethod
     def _size(image):
@@ -203,15 +204,18 @@ class VaeImageProcessor:
         return tuple(int(v) for v in image.shape[:2])
 
     def _crop_target(self, image, crops_coords, height, width):
-        """The crop box (the whole image without ``crops_coords``) and the target size (of the crop, by default)."""
+        """The crop box (None: the whole image) and the target size: ``height`` / ``width`` if given, else the
+        crop's (the image's) own, each rounded down to a multiple of 8."""
         ih, iw = self._size(image)
-        crop = (0, 0, iw, ih) if crops_coords is None else tuple(int(v) for v in crops_coords)
-        x1, y1, x2, y2 = crop
-        if not (0 <= x1 < x2 <= iw and 0 <= y1 < y2 <= ih):
-            raise ValueError(f"crops_coords {crop} does not lie inside the {ih} x {iw} image")
+        crop = None if crops_coords is None else tuple(int(v) for v in crops_coords)
+        if crop is not None:
+            x1, y1, x2, y2 = crop
+            if not (0 <= x1 < x2 <= iw and 0 <= y1 < y2 <= ih):
+                raise ValueError(f"crops_coords {crop} does not lie inside the {ih} x {iw} image")
+            ih, iw = y2 - y1, x2 - x1
         f = self.vae_scale_factor
-        h = int(height) if height is not None else y2 - y1
-        w = int(width) if width is not None else x2 - x1
+        h = int(height) if height is not None else ih
+        w = int(width) if width is not None else iw
         h, w = h - h % f, w - w % f
         if h < f or w < f:
             raise ValueError(f"image / panel size {h} x {w} (after rounding down to a multiple of {f}) is too small")
@@ -222,15 +226,10 @@ class VaeImageProcessor:
         if self.is_mask:
             raise ValueError("VaeImageProcessor: this is the mask configuration; use preprocess / "
                              "preprocess_latent_mask")
-        if self._check_resize(resize_mode, crops_coords, image):
-            crop, h, w = self._crop_target(image, crops_coords, height, width)
-            dev = self.device or torch.device("cuda", torch.cuda.current_device())
-            u8 = _DeviceImageProcessor.to_device(image, dev)
-            return ops.vae_fill_preprocess(u8, crop, h, w, fill=resize_mode == "fill", want_out=want_nchw,
-                                           want_out2=want_nhwc4)
-        dev = self.device or torch.device("cuda", torch.cuda.current_device())
-        h, w = self.get_default_height_width(image, height, width)
+        self._check_resize(resize_mode, crops_coords, image)
         if self._is_float_tensor(image):
+            dev = self.device or torch.device("cuda", torch.cuda.current_device())
+            h, w = self.get_default_height_width(image, height, width)
             x = image if image.dim() == 4 else image.unsqueeze(0)
             if x.dim() != 4 or x.shape[0] != 1 or x.shape[1] != 3:
                 raise ValueError(f"a float image must be an NCHW tensor of batch 1 with 3 channels, got "
@@ -240,8 +239,10 @@ class VaeImageProcessor:
                                  f"8), got {tuple(x.shape[-2:])}")
             x = x.to(device=dev, dtype=torch.float32).contiguous()
             return ops.vae_image_pack(x, normalize=bool(x.min() >= 0), want_nchw=want_nchw, want_nhwc4=want_nhwc4)
+        crop, h, w = self._crop_target(image, crops_coords, height, width)
+        dev = self.device or torch.device("cuda", torch.cuda.current_device())
         u8 = _DeviceImageProcessor.to_device(image, dev)
-        return ops.vae_image_preprocess(u8, h, w, want_nchw=want_nchw, want_nhwc4=want_nhwc4)
+        return ops.vae_preprocess(u8, h, w, crop, fill=resize_mode == "fill", want_out=want_nchw, want_out2=want_nhwc4)
 
     def preprocess(self, image, height: Optional[int] = None, width: Optional[int] = None,
                    resize_mode: str = "default", crops_coords=None) -> torch.Tensor:
@@ -389,18 +390,17 @@ class VaeImageProcessor:
                              "do_binarize=True, do_convert_grayscale=True)")
         if isinstance(mask, np.ndarray):
             mask = torch.from_numpy(np.ascontiguousarray(mask))
-        if self._check_resize(resize_mode, crops_coords, mask):
-            crop, h, w = self._crop_target(mask, crops_coords, height, width)
+        self._check_resize(resize_mode, crops_coords, mask)
+        if self._is_float_tensor(mask):
             dev = self.device or torch.device("cuda", torch.cuda.current_device())
-            _, t = self.mask_host(mask, *self._size(mask))
-            return ops.vae_fill_preprocess(t.to(dev).contiguous(), crop, h, w, fill=resize_mode == "fill", mask=True,
-                                           want_out=want_mask, want_out2=want_latent)
-        dev = self.device or torch.device("cuda", torch.cuda.current_device())
-        h, w = self.get_default_height_width(mask, height, width)
-        kind, t = self.mask_host(mask, h, w)
-        if kind == "float":
+            h, w = self.get_default_height_width(mask, height, width)
+            _, t = self.mask_host(mask, h, w)
             return ops.vae_mask_pack(t.to(device=dev, dtype=torch.float32).contiguous(), want_mask, want_latent)
-        return ops.vae_mask_preprocess(t.to(dev).contiguous(), h, w, want_mask, want_latent)
+        crop, h, w = self._crop_target(mask, crops_coords, height, width)
+        dev = self.device or torch.device("cuda", torch.cuda.current_device())
+        _, t = self.mask_host(mask, *self._size(mask))
+        return ops.vae_preprocess(t.to(dev).contiguous(), h, w, crop, fill=resize_mode == "fill", mask=True,
+                                  want_out=want_mask, want_out2=want_latent)
 
     def preprocess_latent_mask(self, mask, height: Optional[int] = None, width: Optional[int] = None,
                                resize_mode: str = "default", crops_coords=None) -> torch.Tensor:

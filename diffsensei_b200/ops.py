@@ -1122,29 +1122,6 @@ def image_preprocess(src: torch.Tensor, sizes, mode: str, offsets=None, out: Opt
     return out
 
 
-def vae_image_preprocess(img: torch.Tensor, out_h: int, out_w: int, want_nchw: bool = True, want_nhwc4: bool = True):
-    """diffusers ``VaeImageProcessor.preprocess`` of one uint8 RGB HWC image ``img`` [H, W, 3] (CUDA): Pillow LANCZOS
-    resize to (out_h, out_w) (none when the size is unchanged), ``float32(u8) / 255``, ``2x - 1``.  Returns
-    (fp32 NCHW [1, 3, out_h, out_w], bf16 NHWC [1, out_h, out_w, 4] with a zero 4th channel), None where not asked."""
-    _req(img, torch.uint8, "vae_image_preprocess.img", 3)
-    H, W, c = img.shape
-    if c != 3:
-        raise DsEngineError("vae_image_preprocess: img must be uint8 RGB [H, W, 3]")
-    out_h, out_w = int(out_h), int(out_w)
-    need = int(lib.ds_vae_image_preprocess_scratch_bytes(H, W, out_h, out_w))
-    if need < 0:
-        raise DsEngineError(f"vae_image_preprocess: unsupported sizes {H} x {W} -> {out_h} x {out_w} "
-                            "(sides must be in [1, 65535])")
-    if not (want_nchw or want_nhwc4):
-        raise DsEngineError("vae_image_preprocess: nothing to compute")
-    scratch = torch.empty(max(need, 16), dtype=torch.uint8, device=img.device)
-    nchw = torch.empty(1, 3, out_h, out_w, dtype=f32, device=img.device) if want_nchw else None
-    nhwc4 = torch.empty(1, out_h, out_w, 4, dtype=bf16, device=img.device) if want_nhwc4 else None
-    check(lib.ds_vae_image_preprocess(img.data_ptr(), H, W, out_h, out_w, _ptr(nchw), _ptr(nhwc4), scratch.data_ptr(),
-                                      scratch.numel(), _stream()), "ds_vae_image_preprocess")
-    return nchw, nhwc4
-
-
 def vae_image_pack(x: torch.Tensor, normalize: bool, want_nchw: bool = True, want_nhwc4: bool = True):
     """A float image batch already at its size, fp32 NCHW [B, 3, H, W] (CUDA) -> (``2x - 1`` if ``normalize`` else x)
     as (fp32 NCHW [B, 3, H, W], bf16 NHWC [B, H, W, 4] with a zero 4th channel), None where not asked."""
@@ -1159,29 +1136,6 @@ def vae_image_pack(x: torch.Tensor, normalize: bool, want_nchw: bool = True, wan
     check(lib.ds_vae_image_pack(x.data_ptr(), _ptr(nchw), _ptr(nhwc4), B, H * W, int(bool(normalize)), _stream()),
           "ds_vae_image_pack")
     return nchw, nhwc4
-
-
-def vae_mask_preprocess(img: torch.Tensor, out_h: int, out_w: int, want_mask: bool = True, want_latent: bool = True):
-    """The inpaint mask processor of one uint8 HWC image ``img`` (CUDA), [H, W] / [H, W, 1] ("L") or [H, W, 3] ("RGB"):
-    Pillow LANCZOS resize to (out_h, out_w) in its own mode, RGB -> L, ``>= 128``.  Returns (fp32 [1, 1, out_h, out_w]
-    in {0, 1}, uint8 [1, out_h / 8, out_w / 8] latent mask), None where not asked."""
-    _req(img, torch.uint8, "vae_mask_preprocess.img")
-    if img.dim() == 2:
-        img = img.unsqueeze(-1)
-    if img.dim() != 3 or img.shape[2] not in (1, 3):
-        raise DsEngineError(f"vae_mask_preprocess: img must be uint8 [H, W], [H, W, 1] or [H, W, 3], got "
-                            f"{tuple(img.shape)}")
-    H, W, c = img.shape
-    out_h, out_w = int(out_h), int(out_w)
-    need = int(lib.ds_vae_mask_preprocess_scratch_bytes(H, W, c, out_h, out_w))
-    if need < 0:
-        raise DsEngineError(f"vae_mask_preprocess: unsupported sizes {H} x {W} -> {out_h} x {out_w} "
-                            "(sides must be in [1, 65535])")
-    mask, lat = _mask_outputs("vae_mask_preprocess", out_h, out_w, want_mask, want_latent, img.device)
-    scratch = torch.empty(max(need, 16), dtype=torch.uint8, device=img.device)
-    check(lib.ds_vae_mask_preprocess(img.data_ptr(), H, W, c, out_h, out_w, _ptr(mask), _ptr(lat), scratch.data_ptr(),
-                                     scratch.numel(), _stream()), "ds_vae_mask_preprocess")
-    return mask, lat
 
 
 def vae_mask_pack(x: torch.Tensor, want_mask: bool = True, want_latent: bool = True):
@@ -1201,15 +1155,16 @@ def _crop_box(name: str, crop, H: int, W: int):
     return x1, y1, x2, y2
 
 
-def vae_fill_preprocess(img: torch.Tensor, crop, out_h: int, out_w: int, fill: bool = True, mask: bool = False,
-                        want_out: bool = True, want_out2: bool = True):
+def vae_preprocess(img: torch.Tensor, out_h: int, out_w: int, crop=None, fill: bool = False, mask: bool = False,
+                   want_out: bool = True, want_out2: bool = True):
     """``VaeImageProcessor.preprocess(..., crops_coords=crop, resize_mode="fill" | "default")`` of one uint8 HWC
-    image (CUDA), ``crop`` = (x1, y1, x2, y2) in its pixels: Pillow's crop, then ``_resize_and_fill`` (``fill``) or a
-    LANCZOS resize to (out_h, out_w).  An image (``mask=False``, [H, W, 3]) returns (fp32 NCHW [1, 3, out_h, out_w]
-    in [-1, 1], bf16 NHWC [1, out_h, out_w, 4]) as ``vae_image_preprocess``; a mask (``mask=True``, [H, W] / [H, W, 1]
-    "L" or [H, W, 3] "RGB") returns (fp32 [1, 1, out_h, out_w] in {0, 1}, uint8 [1, out_h / 8, out_w / 8]) as
-    ``vae_mask_preprocess``; None where not asked."""
-    name = "vae_fill_preprocess"
+    image (CUDA), ``crop`` = (x1, y1, x2, y2) in its pixels (None: the whole image): Pillow's crop, then
+    ``_resize_and_fill`` (``fill``) or a LANCZOS resize to (out_h, out_w) (none along a side that keeps its size).
+    An image (``mask=False``, RGB [H, W, 3]) returns (fp32 NCHW [1, 3, out_h, out_w] of ``2 * float32(u8) / 255 - 1``,
+    bf16 NHWC [1, out_h, out_w, 4] with a zero 4th channel); a mask (``mask=True``, [H, W] / [H, W, 1] "L" or
+    [H, W, 3] "RGB", resized in its own mode) returns (fp32 [1, 1, out_h, out_w] of ``L >= 128`` after RGB -> L,
+    uint8 [1, out_h / 8, out_w / 8] latent mask); None where not asked."""
+    name = "vae_preprocess"
     _req(img, torch.uint8, f"{name}.img")
     if img.dim() == 2:
         img = img.unsqueeze(-1)
@@ -1217,9 +1172,9 @@ def vae_fill_preprocess(img: torch.Tensor, crop, out_h: int, out_w: int, fill: b
         raise DsEngineError(f"{name}: img must be uint8 [H, W, 3]" + (", [H, W] or [H, W, 1]" if mask else "") +
                             f", got {tuple(img.shape)}")
     H, W, c = img.shape
-    x1, y1, x2, y2 = _crop_box(name, crop, H, W)
+    x1, y1, x2, y2 = _crop_box(name, (0, 0, W, H) if crop is None else crop, H, W)
     out_h, out_w = int(out_h), int(out_w)
-    need = int(lib.ds_vae_fill_preprocess_scratch_bytes(H, W, c, x1, y1, x2, y2, out_h, out_w, int(bool(fill))))
+    need = int(lib.ds_vae_preprocess_scratch_bytes(H, W, c, x1, y1, x2, y2, out_h, out_w, int(bool(fill))))
     if need < 0:
         raise DsEngineError(f"{name}: unsupported sizes: crop {(x1, y1, x2, y2)} of {H} x {W} -> {out_h} x {out_w} "
                             "(sides must be in [1, 65535] and the crop must fit at least 1 x 1)")
@@ -1231,9 +1186,9 @@ def vae_fill_preprocess(img: torch.Tensor, crop, out_h: int, out_w: int, fill: b
         out = torch.empty(1, 3, out_h, out_w, dtype=f32, device=img.device) if want_out else None
         out2 = torch.empty(1, out_h, out_w, 4, dtype=bf16, device=img.device) if want_out2 else None
     scratch = torch.empty(max(need, 16), dtype=torch.uint8, device=img.device)
-    check(lib.ds_vae_fill_preprocess(img.data_ptr(), H, W, c, x1, y1, x2, y2, out_h, out_w, int(bool(fill)),
-                                     int(bool(mask)), _ptr(out), _ptr(out2), scratch.data_ptr(), scratch.numel(),
-                                     _stream()), "ds_vae_fill_preprocess")
+    check(lib.ds_vae_preprocess(img.data_ptr(), H, W, c, x1, y1, x2, y2, out_h, out_w, int(bool(fill)), int(bool(mask)),
+                                _ptr(out), _ptr(out2), scratch.data_ptr(), scratch.numel(), _stream()),
+          "ds_vae_preprocess")
     return out, out2
 
 

@@ -443,65 +443,47 @@ int64_t ds_image_preprocess_scratch_bytes(const int* sizes, int n, int mode);
 int ds_image_preprocess(const uint8_t* src, const int64_t* offsets, const int* sizes, int n, int mode, float* out,
                         void* scratch, int64_t scratch_bytes, void* stream);
 
-/* Image preprocessing of the AutoencoderKL encoder (diffusers VaeImageProcessor.preprocess, default config:
- * do_resize with Pillow LANCZOS, do_normalize), bit-exact with Pillow + numpy / torch fp32:
- *   ds_vae_image_preprocess : one uint8 RGB HWC image [H][W][3] -> Image.resize((out_w, out_h), LANCZOS) (skipped when
- *                             the size does not change), then x = float32(u8) / 255, 2x - 1.  Writes `out` fp32 NCHW
- *                             [3][out_h][out_w] and / or `out_nhwc4` bf16 NHWC [out_h][out_w][4] with a zero 4th
- *                             channel (the input of the encoder's conv_in); either may be NULL.  Same 8-bit fixed-point
- *                             resampler as ds_image_preprocess; the Lanczos tap tables are built on the host (with the
- *                             host libm's sin, as Pillow does) and copied into the scratch, so the call is not
- *                             graph-capturable.  scratch: ds_vae_image_preprocess_scratch_bytes(...) bytes, 16-byte
- *                             aligned (-1: sizes the entry point rejects; sides in [1, 65535]).
- *   ds_vae_image_pack       : a float NCHW [B][3][HW] image that is already at its size -> (normalize ? 2x - 1 : x) as
- *                             fp32 NCHW `out` (may alias x) and / or bf16 NHWC `out_nhwc4` [B][HW][4], 4th channel 0. */
-int64_t ds_vae_image_preprocess_scratch_bytes(int H, int W, int out_h, int out_w);
-int ds_vae_image_preprocess(const uint8_t* src, int H, int W, int out_h, int out_w, float* out, void* out_nhwc4,
-                            void* scratch, int64_t scratch_bytes, void* stream);
+/* diffusers VaeImageProcessor.preprocess(image, height, width, resize_mode, crops_coords) of one uint8 HWC image
+ * [H][W][C], bit-exact with Pillow + numpy / torch fp32:
+ *   ds_vae_preprocess : Image.crop((x1, y1, x2, y2)), then
+ *       fill = 0 ("default", Image.resize): LANCZOS to out_w x out_h; a pass whose size does not change is skipped.
+ *                The crop (0, 0, W, H) with fill = 0 is Image.resize((out_w, out_h), LANCZOS) of the whole image;
+ *       fill = 1 ("fill", _resize_and_fill, the SDXL inpaint pipeline's padding_mask_crop): LANCZOS to fit the
+ *                out_w x out_h frame (rw = ratio < src_ratio ? out_w : cw * out_h // ch, rh = ratio >= src_ratio ?
+ *                out_h : ch * out_w // cw, ratio = out_w / out_h, src_ratio = cw / ch), pasted centred on black; the
+ *                stripes above / below (left / right) are Pillow's default BICUBIC over a zero-height (zero-width)
+ *                source box at the resized image's first and last row (column).
+ *     then the epilogue of the processor's configuration:
+ *       mask = 0 (default config: do_resize, do_normalize; the AutoencoderKL encoder's input), C = 3 ("RGB"):
+ *                x = float32(u8) / 255, 2x - 1 -> `out` fp32 NCHW [3][out_h][out_w] and / or `out2` bf16 NHWC
+ *                [out_h][out_w][4] with a zero 4th channel (the input of the encoder's conv_in), 8-byte aligned;
+ *       mask = 1 (do_normalize=False, do_binarize=True, do_convert_grayscale=True; the inpaint mask), C = 1 ("L")
+ *                or 3 ("RGB"), resized in its own mode: for RGB Pillow's convert("L") of the resized pixels,
+ *                (19595 R + 38470 G + 7471 B + 0x8000) >> 16, then binarize float32(L) / 255 at 0.5, i.e.
+ *                L >= 128 -> `out` fp32 [out_h][out_w] in {0, 1} and / or `out2` uint8 [out_h/8][out_w/8] = the mask
+ *                at (8i, 8j) (prepare_mask_latents' F.interpolate nearest; needs sizes that are multiples of 8).
+ *     Either output may be NULL.  The crop must lie inside the H x W source and every side must be in [1, 65535].
+ *     Same 8-bit fixed-point resampler as ds_image_preprocess; the tap tables are built on the host (with the host
+ *     libm's sin, as Pillow does) and copied into the scratch, so the call is not graph-capturable.  scratch:
+ *     ds_vae_preprocess_scratch_bytes(...) bytes, 16-byte aligned (-1: arguments the entry point rejects).
+ *   ds_vae_image_pack : a float NCHW [B][3][HW] image that is already at its size -> (normalize ? 2x - 1 : x) as fp32
+ *                       NCHW `out` (may alias x) and / or bf16 NHWC `out_nhwc4` [B][HW][4], 4th channel 0.
+ *   ds_vae_mask_pack  : a float mask already at its size [H][W] -> (x >= 0.5) as `out` fp32 and / or `out_latent`
+ *                       uint8 [H/8][W/8]. */
+int64_t ds_vae_preprocess_scratch_bytes(int H, int W, int C, int x1, int y1, int x2, int y2, int out_h, int out_w,
+                                        int fill);
+int ds_vae_preprocess(const uint8_t* src, int H, int W, int C, int x1, int y1, int x2, int y2, int out_h, int out_w,
+                      int fill, int mask, float* out, void* out2, void* scratch, int64_t scratch_bytes, void* stream);
 int ds_vae_image_pack(const float* x, float* out, void* out_nhwc4, int B, int HW, int normalize, void* stream);
-
-/* Inpaint mask preprocessing (diffusers VaeImageProcessor(do_normalize=False, do_binarize=True,
- * do_convert_grayscale=True).preprocess, then prepare_mask_latents' F.interpolate(nearest) to H/8 x W/8):
- *   ds_vae_mask_preprocess : one uint8 HWC image with C = 1 ("L") or C = 3 ("RGB") channels -> Image.resize((out_w,
- *                            out_h), LANCZOS) in its own mode (same resampler and host-built tap tables as
- *                            ds_vae_image_preprocess) -> for RGB, Pillow's convert("L") of the resized pixels,
- *                            (19595 R + 38470 G + 7471 B + 0x8000) >> 16 -> binarize float32(L) / 255 at 0.5, i.e.
- *                            L >= 128.  Writes `out` fp32 [out_h][out_w] in {0, 1} and / or `out_latent` uint8
- *                            [out_h/8][out_w/8] = the mask at (8i, 8j); either may be NULL (out_latent needs sizes that
- *                            are multiples of 8).  Not graph-capturable (host tables).  scratch:
- *                            ds_vae_mask_preprocess_scratch_bytes(...) bytes, 16-byte aligned (-1: rejected sizes).
- *   ds_vae_mask_pack       : a float mask already at its size [H][W] -> (x >= 0.5) as `out` fp32 and / or
- *                            `out_latent` uint8 [H/8][W/8]. */
-int64_t ds_vae_mask_preprocess_scratch_bytes(int H, int W, int C, int out_h, int out_w);
-int ds_vae_mask_preprocess(const uint8_t* src, int H, int W, int C, int out_h, int out_w, float* out,
-                           uint8_t* out_latent, void* scratch, int64_t scratch_bytes, void* stream);
 int ds_vae_mask_pack(const float* x, int H, int W, float* out, uint8_t* out_latent, void* stream);
 
-/* diffusers VaeImageProcessor.preprocess(..., crops_coords=(x1, y1, x2, y2), resize_mode) of the SDXL inpaint
- * pipeline's padding_mask_crop, for images and masks, bit-exact with Pillow: Image.crop, then
- *   fill = 1 ("fill", _resize_and_fill): LANCZOS to fit the out_w x out_h frame (rw = ratio < src_ratio ? out_w :
- *            cw * out_h // ch, rh = ratio >= src_ratio ? out_h : ch * out_w // cw, ratio = out_w / out_h, src_ratio =
- *            cw / ch), pasted centred on black; the stripes above / below (left / right) are Pillow's default BICUBIC
- *            over a zero-height (zero-width) source box at the resized image's first and last row (column);
- *   fill = 0 ("default"): LANCZOS to out_w x out_h.
- * Then the existing epilogues: mask = 0, C = 3 -> `out` fp32 NCHW [3][out_h][out_w] of 2 (u8 / 255) - 1 and / or `out2`
- * bf16 NHWC [out_h][out_w][4] (4th channel 0), as ds_vae_image_preprocess; mask = 1, C = 1 ("L") or 3 ("RGB") -> `out`
- * fp32 [out_h][out_w] of L >= 128 and / or `out2` uint8 [out_h/8][out_w/8], as ds_vae_mask_preprocess.  The crop must
- * lie inside the H x W source; the tap tables are built on the host, so the call is not graph-capturable.  scratch:
- * ds_vae_fill_preprocess_scratch_bytes(...) bytes, 16-byte aligned (-1: arguments the entry point rejects).
- *
- * diffusers VaeImageProcessor.apply_overlay(mask, init_image, image, crop_coords) for n decoded crops:
+/* diffusers VaeImageProcessor.apply_overlay(mask, init_image, image, crop_coords) for n decoded crops:
  *   image : fp32 NCHW [n][3][h][w] in [0, 1] (the decoder's output), rounded as numpy_to_pil does
  *   init  : uint8 RGB [H][W][3], the original;  mask: uint8 "L" [H][W]
  *   out   : uint8 RGB [n][H][W][3]: each image resized with _resize_and_crop (LANCZOS to cover, centred) to the crop,
  *           pasted at (x1, y1) on black, then the original premultiplied by 255 - mask alpha-composited over it, all
  *           in Pillow's 8-bit integer arithmetic (mask 0: the original; 255: the resized crop).
  * scratch: ds_vae_overlay_scratch_bytes(...) bytes, 16-byte aligned (-1: rejected arguments). */
-int64_t ds_vae_fill_preprocess_scratch_bytes(int H, int W, int C, int x1, int y1, int x2, int y2, int out_h, int out_w,
-                                             int fill);
-int ds_vae_fill_preprocess(const uint8_t* src, int H, int W, int C, int x1, int y1, int x2, int y2, int out_h,
-                           int out_w, int fill, int mask, float* out, void* out2, void* scratch, int64_t scratch_bytes,
-                           void* stream);
 int64_t ds_vae_overlay_scratch_bytes(int n, int h, int w, int H, int W, int x1, int y1, int x2, int y2);
 int ds_vae_overlay(const float* image, int n, int h, int w, const uint8_t* init, const uint8_t* mask, int H, int W,
                    int x1, int y1, int x2, int y2, uint8_t* out, void* scratch, int64_t scratch_bytes, void* stream);

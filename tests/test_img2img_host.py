@@ -10,7 +10,8 @@ PIL = pytest.importorskip("PIL.Image")
 from oracle import img2img as o  # noqa: E402
 
 SIZES = [((1024, 1024), (2048, 2048)), ((300, 500), (224, 320)), ((203, 317), None), ((64, 96), None),
-         ((216, 312), None), ((230, 390), (224, 386)), ((120, 90), (216, 312))]
+         ((216, 312), None), ((230, 390), (224, 386)), ((120, 90), (216, 312)), ((200, 317), None),
+         ((203, 312), None)]
 
 
 def _image(h, w, mode="RGB", seed=0):

@@ -13,7 +13,7 @@ from oracle import inpaint as oi  # noqa: E402
 
 # (source (h, w), target (h, w) or None: the source's own size rounded down to a multiple of 8)
 MASK_SIZES = [((64, 96), (128, 192)), ((300, 500), (224, 320)), ((128, 192), (128, 192)), ((203, 317), None),
-              ((230, 390), (224, 386)), ((1024, 1024), (512, 768))]
+              ((230, 390), (224, 386)), ((1024, 1024), (512, 768)), ((200, 317), None), ((203, 312), None)]
 
 
 def _mask(h, w, mode="L", seed=0):

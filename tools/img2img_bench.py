@@ -7,8 +7,8 @@
   warm-up (CUDA events, medians), with the rel-L2 of the engine's ``mean`` against the bf16 library path;
 * conv_in of the encoder at 1024x1024 bs 4 (3 -> 128 channels, 4.2 M pixels): the CUDA-core ``ds_conv_in_3x3`` it runs
   on, against ``ds_im2col_latent`` + a K = 64 wgmma GEMM (the tensor-core form of the same conv), alternating;
-* the LANCZOS 1024 -> 2048 upscale + normalise: ``ds_vae_image_preprocess`` against Pillow's ``Image.resize`` + numpy on
-  the host (host wall clock, medians);
+* the LANCZOS 1024 -> 2048 upscale + normalise: ``ds_vae_preprocess`` against Pillow's ``Image.resize`` + numpy on the
+  host (host wall clock, medians);
 * ``pipe(image=..., strength=0.3 / 0.6)`` against text-to-image at 1024x1024, 30 steps, SDXL-size engines with random
   weights (token ids and PIL images in, PIL images out, synchronised host wall clock, alternating, medians);
 * the card's name, power limit and SM clocks, read with `nvidia-smi --query-gpu` (read only) before and after.

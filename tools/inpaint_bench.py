@@ -8,7 +8,7 @@
 * ``pipe(image, mask_image, strength=0.6)`` against ``pipe(image, strength=0.6)`` at 1024x1024, 30 steps, SDXL-size
   engines with random weights, alternating: the denoise per step (CUDA events around ``denoise``) and the whole call
   (synchronised host wall clock), medians;
-* the mask processor: ``ds_vae_mask_preprocess`` (RGB 768 x 768 -> 1024 x 1024 mask and latent mask) against Pillow's
+* the mask processor: ``ds_vae_preprocess`` (RGB 768 x 768 -> 1024 x 1024 mask and latent mask) against Pillow's
   ``resize(LANCZOS).convert("L")`` + numpy on the host (host wall clock, medians), and whether they agree;
 * the card's name, power limit and SM clocks, read with `nvidia-smi --query-gpu` (read only) before and after.
 

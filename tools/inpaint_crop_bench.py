@@ -2,7 +2,7 @@
 """``padding_mask_crop`` on one GPU, one JSON object:
 
 * the two image kernels at a 2048 x 1536 (W x H) panel with a ~256² mask, processed at 2048 x 1536:
-  ``ds_vae_fill_preprocess`` (image: crop + fill resize to the panel size; mask: the same, + the latent mask) and
+  ``ds_vae_preprocess`` (image: crop + fill resize to the panel size; mask: the same, + the latent mask) and
   ``ds_vae_overlay`` (the decoded crop back over the original), CUDA events over ``LAUNCHES`` launches, against the
   same Pillow chain on the host (crop + ``_resize_and_fill``, ``apply_overlay``; host wall clock), medians, and
   whether each kernel's output equals Pillow's;
@@ -48,8 +48,8 @@ def bench_kernels(dev, rounds):
     dec = torch.rand(1, 3, H, W, generator=torch.Generator().manual_seed(1)).to(dev)
     dec_pil = Image.fromarray((dec[0].permute(1, 2, 0).cpu().numpy() * 255).round().astype(np.uint8))
 
-    fill_img = lambda: ops.vae_fill_preprocess(u8, crop, H, W, want_out=False)
-    fill_mask = lambda: ops.vae_fill_preprocess(m8, crop, H, W, mask=True)
+    fill_img = lambda: ops.vae_preprocess(u8, H, W, crop, fill=True, want_out=False)
+    fill_mask = lambda: ops.vae_preprocess(m8, H, W, crop, fill=True, mask=True)
     overlay = lambda: ops.vae_overlay(dec, u8, m8, crop)
     timer = lambda fn: events_ms(fn, LAUNCHES)
     res = alternate({"fill_image_nhwc4": fill_img, "fill_mask_and_latent": fill_mask, "overlay": overlay}, rounds,
@@ -59,7 +59,7 @@ def bench_kernels(dev, rounds):
                       "pillow_overlay": lambda: pillow_overlay(mask, im, dec_pil, crop)}, rounds, host_ms)
     res.update(host)
     want = np.array(pillow_fill(im, crop, W, H))
-    got = ops.vae_fill_preprocess(u8, crop, H, W, want_out2=False)[0][0].permute(1, 2, 0).cpu().numpy()
+    got = ops.vae_preprocess(u8, H, W, crop, fill=True, want_out2=False)[0][0].permute(1, 2, 0).cpu().numpy()
     res["fill_image_equal"] = bool(np.array_equal(got, 2.0 * (want.astype(np.float32) / np.float32(255.0)) - 1.0))
     want_m = np.array(pillow_fill(mask, crop, W, H))[..., 0] >= 128
     res["fill_mask_equal"] = bool(np.array_equal(fill_mask()[0][0, 0].cpu().numpy() == 1.0, want_m))
