@@ -12,6 +12,8 @@ Public surface (mirrors the reference's, SURVEY.md §8b):
     CLIPImageProcessor, ViTImageProcessor  <- transformers' image processors as constructed by
                               pipeline_diffsensei.py:70-71 (shipped defaults; resize / normalise on the GPU)
     DiffSenseiPipeline     <- src/pipelines/pipeline_diffsensei.py  (denoise loop)
+    T2IAdapterEngine       <- diffusers T2IAdapter (full_adapter_xl), the input of UNetMangaModel.forward's
+                              down_intrablock_additional_residuals (``DiffSenseiPipeline(adapter=...)``)
     DDIMScheduler, EulerDiscreteScheduler, scheduler_from_config  <- the diffusers schedulers a checkpoint's
                               scheduler_config.json may name (SDXL-base configuration only)
     AgentEngine, LlamaEngine  <- src/models/mllm/seed_x.py ContinuousLVLM (greedy LLaMA generate of the MLLM agent)
@@ -22,9 +24,10 @@ missing, and nothing in here falls back to PyTorch compute or to the test oracle
 """
 from . import _lib  # noqa: F401  (loads libdsengine.so or raises ImportError)
 from . import ops  # noqa: F401
+from .adapter import T2IAdapterEngine  # noqa: F401
 from .agent import AgentEngine, LlamaEngine  # noqa: F401
 from .attention_processor import AttnProcessor2_0, MaskedIPAttnProcessor2_0  # noqa: F401
-from .config import (AGENT_TINY, LLAMA2_13B, RESAMPLER, RESAMPLER_TINY, SDXL_MANGA, SDXL_VAE, TINY, TINY_VAE, ResamplerConfig, UNetConfig,  # noqa: F401
+from .config import (ADAPTER_TINY, SDXL_ADAPTER, AdapterConfig, AGENT_TINY, LLAMA2_13B, RESAMPLER, RESAMPLER_TINY, SDXL_MANGA, SDXL_VAE, TINY, TINY_VAE, ResamplerConfig, UNetConfig,  # noqa: F401
                      AgentConfig, VaeConfig)
 from .encoders import (CLIP_L_TEXT, CLIP_VIT_H, MAGI_VIT_MAE, OPENCLIP_BIGG_TEXT, ClipTextEncoderEngine,  # noqa: F401
                        ClipVisionEncoderEngine, EncoderConfig, VitMaeEncoderEngine)

@@ -62,6 +62,9 @@ SIGNATURES = {
     "ds_layernorm": [_vp, _vp, _vp, _vp, _i, _i, _f, _vp],
     "ds_freeu_moments": [_vp, _vp, _i, _i, _i, _i, _vp],
     "ds_freeu_apply": [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _f, _f, _i, _i, _i, _vp],
+    "ds_adapter_relu": [_vp, _vp, _i64, _vp],
+    "ds_adapter_avgpool": [_vp, _vp, _i, _i, _i, _i, _vp],
+    "ds_adapter_add": [_vp, _vp, _i, _i, _vp, _vp, _i, _i, _i, _vp],
     "ds_dialog_embed_add": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp],
     "ds_ip_mask": [_vp, _vp, _i, _i, _d, _i, _i, _i, _vp],
     "ds_gemm_bf16": [C.POINTER(GemmArgs), _vp],

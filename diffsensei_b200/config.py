@@ -52,6 +52,49 @@ TINY = UNetConfig(block_out_channels=(64, 128, 256), transformer_layers_per_bloc
 
 
 @dataclass(frozen=True)
+class AdapterConfig:
+    """diffusers' ``T2IAdapter`` config for ``adapter_type="full_adapter_xl"`` (``FullAdapterXL``), the layout of the
+    public SDXL sketch / lineart / canny / depth adapters: ``in_channels`` 1 ("L" images) or 3 ("RGB"), four feature
+    widths, ``num_res_blocks`` AdapterResnetBlocks per AdapterBlock, PixelUnshuffle by ``downscale_factor``."""
+    in_channels: int = 3
+    channels: Tuple[int, ...] = (320, 640, 1280, 1280)
+    num_res_blocks: int = 2
+    downscale_factor: int = 16
+
+    def __post_init__(self):
+        if self.in_channels not in (1, 3):
+            raise ValueError(f"AdapterConfig: in_channels must be 1 or 3, got {self.in_channels}")
+        if len(self.channels) != 4 or self.downscale_factor != 16 or self.num_res_blocks < 1:
+            raise ValueError(f"AdapterConfig: full_adapter_xl has 4 channels, downscale_factor 16 and at least one "
+                             f"res block, got {self.channels}, {self.downscale_factor}, {self.num_res_blocks}")
+
+    @property
+    def total_downscale_factor(self) -> int:      # FullAdapterXL: one AdapterBlock downsamples
+        return self.downscale_factor * 2
+
+    @classmethod
+    def from_config(cls, config: dict) -> "AdapterConfig":
+        """From a diffusers ``T2IAdapter`` ``config.json`` (as a dict).  Only ``adapter_type="full_adapter_xl"`` is
+        supported; ``MultiAdapter`` and the SD1.5 ``full_adapter`` / ``light_adapter`` raise ``ValueError``."""
+        name = config.get("_class_name", "T2IAdapter")
+        if name != "T2IAdapter":
+            raise ValueError(f"AdapterConfig: only a single T2IAdapter is supported, got {name}")
+        kind = config.get("adapter_type", "full_adapter")
+        if kind != "full_adapter_xl":
+            raise ValueError(f"AdapterConfig: only adapter_type='full_adapter_xl' (the SDXL adapters) is supported, "
+                             f"got {kind!r}")
+        return cls(in_channels=int(config.get("in_channels", 3)),
+                   channels=tuple(int(c) for c in config.get("channels", (320, 640, 1280, 1280))),
+                   num_res_blocks=int(config.get("num_res_blocks", 2)),
+                   downscale_factor=int(config.get("downscale_factor", 16)))
+
+
+SDXL_ADAPTER = AdapterConfig()
+# the adapter of the TINY UNet (block_out_channels 64, 128, 256)
+ADAPTER_TINY = AdapterConfig(channels=(64, 128, 256, 256))
+
+
+@dataclass(frozen=True)
 class ResamplerConfig:
     """configs/model/diffsensei.yaml + scripts/demo/gradio_wo_mllm.py:174-185."""
     dim: int = 1280

@@ -22,8 +22,8 @@
 //
 // The same resampler also serves diffusers' VaeImageProcessor.preprocess (ds_vae_preprocess: an optional crop, Pillow
 // LANCZOS to any size or _resize_and_fill, then the AutoencoderKL encoder's 2 * u8 / 255 - 1 or the inpaint mask's
-// RGB -> L and threshold) and apply_overlay (ds_vae_overlay), with host-built tap tables; see the sections below
-// plan_images.
+// RGB -> L and threshold, or the T2I-Adapter's u8 / 255 written pixel-unshuffled) and apply_overlay (ds_vae_overlay),
+// with host-built tap tables; see the sections below plan_images.
 #include <cuda_bf16.h>
 
 #include <cmath>
@@ -463,6 +463,8 @@ static int vae_resample_begin(const uint8_t* src, int H, int W, long long row_px
 //         3 "RGB"): for RGB Pillow's RGB -> L conversion of the resized pixels, L = (19595 R + 38470 G + 7471 B +
 //         0x8000) >> 16, then float32(L) / 255 >= 0.5, i.e. L >= 128 -> fp32; the pixel at (8i, 8j) also writes
 //         latent pixel (i, j) (prepare_mask_latents' F.interpolate nearest to H/8 x W/8).
+//   adapter (diffusers' _preprocess_adapter_image + T2IAdapter's PixelUnshuffle(16); resized in its own mode, C = 1
+//         "L" or 3 "RGB"): float32(u8) / 255, no normalisation, rounded to bf16 and written pixel-unshuffled.
 // One launch of the horizontal pass over the crop (the source rows keep the image's pitch; skipped when the width
 // does not change), then one thread per output pixel: the vertical pass of the resized pixel (a copy when the height
 // does not change), or of the 2 resized rows (columns) a stripe pixel mixes, then the epilogue.
@@ -529,8 +531,9 @@ struct FillArgs {
   int kv, ks;
   int rw, rh, ox, oy, stripe, fill;
   int oh, ow;
-  float* out;                  // image: fp32 NCHW [3][oh][ow]; mask: fp32 [oh][ow]
-  void* out2;                  // image: bf16 NHWC4 [oh][ow][4]; mask: uint8 latent [oh/8][ow/8]
+  float* out;                  // image: fp32 NCHW [3][oh][ow]; mask: fp32 [oh][ow]; adapter: unused
+  void* out2;                  // image: bf16 NHWC4 [oh][ow][4]; mask: uint8 latent [oh/8][ow/8];
+                               // adapter: bf16 NHWC [oh/16][ow/16][C*256]
 };
 
 // one stripe pixel: clip8(2^21 + sum_t k[t] * resized[...]) over the 1-D taps of its stripe table row
@@ -553,7 +556,7 @@ __device__ __forceinline__ void fill_stripe_pixel(const FillArgs& a, const int* 
   for (int c = 0; c < C; ++c) v[c] = clip8(acc[c]);
 }
 
-template <int C, bool kMask>
+template <int C, int kEpi>
 __global__ void vae_preprocess_kernel(FillArgs a) {
   const long long hw = static_cast<long long>(a.oh) * a.ow;
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -572,12 +575,18 @@ __global__ void vae_preprocess_kernel(FillArgs a) {
     if (x < a.fill) fill_stripe_pixel<C>(a, a.coef_s0, x, y, 0, false, v);
     else if (rx >= a.rw && rx - a.rw < a.fill) fill_stripe_pixel<C>(a, a.coef_s1, rx - a.rw, y, 0, false, v);
   }
-  if constexpr (kMask) {
+  if constexpr (kEpi == DS_VAE_EPI_MASK) {
     const int l = C == 3 ? (v[0] * 19595 + v[1] * 38470 + v[2] * 7471 + 0x8000) >> 16 : v[0];
     const bool keep = l >= 128;
     if (a.out) a.out[i] = keep ? 1.0f : 0.0f;
     if (a.out2 && (y & 7) == 0 && (x & 7) == 0)
       static_cast<unsigned char*>(a.out2)[(y >> 3) * (a.ow >> 3) + (x >> 3)] = keep;
+  } else if constexpr (kEpi == DS_VAE_EPI_ADAPTER) {
+    // PixelUnshuffle(16): pixel (16 Y + i, 16 X + j) of channel c -> [Y][X][c * 256 + i * 16 + j]
+    __nv_bfloat16* o = static_cast<__nv_bfloat16*>(a.out2) +
+                       (static_cast<long long>(y >> 4) * (a.ow >> 4) + (x >> 4)) * (C * 256) + (y & 15) * 16 + (x & 15);
+#pragma unroll
+    for (int c = 0; c < C; ++c) o[c * 256] = __float2bfloat16_rn(__fdiv_rn(static_cast<float>(v[c]), 255.0f));
   } else {
     float o[3];
 #pragma unroll
@@ -828,13 +837,19 @@ extern "C" int64_t ds_vae_preprocess_scratch_bytes(int H, int W, int C, int x1, 
 }
 
 extern "C" int ds_vae_preprocess(const uint8_t* src, int H, int W, int C, int x1, int y1, int x2, int y2, int out_h,
-                                 int out_w, int fill, int mask, float* out, void* out2, void* scratch,
+                                 int out_w, int fill, int epilogue, float* out, void* out2, void* scratch,
                                  int64_t scratch_bytes, void* stream) {
   using namespace ds;
   DS_REQUIRE(src && (out || out2), "ds_vae_preprocess: bad arguments");
-  DS_REQUIRE(mask == 0 || mask == 1, "ds_vae_preprocess: mask must be 0 (image) or 1 (mask), got %d", mask);
-  DS_REQUIRE(mask ? (C == 1 || C == 3) : C == 3, "ds_vae_preprocess: C must be 3 for an image, 1 or 3 for a "
-             "mask, got %d", C);
+  DS_REQUIRE(epilogue == DS_VAE_EPI_IMAGE || epilogue == DS_VAE_EPI_MASK || epilogue == DS_VAE_EPI_ADAPTER,
+             "ds_vae_preprocess: unknown epilogue %d", epilogue);
+  const bool mask = epilogue == DS_VAE_EPI_MASK, adapter = epilogue == DS_VAE_EPI_ADAPTER;
+  DS_REQUIRE(epilogue != DS_VAE_EPI_IMAGE ? (C == 1 || C == 3) : C == 3, "ds_vae_preprocess: C must be 3 for an "
+             "image, 1 or 3 for a mask or an adapter input, got %d", C);
+  DS_REQUIRE(!adapter || (!out && out2 && out_h % 16 == 0 && out_w % 16 == 0 &&
+                          (reinterpret_cast<uintptr_t>(out2) & 1) == 0),
+             "ds_vae_preprocess: the adapter epilogue writes out2 only (2-byte aligned) and needs an output size that "
+             "is a multiple of 16, got %d x %d", out_h, out_w);
   FillPlan p;
   DS_REQUIRE(plan_fill(H, W, C, x1, y1, x2, y2, out_h, out_w, fill, &p),
              "ds_vae_preprocess: crop (%d, %d, %d, %d) of a %d x %d image -> %d x %d (fill %d) is not supported: "
@@ -843,7 +858,8 @@ extern "C" int ds_vae_preprocess(const uint8_t* src, int H, int W, int C, int x1
   DS_REQUIRE(!(mask && out2) || (out_h % 8 == 0 && out_w % 8 == 0),
              "ds_vae_preprocess: the latent mask needs an output size that is a multiple of 8, got %d x %d", out_h,
              out_w);
-  DS_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3) == 0 && (mask || (reinterpret_cast<uintptr_t>(out2) & 7) == 0),
+  DS_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3) == 0 && (epilogue != DS_VAE_EPI_IMAGE ||
+                                                             (reinterpret_cast<uintptr_t>(out2) & 7) == 0),
              "ds_vae_preprocess: out must be 4-byte and an image's out2 8-byte aligned");
   DS_REQUIRE(p.total == 0 || (scratch && scratch_bytes >= p.total && (reinterpret_cast<uintptr_t>(scratch) & 15) == 0),
              "ds_vae_preprocess: needs %lld bytes of 16-byte aligned scratch "
@@ -882,12 +898,16 @@ extern "C" int ds_vae_preprocess(const uint8_t* src, int H, int W, int C, int x1
   a.out = out;
   a.out2 = out2;
   const unsigned blocks = static_cast<unsigned>((static_cast<long long>(out_h) * out_w + 255) / 256);
-  if (!mask)
-    vae_preprocess_kernel<3, false><<<blocks, 256, 0, st>>>(a);
+  if (!mask && !adapter)
+    vae_preprocess_kernel<3, DS_VAE_EPI_IMAGE><<<blocks, 256, 0, st>>>(a);
+  else if (mask && C == 3)
+    vae_preprocess_kernel<3, DS_VAE_EPI_MASK><<<blocks, 256, 0, st>>>(a);
+  else if (mask)
+    vae_preprocess_kernel<1, DS_VAE_EPI_MASK><<<blocks, 256, 0, st>>>(a);
   else if (C == 3)
-    vae_preprocess_kernel<3, true><<<blocks, 256, 0, st>>>(a);
+    vae_preprocess_kernel<3, DS_VAE_EPI_ADAPTER><<<blocks, 256, 0, st>>>(a);
   else
-    vae_preprocess_kernel<1, true><<<blocks, 256, 0, st>>>(a);
+    vae_preprocess_kernel<1, DS_VAE_EPI_ADAPTER><<<blocks, 256, 0, st>>>(a);
   DS_LAUNCH_OK("vae_preprocess_kernel");
   return DS_OK;
 }

@@ -407,3 +407,39 @@ class VaeImageProcessor:
         """The mask at latent resolution, uint8 [1, h / 8, w / 8] in {0, 1}: ``F.interpolate(preprocess(mask),
         size=(h / 8, w / 8))`` (nearest), i.e. pixel (8i, 8j), as diffusers' ``prepare_mask_latents``."""
         return self._prepare_mask(mask, height, width, False, True, resize_mode, crops_coords)[1]
+
+
+# ---------------------------------------------------------------------------------------------- T2I-Adapter input
+def adapter_image_info(image):
+    """(channels, height, width, is_float) of a T2I-Adapter image, host-only: a PIL image in its own mode ("L": 1
+    channel, "RGB": 3; diffusers' ``_preprocess_adapter_image`` keeps the mode), a uint8 [H, W] / [H, W, C] array or
+    tensor, or a float NCHW [1, C, H, W] tensor in [0, 1] already at the panel size (diffusers passes tensors through).
+    Any other input raises ``ValueError``."""
+    if isinstance(image, torch.Tensor) and image.is_floating_point():
+        if image.dim() != 4 or image.shape[0] != 1:
+            raise ValueError(f"a float adapter_image must be an NCHW tensor of batch 1, got {tuple(image.shape)}")
+        return int(image.shape[1]), int(image.shape[2]), int(image.shape[3]), True
+    if hasattr(image, "mode") and hasattr(image, "size") and not isinstance(image, (torch.Tensor, np.ndarray)):
+        c = {"L": 1, "RGB": 3}.get(image.mode)
+        if c is None:
+            raise ValueError(f"adapter_image: PIL mode {image.mode!r} is not supported; pass image.convert('RGB') or "
+                             "image.convert('L')")
+        return c, image.size[1], image.size[0], False
+    if isinstance(image, (np.ndarray, torch.Tensor)):
+        if image.dtype not in (np.uint8, torch.uint8) or image.ndim not in (2, 3):
+            raise ValueError(f"an adapter_image array / tensor must be uint8 [H, W] or [H, W, C], or a float NCHW "
+                             f"tensor, got {image.dtype} {tuple(image.shape)}")
+        return 1 if image.ndim == 2 else int(image.shape[2]), int(image.shape[0]), int(image.shape[1]), False
+    raise ValueError(f"adapter_image must be a PIL image, a uint8 array / tensor or a float NCHW tensor, got "
+                     f"{type(image)}")
+
+
+def adapter_image_u8(image, dev: torch.device) -> torch.Tensor:
+    """A PIL / uint8 adapter image as a uint8 [H, W] or [H, W, C] tensor on ``dev``, in its own mode."""
+    if isinstance(image, torch.Tensor):
+        t = image
+    elif isinstance(image, np.ndarray):
+        t = torch.from_numpy(np.ascontiguousarray(image))
+    else:
+        t = torch.from_numpy(np.array(image, dtype=np.uint8))            # PIL: host decode only
+    return t.to(dev).contiguous()

@@ -176,6 +176,53 @@ def freeu_apply(skip: torch.Tensor, hidden: torch.Tensor, moments: torch.Tensor,
     return skip_out, hidden_out, skip_stats, hidden_stats
 
 
+# ---------------------------------------------------------------------------------------------- T2I-Adapter
+def adapter_relu(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``torch.relu`` of bf16 ``x`` (``ds_adapter_relu``); ``out`` may be ``x``."""
+    _req(x, bf16, "adapter_relu.x")
+    if out is None:
+        out = torch.empty_like(x)
+    else:
+        _req(out, bf16, "adapter_relu.out")
+        if out.numel() != x.numel():
+            raise DsEngineError("adapter_relu: out has the wrong number of elements")
+    check(lib.ds_adapter_relu(x.data_ptr(), out.data_ptr(), x.numel(), _stream()), "ds_adapter_relu")
+    return out
+
+
+def adapter_avgpool(x: torch.Tensor) -> torch.Tensor:
+    """``nn.AvgPool2d(2, 2, ceil_mode=True)`` of channels-last bf16 ``x`` [B, H, W, C] -> [B, ceil(H/2), ceil(W/2), C]
+    (``ds_adapter_avgpool``; a partial window is divided by its in-bounds pixel count)."""
+    _req(x, bf16, "adapter_avgpool.x", 4)
+    B, H, W, Cc = x.shape
+    out = torch.empty(B, (H + 1) // 2, (W + 1) // 2, Cc, dtype=bf16, device=x.device)
+    check(lib.ds_adapter_avgpool(x.data_ptr(), out.data_ptr(), B, H, W, Cc, _stream()), "ds_adapter_avgpool")
+    return out
+
+
+def adapter_add_(h: torch.Tensor, f: torch.Tensor, gate: torch.Tensor, row0: int = 0,
+                 stats: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """In place on channels-last bf16 ``h`` [B, H, W, C]: ``h[b] += gate * f[(b + row0) % F]`` for the F feature rows
+    ``f`` [F, H, W, C] (``ds_adapter_add``; ``gate`` a CUDA fp32 scalar).  Returns the GroupNorm statistics of the
+    result, fp64 [B, C, 2], accumulated into ``stats`` (which must be zero; allocated zeroed when not given)."""
+    _req(h, bf16, "adapter_add.h", 4)
+    _req(f, bf16, "adapter_add.f", 4)
+    _req(gate, f32, "adapter_add.gate")
+    B, H, W, Cc = h.shape
+    if tuple(f.shape[1:]) != (H, W, Cc) or gate.numel() != 1:
+        raise DsEngineError(f"adapter_add: features {tuple(f.shape)} do not match h {tuple(h.shape)}, or gate is not "
+                            "a scalar")
+    if stats is None:
+        stats = zero_(torch.empty(B, Cc, 2, dtype=torch.float64, device=h.device))
+    else:
+        _req(stats, torch.float64, "adapter_add.stats")
+        if stats.numel() != 2 * B * Cc:
+            raise DsEngineError("adapter_add: stats must hold B*C*2 doubles")
+    check(lib.ds_adapter_add(h.data_ptr(), f.data_ptr(), f.shape[0], int(row0), gate.data_ptr(), stats.data_ptr(), B,
+                             H * W, Cc, _stream()), "ds_adapter_add")
+    return stats
+
+
 def groupnorm_silu(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, groups: int, eps: float,
                    silu: bool = True, out: Optional[torch.Tensor] = None,
                    stats: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -1190,6 +1237,31 @@ def vae_preprocess(img: torch.Tensor, out_h: int, out_w: int, crop=None, fill: b
                                 _ptr(out), _ptr(out2), scratch.data_ptr(), scratch.numel(), _stream()),
           "ds_vae_preprocess")
     return out, out2
+
+
+def adapter_preprocess(img: torch.Tensor, out_h: int, out_w: int) -> torch.Tensor:
+    """diffusers' ``_preprocess_adapter_image`` of one uint8 image (CUDA; [H, W] / [H, W, 1] "L" or [H, W, 3] "RGB",
+    resized in its own mode) and the T2I-Adapter's ``PixelUnshuffle(16)``: a Pillow LANCZOS resize to
+    (out_h, out_w), ``float32(u8) / 255``, as bf16 NHWC [1, out_h / 16, out_w / 16, C * 256] with channel
+    ``c * 256 + i * 16 + j`` = pixel (16 y + i, 16 x + j) of channel c (``ds_vae_preprocess``' adapter epilogue)."""
+    name = "adapter_preprocess"
+    _req(img, torch.uint8, f"{name}.img")
+    if img.dim() == 2:
+        img = img.unsqueeze(-1)
+    if img.dim() != 3 or img.shape[2] not in (1, 3):
+        raise DsEngineError(f"{name}: img must be uint8 [H, W], [H, W, 1] or [H, W, 3], got {tuple(img.shape)}")
+    H, W, c = img.shape
+    out_h, out_w = int(out_h), int(out_w)
+    if out_h % 16 or out_w % 16:
+        raise DsEngineError(f"{name}: the output size must be a multiple of 16, got {out_h} x {out_w}")
+    need = int(lib.ds_vae_preprocess_scratch_bytes(H, W, c, 0, 0, W, H, out_h, out_w, 0))
+    if need < 0:
+        raise DsEngineError(f"{name}: unsupported sizes {H} x {W} -> {out_h} x {out_w} (sides in [1, 65535])")
+    out = torch.empty(1, out_h // 16, out_w // 16, c * 256, dtype=bf16, device=img.device)
+    scratch = torch.empty(max(need, 16), dtype=torch.uint8, device=img.device)
+    check(lib.ds_vae_preprocess(img.data_ptr(), H, W, c, 0, 0, W, H, out_h, out_w, 0, 2, None, out.data_ptr(),
+                                scratch.data_ptr(), scratch.numel(), _stream()), "ds_vae_preprocess")
+    return out
 
 
 def vae_overlay(image: torch.Tensor, init: torch.Tensor, mask: torch.Tensor, crop) -> torch.Tensor:

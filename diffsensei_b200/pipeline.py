@@ -41,23 +41,25 @@ import numpy as np
 import torch
 
 from . import ops
-from .image_processor import CLIPImageProcessor, VaeImageProcessor, ViTImageProcessor
+from .image_processor import (CLIPImageProcessor, VaeImageProcessor, ViTImageProcessor, adapter_image_info,
+                              adapter_image_u8)
 from .lora import AdapterRegistry, lora_targets, normalize_lora, split_components
 from .scheduler import DDIMScheduler, EulerDiscreteScheduler, get_timesteps, pag_scales, step_table, with_pag_column
-from .unet import UNetMangaEngine, resolve_pag_layers
+from .unet import AdapterResiduals, UNetMangaEngine, resolve_pag_layers
 
 bf16, f32 = torch.bfloat16, torch.float32
 
 # generate_page: what a captured stepper bakes in is the same for the whole page; everything else is per panel
 PAGE_KEYS = frozenset({"num_inference_steps", "guidance_scale", "ip_scale", "output_type", "use_graph",
-                       "max_batch_panels", "strength", "pag_scale", "pag_adaptive_scale"})
+                       "max_batch_panels", "strength", "pag_scale", "pag_adaptive_scale",
+                       "adapter_conditioning_factor"})
 PANEL_KEYS = frozenset({
     "prompt", "prompt_2", "negative_prompt", "negative_prompt_2", "height", "width", "num_samples", "generator",
     "latents", "original_size", "crops_coords_top_left", "target_size", "min_size_step", "ip_images",
     "ip_image_embeds", "clip_image_embeds", "magi_image_embeds", "clip_pixel_values", "magi_pixel_values", "ip_bbox",
     "dialog_bbox", "prompt_embeds", "negative_prompt_embeds", "pooled_prompt_embeds", "negative_pooled_prompt_embeds",
     "prompt_input_ids", "prompt_input_ids_2", "negative_prompt_input_ids", "negative_prompt_input_ids_2", "image",
-    "mask_image", "padding_mask_crop"})
+    "mask_image", "padding_mask_crop", "adapter_image", "adapter_conditioning_scale"})
 PAGE_MAX_ROWS = 8       # samples per page denoise: a UNet batch of 16 rows, as __call__(num_samples=8)
 
 
@@ -161,8 +163,11 @@ class DiffSenseiPipeline:
     def __init__(self, unet: UNetMangaEngine,
                  scheduler: Optional[Union[DDIMScheduler, EulerDiscreteScheduler]] = None, vae_scale_factor: int = 8,
                  default_sample_size: int = 128, vae=None, text_encoder=None, text_encoder_2=None, image_encoder=None,
-                 tokenizer=None, tokenizer_2=None, vae_encoder=None, pag_applied_layers="mid"):
+                 tokenizer=None, tokenizer_2=None, vae_encoder=None, pag_applied_layers="mid", adapter=None):
         self.unet = unet
+        if adapter is not None:
+            unet.check_adapter(adapter.channels)
+        self.adapter = adapter              # T2IAdapterEngine (or None: no adapter_image=)
         self.vae = vae                      # VaeDecoderEngine (or None: latents out only)
         self.vae_encoder = vae_encoder      # VaeEncoderEngine (or None: no image= / img2img)
         self.vae_image_processor = VaeImageProcessor()
@@ -409,41 +414,44 @@ class DiffSenseiPipeline:
                      add_time_ids: torch.Tensor, bbox: torch.Tensor, aspect_ratio: float,
                      dialog_bbox: Optional[torch.Tensor], num_inference_steps: int, guidance_scale: float,
                      use_graph: bool = True, chains: Optional[int] = None, start_index: int = 0,
-                     inpaint=None, pag=None) -> "DenoiseStepper":
+                     inpaint=None, pag=None, adapter=None) -> "DenoiseStepper":
         return DenoiseStepper(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                               dialog_bbox, num_inference_steps, guidance_scale, use_graph, chains, start_index,
-                              inpaint, pag)
+                              inpaint, pag, adapter)
 
     def stepper_key(self, latents, prompt_embeds, aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale,
-                    chains=None, start_index: int = 0, inpaint=None, pag=None) -> tuple:
-        """Everything a captured stepper bakes in (``stepper_for``), FreeU's values (``unet.freeu``) included."""
+                    chains=None, start_index: int = 0, inpaint=None, pag=None, adapter=None) -> tuple:
+        """Everything a captured stepper bakes in (``stepper_for``), FreeU's values (``unet.freeu``) and whether a
+        T2I-Adapter's features are added included."""
         return (tuple(latents.shape), tuple(prompt_embeds.shape), None if dialog_bbox is None else
                 (tuple(dialog_bbox.shape), dialog_bbox.dtype == bf16), float(aspect_ratio), int(num_inference_steps),
                 float(guidance_scale), self.unet.scales_key(), chains, self.unet._ip_weights_version(),
                 type(self.scheduler).__name__, tuple(sorted(self.scheduler.config.items())), int(start_index),
-                inpaint is not None, None if pag is None else tuple(sorted(pag[0])), self.unet.freeu)
+                inpaint is not None, None if pag is None else tuple(sorted(pag[0])), self.unet.freeu,
+                adapter is not None)
 
     def stepper_for(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio, dialog_bbox,
                     num_inference_steps, guidance_scale, chains=None, start_index: int = 0,
-                    inpaint=None, pag=None) -> "DenoiseStepper":
+                    inpaint=None, pag=None, adapter=None) -> "DenoiseStepper":
         """A graph-captured stepper loaded with this panel: a cached one of the same key is refilled in place
         (no re-capture), otherwise a new one is built and cached.  The start index is part of the key: the stepper
         bakes in its slice of the schedule (``set_timesteps`` would reset any scheduler state); so is whether it
         inpaints, which selects the step kernel, the perturbed-attention sites (``pag``: None when off) and FreeU's
-        values, which the graph bakes in.  The PAG scales are not: they live in the coefficient table, which
-        ``load_panel`` rewrites."""
+        values, which the graph bakes in, and whether it adds adapter features.  The PAG scales are not: they live in
+        the coefficient table, which ``load_panel`` rewrites, as it rewrites the adapter features and gates."""
         key = self.stepper_key(latents, prompt_embeds, aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale,
-                               chains, start_index, inpaint, pag)
+                               chains, start_index, inpaint, pag, adapter)
         st = self._steppers.get(key)
         if st is None:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                    dialog_bbox, num_inference_steps, guidance_scale, True, chains, start_index,
-                                   inpaint, pag)
+                                   inpaint, pag, adapter)
             while len(self._steppers) >= self.max_cached_steppers:
                 self._steppers.pop(next(iter(self._steppers)))
             self._steppers[key] = st
         else:
-            st.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox, inpaint, pag)
+            st.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox, inpaint, pag,
+                          adapter)
         return st
 
     @torch.no_grad()
@@ -451,25 +459,27 @@ class DiffSenseiPipeline:
                 add_time_ids: torch.Tensor, bbox: torch.Tensor, aspect_ratio: float,
                 dialog_bbox: Optional[torch.Tensor], num_inference_steps: int, guidance_scale: float,
                 use_graph: bool = True, on_step=None, start_index: int = 0, inpaint=None, pag_scale: float = 0.0,
-                pag_adaptive_scale: float = 0.0) -> torch.Tensor:
+                pag_adaptive_scale: float = 0.0, adapter=None) -> torch.Tensor:
         """pipeline_diffsensei.py:306-337.  ``latents`` NCHW fp32 (bs,4,h,w); conditions already concatenated
         [negative ; positive] along batch (:293-304), or [negative ; positive ; positive] with perturbed-attention
         guidance (``pag_scale > 0``: diffusers' PAGMixin; the third chunk takes the identity attention map at the
         ``pag_applied_layers`` sites and eps = u + g (t - u) + s_i (t - p), s_i per ``scheduler.pag_scales``).  ``start_index``: run steps start_index .. T-1 of the
         ``num_inference_steps`` schedule (img2img; ``on_step`` then counts from 0).  ``inpaint``: (image_latents fp32
         (bs,4,h,w), noise fp32 (bs,4,h,w), latent mask uint8 (bs,h,w)); after every step the pixels where the mask is
-        0 become the image latents noised to the next timestep (the image latents on the last step).  Returns the
-        final latents, NCHW fp32."""
+        0 become the image latents noised to the next timestep (the image latents on the last step).  ``adapter``:
+        (features, gates), T2I-Adapter features bf16 NHWC [bs, h, w, c] (one row per sample, every UNet row of the
+        sample gets it) and per loop step a gate, 1.0 (added) or 0.0 (``DenoiseStepper``).  Returns the final latents,
+        NCHW fp32."""
         self.unet.set_lora_scale(1.0)            # a direct unet(..., cross_attention_kwargs={"scale": s}) call may have left s
         pag = self._pag(pag_scale, pag_adaptive_scale)
         if use_graph:
             st = self.stepper_for(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                   dialog_bbox, num_inference_steps, guidance_scale, start_index=start_index,
-                                  inpaint=inpaint, pag=pag)
+                                  inpaint=inpaint, pag=pag, adapter=adapter)
         else:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                    dialog_bbox, num_inference_steps, guidance_scale, False, start_index=start_index,
-                                   inpaint=inpaint, pag=pag)
+                                   inpaint=inpaint, pag=pag, adapter=adapter)
         for i, t in enumerate(st.timesteps):
             st.step(i)
             if on_step is not None:
@@ -499,14 +509,17 @@ class DiffSenseiPipeline:
                  # with mask_image: inpaint a crop around the mask at the full panel resolution, then paste it back
                  padding_mask_crop: Optional[int] = None,
                  # perturbed-attention guidance (diffusers' StableDiffusionXLPAGPipeline): on when pag_scale > 0
-                 pag_scale: float = 0.0, pag_adaptive_scale: float = 0.0):
+                 pag_scale: float = 0.0, pag_adaptive_scale: float = 0.0,
+                 # T2I-Adapter (diffusers' StableDiffusionXLAdapterPipeline): follow this sketch / line art
+                 adapter_image=None, adapter_conditioning_scale: float = 1.0,
+                 adapter_conditioning_factor: float = 1.0):
         """A page of one panel: ``generate_page([panel], ...)[0]``, the panel holding this call's per-panel keywords
         (``PANEL_KEYS``) and the page the others.  Its input errors carry no panel index."""
         args = locals()
         panel = {k: args[k] for k in PANEL_KEYS}                    # as given, defaults included
         page = dict(num_inference_steps=num_inference_steps, guidance_scale=guidance_scale, output_type=output_type,
                     max_batch_panels=PAGE_MAX_ROWS, strength=strength, pag_scale=pag_scale,
-                    pag_adaptive_scale=pag_adaptive_scale)
+                    pag_adaptive_scale=pag_adaptive_scale, adapter_conditioning_factor=adapter_conditioning_factor)
         t_start = self._check_page([panel], **page)
         return self._run_page([self._panel_job(panel, output_type)], t_start, ip_scale=ip_scale, use_graph=use_graph,
                               **page)[0]
@@ -552,7 +565,7 @@ class DiffSenseiPipeline:
         return height, width
 
     def _check_page(self, panels, num_inference_steps, guidance_scale, output_type, max_batch_panels,
-                    strength, pag_scale, pag_adaptive_scale) -> int:
+                    strength, pag_scale, pag_adaptive_scale, adapter_conditioning_factor) -> int:
         """The host-only checks of the page keywords.  Returns the first step of the schedule that image panels run
         (0 on a page without them, where ``strength`` is not used)."""
         if output_type not in ("latent", "pt", "np", "pil"):
@@ -568,6 +581,9 @@ class DiffSenseiPipeline:
         for name, v in (("pag_scale", pag_scale), ("pag_adaptive_scale", pag_adaptive_scale)):
             if isinstance(v, bool) or not isinstance(v, (int, float)) or v != v or abs(v) == float("inf"):
                 raise ValueError(f"`{name}` must be a finite number, got {v!r}")
+        f = adapter_conditioning_factor
+        if isinstance(f, bool) or not isinstance(f, (int, float)) or not 0.0 <= f <= 1.0:
+            raise ValueError(f"`adapter_conditioning_factor` must be a number in [0, 1], got {f!r}")
         if any(p.get("image") is not None for p in panels):
             return get_timesteps(num_inference_steps, strength)[0]
         return 0
@@ -579,7 +595,8 @@ class DiffSenseiPipeline:
                       max_batch_panels: int = PAGE_MAX_ROWS, agent=None, tokenizer_mllm=None,
                       mllm_scale: float = 0.4, max_new_tokens: int = 500,
                       strength: float = 0.3, pag_scale: float = 0.0,
-                      pag_adaptive_scale: float = 0.0) -> List[SimpleNamespace]:
+                      pag_adaptive_scale: float = 0.0,
+                      adapter_conditioning_factor: float = 1.0) -> List[SimpleNamespace]:
         """Several panels of a page in one call.  ``panels`` holds one dict per panel with the per-panel keywords of
         ``__call__`` (``PANEL_KEYS``); the keywords here are the same for the whole page.  Returns one
         ``SimpleNamespace(images=..., latents=...)`` per panel, in panel order, each ``torch.equal`` to
@@ -616,7 +633,14 @@ class DiffSenseiPipeline:
         ``pag_applied_layers`` sites: every denoise runs [all negatives ; all positives ; all positives again], the
         third block with the identity self-attention map, and guides with ``u + g (t - u) + s_i (t - p)``;
         ``pag_adaptive_scale > 0`` lowers s_i with the timestep as diffusers does.  Departure: ``pag_scale`` defaults
-        to 0 (off), not diffusers' 3.0."""
+        to 0 (off), not diffusers' 3.0.
+
+        A panel with ``adapter_image`` (needs ``adapter=``) follows that sketch / line art as diffusers'
+        ``StableDiffusionXLAdapterPipeline`` does: the adapter runs once per panel, its four features are multiplied
+        by the panel's ``adapter_conditioning_scale`` (rounded to bf16) and added to the UNet's down path on every
+        row of the panel at loop steps ``i < int(num_inference_steps * adapter_conditioning_factor)`` (``i`` counts
+        the steps the loop runs).  A scale of 0, or a factor that gives no step, runs the panel without the adapter.
+        Adapter panels share a denoise only with adapter panels."""
         if not isinstance(panels, (list, tuple)) or len(panels) == 0:
             raise ValueError("generate_page needs a non-empty list of panel dicts")
         panels = [dict(p) for p in panels]
@@ -628,7 +652,7 @@ class DiffSenseiPipeline:
                     raise ValueError(f"panel {i}: unknown key `{k}`")
         page = dict(num_inference_steps=num_inference_steps, guidance_scale=guidance_scale, output_type=output_type,
                     max_batch_panels=max_batch_panels, strength=strength, pag_scale=pag_scale,
-                    pag_adaptive_scale=pag_adaptive_scale)
+                    pag_adaptive_scale=pag_adaptive_scale, adapter_conditioning_factor=adapter_conditioning_factor)
         t_start = self._check_page(panels, **page)
         if agent is not None:
             self._check_agent_panels(panels, tokenizer_mllm)
@@ -648,7 +672,8 @@ class DiffSenseiPipeline:
         return jobs
 
     def _run_page(self, jobs, t_start: int, *, num_inference_steps, guidance_scale, ip_scale, output_type, use_graph,
-                  max_batch_panels, strength, pag_scale, pag_adaptive_scale) -> List[SimpleNamespace]:
+                  max_batch_panels, strength, pag_scale, pag_adaptive_scale,
+                  adapter_conditioning_factor) -> List[SimpleNamespace]:
         """The GPU half of a page whose panels (``_panel_job``) and keywords (``_check_page``) passed their checks."""
         # ---- front end, once per page
         dev = self.unet.device
@@ -686,8 +711,11 @@ class DiffSenseiPipeline:
             else:
                 j.latents = j.latents * self.scheduler.init_noise_sigma    # diffusers' prepare_latents
         self._encode_page_latents([j for j in jobs if j.image is not None], t_start, strength)
+        ad_steps = int(num_inference_steps * adapter_conditioning_factor)    # diffusers' adapter step count
+        self._adapter_features(jobs, ad_steps)
         results = [None] * len(jobs)
-        kind = lambda j: () if j.image is None else ("inpaint",) if j.mask_image is not None else ("image",)
+        kind = lambda j: (() if j.image is None else ("inpaint",) if j.mask_image is not None else ("image",)) + \
+            (() if j.adapter_feats is None else ("adapter",))
         shapes = [(j.ns,) + tuple(j.latents.shape[-2:]) + kind(j) for j in jobs]
         for chunk in plan_page(shapes, max_batch_panels):
             rows = [self._panel_rows(jobs[i]) for i in chunk]
@@ -698,10 +726,16 @@ class DiffSenseiPipeline:
             inpaint = None
             if jobs[chunk[0]].inpaint is not None:
                 inpaint = tuple(torch.cat([jobs[i].inpaint[k] for i in chunk], dim=0) for k in range(3))
+            adapter = None
+            if jobs[chunk[0]].adapter_feats is not None:        # one feature row per sample of the chunk
+                feats = [torch.cat([jobs[i].adapter_feats[k].expand(jobs[i].ns, -1, -1, -1) for i in chunk])
+                         for k in range(len(jobs[chunk[0]].adapter_feats))]
+                steps = num_inference_steps - (t_start if jobs[chunk[0]].image is not None else 0)
+                adapter = (feats, [1.0 if i < ad_steps else 0.0 for i in range(steps)])   # i: the loop's step
             final = self.denoise(lat, cat("pe"), cat("te"), cat("ti"), cat("bbox"), lat.shape[-2] / lat.shape[-1],
                                  cat("db"), num_inference_steps, guidance_scale, use_graph=use_graph,
                                  start_index=t_start if jobs[chunk[0]].image is not None else 0, inpaint=inpaint,
-                                 pag_scale=pag_scale, pag_adaptive_scale=pag_adaptive_scale)
+                                 pag_scale=pag_scale, pag_adaptive_scale=pag_adaptive_scale, adapter=adapter)
             # pipeline_diffsensei.py:339-363: latents / scaling_factor -> vae.decode -> image_processor.postprocess
             image = self.vae.decode_image(final) if output_type != "latent" else final
             r0 = 0
@@ -716,6 +750,21 @@ class DiffSenseiPipeline:
                 results[i] = SimpleNamespace(images=images, latents=final[r0:r1])
                 r0 = r1
         return results
+
+    def _adapter_features(self, jobs, ad_steps: int) -> None:
+        """The T2I-Adapter features of every panel that adds them (``adapter_feats``, bf16 NHWC [1, h, w, c] each,
+        times the panel's scale and rounded to bf16, as diffusers scales them before the repeat and the CFG concat):
+        one adapter call per panel.  A panel with scale 0, or a page whose factor gives no adapter step
+        (``ad_steps == 0``), keeps ``adapter_feats = None`` and runs the plain path."""
+        dev = self.unet.device
+        for j in jobs:
+            if j.adapter_image is None or j.adapter_scale == 0.0 or ad_steps == 0:
+                continue
+            if j.adapter_float:
+                x = self.adapter.unshuffle(j.adapter_image)
+            else:
+                x = ops.adapter_preprocess(adapter_image_u8(j.adapter_image, dev), j.height, j.width)
+            j.adapter_feats = [f * j.adapter_scale for f in self.adapter.forward_nhwc(x)]
 
     def _encode_page_latents(self, jobs, t_start: int, strength: float) -> None:
         """The img2img and inpaint panels' initial latents: every image processed to its panel size, same-size images
@@ -742,6 +791,21 @@ class DiffSenseiPipeline:
         if g("mask_image") is not None and g("image") is None:
             raise ValueError("`mask_image` needs `image`: inpainting redraws the masked part of that image")
         crop = mask_l = None
+        ad_image = g("adapter_image")
+        ad_scale = g("adapter_conditioning_scale", 1.0)
+        if ad_image is not None:
+            if self.adapter is None:
+                raise ValueError("adapter_image= needs a T2I-Adapter: DiffSenseiPipeline(..., "
+                                 "adapter=T2IAdapterEngine)")
+            if g("padding_mask_crop") is not None:
+                raise ValueError("`padding_mask_crop` and `adapter_image` can not be input together (the adapter "
+                                 "image is not cropped)")
+            if isinstance(ad_scale, bool) or not isinstance(ad_scale, (int, float)) or ad_scale != ad_scale or \
+                    abs(ad_scale) == float("inf"):
+                raise ValueError(f"`adapter_conditioning_scale` must be a finite number, got {ad_scale!r}")
+            ad_c, ad_h, ad_w, ad_float = adapter_image_info(ad_image)
+            if ad_c != self.adapter.cfg.in_channels:
+                raise ValueError(self.adapter._mode_message(ad_c))
         if g("padding_mask_crop") is not None:
             mask_l = self._check_crop(g("padding_mask_crop"), g("image"), g("mask_image"), g("latents"), output_type)
         if g("image") is not None:
@@ -752,6 +816,16 @@ class DiffSenseiPipeline:
             crop = VaeImageProcessor.get_crop_region(mask_l, width, height, int(g("padding_mask_crop")))
             p = self._crop_panel(p, crop, mask_l.shape, (height, width))
             g = lambda k, d=None: p.get(k, d)
+        if ad_image is not None:
+            f = self.adapter.downscale_factor           # diffusers' _default_height_width: the image's, rounded down
+            height = height if height is not None else ad_h - ad_h % f
+            width = width if width is not None else ad_w - ad_w % f
+            if height % f or width % f or height < f or width < f:
+                raise ValueError(f"with adapter_image the panel size must be a positive multiple of {f}, got "
+                                 f"{height} x {width}")
+            if ad_float and (ad_h, ad_w) != (height, width):
+                raise ValueError(f"a float adapter_image tensor is not resized: it must already be {height} x {width}, "
+                                 f"got {ad_h} x {ad_w}")
         height = height or self.default_sample_size * self.vae_scale_factor
         width = width or self.default_sample_size * self.vae_scale_factor
         ip_images, ip_bbox = list(g("ip_images", ())), list(g("ip_bbox", ()))
@@ -808,6 +882,8 @@ class DiffSenseiPipeline:
         return SimpleNamespace(
             ns=int(g("num_samples", 1)), height=height, width=width, generator=g("generator"), latents=g("latents"),
             ids=ids, image=g("image"), mask_image=g("mask_image"), inpaint=None, crop=crop, mask_l=mask_l,
+            adapter_image=ad_image, adapter_scale=float(ad_scale), adapter_float=ad_image is not None and ad_float,
+            adapter_feats=None,
             pe=g("prompt_embeds"), npe=g("negative_prompt_embeds"), pp=g("pooled_prompt_embeds"),
             npp=g("negative_pooled_prompt_embeds"), ip_images=ip_images, clip_pv=clip_pv, magi_pv=magi_pv,
             clip=g("clip_image_embeds"), magi=g("magi_image_embeds"), ip_image_embeds=ip_image_embeds,
@@ -1009,12 +1085,15 @@ class DenoiseStepper:
     With ``pag`` = (sites, pag_scale, pag_adaptive_scale) the batch is [uncond ; text ; perturbed] (3 bs rows), the
     UNet perturbs the self-attention ``sites`` of the third chunk, and the table has each step's PAG scale appended
     (``with_pag_column``).
+    With ``adapter`` = (features, gates) the UNet adds T2I-Adapter features (bf16 NHWC [bs, h, w, c] each; UNet row b
+    reads row b % bs) at its down-path sites, times the step's gate (1.0 or 0.0), which ``step`` copies into a device
+    scalar like the time embedding's row.
     """
 
     @torch.no_grad()
     def __init__(self, pipe: DiffSenseiPipeline, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox,
                  aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale, use_graph=True, chains=None,
-                 start_index: int = 0, inpaint=None, pag=None):
+                 start_index: int = 0, inpaint=None, pag=None, adapter=None):
         unet, dev = pipe.unet, pipe.unet.device
         self.unet, self.dev, self.guidance = unet, dev, float(guidance_scale)
         self.scheduler = pipe.scheduler
@@ -1038,8 +1117,12 @@ class DenoiseStepper:
         self.inp_z = self.inp_n = self.inp_m = None
         self.round_bf16 = True
         self.graph = None
-        self.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox, inpaint, pag)
+        self.has_adapter = adapter is not None
+        self.ad_feats = self.ad_gates = None
+        self.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox, inpaint, pag,
+                        adapter)
         self.temb_cur = self.temb_table[0].clone()
+        self.ad_gate_cur = None if adapter is None else self.ad_gates[0].clone()
         self.coef_cur = self.coef_table[0].clone()
         self._host_in = None
         # Independent batch rows (the CFG halves, the panels) CAN run as `chains` concurrent kernel chains on separate
@@ -1076,11 +1159,11 @@ class DenoiseStepper:
 
     @torch.no_grad()
     def load_panel(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox,
-                   inpaint=None, pag=None) -> None:
+                   inpaint=None, pag=None, adapter=None) -> None:
         """Everything that is per panel and timestep-invariant, written INTO the buffers the captured graph reads:
         K|V of the text / IP tokens for all cross-attention layers, the time-embedding row-bias table for all T
-        steps, the bbox tables, the initial latents, the inpaint state, and the PAG scale of every step.  First call
-        allocates; later calls (same shapes) refill."""
+        steps, the bbox tables, the initial latents, the inpaint state, the PAG scale of every step, and the adapter
+        features and per-step gates.  First call allocates; later calls (same shapes) refill."""
         unet, dev = self.unet, self.dev
         bs = latents.shape[0]
         k = self.n_chunks
@@ -1094,6 +1177,22 @@ class DenoiseStepper:
                              "conditions: prompt_embeds.shape[0] == 3 * num_samples")
         if (inpaint is not None) != self.inpaint:
             raise ValueError("load_panel: inpaint state presence differs from the stepper's")
+        if (adapter is not None) != self.has_adapter:
+            raise ValueError("load_panel: adapter presence differs from the stepper's")
+        if adapter is not None:
+            feats, gates = adapter
+            if len(gates) != len(self.timesteps) or any(f.shape[0] != bs for f in feats):
+                raise ValueError("adapter: one gate per loop step and one feature row per sample are needed")
+            gates = torch.tensor([float(v) for v in gates], dtype=f32, device=dev)
+            feats = [f.to(device=dev, dtype=bf16).contiguous() for f in feats]
+            if self.ad_feats is None:
+                self.ad_feats, self.ad_gates = feats, gates
+            else:
+                if [tuple(f.shape) for f in feats] != [tuple(f.shape) for f in self.ad_feats]:
+                    raise ValueError("load_panel: adapter feature shapes differ from the captured panel")
+                for d, f in zip(self.ad_feats, feats):
+                    d.copy_(f)
+                self.ad_gates.copy_(gates)
         if pag is not None:                                             # s_i of every step as the table's last column
             self.coef_table = with_pag_column(self.base_coef_table, pag_scales(self.timesteps, pag[1], pag[2]))
         if inpaint is not None:
@@ -1140,10 +1239,17 @@ class DenoiseStepper:
             return {}
         return dict(pag_sites=self.pag_sites, pag_row0=min(max(self._pag_row0 - s, 0), e - s))
 
+    def _adapter_args(self, s: int) -> dict:
+        """forward_nhwc's adapter keyword for batch rows from ``s`` on (feature row = global row % bs)."""
+        if not self.has_adapter:
+            return {}
+        return dict(adapter=AdapterResiduals(self.ad_feats, self.ad_gate_cur, s))
+
     def _launch(self):
         if len(self._parts) == 1:
             eps = self.unet.forward_nhwc(self.model_in, self.temb_cur, self.cond, self.db, self.round_bf16,
-                                         **self._pag_args(0, self.model_in.shape[0]))                     # :322-329
+                                         **self._pag_args(0, self.model_in.shape[0]),
+                                         **self._adapter_args(0))                                          # :322-329
         else:
             main = torch.cuda.current_stream(self.dev)
             eps = self._eps
@@ -1159,7 +1265,7 @@ class DenoiseStepper:
                     with torch.cuda.stream(st):
                         self.unet.forward_nhwc(self.model_in[s:e], self.temb_cur[s:e], self._cond_parts[k],
                                                None if self.db is None else self.db[s:e], self.round_bf16,
-                                               out=eps[s:e], **self._pag_args(s, e))
+                                               out=eps[s:e], **self._pag_args(s, e), **self._adapter_args(s))
                 for st in self._side:
                     main.wait_stream(st)                       # join before the CFG blend needs both halves
             finally:
@@ -1172,6 +1278,8 @@ class DenoiseStepper:
     def step(self, i: int) -> None:
         self.temb_cur.copy_(self.temb_table[i])
         self.coef_cur.copy_(self.coef_table[i])
+        if self.has_adapter:
+            self.ad_gate_cur.copy_(self.ad_gates[i])
         if self.graph is not None:
             self.graph.replay()
         else:

@@ -91,6 +91,17 @@ class Conditions:
                           bbox=self.bbox[s:e], aspect_ratio=self.aspect_ratio, batch=e - s)
 
 
+@dataclass
+class AdapterResiduals:
+    """T2I-Adapter features as ``forward_nhwc`` adds them (diffusers' ``down_intrablock_additional_residuals``):
+    bf16 NHWC [F, h, w, c] each, in the order the down path consumes them; batch row b of the forward gets feature row
+    (row0 + b) % F, times the device fp32 scalar ``gate`` (1 adds, 0 leaves the stream as it is: one captured graph
+    serves the steps with and without the features)."""
+    features: List[torch.Tensor]
+    gate: torch.Tensor
+    row0: int = 0
+
+
 class _Resnet:
     __slots__ = ("cin", "cout", "n1", "n2", "w1", "b1", "w2", "b2", "wsc", "bsc", "temb_off")
 
@@ -191,6 +202,14 @@ class UNetMangaEngine:
                 c_skip = rch[i] if j < nres - 1 else rch[min(i + 1, len(ch) - 1)]
                 n += -(-(9 * c_skip + 2 * c_hidden) // (2 * cmax))
         return n
+
+    def check_adapter(self, channels) -> None:
+        """A T2I-Adapter's four feature widths must be the down path's sites: the last output of every level
+        (``block_out_channels``) and the mid block (the last width again)."""
+        want = tuple(self.cfg.block_out_channels) + (self.cfg.block_out_channels[-1],)
+        if tuple(channels) != want:
+            raise ValueError(f"the adapter's channels {tuple(channels)} do not fit this UNet: its "
+                             f"down_intrablock_additional_residuals sites have {want}")
 
     def _ip_weights_version(self) -> int:
         """Moves when a checkpoint is loaded INTO the processors (their Parameters alias the packed IP weights)."""
@@ -515,12 +534,17 @@ class UNetMangaEngine:
     def forward_nhwc(self, x: torch.Tensor, temb: torch.Tensor, cond: Conditions,
                      dialog_bbox: Optional[torch.Tensor] = None, round_bf16: bool = True,
                      out: Optional[torch.Tensor] = None, pag_sites: frozenset = frozenset(),
-                     pag_row0: Optional[int] = None) -> torch.Tensor:
+                     pag_row0: Optional[int] = None, adapter: Optional[AdapterResiduals] = None) -> torch.Tensor:
         """x: bf16 [B,H,W,4]; temb: fp32 [B, sum(Cout)] from ``time_rowbias``; returns eps bf16 [B,H,W,4]
         (written into ``out`` when given — a contiguous batch slice of a larger buffer is fine).
         Perturbed-attention guidance: at the self-attention sites named in ``pag_sites`` (``resolve_pag_layers``),
         batch rows ``pag_row0`` .. B-1 take the identity attention map, ``to_out(to_v(x))``.
-        FreeU (``enable_freeu``) acts on every row."""
+        FreeU (``enable_freeu``) acts on every row.
+        ``adapter``: T2I-Adapter features added in place where diffusers' UNet2DConditionModel adds
+        ``down_intrablock_additional_residuals`` (unet.py:243-298): after a down block without attention (its
+        downsampler included), after the last resnet / attention pair of a down block with attention (before its
+        skip is pushed and before its downsampler), and after the mid block if a feature of its shape remains; the
+        stream and its skip both see the sum.  Without it the launches are exactly those of the plain UNet."""
         cfg = self.cfg
         tr = lambda p, h, st, **kw: self._transformer(p, h, st, cond, pool, pag_sites=pag_sites, pag_row0=pag_row0,
                                                       **kw)
@@ -529,7 +553,11 @@ class UNetMangaEngine:
         B, H, W, _ = x.shape
         need_size = (H % (2 ** (nlev - 1)) != 0) or (W % (2 ** (nlev - 1)) != 0)       # unet.py:152-162
         freeu = self.freeu
-        pool = self._Pool(B, max(ch), x.device, 64 + (self._freeu_pool_slots() if freeu else 0))
+        feats = [] if adapter is None else list(adapter.features)
+        pool = self._Pool(B, max(ch), x.device, 64 + (self._freeu_pool_slots() if freeu else 0) + len(feats))
+
+        def adapter_site(h):       # the producer's statistics are stale after the add: the kernel emits new ones
+            return h, ops.adapter_add_(h, feats.pop(0), adapter.gate, adapter.row0, stats=pool.take(h.shape[-1]))
         # conv_in on the tensor cores: im2col of the 4-channel latent (K = 36 -> 64) + one GEMM whose epilogue also
         # takes the GroupNorm statistics — unless the dialog embedding is added afterwards (it changes them)
         st = None
@@ -548,15 +576,22 @@ class UNetMangaEngine:
                 h, st = self._resnet(f"down_blocks.{i}.resnets.{j}", h, st, temb, pool)
                 if depth[i] > 0:
                     h, st = tr(f"down_blocks.{i}.attentions.{j}", h, st)
+                    if j == cfg.layers_per_block - 1 and feats:
+                        h, st = adapter_site(h)
                 skips.append((h, st))
             if i < nlev - 1:
                 w, b = self.down_convs[i]
                 st = pool.take(ch[i])
                 h = ops.conv3x3(h, w, b, stride=2, chan_stats=st)
                 skips.append((h, st))
+            if depth[i] == 0 and feats:             # in place: the block's last skip is h itself
+                h, st = adapter_site(h)
+                skips[-1] = (h, st)
         h, st = self._resnet("mid_block.resnets.0", h, st, temb, pool)
         h, st = tr("mid_block.attentions.0", h, st)
         h, st = self._resnet("mid_block.resnets.1", h, st, temb, pool)
+        if feats and tuple(feats[0].shape[1:]) == tuple(h.shape[1:]):
+            h, st = adapter_site(h)
         rdepth = list(reversed(depth))
         rch = list(reversed(ch))
         for i in range(nlev):
@@ -616,7 +651,6 @@ class UNetMangaEngine:
         for name, v in (("timestep_cond", timestep_cond), ("attention_mask", attention_mask),
                         ("down_block_additional_residuals", down_block_additional_residuals),
                         ("mid_block_additional_residual", mid_block_additional_residual),
-                        ("down_intrablock_additional_residuals", down_intrablock_additional_residuals),
                         ("encoder_attention_mask", encoder_attention_mask)):
             if v is not None:
                 raise NotImplementedError(f"UNetMangaEngine: `{name}` is not on the DiffSensei sampling path")
@@ -646,7 +680,18 @@ class UNetMangaEngine:
             db = dialog_bbox.to(device=self.device, dtype=f32).contiguous()
         else:
             round_bf16 = True
-        eps = self.forward_nhwc(ops.nchw_to_nhwc(sample), temb, cond, db, round_bf16)
+        adapter = None
+        if down_intrablock_additional_residuals is not None:
+            # T2I-Adapter features of the whole batch, NCHW (unet.py:243-298); the caller's list is left as it is
+            feats = []
+            for r in down_intrablock_additional_residuals:
+                r = r.to(self.device).contiguous()
+                if r.dim() != 4 or r.shape[0] != B:
+                    raise ValueError(f"down_intrablock_additional_residuals: expected NCHW tensors of batch {B}, got "
+                                     f"{tuple(r.shape)}")
+                feats.append(ops.nchw_to_nhwc(r if r.dtype in (f32, bf16) else r.float()))
+            adapter = AdapterResiduals(feats, torch.ones((), dtype=f32, device=self.device))
+        eps = self.forward_nhwc(ops.nchw_to_nhwc(sample), temb, cond, db, round_bf16, adapter=adapter)
         out = ops.nhwc_to_nchw(eps, f32 if out_dtype != bf16 else bf16)
         if out.dtype != out_dtype:
             out = out.to(out_dtype)

@@ -87,6 +87,23 @@ int ds_freeu_apply(const void* skip, const double* moments, void* skip_out, doub
                    const void* hidden, void* hidden_out, double* hidden_stats, int C_hidden, float s, float b, int B,
                    int H, int W, void* stream);
 
+/* SDXL T2I-Adapter (diffusers' T2IAdapter, adapter_type "full_adapter_xl"; the reference's seam is
+ * UNetMangaModel.forward's down_intrablock_additional_residuals, src/models/unet.py:125-127,225-263,292-298).  NHWC bf16,
+ * 16-byte aligned pointers, C a multiple of 8 (adapter_kernels.cu).  The adapter's input is ds_vae_preprocess with
+ * epilogue DS_VAE_EPI_ADAPTER; its 3x3 convs are ds_conv3x3_nhwc, its 1x1 convs (+ residual) ds_gemm_bf16.
+ *   ds_adapter_relu    : y = relu(x) over n elements (n % 8 == 0); y may be x.  AdapterResnetBlock.act.
+ *   ds_adapter_avgpool : y [B][ceil(H/2)][ceil(W/2)][C] = nn.AvgPool2d(2, 2, ceil_mode=True)(x [B][H][W][C]): the
+ *                        window's in-bounds pixels summed row by row in fp32, divided by their count, one rounding.
+ *   ds_adapter_add     : the per-step residual add, in place: h[b] = bf16(h[b] + gate * f[(b + row0) % F]) for
+ *                        h [B][HW][C] and the F stored feature rows f [F][HW][C] (gate 1: torch's bf16 `h + f`; gate
+ *                        0: h unchanged).  `gate` is a DEVICE fp32 scalar, so one captured graph serves steps with and
+ *                        without the add.  It also ACCUMULATES the GroupNorm statistics of the result (ds_channel_stats'
+ *                        layout fp64 [B][C][2], caller zeroes) — the same bits ds_channel_stats gives.  C <= 4096. */
+int ds_adapter_relu(const void* x, void* y, int64_t n, void* stream);
+int ds_adapter_avgpool(const void* x, void* y, int B, int H, int W, int C, void* stream);
+int ds_adapter_add(void* h, const void* f, int F, int row0, const float* gate, double* stats, int B, int HW, int C,
+                   void* stream);
+
 /* LayerNorm over the last dim, bf16 in/out, fp32 affine.     [HBM-bound]
  * Replaces BasicTransformerBlock.norm1/2/3 (eps 1e-5) and Resampler LayerNorms
  * (src/models/resampler.py:14,40-41,104). rows x C, C % 8 == 0, C <= 5120. */
@@ -454,15 +471,21 @@ int ds_image_preprocess(const uint8_t* src, const int64_t* offsets, const int* s
  *                stripes above / below (left / right) are Pillow's default BICUBIC over a zero-height (zero-width)
  *                source box at the resized image's first and last row (column).
  *     then the epilogue of the processor's configuration:
- *       mask = 0 (default config: do_resize, do_normalize; the AutoencoderKL encoder's input), C = 3 ("RGB"):
+ *       epilogue = 0 (DS_VAE_EPI_IMAGE, default config: do_resize, do_normalize; the AutoencoderKL encoder's
+ *                input), C = 3 ("RGB"):
  *                x = float32(u8) / 255, 2x - 1 -> `out` fp32 NCHW [3][out_h][out_w] and / or `out2` bf16 NHWC
  *                [out_h][out_w][4] with a zero 4th channel (the input of the encoder's conv_in), 8-byte aligned;
- *       mask = 1 (do_normalize=False, do_binarize=True, do_convert_grayscale=True; the inpaint mask), C = 1 ("L")
- *                or 3 ("RGB"), resized in its own mode: for RGB Pillow's convert("L") of the resized pixels,
+ *       epilogue = 1 (DS_VAE_EPI_MASK, do_normalize=False, do_binarize=True, do_convert_grayscale=True; the
+ *                inpaint mask), C = 1 ("L") or 3 ("RGB"), resized in its own mode: for RGB Pillow's convert("L") of the resized pixels,
  *                (19595 R + 38470 G + 7471 B + 0x8000) >> 16, then binarize float32(L) / 255 at 0.5, i.e.
  *                L >= 128 -> `out` fp32 [out_h][out_w] in {0, 1} and / or `out2` uint8 [out_h/8][out_w/8] = the mask
  *                at (8i, 8j) (prepare_mask_latents' F.interpolate nearest; needs sizes that are multiples of 8).
- *     Either output may be NULL.  The crop must lie inside the H x W source and every side must be in [1, 65535].
+ *       epilogue = 2 (DS_VAE_EPI_ADAPTER: diffusers' _preprocess_adapter_image, then the T2I-Adapter's
+ *                PixelUnshuffle(16)), C = 1 ("L") or 3 ("RGB"), resized in its own mode: float32(u8) / 255 (no normalisation) rounded to
+ *                bf16 -> `out2` bf16 NHWC [out_h/16][out_w/16][C*256], channel c * 256 + i * 16 + j holding pixel
+ *                (16 Y + i, 16 X + j) of channel c; `out` must be NULL and the sizes multiples of 16.
+ *     Either output may be NULL (the image and mask epilogues).  The crop must lie inside the H x W source and
+ *     every side must be in [1, 65535].
  *     Same 8-bit fixed-point resampler as ds_image_preprocess; the tap tables are built on the host (with the host
  *     libm's sin, as Pillow does) and copied into the scratch, so the call is not graph-capturable.  scratch:
  *     ds_vae_preprocess_scratch_bytes(...) bytes, 16-byte aligned (-1: arguments the entry point rejects).
@@ -470,10 +493,14 @@ int ds_image_preprocess(const uint8_t* src, const int64_t* offsets, const int* s
  *                       NCHW `out` (may alias x) and / or bf16 NHWC `out_nhwc4` [B][HW][4], 4th channel 0.
  *   ds_vae_mask_pack  : a float mask already at its size [H][W] -> (x >= 0.5) as `out` fp32 and / or `out_latent`
  *                       uint8 [H/8][W/8]. */
+#define DS_VAE_EPI_IMAGE 0
+#define DS_VAE_EPI_MASK 1
+#define DS_VAE_EPI_ADAPTER 2
 int64_t ds_vae_preprocess_scratch_bytes(int H, int W, int C, int x1, int y1, int x2, int y2, int out_h, int out_w,
                                         int fill);
 int ds_vae_preprocess(const uint8_t* src, int H, int W, int C, int x1, int y1, int x2, int y2, int out_h, int out_w,
-                      int fill, int mask, float* out, void* out2, void* scratch, int64_t scratch_bytes, void* stream);
+                      int fill, int epilogue, float* out, void* out2, void* scratch, int64_t scratch_bytes,
+                      void* stream);
 int ds_vae_image_pack(const float* x, float* out, void* out_nhwc4, int B, int HW, int normalize, void* stream);
 int ds_vae_mask_pack(const float* x, int H, int W, float* out, uint8_t* out_latent, void* stream);
 
