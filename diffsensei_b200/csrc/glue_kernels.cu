@@ -1,7 +1,9 @@
 // glue_kernels.cu — small HBM-bound kernels around the tensor-core ops: conv_in (Cin = 4), layout changes at
 // the diffusers-facing boundary, nearest upsample, channel concat, SiLU, sinusoidal timestep features, and the
-// fused CFG + DDIM and CFG + Euler updates (plain and
-// inpaint).  All vectorised to 16-byte accesses where the shape allows.
+// fused CFG + DDIM and CFG + Euler updates (plain and inpaint, with or without guidance_rescale) and the per-sample
+// factors of that rescale.  All vectorised to 16-byte accesses where the shape allows.
+#include <cmath>
+
 #include "ds_common.cuh"
 #include "ds_host.h"
 
@@ -230,6 +232,30 @@ __device__ __forceinline__ void inpaint_blend(float xv[4], long long i, const fl
   xv[3] = __fadd_rn(__fmul_rn(c0, z.w), __fmul_rn(c1, n.w));
 }
 
+// The guided eps of one pixel, each operation rounded on its own: u + g (t - u), then + s (t - p) with 3 chunks (the
+// perturbed chunk read here).  The step kernel and the rescale factors both use it, so the values the factors reduce
+// are bit for bit the values the step rescales.
+template <int kChunks>
+__device__ __forceinline__ void guided_eps_rn(const uint2* __restrict__ noise_pred, long long i, long long n_pix,
+                                              const float u[4], const float tt[4], float guidance, float s,
+                                              float eps[4]) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) eps[j] = __fadd_rn(u[j], __fmul_rn(guidance, __fsub_rn(tt[j], u[j])));
+  if constexpr (kChunks == 3) {
+    const uint2 ep = __ldg(noise_pred + 2 * n_pix + i);  // perturbed chunk
+    const float pp[4] = {bf16_lo(ep.x), bf16_hi(ep.x), bf16_lo(ep.y), bf16_hi(ep.y)};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) eps[j] = __fadd_rn(eps[j], __fmul_rn(s, __fsub_rn(tt[j], pp[j])));
+  }
+}
+
+// diffusers' rescale_noise_cfg on one pixel of the guided eps, in its eager fp32 order:
+// phi * (eps * r) + (1 - phi) * eps, each product and the sum rounded on its own; one_m_phi = fp32(1 - phi).
+__device__ __forceinline__ void rescale_eps(float eps[4], float r, float phi, float one_m_phi) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) eps[j] = __fadd_rn(__fmul_rn(phi, __fmul_rn(eps[j], r)), __fmul_rn(one_m_phi, eps[j]));
+}
+
 // the fp32 master and all kChunks chunks of the next UNet input: bf16(xv / in_div), or bf16(xv) when in_div is NULL
 template <int kChunks>
 __device__ __forceinline__ void store_step(float4* __restrict__ latents, uint2* __restrict__ model_in, long long i,
@@ -248,12 +274,14 @@ __device__ __forceinline__ void store_step(float4* __restrict__ latents, uint2* 
 }
 
 // noise_pred holds kChunks chunks of n_pix pixels, [uncond ; text (; perturbed)]; coef is the step's row
-// {update (2 DDIM, 3 Euler) | c0, c1 if kInpaint | s if kChunks == 3}.
-template <bool kEuler, int kChunks, bool kInpaint>
+// {update (2 DDIM, 3 Euler) | c0, c1 if kInpaint | s if kChunks == 3}.  kRescale: the guided eps of sample i / HW is
+// rescaled with the factor rescale[i / HW] (cfg_rescale_factors_kernel) before the update.
+template <bool kEuler, int kChunks, bool kInpaint, bool kRescale>
 __global__ void cfg_step_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
                                 uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
                                 long long n_pix /* bs*HW */, const float4* __restrict__ image_latents,
-                                const float4* __restrict__ noise, const unsigned char* __restrict__ mask) {
+                                const float4* __restrict__ noise, const unsigned char* __restrict__ mask,
+                                const float* __restrict__ rescale, float phi, float one_m_phi, int HW) {
   static_assert(kChunks == 2 || kChunks == 3, "CFG (2 chunks) or CFG + PAG (3 chunks)");
   constexpr int kC0 = kEuler ? 3 : 2;                 // {c0, c1} follow the update's coefficients
   constexpr int kS = kC0 + (kInpaint ? 2 : 0);         // then the PAG scale
@@ -263,20 +291,13 @@ __global__ void cfg_step_kernel(const uint2* __restrict__ noise_pred, float4* __
   load_cfg_halves(noise_pred, i, n_pix, u, tt);
   const float4 x = latents[i];
   float xv[4] = {x.x, x.y, x.z, x.w};
-  if constexpr (!kEuler && kChunks == 2) {
+  if constexpr (!kEuler && kChunks == 2 && !kRescale) {
     // the CFG-only DDIM step has always let the compiler contract into FMAs; rounding it op by op changes its bits
     cfg_ddim_pixel(u, tt, xv, coef, guidance);
   } else {
     float eps[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) eps[j] = __fadd_rn(u[j], __fmul_rn(guidance, __fsub_rn(tt[j], u[j])));
-    if constexpr (kChunks == 3) {
-      const float s = coef[kS];
-      const uint2 ep = __ldg(noise_pred + 2 * n_pix + i);  // perturbed chunk
-      const float pp[4] = {bf16_lo(ep.x), bf16_hi(ep.x), bf16_lo(ep.y), bf16_hi(ep.y)};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) eps[j] = __fadd_rn(eps[j], __fmul_rn(s, __fsub_rn(tt[j], pp[j])));
-    }
+    guided_eps_rn<kChunks>(noise_pred, i, n_pix, u, tt, guidance, kChunks == 3 ? coef[kS] : 0.f, eps);
+    if constexpr (kRescale) rescale_eps(eps, __ldg(rescale + i / HW), phi, one_m_phi);
     if constexpr (kEuler)
       euler_update_rn(eps, xv, coef);
     else
@@ -284,6 +305,60 @@ __global__ void cfg_step_kernel(const uint2* __restrict__ noise_pred, float4* __
   }
   if constexpr (kInpaint) inpaint_blend(xv, i, image_latents, noise, mask, coef[kC0], coef[kC0 + 1]);
   store_step<kChunks>(latents, model_in, i, n_pix, xv, kEuler ? coef + 2 : nullptr);
+}
+
+// guidance_rescale's per-sample factor r_b = fp32(std(text_b)) / fp32(std(guided_b)), both unbiased over the sample's
+// 4 * HW values.  One CTA per sample: every thread walks a fixed set of pixels, accumulating in fp64 the sums of
+// x - k and (x - k)^2 (k: the sample's first value, so a constant sample gives exactly 0), then a fixed-order tree
+// (warp shuffles, then the warps in order) combines them.  No atomics: a sample's factor has the same bits whatever
+// the batch around it.
+constexpr int kRescaleThreads = 512;
+
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  return v;
+}
+
+template <int kChunks>
+__global__ void __launch_bounds__(kRescaleThreads) cfg_rescale_factors_kernel(
+    const uint2* __restrict__ noise_pred, const float* __restrict__ coef, int s_col, float guidance,
+    float* __restrict__ factors, int HW, long long n_pix) {
+  __shared__ double part[kRescaleThreads / 32][4];
+  const long long base = static_cast<long long>(blockIdx.x) * HW;
+  const float s = kChunks == 3 ? coef[s_col] : 0.f;
+  float u[4], tt[4], e[4];
+  load_cfg_halves(noise_pred, base, n_pix, u, tt);
+  guided_eps_rn<kChunks>(noise_pred, base, n_pix, u, tt, guidance, s, e);
+  const double kt = tt[0], kc = e[0];
+  double st = 0.0, st2 = 0.0, sc = 0.0, sc2 = 0.0;
+  for (int p = threadIdx.x; p < HW; p += kRescaleThreads) {
+    load_cfg_halves(noise_pred, base + p, n_pix, u, tt);
+    guided_eps_rn<kChunks>(noise_pred, base + p, n_pix, u, tt, guidance, s, e);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const double dt = static_cast<double>(tt[j]) - kt, dc = static_cast<double>(e[j]) - kc;
+      st += dt;
+      st2 = fma(dt, dt, st2);
+      sc += dc;
+      sc2 = fma(dc, dc, sc2);
+    }
+  }
+  st = warp_sum_f64(st), st2 = warp_sum_f64(st2), sc = warp_sum_f64(sc), sc2 = warp_sum_f64(sc2);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) part[warp][0] = st, part[warp][1] = st2, part[warp][2] = sc, part[warp][3] = sc2;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double a[4] = {0.0, 0.0, 0.0, 0.0};
+    for (int w = 0; w < kRescaleThreads / 32; ++w)
+#pragma unroll
+      for (int k = 0; k < 4; ++k) a[k] += part[w][k];
+    const double n = 4.0 * HW;
+    // unbiased variance of the shifted values; rounding can leave it a hair below 0 only when it is ~0
+    const double var_t = fmax((a[1] - a[0] * a[0] / n) / (n - 1.0), 0.0);
+    const double var_c = fmax((a[3] - a[2] * a[2] / n) / (n - 1.0), 0.0);
+    factors[blockIdx.x] = __fdiv_rn(__double2float_rn(sqrt(var_t)), __double2float_rn(sqrt(var_c)));
+  }
 }
 
 }  // namespace ds
@@ -430,8 +505,10 @@ extern "C" int ds_timestep_embedding(const float* t, void* out, int rows, int di
 
 extern "C" int ds_cfg_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
                            int update, int chunks, const float* image_latents, const float* noise, const uint8_t* mask,
-                           int bs, int HW, int C, void* stream) {
+                           const float* rescale_factors, double guidance_rescale, int bs, int HW, int C,
+                           void* stream) {
   const bool inpaint = image_latents || noise || mask;
+  const bool rescale = rescale_factors != nullptr;
   DS_REQUIRE(noise_pred && latents && model_in && coef, "ds_cfg_step: NULL pointer");
   DS_REQUIRE(!inpaint || (image_latents && noise && mask),
              "ds_cfg_step: image_latents / noise / mask must all be given or all be NULL");
@@ -441,20 +518,45 @@ extern "C" int ds_cfg_step(const void* noise_pred, float* latents, void* model_i
   DS_REQUIRE(!inpaint || ((reinterpret_cast<uintptr_t>(image_latents) & 15) == 0 &&
                           (reinterpret_cast<uintptr_t>(noise) & 15) == 0),
              "ds_cfg_step: image_latents / noise must be 16-byte aligned");
+  DS_REQUIRE(rescale ? std::isfinite(guidance_rescale) : guidance_rescale == 0.0,
+             "ds_cfg_step: guidance_rescale must be finite, and 0 when rescale_factors is NULL (got %g)",
+             guidance_rescale);
   DeviceInfo dev;
   if (!get_device(&dev)) return DS_ERR_CUDA;
   using StepKernel = void (*)(const uint2*, float4*, uint2*, const float*, float, long long, const float4*,
-                              const float4*, const unsigned char*);
-  static constexpr StepKernel kKernels[2][2][2] = {  // [update][chunks - 2][inpaint]
-      {{cfg_step_kernel<false, 2, false>, cfg_step_kernel<false, 2, true>},
-       {cfg_step_kernel<false, 3, false>, cfg_step_kernel<false, 3, true>}},
-      {{cfg_step_kernel<true, 2, false>, cfg_step_kernel<true, 2, true>},
-       {cfg_step_kernel<true, 3, false>, cfg_step_kernel<true, 3, true>}}};
+                              const float4*, const unsigned char*, const float*, float, float, int);
+  static constexpr StepKernel kKernels[2][2][2][2] = {  // [update][chunks - 2][inpaint][rescale]
+      {{{cfg_step_kernel<false, 2, false, false>, cfg_step_kernel<false, 2, false, true>},
+        {cfg_step_kernel<false, 2, true, false>, cfg_step_kernel<false, 2, true, true>}},
+       {{cfg_step_kernel<false, 3, false, false>, cfg_step_kernel<false, 3, false, true>},
+        {cfg_step_kernel<false, 3, true, false>, cfg_step_kernel<false, 3, true, true>}}},
+      {{{cfg_step_kernel<true, 2, false, false>, cfg_step_kernel<true, 2, false, true>},
+        {cfg_step_kernel<true, 2, true, false>, cfg_step_kernel<true, 2, true, true>}},
+       {{cfg_step_kernel<true, 3, false, false>, cfg_step_kernel<true, 3, false, true>},
+        {cfg_step_kernel<true, 3, true, false>, cfg_step_kernel<true, 3, true, true>}}}};
   const long long n_pix = static_cast<long long>(bs) * HW;
-  kKernels[update][chunks - 2][inpaint]<<<static_cast<unsigned>((n_pix + 255) / 256), 256, 0,
-                                          static_cast<cudaStream_t>(stream)>>>(
+  kKernels[update][chunks - 2][inpaint][rescale]<<<static_cast<unsigned>((n_pix + 255) / 256), 256, 0,
+                                                   static_cast<cudaStream_t>(stream)>>>(
       static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
-      guidance, n_pix, reinterpret_cast<const float4*>(image_latents), reinterpret_cast<const float4*>(noise), mask);
+      guidance, n_pix, reinterpret_cast<const float4*>(image_latents), reinterpret_cast<const float4*>(noise), mask,
+      // phi and 1 - phi (in double) each rounded to fp32 once: torch's values of the Python scalars for an fp32 tensor
+      rescale_factors, static_cast<float>(guidance_rescale), static_cast<float>(1.0 - guidance_rescale), HW);
   DS_LAUNCH_OK("cfg_step_kernel");
+  return DS_OK;
+}
+
+extern "C" int ds_cfg_rescale_factors(const void* noise_pred, const float* coef, int ncoef, float guidance, int chunks,
+                                      float* factors, int bs, int HW, int C, void* stream) {
+  DS_REQUIRE(noise_pred && coef && factors, "ds_cfg_rescale_factors: NULL pointer");
+  DS_REQUIRE(chunks == 2 || chunks == 3, "ds_cfg_rescale_factors: chunks must be 2 or 3, got %d", chunks);
+  DS_REQUIRE(chunks == 2 || ncoef > 0, "ds_cfg_rescale_factors: 3 chunks read the PAG scale at coef[ncoef - 1]");
+  DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "ds_cfg_rescale_factors: only C == 4 latents are supported (got C=%d)", C);
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  const long long n_pix = static_cast<long long>(bs) * HW;
+  auto kernel = chunks == 2 ? cfg_rescale_factors_kernel<2> : cfg_rescale_factors_kernel<3>;
+  kernel<<<bs, kRescaleThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint2*>(noise_pred), coef, ncoef - 1, guidance, factors, HW, n_pix);
+  DS_LAUNCH_OK("cfg_rescale_factors_kernel");
   return DS_OK;
 }

@@ -695,14 +695,16 @@ def timestep_embedding(t: torch.Tensor, dim: int, out: Optional[torch.Tensor] = 
 
 
 def cfg_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
-              guidance: float, euler: bool, inpaint=None) -> None:
+              guidance: float, euler: bool, inpaint=None, rescale=None) -> None:
     """The fused end of a denoise step (``ds_cfg_step``), in place.  noise_pred bf16 [k*bs,H,W,4] holds k = 2 chunks
     [uncond ; text] (CFG) or k = 3 [uncond ; text ; perturbed] (CFG + perturbed-attention guidance):
     eps = u + guidance (t - u) [+ s (t - p)].  latents fp32 NHWC [bs,H,W,4] <- DDIM or (``euler``) Euler update;
     model_in bf16 [k*bs,H,W,4] <- cat[x]*k (DDIM) or cat[x / coef[2]]*k (Euler).  ``inpaint`` None or
     (image_latents, noise, mask): fp32 NHWC [bs,H,W,4] twice and uint8 [bs,H,W]; where mask is 0 the latents become
-    c0 * image_latents + c1 * noise.  coef: the step's fp32 row on the device, exactly
-    DDIM {alpha_prod_t, alpha_prod_t_prev} / Euler {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1)},
+    c0 * image_latents + c1 * noise.  ``rescale`` None or (factors, guidance_rescale): factors fp32 [bs] from
+    ``cfg_rescale_factors`` of this noise_pred and coef, and eps of sample b becomes
+    phi * (eps * factors[b]) + (1 - phi) * eps (diffusers' ``rescale_noise_cfg``).  coef: the step's fp32 row on the
+    device, exactly DDIM {alpha_prod_t, alpha_prod_t_prev} / Euler {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1)},
     then {c0, c1} with ``inpaint``, then s with 3 chunks."""
     _req(noise_pred, bf16, "cfg_step.noise_pred", 4)
     _req(latents, f32, "cfg_step.latents", 4)
@@ -723,8 +725,37 @@ def cfg_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.T
         if image_latents.shape != latents.shape or noise.shape != latents.shape or mask.shape != (bs, H, W):
             raise DsEngineError("cfg_step: shape mismatch")
         ptrs = [image_latents.data_ptr(), noise.data_ptr(), mask.data_ptr()]
+    factors, phi = None, 0.0
+    if rescale is not None:
+        factors, phi = rescale
+        _req(factors, f32, "cfg_step.rescale_factors", 1)
+        if factors.numel() != bs:
+            raise DsEngineError("cfg_step: rescale factors must hold one value per sample")
+        factors = factors.data_ptr()
     check(lib.ds_cfg_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(),
-                          float(guidance), int(bool(euler)), chunks, *ptrs, bs, H * W, Cc, _stream()), "ds_cfg_step")
+                          float(guidance), int(bool(euler)), chunks, *ptrs, factors, float(phi), bs, H * W, Cc,
+                          _stream()), "ds_cfg_step")
+
+
+def cfg_rescale_factors(noise_pred: torch.Tensor, coef: torch.Tensor, guidance: float,
+                        out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The per-sample factors of diffusers' ``rescale_noise_cfg`` (``ds_cfg_rescale_factors``): fp32 [bs],
+    ``fp32(std(t_b)) / fp32(std(eps_b))`` over each sample's C*H*W values (unbiased, fp64 sums), where noise_pred
+    bf16 [k*bs,H,W,4] and coef (s = its last entry with k = 3) are what ``cfg_step_`` then reads and eps_b is the
+    guided eps it computes.  ``out`` fp32 [bs]; bs = out.numel() when given, else noise_pred.shape[0] // 2."""
+    _req(noise_pred, bf16, "cfg_rescale_factors.noise_pred", 4)
+    _req(coef, f32, "cfg_rescale_factors.coef", 1)
+    rows, H, W, Cc = noise_pred.shape
+    if out is None:
+        out = torch.empty(rows // 2, dtype=f32, device=noise_pred.device)
+    _req(out, f32, "cfg_rescale_factors.out", 1)
+    bs = out.numel()
+    chunks = rows // bs if bs else 0
+    if chunks not in (2, 3) or rows != chunks * bs:
+        raise DsEngineError("cfg_rescale_factors: noise_pred must hold 2 or 3 chunks of out.numel() samples")
+    check(lib.ds_cfg_rescale_factors(noise_pred.data_ptr(), coef.data_ptr(), coef.numel(), float(guidance), chunks,
+                                     out.data_ptr(), bs, H * W, Cc, _stream()), "ds_cfg_rescale_factors")
+    return out
 
 
 # ---------------------------------------------------------------------------------------------- encoder helpers

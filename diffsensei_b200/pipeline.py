@@ -32,6 +32,8 @@ checkpoint's scheduler config.
 """
 from __future__ import annotations
 
+import math
+import numbers
 import os
 
 from types import SimpleNamespace
@@ -52,7 +54,7 @@ bf16, f32 = torch.bfloat16, torch.float32
 # generate_page: what a captured stepper bakes in is the same for the whole page; everything else is per panel
 PAGE_KEYS = frozenset({"num_inference_steps", "guidance_scale", "ip_scale", "output_type", "use_graph",
                        "max_batch_panels", "strength", "pag_scale", "pag_adaptive_scale",
-                       "adapter_conditioning_factor"})
+                       "adapter_conditioning_factor", "guidance_rescale"})
 PANEL_KEYS = frozenset({
     "prompt", "prompt_2", "negative_prompt", "negative_prompt_2", "height", "width", "num_samples", "generator",
     "latents", "original_size", "crops_coords_top_left", "target_size", "min_size_step", "ip_images",
@@ -103,6 +105,15 @@ def _stacked(fn, xs):
             out[i] = tuple(t[r0:r1] for t in res)
             r0 = r1
     return out
+
+
+def check_guidance_rescale(guidance_rescale) -> float:
+    """diffusers' ``guidance_rescale`` as a float: a finite real number (not a bool), else ``ValueError`` naming the
+    keyword.  ``> 0`` turns the rescale on, as in diffusers; 0 and below leave the step as it is."""
+    v = guidance_rescale
+    if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(v):
+        raise ValueError(f"`guidance_rescale` must be a finite real number, got {v!r}")
+    return float(v)
 
 
 def _pad_boxes(boxes, m: int) -> List[List[float]]:
@@ -414,38 +425,44 @@ class DiffSenseiPipeline:
                      add_time_ids: torch.Tensor, bbox: torch.Tensor, aspect_ratio: float,
                      dialog_bbox: Optional[torch.Tensor], num_inference_steps: int, guidance_scale: float,
                      use_graph: bool = True, chains: Optional[int] = None, start_index: int = 0,
-                     inpaint=None, pag=None, adapter=None) -> "DenoiseStepper":
+                     inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0) -> "DenoiseStepper":
         return DenoiseStepper(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                               dialog_bbox, num_inference_steps, guidance_scale, use_graph, chains, start_index,
-                              inpaint, pag, adapter)
+                              inpaint, pag, adapter, guidance_rescale)
 
     def stepper_key(self, latents, prompt_embeds, aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale,
-                    chains=None, start_index: int = 0, inpaint=None, pag=None, adapter=None) -> tuple:
+                    chains=None, start_index: int = 0, inpaint=None, pag=None, adapter=None,
+                    guidance_rescale: float = 0.0) -> tuple:
         """Everything a captured stepper bakes in (``stepper_for``), FreeU's values (``unet.freeu``) and whether a
-        T2I-Adapter's features are added included."""
-        return (tuple(latents.shape), tuple(prompt_embeds.shape), None if dialog_bbox is None else
+        T2I-Adapter's features are added included.  With ``guidance_rescale > 0`` the key ends with its value, which
+        the graph bakes in like ``guidance_scale``; otherwise the key is the one the step without the rescale has."""
+        key = (tuple(latents.shape), tuple(prompt_embeds.shape), None if dialog_bbox is None else
                 (tuple(dialog_bbox.shape), dialog_bbox.dtype == bf16), float(aspect_ratio), int(num_inference_steps),
                 float(guidance_scale), self.unet.scales_key(), chains, self.unet._ip_weights_version(),
                 type(self.scheduler).__name__, tuple(sorted(self.scheduler.config.items())), int(start_index),
                 inpaint is not None, None if pag is None else tuple(sorted(pag[0])), self.unet.freeu,
                 adapter is not None)
+        if guidance_rescale > 0:
+            key += (("guidance_rescale", float(guidance_rescale)),)
+        return key
 
     def stepper_for(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio, dialog_bbox,
                     num_inference_steps, guidance_scale, chains=None, start_index: int = 0,
-                    inpaint=None, pag=None, adapter=None) -> "DenoiseStepper":
+                    inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0) -> "DenoiseStepper":
         """A graph-captured stepper loaded with this panel: a cached one of the same key is refilled in place
         (no re-capture), otherwise a new one is built and cached.  The start index is part of the key: the stepper
         bakes in its slice of the schedule (``set_timesteps`` would reset any scheduler state); so is whether it
         inpaints, which selects the step kernel, the perturbed-attention sites (``pag``: None when off) and FreeU's
-        values, which the graph bakes in, and whether it adds adapter features.  The PAG scales are not: they live in
-        the coefficient table, which ``load_panel`` rewrites, as it rewrites the adapter features and gates."""
+        values, which the graph bakes in, and whether it adds adapter features, and ``guidance_rescale``.  The PAG
+        scales are not: they live in the coefficient table, which ``load_panel`` rewrites, as it rewrites the adapter
+        features and gates."""
         key = self.stepper_key(latents, prompt_embeds, aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale,
-                               chains, start_index, inpaint, pag, adapter)
+                               chains, start_index, inpaint, pag, adapter, guidance_rescale)
         st = self._steppers.get(key)
         if st is None:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                    dialog_bbox, num_inference_steps, guidance_scale, True, chains, start_index,
-                                   inpaint, pag, adapter)
+                                   inpaint, pag, adapter, guidance_rescale)
             while len(self._steppers) >= self.max_cached_steppers:
                 self._steppers.pop(next(iter(self._steppers)))
             self._steppers[key] = st
@@ -459,7 +476,7 @@ class DiffSenseiPipeline:
                 add_time_ids: torch.Tensor, bbox: torch.Tensor, aspect_ratio: float,
                 dialog_bbox: Optional[torch.Tensor], num_inference_steps: int, guidance_scale: float,
                 use_graph: bool = True, on_step=None, start_index: int = 0, inpaint=None, pag_scale: float = 0.0,
-                pag_adaptive_scale: float = 0.0, adapter=None) -> torch.Tensor:
+                pag_adaptive_scale: float = 0.0, adapter=None, guidance_rescale: float = 0.0) -> torch.Tensor:
         """pipeline_diffsensei.py:306-337.  ``latents`` NCHW fp32 (bs,4,h,w); conditions already concatenated
         [negative ; positive] along batch (:293-304), or [negative ; positive ; positive] with perturbed-attention
         guidance (``pag_scale > 0``: diffusers' PAGMixin; the third chunk takes the identity attention map at the
@@ -468,18 +485,20 @@ class DiffSenseiPipeline:
         (bs,4,h,w), noise fp32 (bs,4,h,w), latent mask uint8 (bs,h,w)); after every step the pixels where the mask is
         0 become the image latents noised to the next timestep (the image latents on the last step).  ``adapter``:
         (features, gates), T2I-Adapter features bf16 NHWC [bs, h, w, c] (one row per sample, every UNet row of the
-        sample gets it) and per loop step a gate, 1.0 (added) or 0.0 (``DenoiseStepper``).  Returns the final latents,
-        NCHW fp32."""
+        sample gets it) and per loop step a gate, 1.0 (added) or 0.0 (``DenoiseStepper``).  ``guidance_rescale > 0``:
+        diffusers' ``rescale_noise_cfg`` on the guided eps of every sample before the scheduler step.  Returns the
+        final latents, NCHW fp32."""
+        guidance_rescale = check_guidance_rescale(guidance_rescale)
         self.unet.set_lora_scale(1.0)            # a direct unet(..., cross_attention_kwargs={"scale": s}) call may have left s
         pag = self._pag(pag_scale, pag_adaptive_scale)
         if use_graph:
             st = self.stepper_for(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                   dialog_bbox, num_inference_steps, guidance_scale, start_index=start_index,
-                                  inpaint=inpaint, pag=pag, adapter=adapter)
+                                  inpaint=inpaint, pag=pag, adapter=adapter, guidance_rescale=guidance_rescale)
         else:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                    dialog_bbox, num_inference_steps, guidance_scale, False, start_index=start_index,
-                                   inpaint=inpaint, pag=pag, adapter=adapter)
+                                   inpaint=inpaint, pag=pag, adapter=adapter, guidance_rescale=guidance_rescale)
         for i, t in enumerate(st.timesteps):
             st.step(i)
             if on_step is not None:
@@ -512,14 +531,17 @@ class DiffSenseiPipeline:
                  pag_scale: float = 0.0, pag_adaptive_scale: float = 0.0,
                  # T2I-Adapter (diffusers' StableDiffusionXLAdapterPipeline): follow this sketch / line art
                  adapter_image=None, adapter_conditioning_scale: float = 1.0,
-                 adapter_conditioning_factor: float = 1.0):
+                 adapter_conditioning_factor: float = 1.0,
+                 # diffusers' rescale_noise_cfg (Lin et al., sec. 3.4) after the guidance blend: on when > 0
+                 guidance_rescale: float = 0.0):
         """A page of one panel: ``generate_page([panel], ...)[0]``, the panel holding this call's per-panel keywords
         (``PANEL_KEYS``) and the page the others.  Its input errors carry no panel index."""
         args = locals()
         panel = {k: args[k] for k in PANEL_KEYS}                    # as given, defaults included
         page = dict(num_inference_steps=num_inference_steps, guidance_scale=guidance_scale, output_type=output_type,
                     max_batch_panels=PAGE_MAX_ROWS, strength=strength, pag_scale=pag_scale,
-                    pag_adaptive_scale=pag_adaptive_scale, adapter_conditioning_factor=adapter_conditioning_factor)
+                    pag_adaptive_scale=pag_adaptive_scale, adapter_conditioning_factor=adapter_conditioning_factor,
+                    guidance_rescale=guidance_rescale)
         t_start = self._check_page([panel], **page)
         return self._run_page([self._panel_job(panel, output_type)], t_start, ip_scale=ip_scale, use_graph=use_graph,
                               **page)[0]
@@ -565,7 +587,7 @@ class DiffSenseiPipeline:
         return height, width
 
     def _check_page(self, panels, num_inference_steps, guidance_scale, output_type, max_batch_panels,
-                    strength, pag_scale, pag_adaptive_scale, adapter_conditioning_factor) -> int:
+                    strength, pag_scale, pag_adaptive_scale, adapter_conditioning_factor, guidance_rescale) -> int:
         """The host-only checks of the page keywords.  Returns the first step of the schedule that image panels run
         (0 on a page without them, where ``strength`` is not used)."""
         if output_type not in ("latent", "pt", "np", "pil"):
@@ -584,6 +606,7 @@ class DiffSenseiPipeline:
         f = adapter_conditioning_factor
         if isinstance(f, bool) or not isinstance(f, (int, float)) or not 0.0 <= f <= 1.0:
             raise ValueError(f"`adapter_conditioning_factor` must be a number in [0, 1], got {f!r}")
+        check_guidance_rescale(guidance_rescale)
         if any(p.get("image") is not None for p in panels):
             return get_timesteps(num_inference_steps, strength)[0]
         return 0
@@ -596,7 +619,8 @@ class DiffSenseiPipeline:
                       mllm_scale: float = 0.4, max_new_tokens: int = 500,
                       strength: float = 0.3, pag_scale: float = 0.0,
                       pag_adaptive_scale: float = 0.0,
-                      adapter_conditioning_factor: float = 1.0) -> List[SimpleNamespace]:
+                      adapter_conditioning_factor: float = 1.0,
+                      guidance_rescale: float = 0.0) -> List[SimpleNamespace]:
         """Several panels of a page in one call.  ``panels`` holds one dict per panel with the per-panel keywords of
         ``__call__`` (``PANEL_KEYS``); the keywords here are the same for the whole page.  Returns one
         ``SimpleNamespace(images=..., latents=...)`` per panel, in panel order, each ``torch.equal`` to
@@ -640,7 +664,13 @@ class DiffSenseiPipeline:
         by the panel's ``adapter_conditioning_scale`` (rounded to bf16) and added to the UNet's down path on every
         row of the panel at loop steps ``i < int(num_inference_steps * adapter_conditioning_factor)`` (``i`` counts
         the steps the loop runs).  A scale of 0, or a factor that gives no step, runs the panel without the adapter.
-        Adapter panels share a denoise only with adapter panels."""
+        Adapter panels share a denoise only with adapter panels.
+
+        ``guidance_rescale > 0`` rescales the guided noise of every sample as diffusers' SDXL pipelines do
+        (``rescale_noise_cfg``, Lin et al. 2024, sec. 3.4): eps <- phi * eps * std(text eps) / std(eps) +
+        (1 - phi) * eps, the standard deviations over the sample's C x H x W values, with PAG's term included in eps
+        and before the scheduler step and the inpaint blend.  It counters the over-exposure of high guidance
+        scales; diffusers' pipelines suggest 0.7."""
         if not isinstance(panels, (list, tuple)) or len(panels) == 0:
             raise ValueError("generate_page needs a non-empty list of panel dicts")
         panels = [dict(p) for p in panels]
@@ -652,7 +682,8 @@ class DiffSenseiPipeline:
                     raise ValueError(f"panel {i}: unknown key `{k}`")
         page = dict(num_inference_steps=num_inference_steps, guidance_scale=guidance_scale, output_type=output_type,
                     max_batch_panels=max_batch_panels, strength=strength, pag_scale=pag_scale,
-                    pag_adaptive_scale=pag_adaptive_scale, adapter_conditioning_factor=adapter_conditioning_factor)
+                    pag_adaptive_scale=pag_adaptive_scale, adapter_conditioning_factor=adapter_conditioning_factor,
+                    guidance_rescale=guidance_rescale)
         t_start = self._check_page(panels, **page)
         if agent is not None:
             self._check_agent_panels(panels, tokenizer_mllm)
@@ -673,7 +704,7 @@ class DiffSenseiPipeline:
 
     def _run_page(self, jobs, t_start: int, *, num_inference_steps, guidance_scale, ip_scale, output_type, use_graph,
                   max_batch_panels, strength, pag_scale, pag_adaptive_scale,
-                  adapter_conditioning_factor) -> List[SimpleNamespace]:
+                  adapter_conditioning_factor, guidance_rescale) -> List[SimpleNamespace]:
         """The GPU half of a page whose panels (``_panel_job``) and keywords (``_check_page``) passed their checks."""
         # ---- front end, once per page
         dev = self.unet.device
@@ -735,7 +766,8 @@ class DiffSenseiPipeline:
             final = self.denoise(lat, cat("pe"), cat("te"), cat("ti"), cat("bbox"), lat.shape[-2] / lat.shape[-1],
                                  cat("db"), num_inference_steps, guidance_scale, use_graph=use_graph,
                                  start_index=t_start if jobs[chunk[0]].image is not None else 0, inpaint=inpaint,
-                                 pag_scale=pag_scale, pag_adaptive_scale=pag_adaptive_scale, adapter=adapter)
+                                 pag_scale=pag_scale, pag_adaptive_scale=pag_adaptive_scale, adapter=adapter,
+                                 guidance_rescale=guidance_rescale)
             # pipeline_diffsensei.py:339-363: latents / scaling_factor -> vae.decode -> image_processor.postprocess
             image = self.vae.decode_image(final) if output_type != "latent" else final
             r0 = 0
@@ -1088,12 +1120,15 @@ class DenoiseStepper:
     With ``adapter`` = (features, gates) the UNet adds T2I-Adapter features (bf16 NHWC [bs, h, w, c] each; UNet row b
     reads row b % bs) at its down-path sites, times the step's gate (1.0 or 0.0), which ``step`` copies into a device
     scalar like the time embedding's row.
+    With ``guidance_rescale`` > 0 each step first computes the per-sample factors of diffusers' ``rescale_noise_cfg``
+    from the UNet's eps (``ops.cfg_rescale_factors``, into a [bs] buffer allocated once), then runs the step with the
+    rescale; both launches are in the captured graph, which bakes in the value as it does ``guidance_scale``.
     """
 
     @torch.no_grad()
     def __init__(self, pipe: DiffSenseiPipeline, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox,
                  aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale, use_graph=True, chains=None,
-                 start_index: int = 0, inpaint=None, pag=None, adapter=None):
+                 start_index: int = 0, inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0):
         unet, dev = pipe.unet, pipe.unet.device
         self.unet, self.dev, self.guidance = unet, dev, float(guidance_scale)
         self.scheduler = pipe.scheduler
@@ -1121,6 +1156,11 @@ class DenoiseStepper:
         self.ad_feats = self.ad_gates = None
         self.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox, inpaint, pag,
                         adapter)
+        rescale = check_guidance_rescale(guidance_rescale)
+        self.guidance_rescale = rescale if rescale > 0 else 0.0
+        self.rescale_factors = None
+        if self.guidance_rescale > 0:
+            self.rescale_factors = torch.empty(self.lat.shape[0], dtype=f32, device=dev)
         self.temb_cur = self.temb_table[0].clone()
         self.ad_gate_cur = None if adapter is None else self.ad_gates[0].clone()
         self.coef_cur = self.coef_table[0].clone()
@@ -1271,8 +1311,14 @@ class DenoiseStepper:
             finally:
                 ops.SPLITK = prev_splitk
                 ops.GEMM_CHAINS = prev_chains
-        self.scheduler.fused_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance,     # :332-337,:315-317
-                                   (self.inp_z, self.inp_n, self.inp_m) if self.inpaint else None)
+        inpaint = (self.inp_z, self.inp_n, self.inp_m) if self.inpaint else None
+        if self.guidance_rescale > 0:                  # diffusers' rescale_noise_cfg, before the scheduler step
+            ops.cfg_rescale_factors(eps, self.coef_cur, self.guidance, out=self.rescale_factors)
+            self.scheduler.fused_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance, inpaint,
+                                       (self.rescale_factors, self.guidance_rescale))
+        else:
+            self.scheduler.fused_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance,  # :332-337,:315-317
+                                       inpaint)
 
     @torch.no_grad()
     def step(self, i: int) -> None:

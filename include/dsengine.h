@@ -361,19 +361,35 @@ int ds_timestep_embedding(const float* t, void* out, int rows, int dim, void* st
  *   coef          : device pointer to this step's row, columns in this order:
  *                   DDIM {alpha_prod_t, alpha_prod_t_prev} or Euler {sigma, sigma_next, sqrt(sigma_next^2 + 1)},
  *                   then {c0, c1} when inpainting, then s when chunks == 3
+ *   rescale_factors : NULL (no rescale; guidance_rescale must then be 0) or fp32 [bs], the factors
+ *                   ds_cfg_rescale_factors wrote for this noise_pred and coef row
+ *   guidance_rescale: phi of diffusers' rescale_noise_cfg as the caller's double (finite; on for phi > 0 in diffusers)
  * The arithmetic, per element:
  *   eps   = e_uncond + guidance * (e_text - e_uncond)      [+ s * (e_text - e_perturbed) with 3 chunks]
+ *   rescale (rescale_factors given): eps = fp32(phi) * (eps * r_b) + fp32(1 - phi) * eps, r_b the factor of the
+ *            pixel's sample, 1 - phi evaluated in double: torch's fp32 values of the Python scalars
  *   DDIM  : x0 = (x - sqrt(1-a_t) * eps) / sqrt(a_t);  x_new = sqrt(a_prev) * x0 + sqrt(1-a_prev) * eps
  *   Euler : x0 = x - sigma * eps;  d = (x - x0) / sigma;  x_new = x + d * (sigma_next - sigma)
  *   inpaint: init = c0 * z + c1 * n (add_noise of the image latents at the next timestep; {1, 0} on the last step);
  *            x_new = mask ? x_new : init, and the next UNet input is computed from the blended x_new
- * Rounding: every operation is rounded on its own in diffusers' eager fp32 order, except DDIM with 2 chunks, where
- * the compiler may contract multiply-adds into FMAs.  A pixel with mask != 0 is the result without inpaint bit for
- * bit.
+ * Rounding: every operation is rounded on its own in diffusers' eager fp32 order, except DDIM with 2 chunks and no
+ * rescale, where the compiler may contract multiply-adds into FMAs.  A pixel with mask != 0 is the result without
+ * inpaint bit for bit.
+ *
+ * ds_cfg_rescale_factors: the per-sample factors of diffusers' rescale_noise_cfg (Lin et al. 2024, sec. 3.4), from
+ * the same noise_pred / coef row / guidance / chunks the step then reads (s = coef[ncoef - 1] with 3 chunks):
+ *   factors[b] = fp32(std(e_text_b)) / fp32(std(eps_b))  (fp32 division), eps_b the guided eps of sample b computed
+ *   exactly as ds_cfg_step computes it; both std unbiased (N - 1) over the sample's 4 * HW values, accumulated in fp64
+ *   and rounded to fp32 once.  One CTA per sample, a fixed reduction order and no atomics: a sample's factor has the
+ *   same bits whatever bs is and whichever samples share the batch.  A sample whose guided eps is constant has
+ *   std 0, so its factor is +inf (NaN if its text eps is constant too), and the rescaled step then writes inf / NaN
+ *   into that sample, as diffusers does; there is no guard.
  * --------------------------------------------------------------------------------------------- */
 int ds_cfg_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance, int update,
-                int chunks, const float* image_latents, const float* noise, const uint8_t* mask, int bs, int HW, int C,
-                void* stream);
+                int chunks, const float* image_latents, const float* noise, const uint8_t* mask,
+                const float* rescale_factors, double guidance_rescale, int bs, int HW, int C, void* stream);
+int ds_cfg_rescale_factors(const void* noise_pred, const float* coef, int ncoef, float guidance, int chunks,
+                           float* factors, int bs, int HW, int C, void* stream);
 
 /* Perceiver attention of the character Resampler: 16 latent queries x (n_kv) keys per (character, head),
  * q and k each pre-scaled by dim_head^-0.25, fp32 softmax (src/models/resampler.py:64-74).
