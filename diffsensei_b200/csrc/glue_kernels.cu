@@ -1,7 +1,8 @@
 // glue_kernels.cu — small HBM-bound kernels around the tensor-core ops: conv_in (Cin = 4), layout changes at
 // the diffusers-facing boundary, nearest upsample, channel concat, SiLU, sinusoidal timestep features, and the
-// fused CFG + DDIM and CFG + Euler updates (plain and inpaint, with or without guidance_rescale) and the per-sample
-// factors of that rescale.  All vectorised to 16-byte accesses where the shape allows.
+// fused CFG + DDIM and CFG + Euler updates (plain and inpaint, with or without guidance_rescale), the same update on a
+// canvas denoised as overlapping views (MultiDiffusion), and the per-sample factors of that rescale.  All vectorised to
+// 16-byte accesses where the shape allows.
 #include <cmath>
 
 #include "ds_common.cuh"
@@ -273,6 +274,29 @@ __device__ __forceinline__ void store_step(float4* __restrict__ latents, uint2* 
   for (int c = 0; c < kChunks; ++c) model_in[c * n_pix + i] = o;
 }
 
+// The guided scheduler update of one pixel: xv (the latents, loaded by the caller) <- update(guide(u, tt)), u / tt
+// the pixel's uncond / text eps at index i of noise_pred, kS the PAG scale's column of coef; kRescale: the factor of
+// sample i / HW is rescale[i / HW].  The step kernels share it, so a tiled step's views update exactly as untiled samples.
+template <bool kEuler, int kChunks, bool kRescale, int kS>
+__device__ __forceinline__ void guided_update(const uint2* __restrict__ noise_pred, long long i, long long n_pix,
+                                              const float u[4], const float tt[4], float xv[4],
+                                              const float* __restrict__ coef, float guidance,
+                                              const float* __restrict__ rescale, int HW, float phi,
+                                              float one_m_phi) {
+  if constexpr (!kEuler && kChunks == 2 && !kRescale) {
+    // the CFG-only DDIM step has always let the compiler contract into FMAs; rounding it op by op changes its bits
+    cfg_ddim_pixel(u, tt, xv, coef, guidance);
+  } else {
+    float eps[4];
+    guided_eps_rn<kChunks>(noise_pred, i, n_pix, u, tt, guidance, kChunks == 3 ? coef[kS] : 0.f, eps);
+    if constexpr (kRescale) rescale_eps(eps, __ldg(rescale + i / HW), phi, one_m_phi);
+    if constexpr (kEuler)
+      euler_update_rn(eps, xv, coef);
+    else
+      ddim_update_rn(eps, xv, coef);
+  }
+}
+
 // noise_pred holds kChunks chunks of n_pix pixels, [uncond ; text (; perturbed)]; coef is the step's row
 // {update (2 DDIM, 3 Euler) | c0, c1 if kInpaint | s if kChunks == 3}.  kRescale: the guided eps of sample i / HW is
 // rescaled with the factor rescale[i / HW] (cfg_rescale_factors_kernel) before the update.
@@ -291,20 +315,92 @@ __global__ void cfg_step_kernel(const uint2* __restrict__ noise_pred, float4* __
   load_cfg_halves(noise_pred, i, n_pix, u, tt);
   const float4 x = latents[i];
   float xv[4] = {x.x, x.y, x.z, x.w};
-  if constexpr (!kEuler && kChunks == 2 && !kRescale) {
-    // the CFG-only DDIM step has always let the compiler contract into FMAs; rounding it op by op changes its bits
-    cfg_ddim_pixel(u, tt, xv, coef, guidance);
-  } else {
-    float eps[4];
-    guided_eps_rn<kChunks>(noise_pred, i, n_pix, u, tt, guidance, kChunks == 3 ? coef[kS] : 0.f, eps);
-    if constexpr (kRescale) rescale_eps(eps, __ldg(rescale + i / HW), phi, one_m_phi);
-    if constexpr (kEuler)
-      euler_update_rn(eps, xv, coef);
-    else
-      ddim_update_rn(eps, xv, coef);
-  }
+  guided_update<kEuler, kChunks, kRescale, kS>(noise_pred, i, n_pix, u, tt, xv, coef, guidance, rescale, HW, phi,
+                                               one_m_phi);
   if constexpr (kInpaint) inpaint_blend(xv, i, image_latents, noise, mask, coef[kC0], coef[kC0 + 1]);
   store_step<kChunks>(latents, model_in, i, n_pix, xv, kEuler ? coef + 2 : nullptr);
+}
+
+// MultiDiffusion's view grid on one latent axis: n views of `size` pixels, view k at min(k * stride, dim - size) (the
+// last one flush with the far edge), 0 < stride <= size <= dim.  Every coordinate has at least one covering view.
+struct TileAxis {
+  int dim, size, stride, n;
+};
+
+__device__ __forceinline__ int tile_origin(const TileAxis& a, int k) { return min(k * a.stride, a.dim - a.size); }
+
+// the views [lo, hi] that cover coordinate p: a contiguous range, from integer arithmetic on the grid alone
+__device__ __forceinline__ void tile_cover(const TileAxis& a, int p, int& lo, int& hi) {
+  lo = p < a.size ? 0 : min((p - a.size) / a.stride + 1, a.n - 1);
+  hi = p >= a.dim - a.size ? a.n - 1 : p / a.stride;
+}
+
+// The tiled step (MultiDiffusion, Bar-Tal et al. 2023), one thread per canvas pixel.  latents: the fp32 canvas
+// [bs][H][W][4]; noise_pred / model_in: kChunks chunks of bs * V views (row b * V + v, v = vy * ax.n + vx) of
+// ay.size x ax.size pixels.  Every covering view's x_new is computed from the canvas pixel as the untiled step
+// computes a sample's (rescale factor: the view row's); their fp32 sum, in view order from 0, over the count is the
+// new canvas pixel (diffusers' panorama loop: value += x_view, then value / count), then the inpaint blend on the
+// canvas, then the next UNet input into every covering view of every chunk.  Each output element is written once.
+template <bool kEuler, int kChunks, bool kInpaint, bool kRescale>
+__global__ void tile_step_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
+                                 uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
+                                 TileAxis ay, TileAxis ax, int bs,
+                                 const float4* __restrict__ image_latents, const float4* __restrict__ noise,
+                                 const unsigned char* __restrict__ mask, const float* __restrict__ rescale, float phi,
+                                 float one_m_phi) {
+  static_assert(kChunks == 2 || kChunks == 3, "CFG (2 chunks) or CFG + PAG (3 chunks)");
+  constexpr int kC0 = kEuler ? 3 : 2;
+  constexpr int kS = kC0 + (kInpaint ? 2 : 0);
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<long long>(bs) * ay.dim * ax.dim) return;
+  const int x = static_cast<int>(i % ax.dim);
+  const long long by = i / ax.dim;
+  const int y = static_cast<int>(by % ay.dim);
+  const int b = static_cast<int>(by / ay.dim);
+  const int views = ay.n * ax.n, view_hw = ay.size * ax.size;
+  const long long n_pix = static_cast<long long>(bs) * views * view_hw;  // pixels per chunk
+  int ylo, yhi, xlo, xhi;
+  tile_cover(ay, y, ylo, yhi);
+  tile_cover(ax, x, xlo, xhi);
+  const float4 xc = latents[i];
+  float sum[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int vy = ylo; vy <= yhi; ++vy) {
+    const long long row0 = (static_cast<long long>(b) * views + vy * ax.n) * view_hw +
+                           static_cast<long long>(y - tile_origin(ay, vy)) * ax.size;
+    for (int vx = xlo; vx <= xhi; ++vx) {
+      const long long j = row0 + vx * static_cast<long long>(view_hw) + (x - tile_origin(ax, vx));
+      float u[4], tt[4];
+      load_cfg_halves(noise_pred, j, n_pix, u, tt);
+      float xv[4] = {xc.x, xc.y, xc.z, xc.w};
+      guided_update<kEuler, kChunks, kRescale, kS>(noise_pred, j, n_pix, u, tt, xv, coef, guidance, rescale, view_hw,
+                                                   phi, one_m_phi);
+#pragma unroll
+      for (int c = 0; c < 4; ++c) sum[c] = __fadd_rn(sum[c], xv[c]);
+    }
+  }
+  const float count = static_cast<float>((yhi - ylo + 1) * (xhi - xlo + 1));
+  float xv[4];
+#pragma unroll
+  for (int c = 0; c < 4; ++c) xv[c] = __fdiv_rn(sum[c], count);
+  if constexpr (kInpaint) inpaint_blend(xv, i, image_latents, noise, mask, coef[kC0], coef[kC0 + 1]);
+  latents[i] = make_float4(xv[0], xv[1], xv[2], xv[3]);
+  uint2 o;
+  if constexpr (kEuler) {
+    const float d = coef[2];
+    o = make_uint2(pack_bf16(__fdiv_rn(xv[0], d), __fdiv_rn(xv[1], d)),
+                   pack_bf16(__fdiv_rn(xv[2], d), __fdiv_rn(xv[3], d)));
+  } else {
+    o = make_uint2(pack_bf16(xv[0], xv[1]), pack_bf16(xv[2], xv[3]));
+  }
+  for (int vy = ylo; vy <= yhi; ++vy) {
+    const long long row0 = (static_cast<long long>(b) * views + vy * ax.n) * view_hw +
+                           static_cast<long long>(y - tile_origin(ay, vy)) * ax.size;
+    for (int vx = xlo; vx <= xhi; ++vx) {
+      const long long j = row0 + vx * static_cast<long long>(view_hw) + (x - tile_origin(ax, vx));
+#pragma unroll
+      for (int c = 0; c < kChunks; ++c) model_in[c * n_pix + j] = o;
+    }
+  }
 }
 
 // guidance_rescale's per-sample factor r_b = fp32(std(text_b)) / fp32(std(guided_b)), both unbiased over the sample's
@@ -542,6 +638,54 @@ extern "C" int ds_cfg_step(const void* noise_pred, float* latents, void* model_i
       // phi and 1 - phi (in double) each rounded to fp32 once: torch's values of the Python scalars for an fp32 tensor
       rescale_factors, static_cast<float>(guidance_rescale), static_cast<float>(1.0 - guidance_rescale), HW);
   DS_LAUNCH_OK("cfg_step_kernel");
+  return DS_OK;
+}
+
+extern "C" int ds_tile_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
+                            int update, int chunks, const float* image_latents, const float* noise, const uint8_t* mask,
+                            const float* rescale_factors, double guidance_rescale, int bs, int H, int W, int tile_h,
+                            int tile_w, int stride_h, int stride_w, int C, void* stream) {
+  const bool inpaint = image_latents || noise || mask;
+  const bool rescale = rescale_factors != nullptr;
+  DS_REQUIRE(noise_pred && latents && model_in && coef, "ds_tile_step: NULL pointer");
+  DS_REQUIRE(!inpaint || (image_latents && noise && mask),
+             "ds_tile_step: image_latents / noise / mask must all be given or all be NULL");
+  DS_REQUIRE(update == 0 || update == 1, "ds_tile_step: update must be 0 (DDIM) or 1 (Euler), got %d", update);
+  DS_REQUIRE(chunks == 2 || chunks == 3, "ds_tile_step: chunks must be 2 or 3, got %d", chunks);
+  DS_REQUIRE(bs > 0 && C == 4, "ds_tile_step: only C == 4 latents are supported (got C=%d)", C);
+  DS_REQUIRE(0 < tile_h && tile_h <= H && 0 < tile_w && tile_w <= W,
+             "ds_tile_step: the view (%d x %d) must fit the canvas (%d x %d)", tile_h, tile_w, H, W);
+  DS_REQUIRE(0 < stride_h && stride_h <= tile_h && 0 < stride_w && stride_w <= tile_w,
+             "ds_tile_step: the stride (%d, %d) must be in (0, view size]", stride_h, stride_w);
+  DS_REQUIRE(!inpaint || ((reinterpret_cast<uintptr_t>(image_latents) & 15) == 0 &&
+                          (reinterpret_cast<uintptr_t>(noise) & 15) == 0),
+             "ds_tile_step: image_latents / noise must be 16-byte aligned");
+  DS_REQUIRE(rescale ? std::isfinite(guidance_rescale) : guidance_rescale == 0.0,
+             "ds_tile_step: guidance_rescale must be finite, and 0 when rescale_factors is NULL (got %g)",
+             guidance_rescale);
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  // n views per axis: ceil((dim - size) / stride) + 1, the last one flush with the far edge
+  const TileAxis ay{H, tile_h, stride_h, (H - tile_h + stride_h - 1) / stride_h + 1};
+  const TileAxis ax{W, tile_w, stride_w, (W - tile_w + stride_w - 1) / stride_w + 1};
+  using TileKernel = void (*)(const uint2*, float4*, uint2*, const float*, float, TileAxis, TileAxis, int,
+                              const float4*, const float4*, const unsigned char*, const float*, float, float);
+  static constexpr TileKernel kKernels[2][2][2][2] = {  // [update][chunks - 2][inpaint][rescale]
+      {{{tile_step_kernel<false, 2, false, false>, tile_step_kernel<false, 2, false, true>},
+        {tile_step_kernel<false, 2, true, false>, tile_step_kernel<false, 2, true, true>}},
+       {{tile_step_kernel<false, 3, false, false>, tile_step_kernel<false, 3, false, true>},
+        {tile_step_kernel<false, 3, true, false>, tile_step_kernel<false, 3, true, true>}}},
+      {{{tile_step_kernel<true, 2, false, false>, tile_step_kernel<true, 2, false, true>},
+        {tile_step_kernel<true, 2, true, false>, tile_step_kernel<true, 2, true, true>}},
+       {{tile_step_kernel<true, 3, false, false>, tile_step_kernel<true, 3, false, true>},
+        {tile_step_kernel<true, 3, true, false>, tile_step_kernel<true, 3, true, true>}}}};
+  const long long n_canvas = static_cast<long long>(bs) * H * W;
+  kKernels[update][chunks - 2][inpaint][rescale]<<<static_cast<unsigned>((n_canvas + 255) / 256), 256, 0,
+                                                   static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
+      guidance, ay, ax, bs, reinterpret_cast<const float4*>(image_latents), reinterpret_cast<const float4*>(noise),
+      mask, rescale_factors, static_cast<float>(guidance_rescale), static_cast<float>(1.0 - guidance_rescale));
+  DS_LAUNCH_OK("tile_step_kernel");
   return DS_OK;
 }
 

@@ -716,25 +716,59 @@ def cfg_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.T
     if chunks not in (2, 3) or noise_pred.shape != (chunks * bs, H, W, Cc) or model_in.shape != noise_pred.shape \
             or coef.numel() != ncoef:
         raise DsEngineError("cfg_step: shape mismatch")
+    ptrs, factors, phi = _step_state("cfg_step", latents, bs, inpaint, rescale)
+    check(lib.ds_cfg_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(),
+                          float(guidance), int(bool(euler)), chunks, *ptrs, factors, float(phi), bs, H * W, Cc,
+                          _stream()), "ds_cfg_step")
+
+
+def _step_state(what: str, latents: torch.Tensor, rows: int, inpaint, rescale):
+    """The inpaint pointers (latent-shaped image latents and noise, a [bs, H, W] mask; NULLs without) and the rescale
+    factors (``rows`` values) and value of a step launch, checked."""
+    bs, H, W, _ = latents.shape
     ptrs = [None] * 3
     if inpaint is not None:
         image_latents, noise, mask = inpaint
-        _req(image_latents, f32, "cfg_step.image_latents", 4)
-        _req(noise, f32, "cfg_step.noise", 4)
-        _req(mask, torch.uint8, "cfg_step.mask", 3)
+        _req(image_latents, f32, f"{what}.image_latents", 4)
+        _req(noise, f32, f"{what}.noise", 4)
+        _req(mask, torch.uint8, f"{what}.mask", 3)
         if image_latents.shape != latents.shape or noise.shape != latents.shape or mask.shape != (bs, H, W):
-            raise DsEngineError("cfg_step: shape mismatch")
+            raise DsEngineError(f"{what}: shape mismatch")
         ptrs = [image_latents.data_ptr(), noise.data_ptr(), mask.data_ptr()]
     factors, phi = None, 0.0
     if rescale is not None:
         factors, phi = rescale
-        _req(factors, f32, "cfg_step.rescale_factors", 1)
-        if factors.numel() != bs:
-            raise DsEngineError("cfg_step: rescale factors must hold one value per sample")
+        _req(factors, f32, f"{what}.rescale_factors", 1)
+        if factors.numel() != rows:
+            raise DsEngineError(f"{what}: rescale factors must hold one value per sample")
         factors = factors.data_ptr()
-    check(lib.ds_cfg_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(),
-                          float(guidance), int(bool(euler)), chunks, *ptrs, factors, float(phi), bs, H * W, Cc,
-                          _stream()), "ds_cfg_step")
+    return ptrs, factors, phi
+
+
+def tile_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
+               guidance: float, euler: bool, tiles, inpaint=None, rescale=None) -> None:
+    """``cfg_step_`` on a canvas denoised as the overlapping views of ``tiles`` (a ``tiles.TileGrid``; ``ds_tile_step``),
+    in place.  latents fp32 NHWC [bs,H,W,4] is the canvas, (H, W) the grid's; noise_pred and model_in bf16
+    [k*bs*V, tile_h, tile_w, 4] hold k chunks of the V views of every canvas sample, row c*bs*V + b*V + v.  Each canvas
+    pixel becomes the mean, in view order, of the updates its covering views give it (MultiDiffusion), then the inpaint
+    blend; every covering view's rows of model_in get the next UNet input.  ``inpaint`` canvas-sized as in
+    ``cfg_step_``; ``rescale`` factors fp32 [bs*V], one per view row.  coef as in ``cfg_step_``."""
+    _req(noise_pred, bf16, "tile_step.noise_pred", 4)
+    _req(latents, f32, "tile_step.latents", 4)
+    _req(model_in, bf16, "tile_step.model_in", 4)
+    _req(coef, f32, "tile_step.coef", 1)
+    bs, H, W, Cc = latents.shape
+    rows = bs * tiles.n_views
+    chunks = noise_pred.shape[0] // rows if rows else 0
+    ncoef = (3 if euler else 2) + (0 if inpaint is None else 2) + (chunks == 3)
+    if (H, W) != (tiles.height, tiles.width) or chunks not in (2, 3) or \
+            noise_pred.shape != (chunks * rows, tiles.tile_h, tiles.tile_w, Cc) or \
+            model_in.shape != noise_pred.shape or coef.numel() != ncoef:
+        raise DsEngineError("tile_step: shape mismatch")
+    ptrs, factors, phi = _step_state("tile_step", latents, rows, inpaint, rescale)
+    check(lib.ds_tile_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(),
+                           float(guidance), int(bool(euler)), chunks, *ptrs, factors, float(phi), bs, H, W,
+                           tiles.tile_h, tiles.tile_w, tiles.stride_h, tiles.stride_w, Cc, _stream()), "ds_tile_step")
 
 
 def cfg_rescale_factors(noise_pred: torch.Tensor, coef: torch.Tensor, guidance: float,

@@ -16,6 +16,7 @@ GPU (image_processor.py).  Without them the encoders' inputs (token ids, pixel v
 raises, it does not fall back to anything.
 ``image=`` / ``strength=`` start a panel from an image as diffusers' ``StableDiffusionXLImg2ImgPipeline`` does (needs
 ``vae_encoder=``): the image is encoded, noised to the schedule's step ``t_start`` and denoised from there.
+``tile_size=`` denoises a large panel as overlapping views of a trained size (MultiDiffusion; ``tiles.py``).
 ``mask_image=`` with ``image=`` redraws only the masked part, as diffusers' ``StableDiffusionXLInpaintPipeline`` does
 with a 4-channel UNet: after every step the unmasked latent pixels are reset to the image latents noised to the next
 timestep (fused into the step kernel, ``ds_cfg_step``).  Departures from that pipeline's defaults: the
@@ -47,6 +48,7 @@ from .image_processor import (CLIPImageProcessor, VaeImageProcessor, ViTImagePro
                               adapter_image_u8)
 from .lora import AdapterRegistry, lora_targets, normalize_lora, split_components
 from .scheduler import DDIMScheduler, EulerDiscreteScheduler, get_timesteps, pag_scales, step_table, with_pag_column
+from .tiles import TILE_OVERLAP, TileGrid, check_tiles
 from .unet import AdapterResiduals, UNetMangaEngine, resolve_pag_layers
 
 bf16, f32 = torch.bfloat16, torch.float32
@@ -61,7 +63,7 @@ PANEL_KEYS = frozenset({
     "ip_image_embeds", "clip_image_embeds", "magi_image_embeds", "clip_pixel_values", "magi_pixel_values", "ip_bbox",
     "dialog_bbox", "prompt_embeds", "negative_prompt_embeds", "pooled_prompt_embeds", "negative_pooled_prompt_embeds",
     "prompt_input_ids", "prompt_input_ids_2", "negative_prompt_input_ids", "negative_prompt_input_ids_2", "image",
-    "mask_image", "padding_mask_crop", "adapter_image", "adapter_conditioning_scale"})
+    "mask_image", "padding_mask_crop", "adapter_image", "adapter_conditioning_scale", "tile_size", "tile_overlap"})
 PAGE_MAX_ROWS = 8       # samples per page denoise: a UNet batch of 16 rows, as __call__(num_samples=8)
 
 
@@ -425,17 +427,21 @@ class DiffSenseiPipeline:
                      add_time_ids: torch.Tensor, bbox: torch.Tensor, aspect_ratio: float,
                      dialog_bbox: Optional[torch.Tensor], num_inference_steps: int, guidance_scale: float,
                      use_graph: bool = True, chains: Optional[int] = None, start_index: int = 0,
-                     inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0) -> "DenoiseStepper":
+                     inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0,
+                     tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS) -> "DenoiseStepper":
         return DenoiseStepper(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                               dialog_bbox, num_inference_steps, guidance_scale, use_graph, chains, start_index,
-                              inpaint, pag, adapter, guidance_rescale)
+                              inpaint, pag, adapter, guidance_rescale, tiles, max_batch_panels)
 
     def stepper_key(self, latents, prompt_embeds, aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale,
                     chains=None, start_index: int = 0, inpaint=None, pag=None, adapter=None,
-                    guidance_rescale: float = 0.0) -> tuple:
+                    guidance_rescale: float = 0.0, tiles: Optional[TileGrid] = None,
+                    max_batch_panels: int = PAGE_MAX_ROWS) -> tuple:
         """Everything a captured stepper bakes in (``stepper_for``), FreeU's values (``unet.freeu``) and whether a
         T2I-Adapter's features are added included.  With ``guidance_rescale > 0`` the key ends with its value, which
-        the graph bakes in like ``guidance_scale``; otherwise the key is the one the step without the rescale has."""
+        the graph bakes in like ``guidance_scale``; otherwise the key is the one the step without the rescale has.
+        With ``tiles`` it ends with the view grid and the UNet slice size (``max_batch_panels``); without, neither is
+        in it."""
         key = (tuple(latents.shape), tuple(prompt_embeds.shape), None if dialog_bbox is None else
                 (tuple(dialog_bbox.shape), dialog_bbox.dtype == bf16), float(aspect_ratio), int(num_inference_steps),
                 float(guidance_scale), self.unet.scales_key(), chains, self.unet._ip_weights_version(),
@@ -444,11 +450,14 @@ class DiffSenseiPipeline:
                 adapter is not None)
         if guidance_rescale > 0:
             key += (("guidance_rescale", float(guidance_rescale)),)
+        if tiles is not None:
+            key += (("tiles", tiles, int(max_batch_panels)),)
         return key
 
     def stepper_for(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio, dialog_bbox,
                     num_inference_steps, guidance_scale, chains=None, start_index: int = 0,
-                    inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0) -> "DenoiseStepper":
+                    inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0,
+                    tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS) -> "DenoiseStepper":
         """A graph-captured stepper loaded with this panel: a cached one of the same key is refilled in place
         (no re-capture), otherwise a new one is built and cached.  The start index is part of the key: the stepper
         bakes in its slice of the schedule (``set_timesteps`` would reset any scheduler state); so is whether it
@@ -457,12 +466,12 @@ class DiffSenseiPipeline:
         scales are not: they live in the coefficient table, which ``load_panel`` rewrites, as it rewrites the adapter
         features and gates."""
         key = self.stepper_key(latents, prompt_embeds, aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale,
-                               chains, start_index, inpaint, pag, adapter, guidance_rescale)
+                               chains, start_index, inpaint, pag, adapter, guidance_rescale, tiles, max_batch_panels)
         st = self._steppers.get(key)
         if st is None:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                    dialog_bbox, num_inference_steps, guidance_scale, True, chains, start_index,
-                                   inpaint, pag, adapter, guidance_rescale)
+                                   inpaint, pag, adapter, guidance_rescale, tiles, max_batch_panels)
             while len(self._steppers) >= self.max_cached_steppers:
                 self._steppers.pop(next(iter(self._steppers)))
             self._steppers[key] = st
@@ -476,7 +485,8 @@ class DiffSenseiPipeline:
                 add_time_ids: torch.Tensor, bbox: torch.Tensor, aspect_ratio: float,
                 dialog_bbox: Optional[torch.Tensor], num_inference_steps: int, guidance_scale: float,
                 use_graph: bool = True, on_step=None, start_index: int = 0, inpaint=None, pag_scale: float = 0.0,
-                pag_adaptive_scale: float = 0.0, adapter=None, guidance_rescale: float = 0.0) -> torch.Tensor:
+                pag_adaptive_scale: float = 0.0, adapter=None, guidance_rescale: float = 0.0,
+                tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS) -> torch.Tensor:
         """pipeline_diffsensei.py:306-337.  ``latents`` NCHW fp32 (bs,4,h,w); conditions already concatenated
         [negative ; positive] along batch (:293-304), or [negative ; positive ; positive] with perturbed-attention
         guidance (``pag_scale > 0``: diffusers' PAGMixin; the third chunk takes the identity attention map at the
@@ -486,19 +496,24 @@ class DiffSenseiPipeline:
         0 become the image latents noised to the next timestep (the image latents on the last step).  ``adapter``:
         (features, gates), T2I-Adapter features bf16 NHWC [bs, h, w, c] (one row per sample, every UNet row of the
         sample gets it) and per loop step a gate, 1.0 (added) or 0.0 (``DenoiseStepper``).  ``guidance_rescale > 0``:
-        diffusers' ``rescale_noise_cfg`` on the guided eps of every sample before the scheduler step.  Returns the
-        final latents, NCHW fp32."""
+        diffusers' ``rescale_noise_cfg`` on the guided eps of every sample before the scheduler step.  ``tiles``: a
+        ``TileGrid`` (MultiDiffusion): ``latents`` is the canvas and the conditions (and ``adapter`` may not be given)
+        have one row per view of every sample, row b * V + v of each chunk, ``aspect_ratio`` the view's; the UNet runs
+        the view rows in slices of at most ``max_batch_panels`` view-samples, and ``ds_tile_step`` averages the views'
+        updates on the canvas.  Returns the final latents, NCHW fp32."""
         guidance_rescale = check_guidance_rescale(guidance_rescale)
         self.unet.set_lora_scale(1.0)            # a direct unet(..., cross_attention_kwargs={"scale": s}) call may have left s
         pag = self._pag(pag_scale, pag_adaptive_scale)
         if use_graph:
             st = self.stepper_for(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                   dialog_bbox, num_inference_steps, guidance_scale, start_index=start_index,
-                                  inpaint=inpaint, pag=pag, adapter=adapter, guidance_rescale=guidance_rescale)
+                                  inpaint=inpaint, pag=pag, adapter=adapter, guidance_rescale=guidance_rescale,
+                                  tiles=tiles, max_batch_panels=max_batch_panels)
         else:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                    dialog_bbox, num_inference_steps, guidance_scale, False, start_index=start_index,
-                                   inpaint=inpaint, pag=pag, adapter=adapter, guidance_rescale=guidance_rescale)
+                                   inpaint=inpaint, pag=pag, adapter=adapter, guidance_rescale=guidance_rescale,
+                                   tiles=tiles, max_batch_panels=max_batch_panels)
         for i, t in enumerate(st.timesteps):
             st.step(i)
             if on_step is not None:
@@ -533,7 +548,9 @@ class DiffSenseiPipeline:
                  adapter_image=None, adapter_conditioning_scale: float = 1.0,
                  adapter_conditioning_factor: float = 1.0,
                  # diffusers' rescale_noise_cfg (Lin et al., sec. 3.4) after the guidance blend: on when > 0
-                 guidance_rescale: float = 0.0):
+                 guidance_rescale: float = 0.0,
+                 # MultiDiffusion (diffusers' StableDiffusionPanoramaPipeline): denoise as overlapping views of this size
+                 tile_size=None, tile_overlap: int = TILE_OVERLAP):
         """A page of one panel: ``generate_page([panel], ...)[0]``, the panel holding this call's per-panel keywords
         (``PANEL_KEYS``) and the page the others.  Its input errors carry no panel index."""
         args = locals()
@@ -670,7 +687,14 @@ class DiffSenseiPipeline:
         (``rescale_noise_cfg``, Lin et al. 2024, sec. 3.4): eps <- phi * eps * std(text eps) / std(eps) +
         (1 - phi) * eps, the standard deviations over the sample's C x H x W values, with PAG's term included in eps
         and before the scheduler step and the inpaint blend.  It counters the over-exposure of high guidance
-        scales; diffusers' pipelines suggest 0.7."""
+        scales; diffusers' pipelines suggest 0.7.
+
+        A panel with ``tile_size`` (an int or ``(height, width)`` in pixels; ``tile_overlap``, default 256) is denoised
+        as overlapping views of that size, MultiDiffusion (Bar-Tal et al. 2023) as diffusers'
+        ``StableDiffusionPanoramaPipeline`` runs it (``tiles.TileGrid``; ``_tile_rows`` gives each view's conditions):
+        every step the UNet runs all views, ``max_batch_panels`` view-samples per call, and ``ds_tile_step`` averages
+        the views' updated latents on the canvas before the inpaint blend.  A tiled panel is a denoise of its own; its
+        noise, image and mask are canvas-sized as untiled, and the canvas is decoded whole."""
         if not isinstance(panels, (list, tuple)) or len(panels) == 0:
             raise ValueError("generate_page needs a non-empty list of panel dicts")
         panels = [dict(p) for p in panels]
@@ -747,9 +771,11 @@ class DiffSenseiPipeline:
         results = [None] * len(jobs)
         kind = lambda j: (() if j.image is None else ("inpaint",) if j.mask_image is not None else ("image",)) + \
             (() if j.adapter_feats is None else ("adapter",))
-        shapes = [(j.ns,) + tuple(j.latents.shape[-2:]) + kind(j) for j in jobs]
+        alone = lambda i: () if jobs[i].tiles is None else (("tiles", i),)    # a tiled panel is a denoise of its own
+        shapes = [(j.ns,) + tuple(j.latents.shape[-2:]) + kind(j) + alone(i) for i, j in enumerate(jobs)]
         for chunk in plan_page(shapes, max_batch_panels):
-            rows = [self._panel_rows(jobs[i]) for i in chunk]
+            tiles = jobs[chunk[0]].tiles
+            rows = [self._panel_rows(jobs[i]) if tiles is None else self._tile_rows(jobs[i]) for i in chunk]
             # [negatives ; positives], and the positives again as the perturbed block with PAG (diffusers' PAGMixin)
             sides = (0, 1, 1) if self.do_perturbed_attention_guidance else (0, 1)
             cat = lambda k: torch.cat([r[side][k] for side in sides for r in rows], dim=0)
@@ -763,11 +789,13 @@ class DiffSenseiPipeline:
                          for k in range(len(jobs[chunk[0]].adapter_feats))]
                 steps = num_inference_steps - (t_start if jobs[chunk[0]].image is not None else 0)
                 adapter = (feats, [1.0 if i < ad_steps else 0.0 for i in range(steps)])   # i: the loop's step
-            final = self.denoise(lat, cat("pe"), cat("te"), cat("ti"), cat("bbox"), lat.shape[-2] / lat.shape[-1],
+            aspect = lat.shape[-2] / lat.shape[-1] if tiles is None else tiles.tile_h / tiles.tile_w
+            tiled = {} if tiles is None else dict(tiles=tiles, max_batch_panels=max_batch_panels)
+            final = self.denoise(lat, cat("pe"), cat("te"), cat("ti"), cat("bbox"), aspect,
                                  cat("db"), num_inference_steps, guidance_scale, use_graph=use_graph,
                                  start_index=t_start if jobs[chunk[0]].image is not None else 0, inpaint=inpaint,
                                  pag_scale=pag_scale, pag_adaptive_scale=pag_adaptive_scale, adapter=adapter,
-                                 guidance_rescale=guidance_rescale)
+                                 guidance_rescale=guidance_rescale, **tiled)
             # pipeline_diffsensei.py:339-363: latents / scaling_factor -> vae.decode -> image_processor.postprocess
             image = self.vae.decode_image(final) if output_type != "latent" else final
             r0 = 0
@@ -822,6 +850,10 @@ class DiffSenseiPipeline:
         height, width = g("height"), g("width")
         if g("mask_image") is not None and g("image") is None:
             raise ValueError("`mask_image` needs `image`: inpainting redraws the masked part of that image")
+        if g("tile_size") is not None:
+            for k in ("adapter_image", "padding_mask_crop"):
+                if g(k) is not None:
+                    raise ValueError(f"`tile_size` and `{k}` can not be input together")
         crop = mask_l = None
         ad_image = g("adapter_image")
         ad_scale = g("adapter_conditioning_scale", 1.0)
@@ -860,6 +892,7 @@ class DiffSenseiPipeline:
                                  f"got {ad_h} x {ad_w}")
         height = height or self.default_sample_size * self.vae_scale_factor
         width = width or self.default_sample_size * self.vae_scale_factor
+        tiles = check_tiles(g("tile_size"), g("tile_overlap", TILE_OVERLAP), height, width, self.vae_scale_factor)
         ip_images, ip_bbox = list(g("ip_images", ())), list(g("ip_bbox", ()))
         ip_image_embeds = g("ip_image_embeds")
         if len(ip_images) > 0:
@@ -915,7 +948,7 @@ class DiffSenseiPipeline:
             ns=int(g("num_samples", 1)), height=height, width=width, generator=g("generator"), latents=g("latents"),
             ids=ids, image=g("image"), mask_image=g("mask_image"), inpaint=None, crop=crop, mask_l=mask_l,
             adapter_image=ad_image, adapter_scale=float(ad_scale), adapter_float=ad_image is not None and ad_float,
-            adapter_feats=None,
+            adapter_feats=None, tiles=tiles,
             pe=g("prompt_embeds"), npe=g("negative_prompt_embeds"), pp=g("pooled_prompt_embeds"),
             npp=g("negative_pooled_prompt_embeds"), ip_images=ip_images, clip_pv=clip_pv, magi_pv=magi_pv,
             clip=g("clip_image_embeds"), magi=g("magi_image_embeds"), ip_image_embeds=ip_image_embeds,
@@ -1053,6 +1086,33 @@ class DiffSenseiPipeline:
                                               db=d)
         return side(j.npe, j.npp, neg_img, neg_bbox, neg_db), side(j.pe, j.pp, img, bbox, db)
 
+    def _tile_rows(self, j):
+        """A tiled panel's [negative, positive] condition rows: one per view of every sample, row b * V + v.  Each
+        view takes the panel's prompt and character embeddings; its ``ip_bbox`` / ``dialog_bbox`` are the panel's
+        mapped into the view by ``crop_boxes`` (the view as the crop, at scale 1, clamped to [0, 1]), a box without a
+        positive-area overlap dropped, with its character's image tokens, and the rest moved up and re-padded as a
+        panel with fewer characters is; its SDXL time ids are the panel's ``original_size``, the panel's
+        ``crops_coords_top_left`` plus the view's (top, left) pixel offset, and the tile as ``target_size``."""
+        g, s = j.tiles, self.vae_scale_factor
+        th, tw = g.tile_h * s, g.tile_w * s
+        nv, m = self.unet.cfg.num_vision_tokens, self.unet.cfg.max_num_ips
+        views = ([], [])
+        for top, left in g.views:
+            y0, x0 = top * s, left * s
+            crop = (x0, y0, x0 + tw, y0 + th)
+            db, _ = crop_boxes(j.dialog_bbox, crop, (j.height, j.width), (th, tw))
+            ib, keep = crop_boxes(j.ip_bbox[:m], crop, (j.height, j.width), (th, tw))
+            img = j.img
+            if len(keep) < len(j.ip_bbox[:m]):          # the kept characters' tokens, then the zero characters' padding
+                img = j.neg_img.clone()
+                for k, i in enumerate(keep):
+                    img[:, (1 + k) * nv:(2 + k) * nv] = j.img[:, (1 + i) * nv:(2 + i) * nv]
+            ti = list(j.time_ids[:2]) + [j.time_ids[2] + y0, j.time_ids[3] + x0, th, tw]
+            v = SimpleNamespace(**{**vars(j), "ns": 1, "img": img, "ip_bbox": ib, "dialog_bbox": db, "time_ids": ti})
+            for side, rows in zip(views, self._panel_rows(v)):
+                side.append(rows)
+        return tuple({k: torch.cat([torch.cat([r[k] for r in side])] * j.ns) for k in side[0]} for side in views)
+
     def _check_agent_panels(self, panels, tokenizer_mllm) -> None:
         """The host-only checks of the ``agent=`` path (each panel's own checks follow: ``_panel_job``)."""
         if tokenizer_mllm is None:
@@ -1123,12 +1183,18 @@ class DenoiseStepper:
     With ``guidance_rescale`` > 0 each step first computes the per-sample factors of diffusers' ``rescale_noise_cfg``
     from the UNet's eps (``ops.cfg_rescale_factors``, into a [bs] buffer allocated once), then runs the step with the
     rescale; both launches are in the captured graph, which bakes in the value as it does ``guidance_scale``.
+    With ``tiles`` (a ``TileGrid``, MultiDiffusion) the fp32 master latents are the canvas and ``model_in`` holds the
+    k chunks of its view rows (row b * V + v of each chunk; ``load_panel`` gathers the first input on the host); a
+    step runs the UNet on the view rows in slices of at most k * ``max_batch_panels`` rows, one after another into
+    slices of one eps buffer, then ``ds_tile_step`` (with the factors of every view row when rescaling).  Every kernel
+    gives a row the same bits whatever batch surrounds it, so the slicing changes no bit.
     """
 
     @torch.no_grad()
     def __init__(self, pipe: DiffSenseiPipeline, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox,
                  aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale, use_graph=True, chains=None,
-                 start_index: int = 0, inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0):
+                 start_index: int = 0, inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0,
+                 tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS):
         unet, dev = pipe.unet, pipe.unet.device
         self.unet, self.dev, self.guidance = unet, dev, float(guidance_scale)
         self.scheduler = pipe.scheduler
@@ -1154,13 +1220,16 @@ class DenoiseStepper:
         self.graph = None
         self.has_adapter = adapter is not None
         self.ad_feats = self.ad_gates = None
+        self.tiles = tiles
+        if tiles is not None and (adapter is not None or int(max_batch_panels) < 1):
+            raise ValueError("a tiled denoise takes no adapter features, and max_batch_panels must be >= 1")
         self.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox, inpaint, pag,
                         adapter)
         rescale = check_guidance_rescale(guidance_rescale)
         self.guidance_rescale = rescale if rescale > 0 else 0.0
         self.rescale_factors = None
-        if self.guidance_rescale > 0:
-            self.rescale_factors = torch.empty(self.lat.shape[0], dtype=f32, device=dev)
+        if self.guidance_rescale > 0:                 # one factor per sample, or per view row of a tiled canvas
+            self.rescale_factors = torch.empty(self.model_in.shape[0] // self.n_chunks, dtype=f32, device=dev)
         self.temb_cur = self.temb_table[0].clone()
         self.ad_gate_cur = None if adapter is None else self.ad_gates[0].clone()
         self.coef_cur = self.coef_table[0].clone()
@@ -1175,8 +1244,13 @@ class DenoiseStepper:
         self.chains = max(1, min(want, B2))
         self._parts, self._side = [(0, B2)], []
         # first perturbed row of the whole batch (None: no PAG); each part gets it relative to its own slice
-        self._pag_row0 = None if pag is None else 2 * self.lat.shape[0]
-        if self.chains > 1:
+        self._pag_row0 = None if pag is None else 2 * (B2 // self.n_chunks)
+        if tiles is not None:                       # UNet slices of at most max_batch_panels view-samples' rows
+            cap, self.chains = self.n_chunks * int(max_batch_panels), 1
+            self._parts = [(r, min(r + cap, B2)) for r in range(0, B2, cap)]
+            self._cond_parts = [self.cond.rows(s, e) for s, e in self._parts]
+            self._eps = torch.empty_like(self.model_in)
+        elif self.chains > 1:
             cuts = [round(k * B2 / self.chains) for k in range(self.chains + 1)]
             self._parts = [(cuts[k], cuts[k + 1]) for k in range(self.chains) if cuts[k + 1] > cuts[k]]
             self._cond_parts = [self.cond.rows(s, e) for s, e in self._parts]
@@ -1207,9 +1281,15 @@ class DenoiseStepper:
         unet, dev = self.unet, self.dev
         bs = latents.shape[0]
         k = self.n_chunks
+        rows = bs if self.tiles is None else bs * self.tiles.n_views      # UNet rows per chunk
+        if self.tiles is not None and tuple(latents.shape[-2:]) != (self.tiles.height, self.tiles.width):
+            raise ValueError("load_panel: the latents are not the tile grid's canvas")
         if (pag is None) != (self.pag_sites is None) or (pag is not None and frozenset(pag[0]) != self.pag_sites):
             raise ValueError("load_panel: perturbed-attention sites differ from the stepper's")
-        if prompt_embeds.shape[0] != k * bs:
+        if prompt_embeds.shape[0] != k * rows:
+            if self.tiles is not None:
+                raise ValueError("a tiled denoise expects one condition row per view of every sample in each chunk: "
+                                 "prompt_embeds.shape[0] == chunks * num_samples * views")
             if k == 2:
                 raise ValueError("denoise expects CFG-concatenated conditions: prompt_embeds.shape[0] == 2 * "
                                  "num_samples")
@@ -1252,7 +1332,7 @@ class DenoiseStepper:
         self.cond = unet.prepare_conditions(prompt_embeds.to(dev), bbox, self.aspect_ratio, out=self.cond)
         self.temb_table = unet.time_rowbias_table(self.timesteps, add_text_embeds, add_time_ids)   # [T, 2bs, sumC]
         lat = latents.to(device=dev, dtype=f32).permute(0, 2, 3, 1).contiguous()         # fp32 NHWC master copy
-        x = lat / self.in_div[0]                                                        # :317 (x / 1.0 for DDIM)
+        x = self._rows(lat / self.in_div[0])                                            # :317 (x / 1.0 for DDIM)
         first = self.lat is None
         if first:
             self.lat = lat
@@ -1262,7 +1342,7 @@ class DenoiseStepper:
                 raise ValueError("load_panel: latent shape / dialog_bbox presence differs from the captured panel")
             self.lat.copy_(lat)
             for c in range(k):
-                self.model_in[c * bs:(c + 1) * bs].copy_(x)
+                self.model_in[c * rows:(c + 1) * rows].copy_(x)
         if dialog_bbox is not None:
             rb = dialog_bbox.dtype == bf16
             db = dialog_bbox.to(device=dev, dtype=f32).contiguous()
@@ -1272,6 +1352,10 @@ class DenoiseStepper:
                 if rb != self.round_bf16 or db.shape != self.db.shape:
                     raise ValueError("load_panel: dialog_bbox dtype / shape differs from the captured panel")
                 self.db.copy_(db)
+
+    def _rows(self, x: torch.Tensor) -> torch.Tensor:
+        """The UNet rows of one chunk from NHWC latents: the latents themselves, or a tiled canvas's view rows."""
+        return x if self.tiles is None else self.tiles.gather(x)
 
     def _pag_args(self, s: int, e: int) -> dict:
         """forward_nhwc's PAG keywords for batch rows [s, e): the first perturbed row relative to the slice."""
@@ -1290,6 +1374,12 @@ class DenoiseStepper:
             eps = self.unet.forward_nhwc(self.model_in, self.temb_cur, self.cond, self.db, self.round_bf16,
                                          **self._pag_args(0, self.model_in.shape[0]),
                                          **self._adapter_args(0))                                          # :322-329
+        elif self.tiles is not None:                   # the view rows' slices, one after another, into one buffer
+            eps = self._eps
+            for k, (s, e) in enumerate(self._parts):
+                self.unet.forward_nhwc(self.model_in[s:e], self.temb_cur[s:e], self._cond_parts[k],
+                                       None if self.db is None else self.db[s:e], self.round_bf16, out=eps[s:e],
+                                       **self._pag_args(s, e))
         else:
             main = torch.cuda.current_stream(self.dev)
             eps = self._eps
@@ -1312,13 +1402,14 @@ class DenoiseStepper:
                 ops.SPLITK = prev_splitk
                 ops.GEMM_CHAINS = prev_chains
         inpaint = (self.inp_z, self.inp_n, self.inp_m) if self.inpaint else None
+        tiled = {} if self.tiles is None else dict(tiles=self.tiles)
         if self.guidance_rescale > 0:                  # diffusers' rescale_noise_cfg, before the scheduler step
             ops.cfg_rescale_factors(eps, self.coef_cur, self.guidance, out=self.rescale_factors)
             self.scheduler.fused_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance, inpaint,
-                                       (self.rescale_factors, self.guidance_rescale))
+                                       (self.rescale_factors, self.guidance_rescale), **tiled)
         else:
             self.scheduler.fused_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance,  # :332-337,:315-317
-                                       inpaint)
+                                       inpaint, **tiled)
 
     @torch.no_grad()
     def step(self, i: int) -> None:
@@ -1339,10 +1430,10 @@ class DenoiseStepper:
         self._host_in.copy_(latents_host, non_blocking=True)                            # H2D
         nhwc = self._host_in.permute(0, 2, 3, 1)
         self.lat.copy_(nhwc)
-        bs = self.lat.shape[0]
-        x = nhwc / self.in_div[i]                                                       # step i's scale_model_input
+        x = self._rows(nhwc / self.in_div[i])                                           # step i's scale_model_input
+        rows = x.shape[0]
         for c in range(self.n_chunks):
-            self.model_in[c * bs:(c + 1) * bs].copy_(x)
+            self.model_in[c * rows:(c + 1) * rows].copy_(x)
         self.step(i)
         out_host.copy_(self.lat.permute(0, 3, 1, 2), non_blocking=True)                 # D2H
         torch.cuda.current_stream(self.dev).synchronize()

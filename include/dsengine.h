@@ -391,6 +391,26 @@ int ds_cfg_step(const void* noise_pred, float* latents, void* model_in, const fl
 int ds_cfg_rescale_factors(const void* noise_pred, const float* coef, int ncoef, float guidance, int chunks,
                            float* factors, int bs, int HW, int C, void* stream);
 
+/* ds_tile_step: ds_cfg_step on a canvas denoised as overlapping views (MultiDiffusion, Bar-Tal et al. 2023; diffusers'
+ * StableDiffusionPanoramaPipeline).                                                [HBM-bound]
+ *   latents       : fp32 NHWC [bs][H][W][4], the canvas (updated in place)
+ *   noise_pred    : bf16 NHWC [chunks * bs * V][tile_h][tile_w][4], model_in the same shape; row c * bs * V + b * V + v
+ *                   is chunk c of view v of canvas sample b
+ *   views         : per axis n = ceil((dim - tile) / stride) + 1 views, view k at min(k * stride, dim - tile) (the last
+ *                   flush with the far edge); V = n_h * n_w in row-major order; 0 < stride <= tile <= dim
+ *   image_latents / noise / mask : canvas-sized as in ds_cfg_step (all three or none)
+ *   rescale_factors : NULL or fp32 [bs * V], one factor per view row (ds_cfg_rescale_factors over the view rows)
+ *   update, chunks, coef, guidance, guidance_rescale : as ds_cfg_step
+ * Per canvas pixel: each covering view, in view order, gives x_v = ds_cfg_step's update of the canvas pixel from that
+ * view's eps (and that view's factor); x_new = (0 + x_v1 + x_v2 + ...) / count in fp32, each sum and the division
+ * rounded on their own (one view: ds_cfg_step's bits); then the inpaint blend on the canvas pixel; then the canvas and
+ * the next UNet input (ds_cfg_step's) in every chunk of every covering view.  No atomics: every output element is
+ * written by one thread once. */
+int ds_tile_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance, int update,
+                 int chunks, const float* image_latents, const float* noise, const uint8_t* mask,
+                 const float* rescale_factors, double guidance_rescale, int bs, int H, int W, int tile_h, int tile_w,
+                 int stride_h, int stride_w, int C, void* stream);
+
 /* Perceiver attention of the character Resampler: 16 latent queries x (n_kv) keys per (character, head),
  * q and k each pre-scaled by dim_head^-0.25, fp32 softmax (src/models/resampler.py:64-74).
  *   q: bf16 [Bc][nq][C], kv: bf16 [Bc][n_kv][2*C] (k | v), out: bf16 [Bc][nq][C]; C = heads*64 */
