@@ -23,6 +23,7 @@ struct DeviceInfo {
   int num_sms;
   int cc_major;
   int cc_minor;
+  int smem_optin;   // dynamic shared memory a block may opt in to, bytes
 };
 bool get_device(DeviceInfo* out);
 

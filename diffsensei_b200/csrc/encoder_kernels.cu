@@ -2,8 +2,9 @@
 // the CLIP ViT-H and Magi ViT-MAE image encoders of prepare_ip_image_embeds, src/pipelines/pipeline_diffsensei.py:125-128,
 // and the two SDXL CLIP text encoders of encode_prompt, :232-245).  Their linears / MLPs run on the wgmma GEMM
 // (ds_gemm_bf16, bias / GELU / quick-GELU / residual epilogues) and their LayerNorms on ds_layernorm; this file adds
-//   ds_attention_small : softmax(scale * Q K^T [+ causal mask]) V for SHORT sequences (<= 320 keys) and any head
-//                        width that is a multiple of 8 up to 128 — 77 text tokens (causal), 197 / 257 image tokens, heads
+//   ds_attention_small : softmax(scale * Q K^T [+ causal mask]) V for SHORT sequences (<= 320 keys, fewer above head
+//                        width 168: K and V must fit in shared memory) and any head width that is a multiple of 8 up
+//                        to 256 — 77 text tokens (causal), 197 / 257 image tokens, heads
 //                        of 64 (text, ViT-MAE) and 80 (ViT-H, outside the flash kernel's head_dim 64).  These encoders
 //                        run once per panel (1.3 TFLOP of GEMMs for four 224x224 character crops, 43 GFLOP of
 //                        attention), so the attention is a plain CUDA-core kernel: K / V of one (batch, head) staged
@@ -141,7 +142,13 @@ extern "C" int ds_attention_small(const void* q, const void* k, const void* v, v
   if (!get_device(&dev)) return DS_ERR_CUDA;
   const int hw = head_dim / 2;
   const int row_words = (hw & 1) ? hw : hw + 1;
-  const size_t smem = static_cast<size_t>(2) * Nk * row_words * 4 + 4 * head_dim * 4 + static_cast<size_t>(4) * Nk * 4;
+  // K and V rows [Nk][row_words] words, the 4 warps' q rows [4][hd] and probabilities [4][Nk] floats
+  const size_t per_key = static_cast<size_t>(2) * row_words * 4 + 4 * 4;
+  const size_t smem = per_key * Nk + 4 * head_dim * 4;
+  DS_REQUIRE(smem <= static_cast<size_t>(dev.smem_optin),
+             "ds_attention_small: %d keys at head_dim %d need %zu bytes of shared memory > %d; at most %d keys fit",
+             Nk, head_dim, smem, dev.smem_optin,
+             static_cast<int>((static_cast<size_t>(dev.smem_optin) - 4 * head_dim * 4) / per_key));
   static size_t attr[kMaxDevices] = {};
   if (smem > 48 * 1024 && smem > attr[device_slot()]) {
     DS_CUDA_OK(cudaFuncSetAttribute(attention_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));

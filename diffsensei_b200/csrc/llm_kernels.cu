@@ -389,9 +389,13 @@ __global__ void silu_mul_kernel(const uint4* __restrict__ gu, uint4* __restrict_
 // ----------------------------------------------------------------------------------------------- next token
 constexpr int kTokThreads = 1024;
 
-// (value, index) argmax of one block; ties go to the smaller index (torch.argmax)
+// (value, index) argmax of one block, ranked as torch.argmax ranks: NaN above every number, ties (NaN included) to
+// the smaller index.  The merge is order-independent, so the index is the first maximum however the block splits V,
+// and any V > 0 yields an index in [0, V).
 __device__ __forceinline__ void argmax_merge(float& v, int& i, float v2, int i2) {
-  if (v2 > v || (v2 == v && i2 < i)) { v = v2; i = i2; }
+  const bool n = isnan(v), n2 = isnan(v2);
+  const bool take = n2 != n ? n2 : (v2 > v || ((n || v2 == v) && i2 < i));
+  if (take) { v = v2; i = i2; }
 }
 
 __device__ __forceinline__ void block_argmax(const float* s, int V, float* sv, int* si, float& best_v, int& best_i) {

@@ -795,7 +795,8 @@ def cfg_rescale_factors(noise_pred: torch.Tensor, coef: torch.Tensor, guidance: 
 # ---------------------------------------------------------------------------------------------- encoder helpers
 def attention_small(qkv: torch.Tensor, heads: int, causal: bool = False, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """softmax(Q K^T / sqrt(d) [+ causal]) V from a fused projection ``qkv`` [B, N, 3*heads*d] (N <= 320, d % 8 == 0,
-    d <= 128) -> [B, N, heads*d].  The short-sequence attention of the CLIP / ViT-MAE encoders."""
+    d <= 256, fewer keys above d = 168: include/dsengine.h) -> [B, N, heads*d].  The short-sequence attention of the
+    CLIP / ViT-MAE encoders."""
     _req(qkv, bf16, "attention_small.qkv", 3)
     B, N, C3 = qkv.shape
     if C3 % (3 * heads) != 0:

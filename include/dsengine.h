@@ -463,7 +463,10 @@ int ds_attention_single_head(const void* q, const void* k, const void* v, void* 
  * Their linears run on ds_gemm_bf16 and their LayerNorms on ds_layernorm.                    [latency-bound]
  *   ds_attention_small : out = softmax(scale * Q K^T [+ causal mask]) V for short sequences (Nk <= 320) and any
  *                        head_dim that is a multiple of 8 up to 256 (80 for ViT-H, 160 for the MLLM input resampler: outside the flash
- *                        kernel's 64).
+ *                        kernel's 64), as long as K and V of one head fit in shared memory: the kernel needs
+ *                        8 Nk rw + 16 head_dim + 16 Nk bytes (rw = head_dim / 2 rounded up to odd) within the device's
+ *                        opt-in limit (227 KB on the H100), so head_dim <= 168 takes all 320 keys, 176 up to 315,
+ *                        192 up to 289 and 256 up to 217.  A larger launch is rejected with DS_ERR_INVALID.
  *                        q/k/v/out: bf16 [B][N][ld*] with head h at columns [h*head_dim, (h+1)*head_dim); the row
  *                        strides ld* are in elements, so q/k/v may point into one fused [B][N][3C] projection.
  *                        causal != 0: key j visible from query i iff j <= i (CLIP text), needs Nq == Nk.
@@ -575,7 +578,8 @@ int ds_vae_overlay(const float* image, int n, int h, int w, const uint8_t* init,
  *                        NULL); the image-token rule of AutoImageTokenGenerationProcessor (src/models/mllm/
  *                        generation.py:18-30) on logits fp32 [V], IN PLACE: if `last` is in img_ids[0 .. n_img-2],
  *                        the next entry's score becomes max + 10, else the scores of img_ids[1 ..] become 0.0; then
- *                        tok = argmax (first index on ties); out_ids[generated] = tok; next_x = embed[tok] (bf16
+ *                        tok = argmax as torch.argmax takes it (NaN ranks above every number; first index on
+ *                        ties); out_ids[generated] = tok; next_x = embed[tok] (bf16
  *                        [V][C]); pos += 1; generated += 1; last = tok; done = (tok == eos || generated >= max_new).
  * B sequences decoded together, one row each (B <= 8 in the engine, the GEMV's limit).  Row b has its own position
  * pos[b * pos_stride] (device int32; the engine passes its [B][4] state with pos_stride 4) and its own cache slice
