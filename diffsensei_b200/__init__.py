@@ -5,6 +5,8 @@ Public surface (mirrors the reference's, SURVEY.md §8b):
     AttnProcessor2_0, MaskedIPAttnProcessor2_0  <- src/models/attention_processor.py
     ResamplerEngine        <- src/models/resampler.py       Resampler
     VaeDecoderEngine       <- diffusers AutoencoderKL.decode as used by pipeline_diffsensei.py:339-363
+    TinyVaeDecoderEngine, TinyVaeConfig  <- diffusers AutoencoderTiny.decode (TAESDXL), a cheap drop-in ``vae`` for
+                              previews (``callback_on_step_end``) and drafts
     VaeEncoderEngine, VaeImageProcessor  <- diffusers AutoencoderKL.encode + VaeImageProcessor.preprocess, for
                               img2img (``DiffSenseiPipeline(vae_encoder=...)(image=..., strength=...)``)
     ClipTextEncoderEngine, ClipVisionEncoderEngine, VitMaeEncoderEngine  <- transformers CLIP / ViT-MAE encoders as
@@ -36,6 +38,7 @@ from .pipeline import DiffSenseiPipeline  # noqa: F401
 from .resampler import QwenResamplerEngine, ResamplerEngine  # noqa: F401
 from .scheduler import DDIMScheduler, EulerDiscreteScheduler, get_timesteps, scheduler_from_config  # noqa: F401
 from .unet import UNet2DConditionOutput, UNetMangaEngine  # noqa: F401
+from .tiny_vae import TinyVaeConfig, TinyVaeDecoderEngine  # noqa: F401
 from .vae import VaeDecoderEngine, VaeEncoderEngine  # noqa: F401
 
 __version__ = "0.1.0"

@@ -92,6 +92,9 @@ SIGNATURES = {
     "ds_latent_pointwise": [_vp, _vp, _vp, _vp, _f, _i, _i, _vp],
     "ds_softmax_rows": [_vp, _vp, _i, _i, _i64, _i64, _f, _vp],
     "ds_image_postprocess": [_vp, _vp, _i, _i, _i, _vp],
+    "ds_tiny_latent_in": [_vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp],
+    "ds_tiny_conv64": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp],
+    "ds_tiny_conv_out": [_vp, _vp, _vp, _vp, _i, _i, _i, _vp],
     "ds_attention_single_head": [_vp, _vp, _vp, _vp, _i, _i, _i, _i64, _vp],
     "ds_image_preprocess": [_vp, _vp, _vp, _i, _i, _vp, _vp, _i64, _vp],
     "ds_vae_preprocess": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i64, _vp],

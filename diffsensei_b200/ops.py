@@ -1137,6 +1137,88 @@ def image_postprocess(x: torch.Tensor) -> torch.Tensor:
     return out
 
 
+# ---------------------------------------------------------------------------------------------- tiny VAE decoder
+def _req_aligned(t: torch.Tensor, n: int, name: str) -> None:
+    if t.data_ptr() % n:
+        raise DsEngineError(f"{name}: data must be {n}-byte aligned")
+
+
+def tiny_latent_in(latents: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, inv_scale: float = 1.0) -> torch.Tensor:
+    """DecoderTiny's first layer on ``x = latents * inv_scale``, ReLU(conv3x3(tanh(x / 3) * 3) + bias): fp32 NCHW
+    [B, 4, H, W] -> bf16 NHWC
+    [B, H, W, 64]; ``w`` fp32 [64, 3, 3, 4] (OIHW permuted to OHWI), ``bias`` fp32 [64] (ds_tiny_latent_in)."""
+    _req(latents, f32, "tiny_latent_in.latents", 4)
+    B, Cc, H, W = latents.shape
+    _req(w, f32, "tiny_latent_in.w", 4)
+    _req(bias, f32, "tiny_latent_in.bias", 1)
+    if Cc != 4 or tuple(w.shape) != (64, 3, 3, 4) or tuple(bias.shape) != (64,):
+        raise DsEngineError(f"tiny_latent_in: latents must be [B, 4, H, W], w [64, 3, 3, 4] and bias [64], got "
+                            f"{tuple(latents.shape)}, {tuple(w.shape)}, {tuple(bias.shape)}")
+    out = torch.empty(B, H, W, 64, dtype=bf16, device=latents.device)
+    check(lib.ds_tiny_latent_in(latents.data_ptr(), w.data_ptr(), bias.data_ptr(), out.data_ptr(), float(inv_scale), B,
+                               H, W, _stream()),
+          "ds_tiny_latent_in")
+    return out
+
+
+def tiny_conv64(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, *,
+                residual: Optional[torch.Tensor] = None, relu: bool = False, upsample2: bool = False,
+                out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """3x3 / pad 1 conv with 64 input and 64 output channels on NHWC bf16 ``x`` [B, H, W, 64]: ``ReLU?(conv(x) + bias
+    + residual)``, each term optional, ReLU last.  ``w`` is bf16 [64, 3, 3, 64] (weights.pack_conv3x3); with
+    ``upsample2`` the conv reads nearest_x2(x): ``w`` is then [4, 64, 2, 2, 64] (weights.pack_conv3x3_up2) and the output
+    [B, 2H, 2W, 64].  ``residual`` is bf16 shaped like the output (ds_tiny_conv64)."""
+    _req(x, bf16, "tiny_conv64.x", 4)
+    B, H, W, Cin = x.shape
+    if Cin != 64:
+        raise DsEngineError(f"tiny_conv64: x must have 64 channels, got {tuple(x.shape)}")
+    _req(w, bf16, "tiny_conv64.w")
+    want_w = (4, 64, 2, 2, 64) if upsample2 else (64, 3, 3, 64)
+    if tuple(w.shape) != want_w:
+        raise DsEngineError(f"tiny_conv64: w must be {list(want_w)}, got {tuple(w.shape)}")
+    Ho, Wo = (2 * H, 2 * W) if upsample2 else (H, W)
+    if bias is not None:
+        _req(bias, f32, "tiny_conv64.bias", 1)
+        if bias.numel() != 64:
+            raise DsEngineError("tiny_conv64: bias must be fp32 [64]")
+    if residual is not None:
+        _req(residual, bf16, "tiny_conv64.residual")
+        if tuple(residual.shape) != (B, Ho, Wo, 64):
+            raise DsEngineError(f"tiny_conv64: residual must be {[B, Ho, Wo, 64]}, got {tuple(residual.shape)}")
+        _req_aligned(residual, 4, "tiny_conv64.residual")
+    if out is None:
+        out = torch.empty(B, Ho, Wo, 64, dtype=bf16, device=x.device)
+    else:
+        _req(out, bf16, "tiny_conv64.out")
+        if tuple(out.shape) != (B, Ho, Wo, 64):
+            raise DsEngineError(f"tiny_conv64: out must be {[B, Ho, Wo, 64]}, got {tuple(out.shape)}")
+        _req_aligned(out, 4, "tiny_conv64.out")
+    _req_aligned(x, 16, "tiny_conv64.x")
+    _req_aligned(w, 16, "tiny_conv64.w")
+    check(lib.ds_tiny_conv64(x.data_ptr(), w.data_ptr(), _ptr(bias), _ptr(residual), out.data_ptr(), B, H, W,
+                             int(bool(relu)), int(bool(upsample2)), _stream()), "ds_tiny_conv64")
+    return out
+
+
+def tiny_conv_out(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
+    """DecoderTiny's final conv, 64 -> 3 channels + bias: bf16 NHWC [B, H, W, 64] -> bf16 NHWC [B, H, W, 3].  ``w`` is
+    bf16 [8, 3, 3, 64], output channels 3..7 zero (weights.pack_conv3x3 of the filter padded to 8), ``bias`` fp32 [3]
+    (ds_tiny_conv_out)."""
+    _req(x, bf16, "tiny_conv_out.x", 4)
+    B, H, W, Cin = x.shape
+    _req(w, bf16, "tiny_conv_out.w", 4)
+    _req(bias, f32, "tiny_conv_out.bias", 1)
+    if Cin != 64 or tuple(w.shape) != (8, 3, 3, 64) or bias.numel() != 3:
+        raise DsEngineError(f"tiny_conv_out: x must have 64 channels, w be [8, 3, 3, 64] and bias [3], got "
+                            f"{tuple(x.shape)}, {tuple(w.shape)}, {tuple(bias.shape)}")
+    _req_aligned(x, 16, "tiny_conv_out.x")
+    _req_aligned(w, 16, "tiny_conv_out.w")
+    out = torch.empty(B, H, W, 3, dtype=bf16, device=x.device)
+    check(lib.ds_tiny_conv_out(x.data_ptr(), w.data_ptr(), bias.data_ptr(), out.data_ptr(), B, H, W, _stream()),
+          "ds_tiny_conv_out")
+    return out
+
+
 def vae_posterior(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, *, eps: Optional[torch.Tensor] = None,
                   scale: float = 1.0, noise: Optional[torch.Tensor] = None, coef: Optional[torch.Tensor] = None,
                   repeat: int = 1, want_mean: bool = False, want_logvar: bool = False, want_out: bool = True):

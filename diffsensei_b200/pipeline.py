@@ -56,7 +56,8 @@ bf16, f32 = torch.bfloat16, torch.float32
 # generate_page: what a captured stepper bakes in is the same for the whole page; everything else is per panel
 PAGE_KEYS = frozenset({"num_inference_steps", "guidance_scale", "ip_scale", "output_type", "use_graph",
                        "max_batch_panels", "strength", "pag_scale", "pag_adaptive_scale",
-                       "adapter_conditioning_factor", "guidance_rescale"})
+                       "adapter_conditioning_factor", "guidance_rescale", "callback_on_step_end",
+                       "callback_on_step_end_tensor_inputs"})
 PANEL_KEYS = frozenset({
     "prompt", "prompt_2", "negative_prompt", "negative_prompt_2", "height", "width", "num_samples", "generator",
     "latents", "original_size", "crops_coords_top_left", "target_size", "min_size_step", "ip_images",
@@ -207,6 +208,13 @@ class DiffSenseiPipeline:
         self._lora = AdapterRegistry()
         self._pag_scale = 0.0
         self.set_pag_applied_layers(pag_applied_layers)
+        # diffusers' step-end callback surface: the tensors a callback may read and replace (condition tensors are
+        # baked into the captured graph's K|V buffers, so only the latents are offered), the stop flag a callback
+        # sets, the current denoise's step count and the (panel, first row, end row) of the chunk being denoised
+        self._callback_tensor_inputs = ["latents"]
+        self._interrupt = False
+        self._num_timesteps = 0
+        self._current_panels = ()
 
     # ------------------------------------------------------------------------------ reference surface
     def register_manga_modules(self, magi_image_encoder=None, image_proj_model=None):
@@ -220,6 +228,24 @@ class DiffSenseiPipeline:
     @property
     def do_classifier_free_guidance(self):
         return self._guidance_scale > 1
+
+    @property
+    def interrupt(self) -> bool:
+        """diffusers' stop flag: a ``callback_on_step_end`` sets ``pipe._interrupt = True`` and the remaining steps of
+        the call are skipped (later chunks of a page included); reset at the start of every ``__call__`` and
+        ``generate_page``."""
+        return self._interrupt
+
+    @property
+    def num_timesteps(self) -> int:
+        """The number of steps the current (or last) denoise runs."""
+        return self._num_timesteps
+
+    @property
+    def current_panels(self) -> tuple:
+        """``(panel_index, first_row, end_row)`` of every panel in the chunk being denoised: which rows of the
+        callback's ``latents`` belong to which panel of the page."""
+        return self._current_panels
 
     # ------------------------------------------------------------------------------ perturbed-attention guidance
     def set_pag_applied_layers(self, pag_applied_layers) -> None:
@@ -486,7 +512,8 @@ class DiffSenseiPipeline:
                 dialog_bbox: Optional[torch.Tensor], num_inference_steps: int, guidance_scale: float,
                 use_graph: bool = True, on_step=None, start_index: int = 0, inpaint=None, pag_scale: float = 0.0,
                 pag_adaptive_scale: float = 0.0, adapter=None, guidance_rescale: float = 0.0,
-                tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS) -> torch.Tensor:
+                tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS, callback_on_step_end=None,
+                callback_on_step_end_tensor_inputs=("latents",)) -> torch.Tensor:
         """pipeline_diffsensei.py:306-337.  ``latents`` NCHW fp32 (bs,4,h,w); conditions already concatenated
         [negative ; positive] along batch (:293-304), or [negative ; positive ; positive] with perturbed-attention
         guidance (``pag_scale > 0``: diffusers' PAGMixin; the third chunk takes the identity attention map at the
@@ -500,7 +527,15 @@ class DiffSenseiPipeline:
         ``TileGrid`` (MultiDiffusion): ``latents`` is the canvas and the conditions (and ``adapter`` may not be given)
         have one row per view of every sample, row b * V + v of each chunk, ``aspect_ratio`` the view's; the UNet runs
         the view rows in slices of at most ``max_batch_panels`` view-samples, and ``ds_tile_step`` averages the views'
-        updates on the canvas.  Returns the final latents, NCHW fp32."""
+        updates on the canvas.  ``callback_on_step_end``: diffusers' step-end callback, called as
+        ``callback(pipe, i, t, {"latents": fp32 NCHW latents})`` after each step (and its inpaint blend); the latents it
+        returns become the loop's (``DenoiseStepper.set_latents``), and once it sets ``pipe._interrupt`` the remaining
+        steps are skipped — a denoise that starts with the flag set returns ``latents`` as given.  Returns the final
+        latents, NCHW fp32."""
+        self._check_callback(callback_on_step_end, callback_on_step_end_tensor_inputs)
+        self._num_timesteps = int(num_inference_steps) - int(start_index)
+        if callback_on_step_end is not None and self._interrupt:
+            return latents.to(device=self.unet.device, dtype=f32).contiguous()
         guidance_rescale = check_guidance_rescale(guidance_rescale)
         self.unet.set_lora_scale(1.0)            # a direct unet(..., cross_attention_kwargs={"scale": s}) call may have left s
         pag = self._pag(pag_scale, pag_adaptive_scale)
@@ -514,11 +549,29 @@ class DiffSenseiPipeline:
                                    dialog_bbox, num_inference_steps, guidance_scale, False, start_index=start_index,
                                    inpaint=inpaint, pag=pag, adapter=adapter, guidance_rescale=guidance_rescale,
                                    tiles=tiles, max_batch_panels=max_batch_panels)
+        offer = "latents" in (callback_on_step_end_tensor_inputs or ())
         for i, t in enumerate(st.timesteps):
+            if callback_on_step_end is not None and self._interrupt:
+                continue                                                 # pipeline_diffsensei.py:311-312
             st.step(i)
             if on_step is not None:
                 on_step(i, t, st.lat)
+            if callback_on_step_end is not None:
+                kw = {"latents": st.latents_nchw()} if offer else {}
+                out = callback_on_step_end(self, i, t, kw)
+                lat = out.pop("latents", kw.get("latents"))
+                if lat is not None:
+                    st.set_latents(i + 1, lat)
         return st.latents_nchw()
+
+    def _check_callback(self, callback_on_step_end, callback_on_step_end_tensor_inputs) -> None:
+        """diffusers' checks of the step-end callback keywords (host only)."""
+        if callback_on_step_end is not None and not callable(callback_on_step_end):
+            raise ValueError(f"`callback_on_step_end` must be callable, got {type(callback_on_step_end).__name__}")
+        bad = [k for k in (callback_on_step_end_tensor_inputs or ()) if k not in self._callback_tensor_inputs]
+        if bad:
+            raise ValueError(f"`callback_on_step_end_tensor_inputs` has to be in {self._callback_tensor_inputs}, but "
+                             f"found {bad}")
 
     # ------------------------------------------------------------------------------ reference-shaped entry point
     @torch.no_grad()
@@ -550,15 +603,19 @@ class DiffSenseiPipeline:
                  # diffusers' rescale_noise_cfg (Lin et al., sec. 3.4) after the guidance blend: on when > 0
                  guidance_rescale: float = 0.0,
                  # MultiDiffusion (diffusers' StableDiffusionPanoramaPipeline): denoise as overlapping views of this size
-                 tile_size=None, tile_overlap: int = TILE_OVERLAP):
+                 tile_size=None, tile_overlap: int = TILE_OVERLAP,
+                 # diffusers' per-step hook: callback(pipe, i, t, {"latents": ...}); pipe._interrupt = True stops
+                 callback_on_step_end=None, callback_on_step_end_tensor_inputs=["latents"]):
         """A page of one panel: ``generate_page([panel], ...)[0]``, the panel holding this call's per-panel keywords
         (``PANEL_KEYS``) and the page the others.  Its input errors carry no panel index."""
+        self._interrupt = False
         args = locals()
         panel = {k: args[k] for k in PANEL_KEYS}                    # as given, defaults included
         page = dict(num_inference_steps=num_inference_steps, guidance_scale=guidance_scale, output_type=output_type,
                     max_batch_panels=PAGE_MAX_ROWS, strength=strength, pag_scale=pag_scale,
                     pag_adaptive_scale=pag_adaptive_scale, adapter_conditioning_factor=adapter_conditioning_factor,
-                    guidance_rescale=guidance_rescale)
+                    guidance_rescale=guidance_rescale, callback_on_step_end=callback_on_step_end,
+                    callback_on_step_end_tensor_inputs=callback_on_step_end_tensor_inputs)
         t_start = self._check_page([panel], **page)
         return self._run_page([self._panel_job(panel, output_type)], t_start, ip_scale=ip_scale, use_graph=use_graph,
                               **page)[0]
@@ -604,7 +661,8 @@ class DiffSenseiPipeline:
         return height, width
 
     def _check_page(self, panels, num_inference_steps, guidance_scale, output_type, max_batch_panels,
-                    strength, pag_scale, pag_adaptive_scale, adapter_conditioning_factor, guidance_rescale) -> int:
+                    strength, pag_scale, pag_adaptive_scale, adapter_conditioning_factor, guidance_rescale,
+                    callback_on_step_end=None, callback_on_step_end_tensor_inputs=("latents",)) -> int:
         """The host-only checks of the page keywords.  Returns the first step of the schedule that image panels run
         (0 on a page without them, where ``strength`` is not used)."""
         if output_type not in ("latent", "pt", "np", "pil"):
@@ -624,6 +682,7 @@ class DiffSenseiPipeline:
         if isinstance(f, bool) or not isinstance(f, (int, float)) or not 0.0 <= f <= 1.0:
             raise ValueError(f"`adapter_conditioning_factor` must be a number in [0, 1], got {f!r}")
         check_guidance_rescale(guidance_rescale)
+        self._check_callback(callback_on_step_end, callback_on_step_end_tensor_inputs)
         if any(p.get("image") is not None for p in panels):
             return get_timesteps(num_inference_steps, strength)[0]
         return 0
@@ -637,7 +696,8 @@ class DiffSenseiPipeline:
                       strength: float = 0.3, pag_scale: float = 0.0,
                       pag_adaptive_scale: float = 0.0,
                       adapter_conditioning_factor: float = 1.0,
-                      guidance_rescale: float = 0.0) -> List[SimpleNamespace]:
+                      guidance_rescale: float = 0.0, callback_on_step_end=None,
+                      callback_on_step_end_tensor_inputs=["latents"]) -> List[SimpleNamespace]:
         """Several panels of a page in one call.  ``panels`` holds one dict per panel with the per-panel keywords of
         ``__call__`` (``PANEL_KEYS``); the keywords here are the same for the whole page.  Returns one
         ``SimpleNamespace(images=..., latents=...)`` per panel, in panel order, each ``torch.equal`` to
@@ -694,7 +754,15 @@ class DiffSenseiPipeline:
         ``StableDiffusionPanoramaPipeline`` runs it (``tiles.TileGrid``; ``_tile_rows`` gives each view's conditions):
         every step the UNet runs all views, ``max_batch_panels`` view-samples per call, and ``ds_tile_step`` averages
         the views' updated latents on the canvas before the inpaint blend.  A tiled panel is a denoise of its own; its
-        noise, image and mask are canvas-sized as untiled, and the canvas is decoded whole."""
+        noise, image and mask are canvas-sized as untiled, and the canvas is decoded whole.
+
+        ``callback_on_step_end`` (diffusers' contract) is called as ``callback(pipe, i, t, callback_kwargs)`` after each
+        step of every chunk's denoise, after the scheduler update and the inpaint blend; ``i`` counts the steps that
+        denoise runs from 0, ``callback_kwargs["latents"]`` holds the chunk's fp32 NCHW latents (a tiled panel's whole
+        canvas) and ``pipe.current_panels`` says which rows belong to which panel.  The ``latents`` the callback returns
+        become the loop's.  ``pipe._interrupt = True`` in a callback skips every remaining step of the page: later
+        chunks keep their initial latents, and every panel is decoded from its latents as they stand."""
+        self._interrupt = False
         if not isinstance(panels, (list, tuple)) or len(panels) == 0:
             raise ValueError("generate_page needs a non-empty list of panel dicts")
         panels = [dict(p) for p in panels]
@@ -707,7 +775,8 @@ class DiffSenseiPipeline:
         page = dict(num_inference_steps=num_inference_steps, guidance_scale=guidance_scale, output_type=output_type,
                     max_batch_panels=max_batch_panels, strength=strength, pag_scale=pag_scale,
                     pag_adaptive_scale=pag_adaptive_scale, adapter_conditioning_factor=adapter_conditioning_factor,
-                    guidance_rescale=guidance_rescale)
+                    guidance_rescale=guidance_rescale, callback_on_step_end=callback_on_step_end,
+                    callback_on_step_end_tensor_inputs=callback_on_step_end_tensor_inputs)
         t_start = self._check_page(panels, **page)
         if agent is not None:
             self._check_agent_panels(panels, tokenizer_mllm)
@@ -728,7 +797,8 @@ class DiffSenseiPipeline:
 
     def _run_page(self, jobs, t_start: int, *, num_inference_steps, guidance_scale, ip_scale, output_type, use_graph,
                   max_batch_panels, strength, pag_scale, pag_adaptive_scale,
-                  adapter_conditioning_factor, guidance_rescale) -> List[SimpleNamespace]:
+                  adapter_conditioning_factor, guidance_rescale, callback_on_step_end=None,
+                  callback_on_step_end_tensor_inputs=("latents",)) -> List[SimpleNamespace]:
         """The GPU half of a page whose panels (``_panel_job``) and keywords (``_check_page``) passed their checks."""
         # ---- front end, once per page
         dev = self.unet.device
@@ -791,6 +861,11 @@ class DiffSenseiPipeline:
                 adapter = (feats, [1.0 if i < ad_steps else 0.0 for i in range(steps)])   # i: the loop's step
             aspect = lat.shape[-2] / lat.shape[-1] if tiles is None else tiles.tile_h / tiles.tile_w
             tiled = {} if tiles is None else dict(tiles=tiles, max_batch_panels=max_batch_panels)
+            if callback_on_step_end is not None:
+                ends = np.cumsum([jobs[i].ns for i in chunk]).tolist()
+                self._current_panels = tuple((i, e - jobs[i].ns, e) for i, e in zip(chunk, ends))
+                tiled.update(callback_on_step_end=callback_on_step_end,
+                             callback_on_step_end_tensor_inputs=callback_on_step_end_tensor_inputs)
             final = self.denoise(lat, cat("pe"), cat("te"), cat("ti"), cat("bbox"), aspect,
                                  cat("db"), num_inference_steps, guidance_scale, use_graph=use_graph,
                                  start_index=t_start if jobs[chunk[0]].image is not None else 0, inpaint=inpaint,
@@ -1438,6 +1513,23 @@ class DenoiseStepper:
         out_host.copy_(self.lat.permute(0, 3, 1, 2), non_blocking=True)                 # D2H
         torch.cuda.current_stream(self.dev).synchronize()
         return out_host
+
+    @torch.no_grad()
+    def set_latents(self, i: int, latents: torch.Tensor) -> None:
+        """Make fp32 NCHW ``latents`` the loop's latents in front of step ``i``: the fp32 master copy and, when step i
+        exists, every chunk of its UNet input (a tiled canvas's view rows) with step i's scale_model_input — the
+        arithmetic of ``step_host`` and of the step kernels' own store, so writing back the latents a step produced
+        changes no bit."""
+        nhwc = latents.to(device=self.dev, dtype=f32).permute(0, 2, 3, 1)
+        if nhwc.shape != self.lat.shape:
+            raise ValueError(f"set_latents: expected latents of shape {tuple(self.latents_nchw().shape)}, got "
+                             f"{tuple(latents.shape)}")
+        self.lat.copy_(nhwc)
+        if i < len(self.timesteps):
+            x = self._rows(self.lat / self.in_div[i])
+            rows = x.shape[0]
+            for c in range(self.n_chunks):
+                self.model_in[c * rows:(c + 1) * rows].copy_(x)
 
     def latents_nchw(self) -> torch.Tensor:
         return self.lat.permute(0, 3, 1, 2).contiguous()

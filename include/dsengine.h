@@ -432,6 +432,29 @@ int ds_latent_pointwise(const float* latents, const float* w, const float* bias,
                         int HW, void* stream);
 int ds_softmax_rows(const float* S, void* P, int rows, int n, int64_t lds, int64_t ldp, float scale, void* stream);
 int ds_image_postprocess(const void* x, float* out, int B, int HW, int C, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * The tiny SDXL autoencoder's decoder (TAESDXL: diffusers AutoencoderTiny / DecoderTiny), a cheap drop-in `vae`
+ * for previews and drafts.  Every layer after the first is a 3x3 / pad 1 conv with 64 input channels.
+ *   ds_tiny_latent_in : DecoderTiny's first layer: ReLU(conv3x3(tanh(x / 3) * 3) + bias), 4 -> 64 channels, on CUDA
+ *                       cores, x = latents * inv_scale (`latents / scaling_factor`).  latents fp32 NCHW [B][4][H][W]; w fp32 [64][3][3][4]; bias fp32 [64];
+ *                       out bf16 NHWC [B][H][W][64], 16-byte aligned.                          [HBM-bound]
+ *   ds_tiny_conv64    : 3x3 / pad 1 conv, 64 -> 64 channels, on wgmma with the whole filter resident in shared
+ *                       memory; out = ReLU?(conv(x) + bias? + residual?), fp32 accumulation, one bf16 rounding.
+ *                       x bf16 NHWC [B][H][W][64], w bf16 [64][3][3][64] (weights.pack_conv3x3), bias fp32 [64]
+ *                       or NULL, residual bf16 shaped like out or NULL, relu 0/1.  upsample2 = 1: out =
+ *                       conv(nearest_x2(x)) + ..., out [B][2H][2W][64], w [4][64][2][2][64] (weights.pack_conv3x3_up2),
+ *                       the upsampled tensor never written.  x, w 16-byte aligned; out, residual 4-byte aligned.
+ *                       No split-K: an image's output does not depend on the batch around it.   [tensor-bound]
+ *   ds_tiny_conv_out  : the final 64 -> 3 conv + bias on the same kernel with 8-column MMAs.  w bf16
+ *                       [8][3][3][64] (output channels 3..7 zero), bias fp32 [3], out bf16 NHWC [B][H][W][3].
+ * --------------------------------------------------------------------------------------------- */
+int ds_tiny_latent_in(const float* latents, const float* w, const float* bias, void* out, float inv_scale, int B,
+                      int H, int W, void* stream);
+int ds_tiny_conv64(const void* x, const void* w, const float* bias, const void* residual, void* out, int B, int H,
+                   int W, int relu, int upsample2, void* stream);
+int ds_tiny_conv_out(const void* x, const void* w, const float* bias, void* out, int B, int H, int W, void* stream);
+
 /* The AutoencoderKL encoder's posterior, from its conv_out output x fp32 NHWC [B][HW][8] (diffusers
  * AutoencoderKL.encode -> DiagonalGaussianDistribution, then StableDiffusionXLImg2ImgPipeline.prepare_latents):
  *   moments = quant_conv(x) (w fp32 [8][8] (out, in), bias fp32 [8]);  mean = moments[:4],
