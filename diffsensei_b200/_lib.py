@@ -86,6 +86,7 @@ SIGNATURES = {
     "ds_cfg_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _vp, _vp, _vp, _vp, _d, _i, _i, _i, _vp],
     "ds_cfg_rescale_factors": [_vp, _vp, _i, _f, _i, _vp, _i, _i, _i, _vp],
     "ds_tile_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _vp, _vp, _vp, _vp, _d, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "ds_region_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _vp, _vp, _vp, _vp, _d, _vp, _i, _i, _i, _i, _vp],
     "ds_resampler_attn": [_vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "ds_attention_small": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i64, _i64, _i64, _i64, _f, _i, _vp],
     "ds_embed_tokens": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],

@@ -1,8 +1,8 @@
 // glue_kernels.cu — small HBM-bound kernels around the tensor-core ops: conv_in (Cin = 4), layout changes at
 // the diffusers-facing boundary, nearest upsample, channel concat, SiLU, sinusoidal timestep features, and the
 // fused CFG + DDIM and CFG + Euler updates (plain and inpaint, with or without guidance_rescale), the same update on a
-// canvas denoised as overlapping views (MultiDiffusion), and the per-sample factors of that rescale.  All vectorised to
-// 16-byte accesses where the shape allows.
+// canvas denoised as overlapping views or under per-region prompts (MultiDiffusion), and the per-sample factors of that
+// rescale.  All vectorised to 16-byte accesses where the shape allows.
 #include <cmath>
 
 #include "ds_common.cuh"
@@ -403,6 +403,62 @@ __global__ void tile_step_kernel(const uint2* __restrict__ noise_pred, float4* _
   }
 }
 
+// The regional step (MultiDiffusion's region-based generation, Bar-Tal et al. 2023 sec. 4.2), one thread per canvas
+// pixel.  latents: the fp32 canvas [bs][HW]; noise_pred / model_in: kChunks chunks of bs * R1 rows of HW pixels, row
+// b * R1 + r sample b under prompt r (r = 0 the background, r = 1 .. R1 - 1 the regions), every row's input the whole
+// canvas; cover: uint8 [bs][HW], bit r - 1 set <=> region r covers the pixel (bits at or above R1 - 1 are ignored), the
+// background covers exactly the pixels whose byte is 0.  Every covering row's x_new is computed from the canvas pixel
+// as the plain step computes a sample's (rescale factor: the row's); their fp32 sum, in row order from 0, over the
+// count is the new canvas pixel, then the inpaint blend, then the next UNet input into all R1 rows of every chunk.
+template <bool kEuler, int kChunks, bool kInpaint, bool kRescale>
+__global__ void region_step_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
+                                   uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
+                                   const unsigned char* __restrict__ cover, int R1, int bs, int HW,
+                                   const float4* __restrict__ image_latents, const float4* __restrict__ noise,
+                                   const unsigned char* __restrict__ mask, const float* __restrict__ rescale,
+                                   float phi, float one_m_phi) {
+  static_assert(kChunks == 2 || kChunks == 3, "CFG (2 chunks) or CFG + PAG (3 chunks)");
+  constexpr int kC0 = kEuler ? 3 : 2;
+  constexpr int kS = kC0 + (kInpaint ? 2 : 0);
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<long long>(bs) * HW) return;
+  const long long b = i / HW;
+  const long long n_pix = static_cast<long long>(bs) * R1 * HW;  // pixels per chunk
+  const long long row0 = b * R1 * HW + (i - b * HW);               // the pixel in row b * R1 (the background)
+  const unsigned bits = __ldg(cover + i) & ((1u << (R1 - 1)) - 1u);
+  const unsigned rows = bits ? bits << 1 : 1u;                     // bit r set <=> row r covers the pixel
+  const float4 xc = latents[i];
+  float sum[4] = {0.f, 0.f, 0.f, 0.f};
+  for (unsigned m = rows; m != 0; m &= m - 1) {
+    const long long j = row0 + static_cast<long long>(__ffs(m) - 1) * HW;
+    float u[4], tt[4];
+    load_cfg_halves(noise_pred, j, n_pix, u, tt);
+    float xv[4] = {xc.x, xc.y, xc.z, xc.w};
+    guided_update<kEuler, kChunks, kRescale, kS>(noise_pred, j, n_pix, u, tt, xv, coef, guidance, rescale, HW, phi,
+                                                 one_m_phi);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) sum[c] = __fadd_rn(sum[c], xv[c]);
+  }
+  const float count = static_cast<float>(__popc(rows));
+  float xv[4];
+#pragma unroll
+  for (int c = 0; c < 4; ++c) xv[c] = __fdiv_rn(sum[c], count);
+  if constexpr (kInpaint) inpaint_blend(xv, i, image_latents, noise, mask, coef[kC0], coef[kC0 + 1]);
+  latents[i] = make_float4(xv[0], xv[1], xv[2], xv[3]);
+  uint2 o;
+  if constexpr (kEuler) {
+    const float d = coef[2];
+    o = make_uint2(pack_bf16(__fdiv_rn(xv[0], d), __fdiv_rn(xv[1], d)),
+                   pack_bf16(__fdiv_rn(xv[2], d), __fdiv_rn(xv[3], d)));
+  } else {
+    o = make_uint2(pack_bf16(xv[0], xv[1]), pack_bf16(xv[2], xv[3]));
+  }
+  for (int r = 0; r < R1; ++r) {
+#pragma unroll
+    for (int c = 0; c < kChunks; ++c) model_in[c * n_pix + row0 + static_cast<long long>(r) * HW] = o;
+  }
+}
+
 // guidance_rescale's per-sample factor r_b = fp32(std(text_b)) / fp32(std(guided_b)), both unbiased over the sample's
 // 4 * HW values.  One CTA per sample: every thread walks a fixed set of pixels, accumulating in fp64 the sums of
 // x - k and (x - k)^2 (k: the sample's first value, so a constant sample gives exactly 0), then a fixed-order tree
@@ -686,6 +742,52 @@ extern "C" int ds_tile_step(const void* noise_pred, float* latents, void* model_
       guidance, ay, ax, bs, reinterpret_cast<const float4*>(image_latents), reinterpret_cast<const float4*>(noise),
       mask, rescale_factors, static_cast<float>(guidance_rescale), static_cast<float>(1.0 - guidance_rescale));
   DS_LAUNCH_OK("tile_step_kernel");
+  return DS_OK;
+}
+
+extern "C" int ds_region_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
+                              float guidance, int update, int chunks, const float* image_latents, const float* noise,
+                              const uint8_t* mask, const float* rescale_factors, double guidance_rescale,
+                              const uint8_t* cover, int n_regions, int bs, int HW, int C, void* stream) {
+  const bool inpaint = image_latents || noise || mask;
+  const bool rescale = rescale_factors != nullptr;
+  DS_REQUIRE(noise_pred && latents && model_in && coef && cover, "ds_region_step: NULL pointer");
+  DS_REQUIRE(!inpaint || (image_latents && noise && mask),
+             "ds_region_step: image_latents / noise / mask must all be given or all be NULL");
+  DS_REQUIRE(update == 0 || update == 1, "ds_region_step: update must be 0 (DDIM) or 1 (Euler), got %d", update);
+  DS_REQUIRE(chunks == 2 || chunks == 3, "ds_region_step: chunks must be 2 or 3, got %d", chunks);
+  DS_REQUIRE(1 <= n_regions && n_regions <= 8, "ds_region_step: n_regions must be in [1, 8], got %d", n_regions);
+  DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "ds_region_step: only C == 4 latents are supported (got C=%d)", C);
+  DS_REQUIRE((reinterpret_cast<uintptr_t>(latents) & 15) == 0 && (reinterpret_cast<uintptr_t>(noise_pred) & 7) == 0 &&
+                 (reinterpret_cast<uintptr_t>(model_in) & 7) == 0,
+             "ds_region_step: latents must be 16-byte and noise_pred / model_in 8-byte aligned");
+  DS_REQUIRE(!inpaint || ((reinterpret_cast<uintptr_t>(image_latents) & 15) == 0 &&
+                          (reinterpret_cast<uintptr_t>(noise) & 15) == 0),
+             "ds_region_step: image_latents / noise must be 16-byte aligned");
+  DS_REQUIRE(rescale ? std::isfinite(guidance_rescale) : guidance_rescale == 0.0,
+             "ds_region_step: guidance_rescale must be finite, and 0 when rescale_factors is NULL (got %g)",
+             guidance_rescale);
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  using RegionKernel = void (*)(const uint2*, float4*, uint2*, const float*, float, const unsigned char*, int, int,
+                                int, const float4*, const float4*, const unsigned char*, const float*, float, float);
+  static constexpr RegionKernel kKernels[2][2][2][2] = {  // [update][chunks - 2][inpaint][rescale]
+      {{{region_step_kernel<false, 2, false, false>, region_step_kernel<false, 2, false, true>},
+        {region_step_kernel<false, 2, true, false>, region_step_kernel<false, 2, true, true>}},
+       {{region_step_kernel<false, 3, false, false>, region_step_kernel<false, 3, false, true>},
+        {region_step_kernel<false, 3, true, false>, region_step_kernel<false, 3, true, true>}}},
+      {{{region_step_kernel<true, 2, false, false>, region_step_kernel<true, 2, false, true>},
+        {region_step_kernel<true, 2, true, false>, region_step_kernel<true, 2, true, true>}},
+       {{region_step_kernel<true, 3, false, false>, region_step_kernel<true, 3, false, true>},
+        {region_step_kernel<true, 3, true, false>, region_step_kernel<true, 3, true, true>}}}};
+  const long long n_canvas = static_cast<long long>(bs) * HW;
+  kKernels[update][chunks - 2][inpaint][rescale]<<<static_cast<unsigned>((n_canvas + 255) / 256), 256, 0,
+                                                   static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
+      guidance, cover, n_regions + 1, bs, HW, reinterpret_cast<const float4*>(image_latents),
+      reinterpret_cast<const float4*>(noise), mask, rescale_factors, static_cast<float>(guidance_rescale),
+      static_cast<float>(1.0 - guidance_rescale));
+  DS_LAUNCH_OK("region_step_kernel");
   return DS_OK;
 }
 

@@ -771,6 +771,35 @@ def tile_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.
                            tiles.tile_h, tiles.tile_w, tiles.stride_h, tiles.stride_w, Cc, _stream()), "ds_tile_step")
 
 
+def region_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
+                 guidance: float, euler: bool, regions, inpaint=None, rescale=None) -> None:
+    """``cfg_step_`` on a canvas denoised under per-region prompts (``ds_region_step``), in place.  ``regions`` is
+    (cover, R): cover uint8 [bs,H,W], bit r - 1 set where region r (1 .. R, R <= 8) covers the pixel; the background
+    covers the pixels whose cover is 0.  latents fp32 NHWC [bs,H,W,4] is the canvas; noise_pred and model_in bf16
+    [k*bs*R',H,W,4], R' = R + 1, hold k chunks of R' rows per canvas sample, row c*bs*R' + b*R' + r (r = 0 the
+    background).  Each canvas pixel becomes the mean, in row order, of the updates its covering rows give it, then the
+    inpaint blend; all R' rows of model_in get the next UNet input.  ``inpaint`` canvas-sized as in ``cfg_step_``;
+    ``rescale`` factors fp32 [bs*R'], one per row.  coef as in ``cfg_step_``."""
+    cover, n_regions = regions
+    _req(noise_pred, bf16, "region_step.noise_pred", 4)
+    _req(latents, f32, "region_step.latents", 4)
+    _req(model_in, bf16, "region_step.model_in", 4)
+    _req(coef, f32, "region_step.coef", 1)
+    _req(cover, torch.uint8, "region_step.cover", 3)
+    bs, H, W, Cc = latents.shape
+    n_regions = int(n_regions)
+    rows = bs * (n_regions + 1)
+    chunks = noise_pred.shape[0] // rows if rows else 0
+    ncoef = (3 if euler else 2) + (0 if inpaint is None else 2) + (chunks == 3)
+    if not 1 <= n_regions <= 8 or chunks not in (2, 3) or noise_pred.shape != (chunks * rows, H, W, Cc) or \
+            model_in.shape != noise_pred.shape or cover.shape != (bs, H, W) or coef.numel() != ncoef:
+        raise DsEngineError("region_step: shape mismatch")
+    ptrs, factors, phi = _step_state("region_step", latents, rows, inpaint, rescale)
+    check(lib.ds_region_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(),
+                             float(guidance), int(bool(euler)), chunks, *ptrs, factors, float(phi), cover.data_ptr(),
+                             n_regions, bs, H * W, Cc, _stream()), "ds_region_step")
+
+
 def cfg_rescale_factors(noise_pred: torch.Tensor, coef: torch.Tensor, guidance: float,
                         out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """The per-sample factors of diffusers' ``rescale_noise_cfg`` (``ds_cfg_rescale_factors``): fp32 [bs],

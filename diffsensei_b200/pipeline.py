@@ -17,6 +17,7 @@ raises, it does not fall back to anything.
 ``image=`` / ``strength=`` start a panel from an image as diffusers' ``StableDiffusionXLImg2ImgPipeline`` does (needs
 ``vae_encoder=``): the image is encoded, noised to the schedule's step ``t_start`` and denoised from there.
 ``tile_size=`` denoises a large panel as overlapping views of a trained size (MultiDiffusion; ``tiles.py``).
+``regions=`` gives parts of a panel their own prompts (MultiDiffusion's region-based generation; ``regions.py``).
 ``mask_image=`` with ``image=`` redraws only the masked part, as diffusers' ``StableDiffusionXLInpaintPipeline`` does
 with a 4-channel UNet: after every step the unmasked latent pixels are reset to the image latents noised to the next
 timestep (fused into the step kernel, ``ds_cfg_step``).  Departures from that pipeline's defaults: the
@@ -47,6 +48,7 @@ from . import ops
 from .image_processor import (CLIPImageProcessor, VaeImageProcessor, ViTImageProcessor, adapter_image_info,
                               adapter_image_u8)
 from .lora import AdapterRegistry, lora_targets, normalize_lora, split_components
+from .regions import NEGATIVE_KEYS, box_cover, check_regions, cover_byte, region_rows
 from .scheduler import DDIMScheduler, EulerDiscreteScheduler, get_timesteps, pag_scales, step_table, with_pag_column
 from .tiles import TILE_OVERLAP, TileGrid, check_tiles
 from .unet import AdapterResiduals, UNetMangaEngine, resolve_pag_layers
@@ -64,7 +66,8 @@ PANEL_KEYS = frozenset({
     "ip_image_embeds", "clip_image_embeds", "magi_image_embeds", "clip_pixel_values", "magi_pixel_values", "ip_bbox",
     "dialog_bbox", "prompt_embeds", "negative_prompt_embeds", "pooled_prompt_embeds", "negative_pooled_prompt_embeds",
     "prompt_input_ids", "prompt_input_ids_2", "negative_prompt_input_ids", "negative_prompt_input_ids_2", "image",
-    "mask_image", "padding_mask_crop", "adapter_image", "adapter_conditioning_scale", "tile_size", "tile_overlap"})
+    "mask_image", "padding_mask_crop", "adapter_image", "adapter_conditioning_scale", "tile_size", "tile_overlap",
+    "regions"})
 PAGE_MAX_ROWS = 8       # samples per page denoise: a UNet batch of 16 rows, as __call__(num_samples=8)
 
 
@@ -454,20 +457,22 @@ class DiffSenseiPipeline:
                      dialog_bbox: Optional[torch.Tensor], num_inference_steps: int, guidance_scale: float,
                      use_graph: bool = True, chains: Optional[int] = None, start_index: int = 0,
                      inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0,
-                     tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS) -> "DenoiseStepper":
+                     tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS,
+                     regions=None) -> "DenoiseStepper":
         return DenoiseStepper(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                               dialog_bbox, num_inference_steps, guidance_scale, use_graph, chains, start_index,
-                              inpaint, pag, adapter, guidance_rescale, tiles, max_batch_panels)
+                              inpaint, pag, adapter, guidance_rescale, tiles, max_batch_panels, regions)
 
     def stepper_key(self, latents, prompt_embeds, aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale,
                     chains=None, start_index: int = 0, inpaint=None, pag=None, adapter=None,
                     guidance_rescale: float = 0.0, tiles: Optional[TileGrid] = None,
-                    max_batch_panels: int = PAGE_MAX_ROWS) -> tuple:
+                    max_batch_panels: int = PAGE_MAX_ROWS, regions=None) -> tuple:
         """Everything a captured stepper bakes in (``stepper_for``), FreeU's values (``unet.freeu``) and whether a
         T2I-Adapter's features are added included.  With ``guidance_rescale > 0`` the key ends with its value, which
         the graph bakes in like ``guidance_scale``; otherwise the key is the one the step without the rescale has.
         With ``tiles`` it ends with the view grid and the UNet slice size (``max_batch_panels``); without, neither is
-        in it."""
+        in it.  With ``regions`` = (cover, R) it ends with ("regions", R + 1, ``max_batch_panels``); the cover is per
+        panel data that ``load_panel`` refills, so it is not in the key."""
         key = (tuple(latents.shape), tuple(prompt_embeds.shape), None if dialog_bbox is None else
                 (tuple(dialog_bbox.shape), dialog_bbox.dtype == bf16), float(aspect_ratio), int(num_inference_steps),
                 float(guidance_scale), self.unet.scales_key(), chains, self.unet._ip_weights_version(),
@@ -478,12 +483,15 @@ class DiffSenseiPipeline:
             key += (("guidance_rescale", float(guidance_rescale)),)
         if tiles is not None:
             key += (("tiles", tiles, int(max_batch_panels)),)
+        if regions is not None:
+            key += (("regions", int(regions[1]) + 1, int(max_batch_panels)),)
         return key
 
     def stepper_for(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio, dialog_bbox,
                     num_inference_steps, guidance_scale, chains=None, start_index: int = 0,
                     inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0,
-                    tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS) -> "DenoiseStepper":
+                    tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS,
+                    regions=None) -> "DenoiseStepper":
         """A graph-captured stepper loaded with this panel: a cached one of the same key is refilled in place
         (no re-capture), otherwise a new one is built and cached.  The start index is part of the key: the stepper
         bakes in its slice of the schedule (``set_timesteps`` would reset any scheduler state); so is whether it
@@ -492,18 +500,19 @@ class DiffSenseiPipeline:
         scales are not: they live in the coefficient table, which ``load_panel`` rewrites, as it rewrites the adapter
         features and gates."""
         key = self.stepper_key(latents, prompt_embeds, aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale,
-                               chains, start_index, inpaint, pag, adapter, guidance_rescale, tiles, max_batch_panels)
+                               chains, start_index, inpaint, pag, adapter, guidance_rescale, tiles, max_batch_panels,
+                               regions)
         st = self._steppers.get(key)
         if st is None:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                    dialog_bbox, num_inference_steps, guidance_scale, True, chains, start_index,
-                                   inpaint, pag, adapter, guidance_rescale, tiles, max_batch_panels)
+                                   inpaint, pag, adapter, guidance_rescale, tiles, max_batch_panels, regions)
             while len(self._steppers) >= self.max_cached_steppers:
                 self._steppers.pop(next(iter(self._steppers)))
             self._steppers[key] = st
         else:
             st.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox, inpaint, pag,
-                          adapter)
+                          adapter, regions)
         return st
 
     @torch.no_grad()
@@ -513,7 +522,7 @@ class DiffSenseiPipeline:
                 use_graph: bool = True, on_step=None, start_index: int = 0, inpaint=None, pag_scale: float = 0.0,
                 pag_adaptive_scale: float = 0.0, adapter=None, guidance_rescale: float = 0.0,
                 tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS, callback_on_step_end=None,
-                callback_on_step_end_tensor_inputs=("latents",)) -> torch.Tensor:
+                callback_on_step_end_tensor_inputs=("latents",), regions=None) -> torch.Tensor:
         """pipeline_diffsensei.py:306-337.  ``latents`` NCHW fp32 (bs,4,h,w); conditions already concatenated
         [negative ; positive] along batch (:293-304), or [negative ; positive ; positive] with perturbed-attention
         guidance (``pag_scale > 0``: diffusers' PAGMixin; the third chunk takes the identity attention map at the
@@ -527,7 +536,11 @@ class DiffSenseiPipeline:
         ``TileGrid`` (MultiDiffusion): ``latents`` is the canvas and the conditions (and ``adapter`` may not be given)
         have one row per view of every sample, row b * V + v of each chunk, ``aspect_ratio`` the view's; the UNet runs
         the view rows in slices of at most ``max_batch_panels`` view-samples, and ``ds_tile_step`` averages the views'
-        updates on the canvas.  ``callback_on_step_end``: diffusers' step-end callback, called as
+        updates on the canvas.  ``regions``: (cover uint8 (bs, h, w), R), regional prompts (MultiDiffusion's
+        region-based generation): ``latents`` is the canvas and the conditions have R' = R + 1 rows per sample, row
+        b * R' + r of each chunk (r = 0 the background); the UNet runs the rows in slices as with ``tiles`` and
+        ``ds_region_step`` averages, per pixel, the updates of the rows whose region covers it (bit r - 1 of the cover
+        for row r, the background where the cover is 0).  ``callback_on_step_end``: diffusers' step-end callback, called as
         ``callback(pipe, i, t, {"latents": fp32 NCHW latents})`` after each step (and its inpaint blend); the latents it
         returns become the loop's (``DenoiseStepper.set_latents``), and once it sets ``pipe._interrupt`` the remaining
         steps are skipped — a denoise that starts with the flag set returns ``latents`` as given.  Returns the final
@@ -543,12 +556,12 @@ class DiffSenseiPipeline:
             st = self.stepper_for(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                   dialog_bbox, num_inference_steps, guidance_scale, start_index=start_index,
                                   inpaint=inpaint, pag=pag, adapter=adapter, guidance_rescale=guidance_rescale,
-                                  tiles=tiles, max_batch_panels=max_batch_panels)
+                                  tiles=tiles, max_batch_panels=max_batch_panels, regions=regions)
         else:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                    dialog_bbox, num_inference_steps, guidance_scale, False, start_index=start_index,
                                    inpaint=inpaint, pag=pag, adapter=adapter, guidance_rescale=guidance_rescale,
-                                   tiles=tiles, max_batch_panels=max_batch_panels)
+                                   tiles=tiles, max_batch_panels=max_batch_panels, regions=regions)
         offer = "latents" in (callback_on_step_end_tensor_inputs or ())
         for i, t in enumerate(st.timesteps):
             if callback_on_step_end is not None and self._interrupt:
@@ -604,6 +617,8 @@ class DiffSenseiPipeline:
                  guidance_rescale: float = 0.0,
                  # MultiDiffusion (diffusers' StableDiffusionPanoramaPipeline): denoise as overlapping views of this size
                  tile_size=None, tile_overlap: int = TILE_OVERLAP,
+                 # MultiDiffusion's region-based generation: [{"prompt": ..., "box": [x1, y1, x2, y2] or "mask": ...}]
+                 regions=None,
                  # diffusers' per-step hook: callback(pipe, i, t, {"latents": ...}); pipe._interrupt = True stops
                  callback_on_step_end=None, callback_on_step_end_tensor_inputs=["latents"]):
         """A page of one panel: ``generate_page([panel], ...)[0]``, the panel holding this call's per-panel keywords
@@ -802,12 +817,16 @@ class DiffSenseiPipeline:
         """The GPU half of a page whose panels (``_panel_job``) and keywords (``_check_page``) passed their checks."""
         # ---- front end, once per page
         dev = self.unet.device
+        for j in jobs:
+            if j.regions:
+                j.cover = self._region_cover(j)
+        texts = jobs + [r for j in jobs for r in j.regions]          # the panels' prompts, then their regions'
         text = _stacked(lambda ids: (self.text_encoder(ids, output_hidden_states=True).hidden_states[-2],),
-                        [x for j in jobs if j.ids is not None for x in (j.ids[0], j.ids[2]) if x is not None])
+                        [x for j in texts if j.ids is not None for x in (j.ids[0], j.ids[2]) if x is not None])
         text_2 = _stacked(lambda ids: (lambda o: (o.hidden_states[-2], o[0]))(
                           self.text_encoder_2(ids, output_hidden_states=True)),
-                          [x for j in jobs if j.ids is not None for x in (j.ids[1], j.ids[3]) if x is not None])
-        for j in jobs:
+                          [x for j in texts if j.ids is not None for x in (j.ids[1], j.ids[3]) if x is not None])
+        for j in texts:
             if j.ids is None:
                 continue
             (h1,), (h2, pooled) = text.pop(0), text_2.pop(0)
@@ -817,6 +836,13 @@ class DiffSenseiPipeline:
             else:
                 (h1,), (h2, pooled) = text.pop(0), text_2.pop(0)
                 j.npe, j.npp = torch.cat([h1, h2], dim=-1), pooled
+        for j in jobs:
+            for k, r in enumerate(j.regions):
+                if not r.own_negative:
+                    r.npe, r.npp = j.npe, j.npp
+                if tuple(r.pe.shape[1:]) != tuple(j.pe.shape[1:]):
+                    raise ValueError(f"region {k}: its prompt embeddings ({tuple(r.pe.shape[1:])}) must have the "
+                                     f"panel's shape ({tuple(j.pe.shape[1:])})")
         self._encode_page_images(jobs)
         for j, (img, neg) in zip(jobs, self._character_embeds([(j.clip, j.magi, j.ip_image_embeds) for j in jobs])):
             j.img, j.neg_img = img, neg
@@ -841,11 +867,13 @@ class DiffSenseiPipeline:
         results = [None] * len(jobs)
         kind = lambda j: (() if j.image is None else ("inpaint",) if j.mask_image is not None else ("image",)) + \
             (() if j.adapter_feats is None else ("adapter",))
-        alone = lambda i: () if jobs[i].tiles is None else (("tiles", i),)    # a tiled panel is a denoise of its own
+        # a tiled panel, and a panel with regions, is a denoise of its own
+        alone = lambda i: () if jobs[i].tiles is None and not jobs[i].regions else (("alone", i),)
         shapes = [(j.ns,) + tuple(j.latents.shape[-2:]) + kind(j) + alone(i) for i, j in enumerate(jobs)]
         for chunk in plan_page(shapes, max_batch_panels):
-            tiles = jobs[chunk[0]].tiles
-            rows = [self._panel_rows(jobs[i]) if tiles is None else self._tile_rows(jobs[i]) for i in chunk]
+            tiles, regions = jobs[chunk[0]].tiles, jobs[chunk[0]].regions
+            rows = [self._tile_rows(jobs[i]) if tiles is not None else self._region_rows(jobs[i]) if regions else
+                    self._panel_rows(jobs[i]) for i in chunk]
             # [negatives ; positives], and the positives again as the perturbed block with PAG (diffusers' PAGMixin)
             sides = (0, 1, 1) if self.do_perturbed_attention_guidance else (0, 1)
             cat = lambda k: torch.cat([r[side][k] for side in sides for r in rows], dim=0)
@@ -861,6 +889,10 @@ class DiffSenseiPipeline:
                 adapter = (feats, [1.0 if i < ad_steps else 0.0 for i in range(steps)])   # i: the loop's step
             aspect = lat.shape[-2] / lat.shape[-1] if tiles is None else tiles.tile_h / tiles.tile_w
             tiled = {} if tiles is None else dict(tiles=tiles, max_batch_panels=max_batch_panels)
+            if regions:                                         # one panel: its cover for every sample
+                j = jobs[chunk[0]]
+                tiled = dict(regions=(j.cover.expand(j.ns, -1, -1).contiguous(), len(regions)),
+                             max_batch_panels=max_batch_panels)
             if callback_on_step_end is not None:
                 ends = np.cumsum([jobs[i].ns for i in chunk]).tolist()
                 self._current_panels = tuple((i, e - jobs[i].ns, e) for i, e in zip(chunk, ends))
@@ -929,6 +961,10 @@ class DiffSenseiPipeline:
             for k in ("adapter_image", "padding_mask_crop"):
                 if g(k) is not None:
                     raise ValueError(f"`tile_size` and `{k}` can not be input together")
+        if g("regions"):
+            for k in ("tile_size", "adapter_image", "padding_mask_crop"):
+                if g(k) is not None:
+                    raise ValueError(f"`regions` and `{k}` can not be input together")
         crop = mask_l = None
         ad_image = g("adapter_image")
         ad_scale = g("adapter_conditioning_scale", 1.0)
@@ -968,6 +1004,7 @@ class DiffSenseiPipeline:
         height = height or self.default_sample_size * self.vae_scale_factor
         width = width or self.default_sample_size * self.vae_scale_factor
         tiles = check_tiles(g("tile_size"), g("tile_overlap", TILE_OVERLAP), height, width, self.vae_scale_factor)
+        regions = check_regions(g("regions"), height, width, self.vae_scale_factor)
         ip_images, ip_bbox = list(g("ip_images", ())), list(g("ip_bbox", ()))
         ip_image_embeds = g("ip_image_embeds")
         if len(ip_images) > 0:
@@ -976,25 +1013,7 @@ class DiffSenseiPipeline:
             if any(g(k) is not None for k in ("clip_pixel_values", "magi_pixel_values", "clip_image_embeds",
                                               "magi_image_embeds")):
                 raise ValueError("`ip_images` and pixel values / image embeddings can not be input together!")
-        ids = None
-        if g("prompt_embeds") is None:
-            if g("prompt_input_ids") is None and isinstance(g("prompt"), str) and \
-                    self.tokenizer is not None and self.tokenizer_2 is not None:
-                ids = self.tokenize_prompt(g("prompt"), g("prompt_2"), g("negative_prompt"), g("negative_prompt_2"))
-            elif g("prompt_input_ids") is not None:
-                ids = (g("prompt_input_ids"), g("prompt_input_ids_2"), g("negative_prompt_input_ids"),
-                       g("negative_prompt_input_ids_2"))
-            if ids is None:
-                self.check_inputs(g("prompt"), g("prompt_2"), ip_images, ip_image_embeds, ip_bbox)
-                raise NotImplementedError(
-                    "raw prompt strings need the CLIP tokenizers (tokenizer= / tokenizer_2=): pass "
-                    "prompt_input_ids with the text-encoder engines registered, or the prompt embeddings")
-            if self.text_encoder is None or self.text_encoder_2 is None:
-                raise ValueError("encode_prompt_ids needs text_encoder and text_encoder_2 engines")
-            as_ids = lambda t: None if t is None else torch.as_tensor(t)
-            # negative_prompt_input_ids_2 without negative_prompt_input_ids: zero negatives, as encode_prompt_ids
-            ids = (as_ids(ids[0]), as_ids(ids[1] if ids[1] is not None else ids[0]), as_ids(ids[2]),
-                   None if ids[2] is None else as_ids(ids[3] if ids[3] is not None else ids[2]))
+        ids = self._prompt_ids(g, ip_images, ip_image_embeds, ip_bbox)
         m = self.unet.cfg.max_num_ips
         clip_pv = magi_pv = None
         n_real = 0
@@ -1023,13 +1042,56 @@ class DiffSenseiPipeline:
             ns=int(g("num_samples", 1)), height=height, width=width, generator=g("generator"), latents=g("latents"),
             ids=ids, image=g("image"), mask_image=g("mask_image"), inpaint=None, crop=crop, mask_l=mask_l,
             adapter_image=ad_image, adapter_scale=float(ad_scale), adapter_float=ad_image is not None and ad_float,
-            adapter_feats=None, tiles=tiles,
+            adapter_feats=None, tiles=tiles, regions=[] if regions is None else self._region_jobs(regions),
             pe=g("prompt_embeds"), npe=g("negative_prompt_embeds"), pp=g("pooled_prompt_embeds"),
             npp=g("negative_pooled_prompt_embeds"), ip_images=ip_images, clip_pv=clip_pv, magi_pv=magi_pv,
             clip=g("clip_image_embeds"), magi=g("magi_image_embeds"), ip_image_embeds=ip_image_embeds,
             ip_bbox=ip_bbox, dialog_bbox=list(g("dialog_bbox", ())),
             time_ids=list(g("original_size") or (height, width)) + list(g("crops_coords_top_left", (0, 0))) +
             list(g("target_size") or (height, width)))                   # _get_add_time_ids
+
+    def _prompt_ids(self, g, ip_images=(), ip_image_embeds=None, ip_bbox=()):
+        """The token ids of a panel's (or a region's) prompt keys, read with ``g(key)``: None when ``prompt_embeds``
+        is given, else (ids, ids_2, negative_ids, negative_ids_2) from the strings (tokenized) or the ids, int64
+        tensors, the negatives None or both set.  Host only; raises as ``__call__`` does when neither can be
+        encoded."""
+        if g("prompt_embeds") is not None:
+            return None
+        ids = None
+        if g("prompt_input_ids") is None and isinstance(g("prompt"), str) and \
+                self.tokenizer is not None and self.tokenizer_2 is not None:
+            ids = self.tokenize_prompt(g("prompt"), g("prompt_2"), g("negative_prompt"), g("negative_prompt_2"))
+        elif g("prompt_input_ids") is not None:
+            ids = (g("prompt_input_ids"), g("prompt_input_ids_2"), g("negative_prompt_input_ids"),
+                   g("negative_prompt_input_ids_2"))
+        if ids is None:
+            self.check_inputs(g("prompt"), g("prompt_2"), ip_images, ip_image_embeds, ip_bbox)
+            raise NotImplementedError(
+                "raw prompt strings need the CLIP tokenizers (tokenizer= / tokenizer_2=): pass "
+                "prompt_input_ids with the text-encoder engines registered, or the prompt embeddings")
+        if self.text_encoder is None or self.text_encoder_2 is None:
+            raise ValueError("encode_prompt_ids needs text_encoder and text_encoder_2 engines")
+        as_ids = lambda t: None if t is None else torch.as_tensor(t)
+        # negative_prompt_input_ids_2 without negative_prompt_input_ids: zero negatives, as encode_prompt_ids
+        return (as_ids(ids[0]), as_ids(ids[1] if ids[1] is not None else ids[0]), as_ids(ids[2]),
+                None if ids[2] is None else as_ids(ids[3] if ids[3] is not None else ids[2]))
+
+    def _region_jobs(self, regions) -> List[SimpleNamespace]:
+        """The checked ``regions`` of a panel (``regions.check_regions``) with their prompts resolved by the panel's
+        code (``_prompt_ids``); host only.  A region without any negative key takes the panel's negative conditioning
+        (``own_negative`` False: ``_run_page`` copies it once the panel's is encoded)."""
+        out = []
+        for k, r in enumerate(regions):
+            g = lambda key, d=None: r.get(key, d)
+            try:
+                ids = self._prompt_ids(g)
+            except (ValueError, NotImplementedError) as e:
+                raise type(e)(f"region {k}: {e}") from e
+            out.append(SimpleNamespace(
+                ids=ids, pe=g("prompt_embeds"), npe=g("negative_prompt_embeds"), pp=g("pooled_prompt_embeds"),
+                npp=g("negative_pooled_prompt_embeds"), box=g("box"), mask=g("mask"),
+                own_negative=any(g(key) is not None for key in NEGATIVE_KEYS)))
+        return out
 
     def _check_crop(self, pad, image, mask_image, latents, output_type):
         """The host-only checks of ``padding_mask_crop``; returns the mask as "L" (uint8 [H, W], host)."""
@@ -1188,6 +1250,32 @@ class DiffSenseiPipeline:
                 side.append(rows)
         return tuple({k: torch.cat([torch.cat([r[k] for r in side])] * j.ns) for k in side[0]} for side in views)
 
+    def _region_cover(self, j) -> torch.Tensor:
+        """A panel's cover (``regions.cover_byte``), uint8 [1, h, w] on the GPU: a ``box`` region's pixels by
+        ``regions.box_cover``, a ``mask`` region's by the inpaint mask processor at the panel size.  A mask whose
+        latent pixels are all 0 raises ``ValueError`` here, before any denoise."""
+        h, w = j.height // self.vae_scale_factor, j.width // self.vae_scale_factor
+        covers = []
+        for k, r in enumerate(j.regions):
+            if r.box is not None:
+                covers.append(box_cover(r.box, h, w)[None].to(self.unet.device))
+            else:
+                c = self.mask_processor.preprocess_latent_mask(r.mask, j.height, j.width)
+                if not bool(c.any()):
+                    raise ValueError(f"region {k}: `mask` covers no pixel of the {h} x {w} latents")
+                covers.append(c)
+        return cover_byte(covers)
+
+    def _region_rows(self, j):
+        """A panel with regions: its [negative, positive] condition rows, R' = 1 + R per sample, row b * R' + r.  Row 0
+        takes the panel's prompt, row r the prompt of region r; every row takes the panel's characters, ``ip_bbox``,
+        ``dialog_bbox`` and SDXL time ids."""
+        one = SimpleNamespace(**{**vars(j), "ns": 1})
+        prompts = [one] + [SimpleNamespace(**{**vars(one), "pe": r.pe, "pp": r.pp, "npe": r.npe, "npp": r.npp})
+                           for r in j.regions]
+        sides = list(zip(*(self._panel_rows(v) for v in prompts)))
+        return tuple({k: torch.cat([torch.cat([r[k] for r in side])] * j.ns) for k in side[0]} for side in sides)
+
     def _check_agent_panels(self, panels, tokenizer_mllm) -> None:
         """The host-only checks of the ``agent=`` path (each panel's own checks follow: ``_panel_job``)."""
         if tokenizer_mllm is None:
@@ -1263,13 +1351,16 @@ class DenoiseStepper:
     step runs the UNet on the view rows in slices of at most k * ``max_batch_panels`` rows, one after another into
     slices of one eps buffer, then ``ds_tile_step`` (with the factors of every view row when rescaling).  Every kernel
     gives a row the same bits whatever batch surrounds it, so the slicing changes no bit.
+    With ``regions`` = (cover, R) (regional prompts) the fp32 master latents are the canvas, ``model_in`` holds R + 1
+    copies of every sample in each chunk (row b * (R + 1) + r), the UNet runs them in slices as with ``tiles``, and
+    the step is ``ds_region_step`` over the cover, a per-panel buffer ``load_panel`` refills.
     """
 
     @torch.no_grad()
     def __init__(self, pipe: DiffSenseiPipeline, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox,
                  aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale, use_graph=True, chains=None,
                  start_index: int = 0, inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0,
-                 tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS):
+                 tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS, regions=None):
         unet, dev = pipe.unet, pipe.unet.device
         self.unet, self.dev, self.guidance = unet, dev, float(guidance_scale)
         self.scheduler = pipe.scheduler
@@ -1298,8 +1389,14 @@ class DenoiseStepper:
         self.tiles = tiles
         if tiles is not None and (adapter is not None or int(max_batch_panels) < 1):
             raise ValueError("a tiled denoise takes no adapter features, and max_batch_panels must be >= 1")
+        self.regions = None if regions is None else int(regions[1])     # R; the rows per sample are R + 1
+        self.cover = None
+        if regions is not None and (tiles is not None or adapter is not None or int(max_batch_panels) < 1 or
+                                    not 1 <= self.regions <= 8):
+            raise ValueError("a denoise with regions takes 1 to 8 regions, no tiles and no adapter features, and "
+                             "max_batch_panels must be >= 1")
         self.load_panel(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox, inpaint, pag,
-                        adapter)
+                        adapter, regions)
         rescale = check_guidance_rescale(guidance_rescale)
         self.guidance_rescale = rescale if rescale > 0 else 0.0
         self.rescale_factors = None
@@ -1320,7 +1417,7 @@ class DenoiseStepper:
         self._parts, self._side = [(0, B2)], []
         # first perturbed row of the whole batch (None: no PAG); each part gets it relative to its own slice
         self._pag_row0 = None if pag is None else 2 * (B2 // self.n_chunks)
-        if tiles is not None:                       # UNet slices of at most max_batch_panels view-samples' rows
+        if tiles is not None or regions is not None:    # UNet slices of at most max_batch_panels samples' rows
             cap, self.chains = self.n_chunks * int(max_batch_panels), 1
             self._parts = [(r, min(r + cap, B2)) for r in range(0, B2, cap)]
             self._cond_parts = [self.cond.rows(s, e) for s, e in self._parts]
@@ -1348,15 +1445,24 @@ class DenoiseStepper:
 
     @torch.no_grad()
     def load_panel(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, dialog_bbox,
-                   inpaint=None, pag=None, adapter=None) -> None:
+                   inpaint=None, pag=None, adapter=None, regions=None) -> None:
         """Everything that is per panel and timestep-invariant, written INTO the buffers the captured graph reads:
         K|V of the text / IP tokens for all cross-attention layers, the time-embedding row-bias table for all T
-        steps, the bbox tables, the initial latents, the inpaint state, the PAG scale of every step, and the adapter
-        features and per-step gates.  First call allocates; later calls (same shapes) refill."""
+        steps, the bbox tables, the initial latents, the inpaint state, the PAG scale of every step, the adapter
+        features and per-step gates, and the regions' cover.  First call allocates; later calls (same shapes)
+        refill."""
         unet, dev = self.unet, self.dev
         bs = latents.shape[0]
         k = self.n_chunks
         rows = bs if self.tiles is None else bs * self.tiles.n_views      # UNet rows per chunk
+        if self.regions is not None:
+            rows = bs * (self.regions + 1)
+            if regions is None or int(regions[1]) != self.regions or \
+                    tuple(regions[0].shape) != (bs,) + tuple(latents.shape[-2:]):
+                raise ValueError("load_panel: the regions' count or cover shape (num_samples, h, w) differs from the "
+                                 "stepper's")
+        elif regions is not None:
+            raise ValueError("load_panel: regions given to a stepper built without them")
         if self.tiles is not None and tuple(latents.shape[-2:]) != (self.tiles.height, self.tiles.width):
             raise ValueError("load_panel: the latents are not the tile grid's canvas")
         if (pag is None) != (self.pag_sites is None) or (pag is not None and frozenset(pag[0]) != self.pag_sites):
@@ -1365,6 +1471,9 @@ class DenoiseStepper:
             if self.tiles is not None:
                 raise ValueError("a tiled denoise expects one condition row per view of every sample in each chunk: "
                                  "prompt_embeds.shape[0] == chunks * num_samples * views")
+            if self.regions is not None:
+                raise ValueError("a denoise with regions expects R + 1 condition rows per sample in each chunk: "
+                                 "prompt_embeds.shape[0] == chunks * num_samples * (R + 1)")
             if k == 2:
                 raise ValueError("denoise expects CFG-concatenated conditions: prompt_embeds.shape[0] == 2 * "
                                  "num_samples")
@@ -1404,6 +1513,12 @@ class DenoiseStepper:
                 self.inp_z.copy_(z)
                 self.inp_n.copy_(n)
                 self.inp_m.copy_(m)
+        if regions is not None:
+            cover = regions[0].to(device=dev, dtype=torch.uint8)
+            if self.cover is None:
+                self.cover = cover.clone(memory_format=torch.contiguous_format)
+            else:
+                self.cover.copy_(cover)
         self.cond = unet.prepare_conditions(prompt_embeds.to(dev), bbox, self.aspect_ratio, out=self.cond)
         self.temb_table = unet.time_rowbias_table(self.timesteps, add_text_embeds, add_time_ids)   # [T, 2bs, sumC]
         lat = latents.to(device=dev, dtype=f32).permute(0, 2, 3, 1).contiguous()         # fp32 NHWC master copy
@@ -1429,7 +1544,10 @@ class DenoiseStepper:
                 self.db.copy_(db)
 
     def _rows(self, x: torch.Tensor) -> torch.Tensor:
-        """The UNet rows of one chunk from NHWC latents: the latents themselves, or a tiled canvas's view rows."""
+        """The UNet rows of one chunk from NHWC latents: the latents themselves, a tiled canvas's view rows, or R + 1
+        copies of every sample with regions."""
+        if self.regions is not None:
+            return region_rows(x, self.regions + 1)
         return x if self.tiles is None else self.tiles.gather(x)
 
     def _pag_args(self, s: int, e: int) -> dict:
@@ -1449,7 +1567,7 @@ class DenoiseStepper:
             eps = self.unet.forward_nhwc(self.model_in, self.temb_cur, self.cond, self.db, self.round_bf16,
                                          **self._pag_args(0, self.model_in.shape[0]),
                                          **self._adapter_args(0))                                          # :322-329
-        elif self.tiles is not None:                   # the view rows' slices, one after another, into one buffer
+        elif self.tiles is not None or self.regions is not None:   # the rows' slices, one after another, into one buffer
             eps = self._eps
             for k, (s, e) in enumerate(self._parts):
                 self.unet.forward_nhwc(self.model_in[s:e], self.temb_cur[s:e], self._cond_parts[k],
@@ -1478,6 +1596,8 @@ class DenoiseStepper:
                 ops.GEMM_CHAINS = prev_chains
         inpaint = (self.inp_z, self.inp_n, self.inp_m) if self.inpaint else None
         tiled = {} if self.tiles is None else dict(tiles=self.tiles)
+        if self.regions is not None:
+            tiled = dict(regions=(self.cover, self.regions))
         if self.guidance_rescale > 0:                  # diffusers' rescale_noise_cfg, before the scheduler step
             ops.cfg_rescale_factors(eps, self.coef_cur, self.guidance, out=self.rescale_factors)
             self.scheduler.fused_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance, inpaint,

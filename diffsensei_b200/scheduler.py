@@ -18,7 +18,7 @@ step's PAG scale (``pag_scales``) to that table.
 and rejects any class or value whose arithmetic is not implemented here.
 
 The per-step update itself runs on the GPU, fused with the guidance blend, the optional guidance rescale, the inpaint
-blend and the next step's input scaling (``fused_step_``, ``ds_cfg_step``, or ``ds_tile_step`` on a tiled canvas); these classes produce the timesteps, the per-step coefficient table
+blend and the next step's input scaling (``fused_step_``, ``ds_cfg_step``, or ``ds_tile_step`` / ``ds_region_step`` on a tiled / regional canvas); these classes produce the timesteps, the per-step coefficient table
 the kernel reads (``coefficient_table``) and the divisor of the first step's UNet input (``model_input_divisors``).
 """
 from __future__ import annotations
@@ -110,13 +110,16 @@ class DDIMScheduler:
         return [1.0] * len(self.timesteps)
 
     def fused_step_(self, noise_pred, latents, model_in, coef, guidance: float, inpaint=None, rescale=None,
-                    tiles=None) -> None:
+                    tiles=None, regions=None) -> None:
         """The guidance blend + DDIM update (``ops.cfg_step_``): ``coef`` is a row of ``step_table``, with the PAG
         scale appended for a 3-chunk ``noise_pred``; ``inpaint`` None or (image_latents, noise, mask); ``rescale``
         None or (factors, guidance_rescale), the guided eps rescaled first (``ops.cfg_rescale_factors``).  ``tiles``:
-        a ``TileGrid`` when ``latents`` is a canvas denoised as its views (``ops.tile_step_``)."""
+        a ``TileGrid`` when ``latents`` is a canvas denoised as its views (``ops.tile_step_``); ``regions``: (cover, R)
+        when it is a canvas denoised under per-region prompts (``ops.region_step_``)."""
         if tiles is not None:
             ops.tile_step_(noise_pred, latents, model_in, coef, guidance, False, tiles, inpaint, rescale)
+        elif regions is not None:
+            ops.region_step_(noise_pred, latents, model_in, coef, guidance, False, regions, inpaint, rescale)
         else:
             ops.cfg_step_(noise_pred, latents, model_in, coef, guidance, euler=False, inpaint=inpaint, rescale=rescale)
 
@@ -187,10 +190,12 @@ class EulerDiscreteScheduler:
         return self._divisors()[:-1].tolist()
 
     def fused_step_(self, noise_pred, latents, model_in, coef, guidance: float, inpaint=None, rescale=None,
-                    tiles=None) -> None:
+                    tiles=None, regions=None) -> None:
         """The guidance blend + Euler update + the next step's scale_model_input (``ops.cfg_step_``); see DDIM's."""
         if tiles is not None:
             ops.tile_step_(noise_pred, latents, model_in, coef, guidance, True, tiles, inpaint, rescale)
+        elif regions is not None:
+            ops.region_step_(noise_pred, latents, model_in, coef, guidance, True, regions, inpaint, rescale)
         else:
             ops.cfg_step_(noise_pred, latents, model_in, coef, guidance, euler=True, inpaint=inpaint, rescale=rescale)
 

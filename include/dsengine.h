@@ -411,6 +411,27 @@ int ds_tile_step(const void* noise_pred, float* latents, void* model_in, const f
                  const float* rescale_factors, double guidance_rescale, int bs, int H, int W, int tile_h, int tile_w,
                  int stride_h, int stride_w, int C, void* stream);
 
+/* ds_region_step: ds_cfg_step on a canvas denoised under per-region prompts (MultiDiffusion's region-based
+ * generation, Bar-Tal et al. 2023 sec. 4.2).                                      [HBM-bound]
+ *   latents       : fp32 NHWC [bs][HW][4], the canvas (updated in place)
+ *   noise_pred    : bf16 NHWC [chunks * bs * R'][HW][4], model_in the same shape; R' = n_regions + 1; row
+ *                   c * bs * R' + b * R' + r is chunk c of canvas sample b under prompt r (r = 0: the background)
+ *   cover         : uint8 [bs][HW]; bit r - 1 set <=> region r covers the pixel (bits >= n_regions are ignored); the
+ *                   background covers exactly the pixels whose byte is 0
+ *   n_regions     : 1 .. 8
+ *   image_latents / noise / mask : canvas-sized as in ds_cfg_step (all three or none)
+ *   rescale_factors : NULL or fp32 [bs * R'], one factor per row (ds_cfg_rescale_factors over the rows)
+ *   update, chunks, coef, guidance, guidance_rescale : as ds_cfg_step
+ * Per canvas pixel: each covering row, in row order, gives x_r = ds_cfg_step's update of the canvas pixel from that
+ * row's eps (and that row's factor); x_new = (0 + x_r1 + x_r2 + ...) / count in fp32, each sum and the division
+ * rounded on their own (one covering row: ds_cfg_step's bits); then the inpaint blend on the canvas pixel; then the
+ * canvas and the next UNet input (ds_cfg_step's) in every chunk of all R' rows.  latents, image_latents and noise must
+ * be 16-byte aligned, noise_pred and model_in 8-byte.  No atomics: every output element is written by one thread once. */
+int ds_region_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
+                   int update, int chunks, const float* image_latents, const float* noise, const uint8_t* mask,
+                   const float* rescale_factors, double guidance_rescale, const uint8_t* cover, int n_regions, int bs,
+                   int HW, int C, void* stream);
+
 /* Perceiver attention of the character Resampler: 16 latent queries x (n_kv) keys per (character, head),
  * q and k each pre-scaled by dim_head^-0.25, fp32 softmax (src/models/resampler.py:64-74).
  *   q: bf16 [Bc][nq][C], kv: bf16 [Bc][n_kv][2*C] (k | v), out: bf16 [Bc][nq][C]; C = heads*64 */
