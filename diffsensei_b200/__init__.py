@@ -16,6 +16,8 @@ Public surface (mirrors the reference's, SURVEY.md §8b):
     DiffSenseiPipeline     <- src/pipelines/pipeline_diffsensei.py  (denoise loop)
     T2IAdapterEngine       <- diffusers T2IAdapter (full_adapter_xl), the input of UNetMangaModel.forward's
                               down_intrablock_additional_residuals (``DiffSenseiPipeline(adapter=...)``)
+    PipelineCallback, MultiPipelineCallbacks, SDXLCFGCutoffCallback  <- diffusers.callbacks (``callback_on_step_end``;
+                              a CFG cutoff runs the late steps on the text rows alone)
     DDIMScheduler, EulerDiscreteScheduler, scheduler_from_config  <- the diffusers schedulers a checkpoint's
                               scheduler_config.json may name (SDXL-base configuration only)
     AgentEngine, LlamaEngine  <- src/models/mllm/seed_x.py ContinuousLVLM (greedy LLaMA generate of the MLLM agent)
@@ -28,6 +30,7 @@ from . import _lib  # noqa: F401  (loads libdsengine.so or raises ImportError)
 from . import ops  # noqa: F401
 from .adapter import T2IAdapterEngine  # noqa: F401
 from .agent import AgentEngine, LlamaEngine  # noqa: F401
+from .callbacks import MultiPipelineCallbacks, PipelineCallback, SDXLCFGCutoffCallback  # noqa: F401
 from .attention_processor import AttnProcessor2_0, MaskedIPAttnProcessor2_0  # noqa: F401
 from .config import (ADAPTER_TINY, SDXL_ADAPTER, AdapterConfig, AGENT_TINY, LLAMA2_13B, RESAMPLER, RESAMPLER_TINY, SDXL_MANGA, SDXL_VAE, TINY, TINY_VAE, ResamplerConfig, UNetConfig,  # noqa: F401
                      AgentConfig, VaeConfig)

@@ -180,6 +180,19 @@ __device__ __forceinline__ void load_cfg_halves(const uint2* __restrict__ noise_
   tt[0] = bf16_lo(et.x), tt[1] = bf16_hi(et.x), tt[2] = bf16_lo(et.y), tt[3] = bf16_hi(et.y);
 }
 
+// A step kernel's eps of pixel i: the uncond and text halves, or with one chunk (no guidance: noise_pred holds the
+// text chunk only) the text eps into tt, u left unread.
+template <int kChunks>
+__device__ __forceinline__ void load_eps(const uint2* __restrict__ noise_pred, long long i, long long n_pix,
+                                         float u[4], float tt[4]) {
+  if constexpr (kChunks == 1) {
+    const uint2 et = __ldg(noise_pred + i);
+    tt[0] = bf16_lo(et.x), tt[1] = bf16_hi(et.x), tt[2] = bf16_lo(et.y), tt[3] = bf16_hi(et.y);
+  } else {
+    load_cfg_halves(noise_pred, i, n_pix, u, tt);
+  }
+}
+
 // xv <- DDIM(CFG(u, tt)) in place, the compiler free to contract into FMAs; coef = {alpha_prod_t, alpha_prod_t_prev}
 __device__ __forceinline__ void cfg_ddim_pixel(const float u[4], const float tt[4], float xv[4],
                                                const float* __restrict__ coef, float guidance) {
@@ -283,7 +296,14 @@ __device__ __forceinline__ void guided_update(const uint2* __restrict__ noise_pr
                                               const float* __restrict__ coef, float guidance,
                                               const float* __restrict__ rescale, int HW, float phi,
                                               float one_m_phi) {
-  if constexpr (!kEuler && kChunks == 2 && !kRescale) {
+  static_assert(kChunks > 1 || !kRescale, "guidance_rescale needs the guided eps");
+  if constexpr (kChunks == 1) {
+    // no guidance: the text eps as it comes, diffusers' eager scheduler.step(noise_pred_text)
+    if constexpr (kEuler)
+      euler_update_rn(tt, xv, coef);
+    else
+      ddim_update_rn(tt, xv, coef);
+  } else if constexpr (!kEuler && kChunks == 2 && !kRescale) {
     // the CFG-only DDIM step has always let the compiler contract into FMAs; rounding it op by op changes its bits
     cfg_ddim_pixel(u, tt, xv, coef, guidance);
   } else {
@@ -297,7 +317,7 @@ __device__ __forceinline__ void guided_update(const uint2* __restrict__ noise_pr
   }
 }
 
-// noise_pred holds kChunks chunks of n_pix pixels, [uncond ; text (; perturbed)]; coef is the step's row
+// noise_pred holds kChunks chunks of n_pix pixels, [uncond ; text (; perturbed)], or [text] with no guidance; coef is the step's row
 // {update (2 DDIM, 3 Euler) | c0, c1 if kInpaint | s if kChunks == 3}.  kRescale: the guided eps of sample i / HW is
 // rescaled with the factor rescale[i / HW] (cfg_rescale_factors_kernel) before the update.
 template <bool kEuler, int kChunks, bool kInpaint, bool kRescale>
@@ -306,13 +326,13 @@ __global__ void cfg_step_kernel(const uint2* __restrict__ noise_pred, float4* __
                                 long long n_pix /* bs*HW */, const float4* __restrict__ image_latents,
                                 const float4* __restrict__ noise, const unsigned char* __restrict__ mask,
                                 const float* __restrict__ rescale, float phi, float one_m_phi, int HW) {
-  static_assert(kChunks == 2 || kChunks == 3, "CFG (2 chunks) or CFG + PAG (3 chunks)");
+  static_assert(1 <= kChunks && kChunks <= 3, "no guidance (1 chunk), CFG (2) or CFG + PAG (3)");
   constexpr int kC0 = kEuler ? 3 : 2;                 // {c0, c1} follow the update's coefficients
   constexpr int kS = kC0 + (kInpaint ? 2 : 0);         // then the PAG scale
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= n_pix) return;
   float u[4], tt[4];
-  load_cfg_halves(noise_pred, i, n_pix, u, tt);
+  load_eps<kChunks>(noise_pred, i, n_pix, u, tt);
   const float4 x = latents[i];
   float xv[4] = {x.x, x.y, x.z, x.w};
   guided_update<kEuler, kChunks, kRescale, kS>(noise_pred, i, n_pix, u, tt, xv, coef, guidance, rescale, HW, phi,
@@ -348,7 +368,7 @@ __global__ void tile_step_kernel(const uint2* __restrict__ noise_pred, float4* _
                                  const float4* __restrict__ image_latents, const float4* __restrict__ noise,
                                  const unsigned char* __restrict__ mask, const float* __restrict__ rescale, float phi,
                                  float one_m_phi) {
-  static_assert(kChunks == 2 || kChunks == 3, "CFG (2 chunks) or CFG + PAG (3 chunks)");
+  static_assert(1 <= kChunks && kChunks <= 3, "no guidance (1 chunk), CFG (2) or CFG + PAG (3)");
   constexpr int kC0 = kEuler ? 3 : 2;
   constexpr int kS = kC0 + (kInpaint ? 2 : 0);
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -370,7 +390,7 @@ __global__ void tile_step_kernel(const uint2* __restrict__ noise_pred, float4* _
     for (int vx = xlo; vx <= xhi; ++vx) {
       const long long j = row0 + vx * static_cast<long long>(view_hw) + (x - tile_origin(ax, vx));
       float u[4], tt[4];
-      load_cfg_halves(noise_pred, j, n_pix, u, tt);
+      load_eps<kChunks>(noise_pred, j, n_pix, u, tt);
       float xv[4] = {xc.x, xc.y, xc.z, xc.w};
       guided_update<kEuler, kChunks, kRescale, kS>(noise_pred, j, n_pix, u, tt, xv, coef, guidance, rescale, view_hw,
                                                    phi, one_m_phi);
@@ -417,7 +437,7 @@ __global__ void region_step_kernel(const uint2* __restrict__ noise_pred, float4*
                                    const float4* __restrict__ image_latents, const float4* __restrict__ noise,
                                    const unsigned char* __restrict__ mask, const float* __restrict__ rescale,
                                    float phi, float one_m_phi) {
-  static_assert(kChunks == 2 || kChunks == 3, "CFG (2 chunks) or CFG + PAG (3 chunks)");
+  static_assert(1 <= kChunks && kChunks <= 3, "no guidance (1 chunk), CFG (2) or CFG + PAG (3)");
   constexpr int kC0 = kEuler ? 3 : 2;
   constexpr int kS = kC0 + (kInpaint ? 2 : 0);
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -432,7 +452,7 @@ __global__ void region_step_kernel(const uint2* __restrict__ noise_pred, float4*
   for (unsigned m = rows; m != 0; m &= m - 1) {
     const long long j = row0 + static_cast<long long>(__ffs(m) - 1) * HW;
     float u[4], tt[4];
-    load_cfg_halves(noise_pred, j, n_pix, u, tt);
+    load_eps<kChunks>(noise_pred, j, n_pix, u, tt);
     float xv[4] = {xc.x, xc.y, xc.z, xc.w};
     guided_update<kEuler, kChunks, kRescale, kS>(noise_pred, j, n_pix, u, tt, xv, coef, guidance, rescale, HW, phi,
                                                  one_m_phi);
@@ -665,7 +685,9 @@ extern "C" int ds_cfg_step(const void* noise_pred, float* latents, void* model_i
   DS_REQUIRE(!inpaint || (image_latents && noise && mask),
              "ds_cfg_step: image_latents / noise / mask must all be given or all be NULL");
   DS_REQUIRE(update == 0 || update == 1, "ds_cfg_step: update must be 0 (DDIM) or 1 (Euler), got %d", update);
-  DS_REQUIRE(chunks == 2 || chunks == 3, "ds_cfg_step: chunks must be 2 or 3, got %d", chunks);
+  DS_REQUIRE(1 <= chunks && chunks <= 3,
+             "ds_cfg_step: chunks must be 2 or 3 (CFG, CFG + PAG) or 1 (no guidance), got %d", chunks);
+  DS_REQUIRE(chunks > 1 || !rescale, "ds_cfg_step: rescale_factors must be NULL with 1 chunk (no guidance)");
   DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "ds_cfg_step: only C == 4 latents are supported (got C=%d)", C);
   DS_REQUIRE(!inpaint || ((reinterpret_cast<uintptr_t>(image_latents) & 15) == 0 &&
                           (reinterpret_cast<uintptr_t>(noise) & 15) == 0),
@@ -677,17 +699,21 @@ extern "C" int ds_cfg_step(const void* noise_pred, float* latents, void* model_i
   if (!get_device(&dev)) return DS_ERR_CUDA;
   using StepKernel = void (*)(const uint2*, float4*, uint2*, const float*, float, long long, const float4*,
                               const float4*, const unsigned char*, const float*, float, float, int);
-  static constexpr StepKernel kKernels[2][2][2][2] = {  // [update][chunks - 2][inpaint][rescale]
-      {{{cfg_step_kernel<false, 2, false, false>, cfg_step_kernel<false, 2, false, true>},
-        {cfg_step_kernel<false, 2, true, false>, cfg_step_kernel<false, 2, true, true>}},
-       {{cfg_step_kernel<false, 3, false, false>, cfg_step_kernel<false, 3, false, true>},
-        {cfg_step_kernel<false, 3, true, false>, cfg_step_kernel<false, 3, true, true>}}},
-      {{{cfg_step_kernel<true, 2, false, false>, cfg_step_kernel<true, 2, false, true>},
-        {cfg_step_kernel<true, 2, true, false>, cfg_step_kernel<true, 2, true, true>}},
-       {{cfg_step_kernel<true, 3, false, false>, cfg_step_kernel<true, 3, false, true>},
-        {cfg_step_kernel<true, 3, true, false>, cfg_step_kernel<true, 3, true, true>}}}};
+  static constexpr StepKernel kKernels[2][3][2][2] = {  // [update][chunks - 1][inpaint][rescale]; 1 chunk never rescales
+      {{{cfg_step_kernel<false, 1, false, false>, nullptr},
+       {cfg_step_kernel<false, 1, true, false>, nullptr}},
+      {{cfg_step_kernel<false, 2, false, false>, cfg_step_kernel<false, 2, false, true>},
+       {cfg_step_kernel<false, 2, true, false>, cfg_step_kernel<false, 2, true, true>}},
+      {{cfg_step_kernel<false, 3, false, false>, cfg_step_kernel<false, 3, false, true>},
+       {cfg_step_kernel<false, 3, true, false>, cfg_step_kernel<false, 3, true, true>}}},
+      {{{cfg_step_kernel<true, 1, false, false>, nullptr},
+       {cfg_step_kernel<true, 1, true, false>, nullptr}},
+      {{cfg_step_kernel<true, 2, false, false>, cfg_step_kernel<true, 2, false, true>},
+       {cfg_step_kernel<true, 2, true, false>, cfg_step_kernel<true, 2, true, true>}},
+      {{cfg_step_kernel<true, 3, false, false>, cfg_step_kernel<true, 3, false, true>},
+       {cfg_step_kernel<true, 3, true, false>, cfg_step_kernel<true, 3, true, true>}}}};
   const long long n_pix = static_cast<long long>(bs) * HW;
-  kKernels[update][chunks - 2][inpaint][rescale]<<<static_cast<unsigned>((n_pix + 255) / 256), 256, 0,
+  kKernels[update][chunks - 1][inpaint][rescale]<<<static_cast<unsigned>((n_pix + 255) / 256), 256, 0,
                                                    static_cast<cudaStream_t>(stream)>>>(
       static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
       guidance, n_pix, reinterpret_cast<const float4*>(image_latents), reinterpret_cast<const float4*>(noise), mask,
@@ -707,7 +733,9 @@ extern "C" int ds_tile_step(const void* noise_pred, float* latents, void* model_
   DS_REQUIRE(!inpaint || (image_latents && noise && mask),
              "ds_tile_step: image_latents / noise / mask must all be given or all be NULL");
   DS_REQUIRE(update == 0 || update == 1, "ds_tile_step: update must be 0 (DDIM) or 1 (Euler), got %d", update);
-  DS_REQUIRE(chunks == 2 || chunks == 3, "ds_tile_step: chunks must be 2 or 3, got %d", chunks);
+  DS_REQUIRE(1 <= chunks && chunks <= 3,
+             "ds_tile_step: chunks must be 2 or 3 (CFG, CFG + PAG) or 1 (no guidance), got %d", chunks);
+  DS_REQUIRE(chunks > 1 || !rescale, "ds_tile_step: rescale_factors must be NULL with 1 chunk (no guidance)");
   DS_REQUIRE(bs > 0 && C == 4, "ds_tile_step: only C == 4 latents are supported (got C=%d)", C);
   DS_REQUIRE(0 < tile_h && tile_h <= H && 0 < tile_w && tile_w <= W,
              "ds_tile_step: the view (%d x %d) must fit the canvas (%d x %d)", tile_h, tile_w, H, W);
@@ -726,17 +754,21 @@ extern "C" int ds_tile_step(const void* noise_pred, float* latents, void* model_
   const TileAxis ax{W, tile_w, stride_w, (W - tile_w + stride_w - 1) / stride_w + 1};
   using TileKernel = void (*)(const uint2*, float4*, uint2*, const float*, float, TileAxis, TileAxis, int,
                               const float4*, const float4*, const unsigned char*, const float*, float, float);
-  static constexpr TileKernel kKernels[2][2][2][2] = {  // [update][chunks - 2][inpaint][rescale]
-      {{{tile_step_kernel<false, 2, false, false>, tile_step_kernel<false, 2, false, true>},
-        {tile_step_kernel<false, 2, true, false>, tile_step_kernel<false, 2, true, true>}},
-       {{tile_step_kernel<false, 3, false, false>, tile_step_kernel<false, 3, false, true>},
-        {tile_step_kernel<false, 3, true, false>, tile_step_kernel<false, 3, true, true>}}},
-      {{{tile_step_kernel<true, 2, false, false>, tile_step_kernel<true, 2, false, true>},
-        {tile_step_kernel<true, 2, true, false>, tile_step_kernel<true, 2, true, true>}},
-       {{tile_step_kernel<true, 3, false, false>, tile_step_kernel<true, 3, false, true>},
-        {tile_step_kernel<true, 3, true, false>, tile_step_kernel<true, 3, true, true>}}}};
+  static constexpr TileKernel kKernels[2][3][2][2] = {  // [update][chunks - 1][inpaint][rescale]; 1 chunk never rescales
+      {{{tile_step_kernel<false, 1, false, false>, nullptr},
+       {tile_step_kernel<false, 1, true, false>, nullptr}},
+      {{tile_step_kernel<false, 2, false, false>, tile_step_kernel<false, 2, false, true>},
+       {tile_step_kernel<false, 2, true, false>, tile_step_kernel<false, 2, true, true>}},
+      {{tile_step_kernel<false, 3, false, false>, tile_step_kernel<false, 3, false, true>},
+       {tile_step_kernel<false, 3, true, false>, tile_step_kernel<false, 3, true, true>}}},
+      {{{tile_step_kernel<true, 1, false, false>, nullptr},
+       {tile_step_kernel<true, 1, true, false>, nullptr}},
+      {{tile_step_kernel<true, 2, false, false>, tile_step_kernel<true, 2, false, true>},
+       {tile_step_kernel<true, 2, true, false>, tile_step_kernel<true, 2, true, true>}},
+      {{tile_step_kernel<true, 3, false, false>, tile_step_kernel<true, 3, false, true>},
+       {tile_step_kernel<true, 3, true, false>, tile_step_kernel<true, 3, true, true>}}}};
   const long long n_canvas = static_cast<long long>(bs) * H * W;
-  kKernels[update][chunks - 2][inpaint][rescale]<<<static_cast<unsigned>((n_canvas + 255) / 256), 256, 0,
+  kKernels[update][chunks - 1][inpaint][rescale]<<<static_cast<unsigned>((n_canvas + 255) / 256), 256, 0,
                                                    static_cast<cudaStream_t>(stream)>>>(
       static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
       guidance, ay, ax, bs, reinterpret_cast<const float4*>(image_latents), reinterpret_cast<const float4*>(noise),
@@ -755,7 +787,9 @@ extern "C" int ds_region_step(const void* noise_pred, float* latents, void* mode
   DS_REQUIRE(!inpaint || (image_latents && noise && mask),
              "ds_region_step: image_latents / noise / mask must all be given or all be NULL");
   DS_REQUIRE(update == 0 || update == 1, "ds_region_step: update must be 0 (DDIM) or 1 (Euler), got %d", update);
-  DS_REQUIRE(chunks == 2 || chunks == 3, "ds_region_step: chunks must be 2 or 3, got %d", chunks);
+  DS_REQUIRE(1 <= chunks && chunks <= 3,
+             "ds_region_step: chunks must be 2 or 3 (CFG, CFG + PAG) or 1 (no guidance), got %d", chunks);
+  DS_REQUIRE(chunks > 1 || !rescale, "ds_region_step: rescale_factors must be NULL with 1 chunk (no guidance)");
   DS_REQUIRE(1 <= n_regions && n_regions <= 8, "ds_region_step: n_regions must be in [1, 8], got %d", n_regions);
   DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "ds_region_step: only C == 4 latents are supported (got C=%d)", C);
   DS_REQUIRE((reinterpret_cast<uintptr_t>(latents) & 15) == 0 && (reinterpret_cast<uintptr_t>(noise_pred) & 7) == 0 &&
@@ -771,17 +805,21 @@ extern "C" int ds_region_step(const void* noise_pred, float* latents, void* mode
   if (!get_device(&dev)) return DS_ERR_CUDA;
   using RegionKernel = void (*)(const uint2*, float4*, uint2*, const float*, float, const unsigned char*, int, int,
                                 int, const float4*, const float4*, const unsigned char*, const float*, float, float);
-  static constexpr RegionKernel kKernels[2][2][2][2] = {  // [update][chunks - 2][inpaint][rescale]
-      {{{region_step_kernel<false, 2, false, false>, region_step_kernel<false, 2, false, true>},
-        {region_step_kernel<false, 2, true, false>, region_step_kernel<false, 2, true, true>}},
-       {{region_step_kernel<false, 3, false, false>, region_step_kernel<false, 3, false, true>},
-        {region_step_kernel<false, 3, true, false>, region_step_kernel<false, 3, true, true>}}},
-      {{{region_step_kernel<true, 2, false, false>, region_step_kernel<true, 2, false, true>},
-        {region_step_kernel<true, 2, true, false>, region_step_kernel<true, 2, true, true>}},
-       {{region_step_kernel<true, 3, false, false>, region_step_kernel<true, 3, false, true>},
-        {region_step_kernel<true, 3, true, false>, region_step_kernel<true, 3, true, true>}}}};
+  static constexpr RegionKernel kKernels[2][3][2][2] = {  // [update][chunks - 1][inpaint][rescale]; 1 chunk never rescales
+      {{{region_step_kernel<false, 1, false, false>, nullptr},
+       {region_step_kernel<false, 1, true, false>, nullptr}},
+      {{region_step_kernel<false, 2, false, false>, region_step_kernel<false, 2, false, true>},
+       {region_step_kernel<false, 2, true, false>, region_step_kernel<false, 2, true, true>}},
+      {{region_step_kernel<false, 3, false, false>, region_step_kernel<false, 3, false, true>},
+       {region_step_kernel<false, 3, true, false>, region_step_kernel<false, 3, true, true>}}},
+      {{{region_step_kernel<true, 1, false, false>, nullptr},
+       {region_step_kernel<true, 1, true, false>, nullptr}},
+      {{region_step_kernel<true, 2, false, false>, region_step_kernel<true, 2, false, true>},
+       {region_step_kernel<true, 2, true, false>, region_step_kernel<true, 2, true, true>}},
+      {{region_step_kernel<true, 3, false, false>, region_step_kernel<true, 3, false, true>},
+       {region_step_kernel<true, 3, true, false>, region_step_kernel<true, 3, true, true>}}}};
   const long long n_canvas = static_cast<long long>(bs) * HW;
-  kKernels[update][chunks - 2][inpaint][rescale]<<<static_cast<unsigned>((n_canvas + 255) / 256), 256, 0,
+  kKernels[update][chunks - 1][inpaint][rescale]<<<static_cast<unsigned>((n_canvas + 255) / 256), 256, 0,
                                                    static_cast<cudaStream_t>(stream)>>>(
       static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
       guidance, cover, n_regions + 1, bs, HW, reinterpret_cast<const float4*>(image_latents),

@@ -698,7 +698,8 @@ def cfg_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.T
               guidance: float, euler: bool, inpaint=None, rescale=None) -> None:
     """The fused end of a denoise step (``ds_cfg_step``), in place.  noise_pred bf16 [k*bs,H,W,4] holds k = 2 chunks
     [uncond ; text] (CFG) or k = 3 [uncond ; text ; perturbed] (CFG + perturbed-attention guidance):
-    eps = u + guidance (t - u) [+ s (t - p)].  latents fp32 NHWC [bs,H,W,4] <- DDIM or (``euler``) Euler update;
+    eps = u + guidance (t - u) [+ s (t - p)]; or k = 1, the text chunk alone (no guidance, after a CFG cutoff):
+    eps = t, ``guidance`` unused and ``rescale`` must be None.  latents fp32 NHWC [bs,H,W,4] <- DDIM or (``euler``) Euler update;
     model_in bf16 [k*bs,H,W,4] <- cat[x]*k (DDIM) or cat[x / coef[2]]*k (Euler).  ``inpaint`` None or
     (image_latents, noise, mask): fp32 NHWC [bs,H,W,4] twice and uint8 [bs,H,W]; where mask is 0 the latents become
     c0 * image_latents + c1 * noise.  ``rescale`` None or (factors, guidance_rescale): factors fp32 [bs] from
@@ -713,7 +714,7 @@ def cfg_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.T
     bs, H, W, Cc = latents.shape
     chunks = noise_pred.shape[0] // bs if bs else 0
     ncoef = (3 if euler else 2) + (0 if inpaint is None else 2) + (chunks == 3)
-    if chunks not in (2, 3) or noise_pred.shape != (chunks * bs, H, W, Cc) or model_in.shape != noise_pred.shape \
+    if chunks not in (1, 2, 3) or noise_pred.shape != (chunks * bs, H, W, Cc) or model_in.shape != noise_pred.shape \
             or coef.numel() != ncoef:
         raise DsEngineError("cfg_step: shape mismatch")
     ptrs, factors, phi = _step_state("cfg_step", latents, bs, inpaint, rescale)
@@ -761,7 +762,7 @@ def tile_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.
     rows = bs * tiles.n_views
     chunks = noise_pred.shape[0] // rows if rows else 0
     ncoef = (3 if euler else 2) + (0 if inpaint is None else 2) + (chunks == 3)
-    if (H, W) != (tiles.height, tiles.width) or chunks not in (2, 3) or \
+    if (H, W) != (tiles.height, tiles.width) or chunks not in (1, 2, 3) or \
             noise_pred.shape != (chunks * rows, tiles.tile_h, tiles.tile_w, Cc) or \
             model_in.shape != noise_pred.shape or coef.numel() != ncoef:
         raise DsEngineError("tile_step: shape mismatch")
@@ -791,7 +792,7 @@ def region_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torc
     rows = bs * (n_regions + 1)
     chunks = noise_pred.shape[0] // rows if rows else 0
     ncoef = (3 if euler else 2) + (0 if inpaint is None else 2) + (chunks == 3)
-    if not 1 <= n_regions <= 8 or chunks not in (2, 3) or noise_pred.shape != (chunks * rows, H, W, Cc) or \
+    if not 1 <= n_regions <= 8 or chunks not in (1, 2, 3) or noise_pred.shape != (chunks * rows, H, W, Cc) or \
             model_in.shape != noise_pred.shape or cover.shape != (bs, H, W) or coef.numel() != ncoef:
         raise DsEngineError("region_step: shape mismatch")
     ptrs, factors, phi = _step_state("region_step", latents, rows, inpaint, rescale)

@@ -44,7 +44,7 @@ from typing import List, Optional, Union
 import numpy as np
 import torch
 
-from . import ops
+from . import callbacks, ops
 from .image_processor import (CLIPImageProcessor, VaeImageProcessor, ViTImageProcessor, adapter_image_info,
                               adapter_image_u8)
 from .lora import AdapterRegistry, lora_targets, normalize_lora, split_components
@@ -120,6 +120,16 @@ def check_guidance_rescale(guidance_rescale) -> float:
     if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(v):
         raise ValueError(f"`guidance_rescale` must be a finite real number, got {v!r}")
     return float(v)
+
+
+def cutoff_in_run(cfg_cutoff, steps: int) -> Optional[int]:
+    """The step k after which a denoise of ``steps`` steps runs without guidance, or None when no step follows the
+    cutoff: steps 0 .. k guide, steps k + 1 .. do not.  A cutoff fires at the step i with ``i == cfg_cutoff``, as
+    diffusers' callback compares, so 2.0 fires at step 2, while 2.5, a negative value, None, or a step at or after the
+    last one leave every step guided."""
+    if cfg_cutoff is None:
+        return None
+    return next((i for i in range(int(steps) - 1) if i == cfg_cutoff), None)
 
 
 def _pad_boxes(boxes, m: int) -> List[List[float]]:
@@ -458,21 +468,23 @@ class DiffSenseiPipeline:
                      use_graph: bool = True, chains: Optional[int] = None, start_index: int = 0,
                      inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0,
                      tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS,
-                     regions=None) -> "DenoiseStepper":
+                     regions=None, cfg_cutoff: Optional[int] = None) -> "DenoiseStepper":
         return DenoiseStepper(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                               dialog_bbox, num_inference_steps, guidance_scale, use_graph, chains, start_index,
-                              inpaint, pag, adapter, guidance_rescale, tiles, max_batch_panels, regions)
+                              inpaint, pag, adapter, guidance_rescale, tiles, max_batch_panels, regions, cfg_cutoff)
 
     def stepper_key(self, latents, prompt_embeds, aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale,
                     chains=None, start_index: int = 0, inpaint=None, pag=None, adapter=None,
                     guidance_rescale: float = 0.0, tiles: Optional[TileGrid] = None,
-                    max_batch_panels: int = PAGE_MAX_ROWS, regions=None) -> tuple:
+                    max_batch_panels: int = PAGE_MAX_ROWS, regions=None, cfg_cutoff: Optional[int] = None) -> tuple:
         """Everything a captured stepper bakes in (``stepper_for``), FreeU's values (``unet.freeu``) and whether a
         T2I-Adapter's features are added included.  With ``guidance_rescale > 0`` the key ends with its value, which
         the graph bakes in like ``guidance_scale``; otherwise the key is the one the step without the rescale has.
         With ``tiles`` it ends with the view grid and the UNet slice size (``max_batch_panels``); without, neither is
         in it.  With ``regions`` = (cover, R) it ends with ("regions", R + 1, ``max_batch_panels``); the cover is per
-        panel data that ``load_panel`` refills, so it is not in the key."""
+        panel data that ``load_panel`` refills, so it is not in the key.  With a CFG cutoff inside the run
+        (``cfg_cutoff`` = k, 0 <= k < steps run - 1) it ends with ("cfg_cutoff", k): the stepper then has a second
+        graph, over the text rows; a cutoff at or after the last step leaves the key as it is."""
         key = (tuple(latents.shape), tuple(prompt_embeds.shape), None if dialog_bbox is None else
                 (tuple(dialog_bbox.shape), dialog_bbox.dtype == bf16), float(aspect_ratio), int(num_inference_steps),
                 float(guidance_scale), self.unet.scales_key(), chains, self.unet._ip_weights_version(),
@@ -485,28 +497,32 @@ class DiffSenseiPipeline:
             key += (("tiles", tiles, int(max_batch_panels)),)
         if regions is not None:
             key += (("regions", int(regions[1]) + 1, int(max_batch_panels)),)
+        k = cutoff_in_run(cfg_cutoff, int(num_inference_steps) - int(start_index))
+        if k is not None:
+            key += (("cfg_cutoff", k),)
         return key
 
     def stepper_for(self, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio, dialog_bbox,
                     num_inference_steps, guidance_scale, chains=None, start_index: int = 0,
                     inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0,
                     tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS,
-                    regions=None) -> "DenoiseStepper":
+                    regions=None, cfg_cutoff: Optional[int] = None) -> "DenoiseStepper":
         """A graph-captured stepper loaded with this panel: a cached one of the same key is refilled in place
         (no re-capture), otherwise a new one is built and cached.  The start index is part of the key: the stepper
         bakes in its slice of the schedule (``set_timesteps`` would reset any scheduler state); so is whether it
         inpaints, which selects the step kernel, the perturbed-attention sites (``pag``: None when off) and FreeU's
         values, which the graph bakes in, and whether it adds adapter features, and ``guidance_rescale``.  The PAG
         scales are not: they live in the coefficient table, which ``load_panel`` rewrites, as it rewrites the adapter
-        features and gates."""
+        features and gates.  A CFG cutoff inside the run (``cfg_cutoff``) is in the key too."""
         key = self.stepper_key(latents, prompt_embeds, aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale,
                                chains, start_index, inpaint, pag, adapter, guidance_rescale, tiles, max_batch_panels,
-                               regions)
+                               regions, cfg_cutoff)
         st = self._steppers.get(key)
         if st is None:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                    dialog_bbox, num_inference_steps, guidance_scale, True, chains, start_index,
-                                   inpaint, pag, adapter, guidance_rescale, tiles, max_batch_panels, regions)
+                                   inpaint, pag, adapter, guidance_rescale, tiles, max_batch_panels, regions,
+                                   cfg_cutoff)
             while len(self._steppers) >= self.max_cached_steppers:
                 self._steppers.pop(next(iter(self._steppers)))
             self._steppers[key] = st
@@ -543,26 +559,40 @@ class DiffSenseiPipeline:
         for row r, the background where the cover is 0).  ``callback_on_step_end``: diffusers' step-end callback, called as
         ``callback(pipe, i, t, {"latents": fp32 NCHW latents})`` after each step (and its inpaint blend); the latents it
         returns become the loop's (``DenoiseStepper.set_latents``), and once it sets ``pipe._interrupt`` the remaining
-        steps are skipped — a denoise that starts with the flag set returns ``latents`` as given.  Returns the final
-        latents, NCHW fp32."""
-        self._check_callback(callback_on_step_end, callback_on_step_end_tensor_inputs)
+        steps are skipped — a denoise that starts with the flag set returns ``latents`` as given.  A
+        ``PipelineCallback`` / ``MultiPipelineCallbacks`` (``callbacks.py``, or diffusers' own) runs with its own
+        ``tensor_inputs``; a CFG cutoff in it (``SDXLCFGCutoffCallback``) is applied by the loop: k is computed from
+        this denoise's step count, the denoise starts at ``guidance_scale``, step k sets ``pipe._guidance_scale = 0.0``
+        at the cutoff's place in the list, and steps k + 1 .. run the UNet on the positive rows alone with no
+        guidance, no ``guidance_rescale`` and the inpaint blend (``DenoiseStepper``).  Returns the final latents, NCHW
+        fp32."""
+        entries, inputs = self._check_callback(callback_on_step_end, callback_on_step_end_tensor_inputs, pag_scale)
         self._num_timesteps = int(num_inference_steps) - int(start_index)
         if callback_on_step_end is not None and self._interrupt:
             return latents.to(device=self.unet.device, dtype=f32).contiguous()
         guidance_rescale = check_guidance_rescale(guidance_rescale)
+        cutoffs = [callbacks.cutoff_step(e.config, self._num_timesteps) for e in entries or ()
+                   if isinstance(e, callbacks.CfgCutoff)]
+        cfg_cutoff = None
+        if cutoffs:
+            self._guidance_scale = guidance_scale
+            # the first cutoff that fires inside the run: one that never fires leaves guidance (and the flag) as is
+            inside = [k for k in (cutoff_in_run(c, self._num_timesteps) for c in cutoffs) if k is not None]
+            cfg_cutoff = min(inside, default=None)
         self.unet.set_lora_scale(1.0)            # a direct unet(..., cross_attention_kwargs={"scale": s}) call may have left s
         pag = self._pag(pag_scale, pag_adaptive_scale)
+        cut = {} if cfg_cutoff is None else dict(cfg_cutoff=cfg_cutoff)
         if use_graph:
             st = self.stepper_for(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                   dialog_bbox, num_inference_steps, guidance_scale, start_index=start_index,
                                   inpaint=inpaint, pag=pag, adapter=adapter, guidance_rescale=guidance_rescale,
-                                  tiles=tiles, max_batch_panels=max_batch_panels, regions=regions)
+                                  tiles=tiles, max_batch_panels=max_batch_panels, regions=regions, **cut)
         else:
             st = self.make_stepper(latents, prompt_embeds, add_text_embeds, add_time_ids, bbox, aspect_ratio,
                                    dialog_bbox, num_inference_steps, guidance_scale, False, start_index=start_index,
                                    inpaint=inpaint, pag=pag, adapter=adapter, guidance_rescale=guidance_rescale,
-                                   tiles=tiles, max_batch_panels=max_batch_panels, regions=regions)
-        offer = "latents" in (callback_on_step_end_tensor_inputs or ())
+                                   tiles=tiles, max_batch_panels=max_batch_panels, regions=regions, **cut)
+        offer = "latents" in (inputs or ())
         for i, t in enumerate(st.timesteps):
             if callback_on_step_end is not None and self._interrupt:
                 continue                                                 # pipeline_diffsensei.py:311-312
@@ -571,20 +601,36 @@ class DiffSenseiPipeline:
                 on_step(i, t, st.lat)
             if callback_on_step_end is not None:
                 kw = {"latents": st.latents_nchw()} if offer else {}
-                out = callback_on_step_end(self, i, t, kw)
+                if entries is None:
+                    out = callback_on_step_end(self, i, t, kw)
+                else:
+                    out = kw
+                    for e in entries:                   # diffusers' MultiPipelineCallbacks order
+                        if not isinstance(e, callbacks.CfgCutoff):
+                            out = e(self, i, t, out)
+                        elif i == callbacks.cutoff_step(e.config, self._num_timesteps):
+                            self._guidance_scale = 0.0
                 lat = out.pop("latents", kw.get("latents"))
                 if lat is not None:
                     st.set_latents(i + 1, lat)
         return st.latents_nchw()
 
-    def _check_callback(self, callback_on_step_end, callback_on_step_end_tensor_inputs) -> None:
-        """diffusers' checks of the step-end callback keywords (host only)."""
+    def _check_callback(self, callback_on_step_end, callback_on_step_end_tensor_inputs, pag_scale=0.0):
+        """diffusers' checks of the step-end callback keywords (host only).  Returns ``callbacks.resolve``'s
+        (entries, tensor inputs): a ``PipelineCallback`` / ``MultiPipelineCallbacks`` brings its own tensor inputs,
+        and a CFG cutoff in it cannot be combined with ``pag_scale > 0``."""
         if callback_on_step_end is not None and not callable(callback_on_step_end):
             raise ValueError(f"`callback_on_step_end` must be callable, got {type(callback_on_step_end).__name__}")
-        bad = [k for k in (callback_on_step_end_tensor_inputs or ()) if k not in self._callback_tensor_inputs]
+        entries, inputs = callbacks.resolve(callback_on_step_end, callback_on_step_end_tensor_inputs)
+        bad = [k for k in (inputs or ()) if k not in self._callback_tensor_inputs]
         if bad:
             raise ValueError(f"`callback_on_step_end_tensor_inputs` has to be in {self._callback_tensor_inputs}, but "
                              f"found {bad}")
+        if any(isinstance(e, callbacks.CfgCutoff) for e in entries or ()):
+            if float(pag_scale) > 0:
+                raise ValueError("a CFG cutoff callback (SDXLCFGCutoffCallback) cannot be combined with "
+                                 "perturbed-attention guidance (pag_scale > 0)")
+        return entries, inputs
 
     # ------------------------------------------------------------------------------ reference-shaped entry point
     @torch.no_grad()
@@ -697,7 +743,7 @@ class DiffSenseiPipeline:
         if isinstance(f, bool) or not isinstance(f, (int, float)) or not 0.0 <= f <= 1.0:
             raise ValueError(f"`adapter_conditioning_factor` must be a number in [0, 1], got {f!r}")
         check_guidance_rescale(guidance_rescale)
-        self._check_callback(callback_on_step_end, callback_on_step_end_tensor_inputs)
+        self._check_callback(callback_on_step_end, callback_on_step_end_tensor_inputs, pag_scale)
         if any(p.get("image") is not None for p in panels):
             return get_timesteps(num_inference_steps, strength)[0]
         return 0
@@ -1354,13 +1400,19 @@ class DenoiseStepper:
     With ``regions`` = (cover, R) (regional prompts) the fp32 master latents are the canvas, ``model_in`` holds R + 1
     copies of every sample in each chunk (row b * (R + 1) + r), the UNet runs them in slices as with ``tiles``, and
     the step is ``ds_region_step`` over the cover, a per-panel buffer ``load_panel`` refills.
+    With ``cfg_cutoff`` = k inside the run (diffusers' ``SDXLCFGCutoffCallback``) steps k + 1 .. run without guidance:
+    the UNet on the text chunk's rows alone (their conditions, time-embedding rows, dialog boxes and adapter rows; the
+    same slicing and chains as the full launch) and the 1-chunk step (eps = text eps, no rescale; the inpaint blend,
+    tiles and regions as before), captured as a second graph.  A guided step writes the text chunk of ``model_in``
+    too, so the switch needs no copy.
     """
 
     @torch.no_grad()
     def __init__(self, pipe: DiffSenseiPipeline, latents, prompt_embeds, add_text_embeds, add_time_ids, bbox,
                  aspect_ratio, dialog_bbox, num_inference_steps, guidance_scale, use_graph=True, chains=None,
                  start_index: int = 0, inpaint=None, pag=None, adapter=None, guidance_rescale: float = 0.0,
-                 tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS, regions=None):
+                 tiles: Optional[TileGrid] = None, max_batch_panels: int = PAGE_MAX_ROWS, regions=None,
+                 cfg_cutoff: Optional[int] = None):
         unet, dev = pipe.unet, pipe.unet.device
         self.unet, self.dev, self.guidance = unet, dev, float(guidance_scale)
         self.scheduler = pipe.scheduler
@@ -1371,6 +1423,9 @@ class DenoiseStepper:
         if not 0 <= s0 < self.num_inference_steps:
             raise ValueError(f"start_index must be in [0, {self.num_inference_steps}), got {start_index}")
         self.timesteps = pipe.scheduler.set_timesteps(num_inference_steps, device=dev)[s0:]
+        self.cfg_cutoff = cutoff_in_run(cfg_cutoff, len(self.timesteps))     # last guided step, None: every step
+        if self.cfg_cutoff is not None and pag is not None:
+            raise ValueError("a CFG cutoff does not combine with perturbed-attention guidance")
         self.inpaint = inpaint is not None
         self.base_coef_table = step_table(pipe.scheduler, s0, dev, self.inpaint)
         self.coef_table = self.base_coef_table
@@ -1414,7 +1469,7 @@ class DenoiseStepper:
         B2 = self.model_in.shape[0]
         want = int(os.environ.get("DS_CHAINS", "1")) if chains is None else int(chains)
         self.chains = max(1, min(want, B2))
-        self._parts, self._side = [(0, B2)], []
+        self._parts, self._cond_parts, self._side = [(0, B2)], [self.cond], []
         # first perturbed row of the whole batch (None: no PAG); each part gets it relative to its own slice
         self._pag_row0 = None if pag is None else 2 * (B2 // self.n_chunks)
         if tiles is not None or regions is not None:    # UNet slices of at most max_batch_panels samples' rows
@@ -1428,6 +1483,18 @@ class DenoiseStepper:
             self._cond_parts = [self.cond.rows(s, e) for s, e in self._parts]
             self._side = [torch.cuda.Stream(device=dev) for _ in self._parts[1:]]
             self._eps = torch.empty_like(self.model_in)
+        self.graph_text = None
+        if self.cfg_cutoff is not None:                 # the text rows [B2 / 2, B2), split as the full launch splits
+            r0 = B2 // 2
+            if tiles is not None or regions is not None:
+                self._text_parts = [(r, min(r + cap, B2)) for r in range(r0, B2, cap)]
+            else:
+                n = min(self.chains, r0)
+                cuts = [r0 + round(k * r0 / n) for k in range(n + 1)]
+                self._text_parts = [(cuts[k], cuts[k + 1]) for k in range(n) if cuts[k + 1] > cuts[k]]
+            self._text_cond_parts = [self.cond.rows(s, e) for s, e in self._text_parts]
+            if len(self._text_parts) > 1:
+                self._eps_text = torch.empty_like(self.model_in[r0:])
         if use_graph:
             side = torch.cuda.Stream(device=dev)
             side.wait_stream(torch.cuda.current_stream(dev))
@@ -1440,6 +1507,20 @@ class DenoiseStepper:
             self.graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self.graph):
                 self._launch()
+            if self.cfg_cutoff is not None:
+                with torch.cuda.stream(side):
+                    self._launch(text=True)
+                torch.cuda.current_stream(dev).wait_stream(side)
+                self.lat.copy_(lat0)
+                self.model_in.copy_(min0)
+                # The text-rows graph allocates from the full graph's pool, so the activations are paid for once.
+                # That is safe because the two graphs replay one after the other on one stream and neither reads a
+                # tensor allocated inside the other's capture: every activation and eps buffer a replay reads, it
+                # has written earlier in the same replay; what persists between steps (latents, model_in, the
+                # tables, conditions and rescale factors) was allocated outside both captures.
+                self.graph_text = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(self.graph_text, pool=self.graph.pool()):
+                    self._launch(text=True)
             self.lat.copy_(lat0)
             self.model_in.copy_(min0)
 
@@ -1562,34 +1643,46 @@ class DenoiseStepper:
             return {}
         return dict(adapter=AdapterResiduals(self.ad_feats, self.ad_gate_cur, s))
 
-    def _launch(self):
-        if len(self._parts) == 1:
+    def _launch(self, text: bool = False):
+        """One step: the UNet on every row, then the guided step; ``text`` (after a CFG cutoff): the UNet on the text
+        chunk's rows [r0, B2) alone, then the 1-chunk step on them."""
+        if text:
+            parts, cond_parts, r0 = self._text_parts, self._text_cond_parts, self.model_in.shape[0] // 2
+        else:
+            parts, cond_parts, r0 = self._parts, self._cond_parts, 0
+        if len(parts) == 1 and not text:
             eps = self.unet.forward_nhwc(self.model_in, self.temb_cur, self.cond, self.db, self.round_bf16,
                                          **self._pag_args(0, self.model_in.shape[0]),
                                          **self._adapter_args(0))                                          # :322-329
+        elif len(parts) == 1:
+            s, e = parts[0]
+            eps = self.unet.forward_nhwc(self.model_in[s:e], self.temb_cur[s:e], cond_parts[0],
+                                         None if self.db is None else self.db[s:e], self.round_bf16,
+                                         **self._adapter_args(s))
         elif self.tiles is not None or self.regions is not None:   # the rows' slices, one after another, into one buffer
-            eps = self._eps
-            for k, (s, e) in enumerate(self._parts):
-                self.unet.forward_nhwc(self.model_in[s:e], self.temb_cur[s:e], self._cond_parts[k],
-                                       None if self.db is None else self.db[s:e], self.round_bf16, out=eps[s:e],
-                                       **self._pag_args(s, e))
+            eps = self._eps_text if text else self._eps
+            for k, (s, e) in enumerate(parts):
+                self.unet.forward_nhwc(self.model_in[s:e], self.temb_cur[s:e], cond_parts[k],
+                                       None if self.db is None else self.db[s:e], self.round_bf16,
+                                       out=eps[s - r0:e - r0], **self._pag_args(s, e))
         else:
             main = torch.cuda.current_stream(self.dev)
-            eps = self._eps
+            eps = self._eps_text if text else self._eps
             # one split-K workspace per device: never shared by kernels that may overlap (also keeps it out of the
             # capture); GEMM chains need every SM resident, which concurrent streams do not guarantee
             prev_splitk, ops.SPLITK = ops.SPLITK, False
             prev_chains, ops.GEMM_CHAINS = ops.GEMM_CHAINS, False
             try:
-                for k, (s, e) in enumerate(self._parts):
+                for k, (s, e) in enumerate(parts):
                     st = main if k == 0 else self._side[k - 1]
                     if k:
                         st.wait_stream(main)                   # fork (inside a capture: joins the captured graph)
                     with torch.cuda.stream(st):
-                        self.unet.forward_nhwc(self.model_in[s:e], self.temb_cur[s:e], self._cond_parts[k],
+                        self.unet.forward_nhwc(self.model_in[s:e], self.temb_cur[s:e], cond_parts[k],
                                                None if self.db is None else self.db[s:e], self.round_bf16,
-                                               out=eps[s:e], **self._pag_args(s, e), **self._adapter_args(s))
-                for st in self._side:
+                                               out=eps[s - r0:e - r0], **self._pag_args(s, e),
+                                               **self._adapter_args(s))
+                for st in self._side[:len(parts) - 1]:
                     main.wait_stream(st)                       # join before the CFG blend needs both halves
             finally:
                 ops.SPLITK = prev_splitk
@@ -1598,7 +1691,10 @@ class DenoiseStepper:
         tiled = {} if self.tiles is None else dict(tiles=self.tiles)
         if self.regions is not None:
             tiled = dict(regions=(self.cover, self.regions))
-        if self.guidance_rescale > 0:                  # diffusers' rescale_noise_cfg, before the scheduler step
+        if text:                                       # no guidance and no rescale: eps is the text eps
+            self.scheduler.fused_step_(eps, self.lat, self.model_in[r0:], self.coef_cur, self.guidance, inpaint,
+                                       **tiled)
+        elif self.guidance_rescale > 0:                # diffusers' rescale_noise_cfg, before the scheduler step
             ops.cfg_rescale_factors(eps, self.coef_cur, self.guidance, out=self.rescale_factors)
             self.scheduler.fused_step_(eps, self.lat, self.model_in, self.coef_cur, self.guidance, inpaint,
                                        (self.rescale_factors, self.guidance_rescale), **tiled)
@@ -1612,10 +1708,11 @@ class DenoiseStepper:
         self.coef_cur.copy_(self.coef_table[i])
         if self.has_adapter:
             self.ad_gate_cur.copy_(self.ad_gates[i])
+        text = self.cfg_cutoff is not None and i > self.cfg_cutoff       # after a CFG cutoff: the text rows alone
         if self.graph is not None:
-            self.graph.replay()
+            (self.graph_text if text else self.graph).replay()
         else:
-            self._launch()
+            self._launch(text)
 
     @torch.no_grad()
     def step_host(self, i: int, latents_host: torch.Tensor, out_host: torch.Tensor) -> torch.Tensor:

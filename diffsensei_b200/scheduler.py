@@ -115,7 +115,8 @@ class DDIMScheduler:
         scale appended for a 3-chunk ``noise_pred``; ``inpaint`` None or (image_latents, noise, mask); ``rescale``
         None or (factors, guidance_rescale), the guided eps rescaled first (``ops.cfg_rescale_factors``).  ``tiles``:
         a ``TileGrid`` when ``latents`` is a canvas denoised as its views (``ops.tile_step_``); ``regions``: (cover, R)
-        when it is a canvas denoised under per-region prompts (``ops.region_step_``)."""
+        when it is a canvas denoised under per-region prompts (``ops.region_step_``).  A 1-chunk ``noise_pred`` (the
+        text rows alone, after a CFG cutoff) steps with the text eps and no guidance."""
         if tiles is not None:
             ops.tile_step_(noise_pred, latents, model_in, coef, guidance, False, tiles, inpaint, rescale)
         elif regions is not None:

@@ -349,7 +349,8 @@ int ds_timestep_embedding(const float* t, void* out, int rows, int dim, void* st
  * torch.cat([latents] * chunks) and scheduler.scale_model_input for the next step).
  *   update        : 0 = DDIMScheduler (eta = 0), 1 = EulerDiscreteScheduler (s_churn = 0); epsilon prediction
  *   chunks        : 2 = CFG, noise_pred [uncond ; text]; 3 = CFG + perturbed-attention guidance (diffusers' PAGMixin
- *                   under classifier-free guidance), noise_pred [uncond ; text ; perturbed]
+ *                   under classifier-free guidance), noise_pred [uncond ; text ; perturbed]; 1 = no guidance (the steps
+ *                   after a CFG cutoff), noise_pred [text]: eps = e_text exactly, guidance unused, rescale_factors NULL
  *   noise_pred    : bf16 NHWC [chunks*bs][H][W][4]
  *   latents       : fp32 [bs][H][W][4] updated in place (fp32 master copy)
  *   model_in      : bf16 NHWC [chunks*bs][H][W][4], the next UNet input in every chunk: x_new (DDIM),
@@ -373,7 +374,8 @@ int ds_timestep_embedding(const float* t, void* out, int rows, int dim, void* st
  *   inpaint: init = c0 * z + c1 * n (add_noise of the image latents at the next timestep; {1, 0} on the last step);
  *            x_new = mask ? x_new : init, and the next UNet input is computed from the blended x_new
  * Rounding: every operation is rounded on its own in diffusers' eager fp32 order, except DDIM with 2 chunks and no
- * rescale, where the compiler may contract multiply-adds into FMAs.  A pixel with mask != 0 is the result without
+ * rescale, where the compiler may contract multiply-adds into FMAs (1 chunk: op by op, diffusers' eager
+ * scheduler.step(noise_pred_text)).  A pixel with mask != 0 is the result without
  * inpaint bit for bit.
  *
  * ds_cfg_rescale_factors: the per-sample factors of diffusers' rescale_noise_cfg (Lin et al. 2024, sec. 3.4), from
@@ -400,7 +402,7 @@ int ds_cfg_rescale_factors(const void* noise_pred, const float* coef, int ncoef,
  *                   flush with the far edge); V = n_h * n_w in row-major order; 0 < stride <= tile <= dim
  *   image_latents / noise / mask : canvas-sized as in ds_cfg_step (all three or none)
  *   rescale_factors : NULL or fp32 [bs * V], one factor per view row (ds_cfg_rescale_factors over the view rows)
- *   update, chunks, coef, guidance, guidance_rescale : as ds_cfg_step
+ *   update, chunks, coef, guidance, guidance_rescale : as ds_cfg_step (chunks 1: the text chunk's view rows only)
  * Per canvas pixel: each covering view, in view order, gives x_v = ds_cfg_step's update of the canvas pixel from that
  * view's eps (and that view's factor); x_new = (0 + x_v1 + x_v2 + ...) / count in fp32, each sum and the division
  * rounded on their own (one view: ds_cfg_step's bits); then the inpaint blend on the canvas pixel; then the canvas and
@@ -421,7 +423,7 @@ int ds_tile_step(const void* noise_pred, float* latents, void* model_in, const f
  *   n_regions     : 1 .. 8
  *   image_latents / noise / mask : canvas-sized as in ds_cfg_step (all three or none)
  *   rescale_factors : NULL or fp32 [bs * R'], one factor per row (ds_cfg_rescale_factors over the rows)
- *   update, chunks, coef, guidance, guidance_rescale : as ds_cfg_step
+ *   update, chunks, coef, guidance, guidance_rescale : as ds_cfg_step (chunks 1: the text chunk's rows only)
  * Per canvas pixel: each covering row, in row order, gives x_r = ds_cfg_step's update of the canvas pixel from that
  * row's eps (and that row's factor); x_new = (0 + x_r1 + x_r2 + ...) / count in fp32, each sum and the division
  * rounded on their own (one covering row: ds_cfg_step's bits); then the inpaint blend on the canvas pixel; then the
