@@ -49,6 +49,11 @@ class CrossIpArgs(C.Structure):
                 ("aspect_ratio", C.c_double), ("ip_scale", C.c_float)]
 
 
+class StepRows(C.Structure):
+    _fields_ = [("tile_h", C.c_int32), ("tile_w", C.c_int32), ("stride_h", C.c_int32), ("stride_w", C.c_int32),
+                ("cover", C.c_void_p), ("n_regions", C.c_int32)]
+
+
 EPI_NONE, EPI_GEGLU, EPI_GELU, EPI_SILU, EPI_QUICKGELU = 0, 1, 2, 3, 4
 
 _vp, _i, _f, _d, _i64 = C.c_void_p, C.c_int, C.c_float, C.c_double, C.c_int64
@@ -83,10 +88,8 @@ SIGNATURES = {
     "ds_concat_channels": [_vp, _vp, _vp, _i, _i, _i, _vp],
     "ds_silu": [_vp, _vp, _i64, _vp],
     "ds_timestep_embedding": [_vp, _vp, _i, _i, _vp],
-    "ds_cfg_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _vp, _vp, _vp, _vp, _d, _i, _i, _i, _vp],
+    "ds_cfg_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _vp, _vp, _vp, _vp, _d, C.POINTER(StepRows), _i, _i, _i, _i, _vp],
     "ds_cfg_rescale_factors": [_vp, _vp, _i, _f, _i, _vp, _i, _i, _i, _vp],
-    "ds_tile_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _vp, _vp, _vp, _vp, _d, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
-    "ds_region_step": [_vp, _vp, _vp, _vp, _f, _i, _i, _vp, _vp, _vp, _vp, _d, _vp, _i, _i, _i, _i, _vp],
     "ds_resampler_attn": [_vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "ds_attention_small": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i64, _i64, _i64, _i64, _f, _i, _vp],
     "ds_embed_tokens": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],

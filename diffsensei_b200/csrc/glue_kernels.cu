@@ -3,6 +3,7 @@
 // fused CFG + DDIM and CFG + Euler updates (plain and inpaint, with or without guidance_rescale), the same update on a
 // canvas denoised as overlapping views or under per-region prompts (MultiDiffusion), and the per-sample factors of that
 // rescale.  All vectorised to 16-byte accesses where the shape allows.
+#include <array>
 #include <cmath>
 
 #include "ds_common.cuh"
@@ -270,21 +271,12 @@ __device__ __forceinline__ void rescale_eps(float eps[4], float r, float phi, fl
   for (int j = 0; j < 4; ++j) eps[j] = __fadd_rn(__fmul_rn(phi, __fmul_rn(eps[j], r)), __fmul_rn(one_m_phi, eps[j]));
 }
 
-// the fp32 master and all kChunks chunks of the next UNet input: bf16(xv / in_div), or bf16(xv) when in_div is NULL
-template <int kChunks>
-__device__ __forceinline__ void store_step(float4* __restrict__ latents, uint2* __restrict__ model_in, long long i,
-                                           long long n_pix, const float xv[4], const float* in_div) {
-  latents[i] = make_float4(xv[0], xv[1], xv[2], xv[3]);
-  uint2 o;
-  if (in_div) {
-    const float d = *in_div;
-    o = make_uint2(pack_bf16(__fdiv_rn(xv[0], d), __fdiv_rn(xv[1], d)),
-                   pack_bf16(__fdiv_rn(xv[2], d), __fdiv_rn(xv[3], d)));
-  } else {
-    o = make_uint2(pack_bf16(xv[0], xv[1]), pack_bf16(xv[2], xv[3]));
-  }
-#pragma unroll
-  for (int c = 0; c < kChunks; ++c) model_in[c * n_pix + i] = o;
+// the next UNet input of one pixel in bf16: xv / in_div, or xv when in_div is NULL
+__device__ __forceinline__ uint2 next_input(const float xv[4], const float* in_div) {
+  if (!in_div) return make_uint2(pack_bf16(xv[0], xv[1]), pack_bf16(xv[2], xv[3]));
+  const float d = *in_div;
+  return make_uint2(pack_bf16(__fdiv_rn(xv[0], d), __fdiv_rn(xv[1], d)),
+                    pack_bf16(__fdiv_rn(xv[2], d), __fdiv_rn(xv[3], d)));
 }
 
 // The guided scheduler update of one pixel: xv (the latents, loaded by the caller) <- update(guide(u, tt)), u / tt
@@ -317,29 +309,24 @@ __device__ __forceinline__ void guided_update(const uint2* __restrict__ noise_pr
   }
 }
 
-// noise_pred holds kChunks chunks of n_pix pixels, [uncond ; text (; perturbed)], or [text] with no guidance; coef is the step's row
-// {update (2 DDIM, 3 Euler) | c0, c1 if kInpaint | s if kChunks == 3}.  kRescale: the guided eps of sample i / HW is
-// rescaled with the factor rescale[i / HW] (cfg_rescale_factors_kernel) before the update.
-template <bool kEuler, int kChunks, bool kInpaint, bool kRescale>
-__global__ void cfg_step_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
-                                uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
-                                long long n_pix /* bs*HW */, const float4* __restrict__ image_latents,
-                                const float4* __restrict__ noise, const unsigned char* __restrict__ mask,
-                                const float* __restrict__ rescale, float phi, float one_m_phi, int HW) {
-  static_assert(1 <= kChunks && kChunks <= 3, "no guidance (1 chunk), CFG (2) or CFG + PAG (3)");
-  constexpr int kC0 = kEuler ? 3 : 2;                 // {c0, c1} follow the update's coefficients
-  constexpr int kS = kC0 + (kInpaint ? 2 : 0);         // then the PAG scale
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= n_pix) return;
-  float u[4], tt[4];
-  load_eps<kChunks>(noise_pred, i, n_pix, u, tt);
-  const float4 x = latents[i];
-  float xv[4] = {x.x, x.y, x.z, x.w};
-  guided_update<kEuler, kChunks, kRescale, kS>(noise_pred, i, n_pix, u, tt, xv, coef, guidance, rescale, HW, phi,
-                                               one_m_phi);
-  if constexpr (kInpaint) inpaint_blend(xv, i, image_latents, noise, mask, coef[kC0], coef[kC0 + 1]);
-  store_step<kChunks>(latents, model_in, i, n_pix, xv, kEuler ? coef + 2 : nullptr);
-}
+// The UNet rows of a step kernel's canvas.  noise_pred / model_in hold kChunks chunks of chunk_pixels() row pixels;
+// every covering row pixel of canvas pixel i (`covering`, from its pixel(i) state) gives an update of it, their mean is
+// the new canvas pixel, and every row pixel `inputs` visits gets the next UNet input.  A row pixel j's rescale factor
+// is rescale[j / row_hw()].
+
+// The plain layout: row pixel i is canvas pixel i, sample b's eps is row b of each chunk.
+struct PlainRows {
+  static constexpr bool kOneRow = true;  // the update is the new pixel as it is: no 0 + x (it turns -0 into +0), no / 1
+  int bs, HW;
+  __device__ long long canvas_pixels() const { return static_cast<long long>(bs) * HW; }
+  __device__ long long chunk_pixels() const { return canvas_pixels(); }
+  __device__ int row_hw() const { return HW; }
+  __device__ long long pixel(long long i) const { return i; }
+  template <class F>
+  __device__ void covering(long long i, F&& f) const { f(i); }
+  template <class F>
+  __device__ void inputs(long long i, F&& f) const { f(i); }
+};
 
 // MultiDiffusion's view grid on one latent axis: n views of `size` pixels, view k at min(k * stride, dim - size) (the
 // last one flush with the far edge), 0 < stride <= size <= dim.  Every coordinate has at least one covering view.
@@ -355,128 +342,163 @@ __device__ __forceinline__ void tile_cover(const TileAxis& a, int p, int& lo, in
   hi = p >= a.dim - a.size ? a.n - 1 : p / a.stride;
 }
 
-// The tiled step (MultiDiffusion, Bar-Tal et al. 2023), one thread per canvas pixel.  latents: the fp32 canvas
-// [bs][H][W][4]; noise_pred / model_in: kChunks chunks of bs * V views (row b * V + v, v = vy * ax.n + vx) of
-// ay.size x ax.size pixels.  Every covering view's x_new is computed from the canvas pixel as the untiled step
-// computes a sample's (rescale factor: the view row's); their fp32 sum, in view order from 0, over the count is the
-// new canvas pixel (diffusers' panorama loop: value += x_view, then value / count), then the inpaint blend on the
-// canvas, then the next UNet input into every covering view of every chunk.  Each output element is written once.
-template <bool kEuler, int kChunks, bool kInpaint, bool kRescale>
-__global__ void tile_step_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
-                                 uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
-                                 TileAxis ay, TileAxis ax, int bs,
-                                 const float4* __restrict__ image_latents, const float4* __restrict__ noise,
-                                 const unsigned char* __restrict__ mask, const float* __restrict__ rescale, float phi,
-                                 float one_m_phi) {
-  static_assert(1 <= kChunks && kChunks <= 3, "no guidance (1 chunk), CFG (2) or CFG + PAG (3)");
-  constexpr int kC0 = kEuler ? 3 : 2;
-  constexpr int kS = kC0 + (kInpaint ? 2 : 0);
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= static_cast<long long>(bs) * ay.dim * ax.dim) return;
-  const int x = static_cast<int>(i % ax.dim);
-  const long long by = i / ax.dim;
-  const int y = static_cast<int>(by % ay.dim);
-  const int b = static_cast<int>(by / ay.dim);
-  const int views = ay.n * ax.n, view_hw = ay.size * ax.size;
-  const long long n_pix = static_cast<long long>(bs) * views * view_hw;  // pixels per chunk
-  int ylo, yhi, xlo, xhi;
-  tile_cover(ay, y, ylo, yhi);
-  tile_cover(ax, x, xlo, xhi);
-  const float4 xc = latents[i];
-  float sum[4] = {0.f, 0.f, 0.f, 0.f};
-  for (int vy = ylo; vy <= yhi; ++vy) {
-    const long long row0 = (static_cast<long long>(b) * views + vy * ax.n) * view_hw +
-                           static_cast<long long>(y - tile_origin(ay, vy)) * ax.size;
-    for (int vx = xlo; vx <= xhi; ++vx) {
-      const long long j = row0 + vx * static_cast<long long>(view_hw) + (x - tile_origin(ax, vx));
-      float u[4], tt[4];
-      load_eps<kChunks>(noise_pred, j, n_pix, u, tt);
-      float xv[4] = {xc.x, xc.y, xc.z, xc.w};
-      guided_update<kEuler, kChunks, kRescale, kS>(noise_pred, j, n_pix, u, tt, xv, coef, guidance, rescale, view_hw,
-                                                   phi, one_m_phi);
-#pragma unroll
-      for (int c = 0; c < 4; ++c) sum[c] = __fadd_rn(sum[c], xv[c]);
+// The tiled layout (MultiDiffusion, Bar-Tal et al. 2023): the canvas [bs][ay.dim][ax.dim] denoised as bs * V views
+// (row b * V + v, v = vy * ax.n + vx) of ay.size x ax.size pixels.  The covering views of a canvas pixel, in view
+// order, update it, and the same views get its next UNet input (diffusers' panorama loop: value += x_view, then
+// value / count).
+struct TileRows {
+  static constexpr bool kOneRow = false;
+  TileAxis ay, ax;
+  int bs;
+  __device__ long long canvas_pixels() const { return static_cast<long long>(bs) * ay.dim * ax.dim; }
+  __device__ long long chunk_pixels() const { return static_cast<long long>(bs) * ay.n * ax.n * row_hw(); }
+  __device__ int row_hw() const { return ay.size * ax.size; }
+  struct Pixel {
+    int b, y, x, ylo, yhi, xlo, xhi;  // the canvas pixel and its covering views [ylo, yhi] x [xlo, xhi]
+  };
+  __device__ Pixel pixel(long long i) const {
+    Pixel p;
+    p.x = static_cast<int>(i % ax.dim);
+    const long long by = i / ax.dim;
+    p.y = static_cast<int>(by % ay.dim);
+    p.b = static_cast<int>(by / ay.dim);
+    tile_cover(ay, p.y, p.ylo, p.yhi);
+    tile_cover(ax, p.x, p.xlo, p.xhi);
+    return p;
+  }
+  template <class F>
+  __device__ void covering(const Pixel& p, F&& f) const {
+    const int views = ay.n * ax.n, view_hw = row_hw();
+    for (int vy = p.ylo; vy <= p.yhi; ++vy) {
+      const long long row0 = (static_cast<long long>(p.b) * views + vy * ax.n) * view_hw +
+                             static_cast<long long>(p.y - tile_origin(ay, vy)) * ax.size;
+      for (int vx = p.xlo; vx <= p.xhi; ++vx)
+        f(row0 + vx * static_cast<long long>(view_hw) + (p.x - tile_origin(ax, vx)));
     }
   }
-  const float count = static_cast<float>((yhi - ylo + 1) * (xhi - xlo + 1));
-  float xv[4];
-#pragma unroll
-  for (int c = 0; c < 4; ++c) xv[c] = __fdiv_rn(sum[c], count);
-  if constexpr (kInpaint) inpaint_blend(xv, i, image_latents, noise, mask, coef[kC0], coef[kC0 + 1]);
-  latents[i] = make_float4(xv[0], xv[1], xv[2], xv[3]);
-  uint2 o;
-  if constexpr (kEuler) {
-    const float d = coef[2];
-    o = make_uint2(pack_bf16(__fdiv_rn(xv[0], d), __fdiv_rn(xv[1], d)),
-                   pack_bf16(__fdiv_rn(xv[2], d), __fdiv_rn(xv[3], d)));
-  } else {
-    o = make_uint2(pack_bf16(xv[0], xv[1]), pack_bf16(xv[2], xv[3]));
-  }
-  for (int vy = ylo; vy <= yhi; ++vy) {
-    const long long row0 = (static_cast<long long>(b) * views + vy * ax.n) * view_hw +
-                           static_cast<long long>(y - tile_origin(ay, vy)) * ax.size;
-    for (int vx = xlo; vx <= xhi; ++vx) {
-      const long long j = row0 + vx * static_cast<long long>(view_hw) + (x - tile_origin(ax, vx));
-#pragma unroll
-      for (int c = 0; c < kChunks; ++c) model_in[c * n_pix + j] = o;
-    }
-  }
-}
+  template <class F>
+  __device__ void inputs(const Pixel& p, F&& f) const { covering(p, f); }
+};
 
-// The regional step (MultiDiffusion's region-based generation, Bar-Tal et al. 2023 sec. 4.2), one thread per canvas
-// pixel.  latents: the fp32 canvas [bs][HW]; noise_pred / model_in: kChunks chunks of bs * R1 rows of HW pixels, row
-// b * R1 + r sample b under prompt r (r = 0 the background, r = 1 .. R1 - 1 the regions), every row's input the whole
-// canvas; cover: uint8 [bs][HW], bit r - 1 set <=> region r covers the pixel (bits at or above R1 - 1 are ignored), the
-// background covers exactly the pixels whose byte is 0.  Every covering row's x_new is computed from the canvas pixel
-// as the plain step computes a sample's (rescale factor: the row's); their fp32 sum, in row order from 0, over the
-// count is the new canvas pixel, then the inpaint blend, then the next UNet input into all R1 rows of every chunk.
-template <bool kEuler, int kChunks, bool kInpaint, bool kRescale>
-__global__ void region_step_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
-                                   uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance,
-                                   const unsigned char* __restrict__ cover, int R1, int bs, int HW,
-                                   const float4* __restrict__ image_latents, const float4* __restrict__ noise,
-                                   const unsigned char* __restrict__ mask, const float* __restrict__ rescale,
-                                   float phi, float one_m_phi) {
+// The regional layout (MultiDiffusion's region-based generation, Bar-Tal et al. 2023 sec. 4.2): the canvas [bs][HW]
+// under R1 prompts, row b * R1 + r sample b under prompt r (r = 0 the background, r = 1 .. R1 - 1 the regions), every
+// row's input the whole canvas.  cover: uint8 [bs][HW], bit r - 1 set <=> region r covers the pixel (bits at or above
+// R1 - 1 are ignored); the background covers exactly the pixels whose byte is 0.  The covering rows, in row order,
+// update a canvas pixel; all R1 rows get its next UNet input.
+struct RegionRows {
+  static constexpr bool kOneRow = false;
+  const unsigned char* cover;
+  int R1, bs, HW;
+  __device__ long long canvas_pixels() const { return static_cast<long long>(bs) * HW; }
+  __device__ long long chunk_pixels() const { return static_cast<long long>(bs) * R1 * HW; }
+  __device__ int row_hw() const { return HW; }
+  struct Pixel {
+    long long row0;  // the pixel in row b * R1 (the background)
+    unsigned rows;   // bit r set <=> row r covers the pixel
+  };
+  __device__ Pixel pixel(long long i) const {
+    const long long b = i / HW;
+    const unsigned bits = __ldg(cover + i) & ((1u << (R1 - 1)) - 1u);
+    return {b * R1 * HW + (i - b * HW), bits ? bits << 1 : 1u};
+  }
+  template <class F>
+  __device__ void covering(const Pixel& p, F&& f) const {
+    for (unsigned m = p.rows; m != 0; m &= m - 1) f(p.row0 + static_cast<long long>(__ffs(m) - 1) * HW);
+  }
+  template <class F>
+  __device__ void inputs(const Pixel& p, F&& f) const {
+    for (int r = 0; r < R1; ++r) f(p.row0 + static_cast<long long>(r) * HW);
+  }
+};
+
+// The step, one thread per canvas pixel.  noise_pred holds kChunks chunks of the layout's rows, [uncond ; text
+// (; perturbed)], or [text] with no guidance; coef is the step's row {update (2 DDIM, 3 Euler) | c0, c1 if kInpaint |
+// s if kChunks == 3}.  kRescale: the guided eps of row pixel j is rescaled with the factor rescale[j / row_hw()]
+// (cfg_rescale_factors_kernel) before the update.  Every covering row's x_new is computed from the canvas pixel by
+// guided_update; their fp32 sum, in the layout's order from 0, over the count is the new canvas pixel (one row in the
+// plain layout: its x_new itself), then the inpaint blend on the canvas, then the canvas and the next UNet input into
+// every chunk of the rows `inputs` visits.  Each output element is written by one thread once.
+template <class Rows, bool kEuler, int kChunks, bool kInpaint, bool kRescale>
+__global__ void cfg_step_kernel(const uint2* __restrict__ noise_pred, float4* __restrict__ latents,
+                                uint2* __restrict__ model_in, const float* __restrict__ coef, float guidance, Rows rows,
+                                const float4* __restrict__ image_latents, const float4* __restrict__ noise,
+                                const unsigned char* __restrict__ mask, const float* __restrict__ rescale, float phi,
+                                float one_m_phi) {
   static_assert(1 <= kChunks && kChunks <= 3, "no guidance (1 chunk), CFG (2) or CFG + PAG (3)");
-  constexpr int kC0 = kEuler ? 3 : 2;
-  constexpr int kS = kC0 + (kInpaint ? 2 : 0);
+  constexpr int kC0 = kEuler ? 3 : 2;                 // {c0, c1} follow the update's coefficients
+  constexpr int kS = kC0 + (kInpaint ? 2 : 0);         // then the PAG scale
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= static_cast<long long>(bs) * HW) return;
-  const long long b = i / HW;
-  const long long n_pix = static_cast<long long>(bs) * R1 * HW;  // pixels per chunk
-  const long long row0 = b * R1 * HW + (i - b * HW);               // the pixel in row b * R1 (the background)
-  const unsigned bits = __ldg(cover + i) & ((1u << (R1 - 1)) - 1u);
-  const unsigned rows = bits ? bits << 1 : 1u;                     // bit r set <=> row r covers the pixel
+  if (i >= rows.canvas_pixels()) return;
+  const long long n_pix = rows.chunk_pixels();
+  const auto px = rows.pixel(i);
   const float4 xc = latents[i];
-  float sum[4] = {0.f, 0.f, 0.f, 0.f};
-  for (unsigned m = rows; m != 0; m &= m - 1) {
-    const long long j = row0 + static_cast<long long>(__ffs(m) - 1) * HW;
+  // x_new of the canvas pixel from row pixel j's eps
+  auto update = [&](long long j, float xv[4]) {
     float u[4], tt[4];
     load_eps<kChunks>(noise_pred, j, n_pix, u, tt);
-    float xv[4] = {xc.x, xc.y, xc.z, xc.w};
-    guided_update<kEuler, kChunks, kRescale, kS>(noise_pred, j, n_pix, u, tt, xv, coef, guidance, rescale, HW, phi,
-                                                 one_m_phi);
-#pragma unroll
-    for (int c = 0; c < 4; ++c) sum[c] = __fadd_rn(sum[c], xv[c]);
-  }
-  const float count = static_cast<float>(__popc(rows));
+    xv[0] = xc.x, xv[1] = xc.y, xv[2] = xc.z, xv[3] = xc.w;
+    guided_update<kEuler, kChunks, kRescale, kS>(noise_pred, j, n_pix, u, tt, xv, coef, guidance, rescale,
+                                                 rows.row_hw(), phi, one_m_phi);
+  };
   float xv[4];
+  if constexpr (Rows::kOneRow) {
+    update(i, xv);
+  } else {
+    float sum[4] = {0.f, 0.f, 0.f, 0.f};
+    int count = 0;
+    rows.covering(px, [&](long long j) {
+      float x[4];
+      update(j, x);
 #pragma unroll
-  for (int c = 0; c < 4; ++c) xv[c] = __fdiv_rn(sum[c], count);
+      for (int c = 0; c < 4; ++c) sum[c] = __fadd_rn(sum[c], x[c]);
+      ++count;
+    });
+#pragma unroll
+    for (int c = 0; c < 4; ++c) xv[c] = __fdiv_rn(sum[c], static_cast<float>(count));
+  }
   if constexpr (kInpaint) inpaint_blend(xv, i, image_latents, noise, mask, coef[kC0], coef[kC0 + 1]);
   latents[i] = make_float4(xv[0], xv[1], xv[2], xv[3]);
-  uint2 o;
-  if constexpr (kEuler) {
-    const float d = coef[2];
-    o = make_uint2(pack_bf16(__fdiv_rn(xv[0], d), __fdiv_rn(xv[1], d)),
-                   pack_bf16(__fdiv_rn(xv[2], d), __fdiv_rn(xv[3], d)));
-  } else {
-    o = make_uint2(pack_bf16(xv[0], xv[1]), pack_bf16(xv[2], xv[3]));
-  }
-  for (int r = 0; r < R1; ++r) {
+  const uint2 o = next_input(xv, kEuler ? coef + 2 : nullptr);
+  rows.inputs(px, [&](long long j) {
 #pragma unroll
-    for (int c = 0; c < kChunks; ++c) model_in[c * n_pix + row0 + static_cast<long long>(r) * HW] = o;
+    for (int c = 0; c < kChunks; ++c) model_in[c * n_pix + j] = o;
+  });
+}
+
+// The 20 step kernels of one row layout, [update][chunks - 1][inpaint][rescale]; 1 chunk has no rescale kernel.
+template <class Rows>
+struct StepKernels {
+  using Fn = void (*)(const uint2*, float4*, uint2*, const float*, float, Rows, const float4*, const float4*,
+                      const unsigned char*, const float*, float, float);
+  using Variants = std::array<std::array<Fn, 2>, 2>;  // [inpaint][rescale]
+  template <bool kEuler, int kChunks, bool kInpaint, bool kRescale>
+  static constexpr Fn kernel() {
+    if constexpr (kChunks == 1 && kRescale)
+      return nullptr;  // guidance_rescale needs the guided eps
+    else
+      return cfg_step_kernel<Rows, kEuler, kChunks, kInpaint, kRescale>;
   }
+  template <bool kEuler, int kChunks>
+  static constexpr Variants variants() {
+    return {{{kernel<kEuler, kChunks, false, false>(), kernel<kEuler, kChunks, false, true>()},
+             {kernel<kEuler, kChunks, true, false>(), kernel<kEuler, kChunks, true, true>()}}};
+  }
+  static constexpr std::array<std::array<Variants, 3>, 2> kTable = {{
+      {variants<false, 1>(), variants<false, 2>(), variants<false, 3>()},
+      {variants<true, 1>(), variants<true, 2>(), variants<true, 3>()}}};
+};
+
+template <class Rows>
+void launch_step(const Rows& rows, long long n_canvas, int update, int chunks, bool inpaint, bool rescale,
+                 const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
+                 const float* image_latents, const float* noise, const uint8_t* mask, const float* rescale_factors,
+                 double guidance_rescale, cudaStream_t stream) {
+  StepKernels<Rows>::kTable[update][chunks - 1][inpaint][rescale]<<<static_cast<unsigned>((n_canvas + 255) / 256), 256,
+                                                                    0, stream>>>(
+      static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
+      guidance, rows, reinterpret_cast<const float4*>(image_latents), reinterpret_cast<const float4*>(noise), mask,
+      // phi and 1 - phi (in double) each rounded to fp32 once: torch's values of the Python scalars for an fp32 tensor
+      rescale_factors, static_cast<float>(guidance_rescale), static_cast<float>(1.0 - guidance_rescale));
 }
 
 // guidance_rescale's per-sample factor r_b = fp32(std(text_b)) / fp32(std(guided_b)), both unbiased over the sample's
@@ -677,18 +699,31 @@ extern "C" int ds_timestep_embedding(const float* t, void* out, int rows, int di
 
 extern "C" int ds_cfg_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
                            int update, int chunks, const float* image_latents, const float* noise, const uint8_t* mask,
-                           const float* rescale_factors, double guidance_rescale, int bs, int HW, int C,
-                           void* stream) {
+                           const float* rescale_factors, double guidance_rescale, const ds_step_rows* rows, int bs,
+                           int H, int W, int C, void* stream) {
   const bool inpaint = image_latents || noise || mask;
   const bool rescale = rescale_factors != nullptr;
-  DS_REQUIRE(noise_pred && latents && model_in && coef, "ds_cfg_step: NULL pointer");
+  const bool views = rows && (rows->tile_h || rows->tile_w || rows->stride_h || rows->stride_w);
+  const bool regions = rows && (rows->cover || rows->n_regions);
+  DS_REQUIRE(noise_pred && latents && model_in && coef && (!regions || rows->cover), "ds_cfg_step: NULL pointer");
   DS_REQUIRE(!inpaint || (image_latents && noise && mask),
              "ds_cfg_step: image_latents / noise / mask must all be given or all be NULL");
   DS_REQUIRE(update == 0 || update == 1, "ds_cfg_step: update must be 0 (DDIM) or 1 (Euler), got %d", update);
   DS_REQUIRE(1 <= chunks && chunks <= 3,
              "ds_cfg_step: chunks must be 2 or 3 (CFG, CFG + PAG) or 1 (no guidance), got %d", chunks);
   DS_REQUIRE(chunks > 1 || !rescale, "ds_cfg_step: rescale_factors must be NULL with 1 chunk (no guidance)");
-  DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "ds_cfg_step: only C == 4 latents are supported (got C=%d)", C);
+  DS_REQUIRE(!(views && regions), "ds_cfg_step: rows sets both views and regions");
+  DS_REQUIRE(!regions || (1 <= rows->n_regions && rows->n_regions <= 8),
+             "ds_cfg_step: n_regions must be in [1, 8], got %d", rows->n_regions);
+  DS_REQUIRE(bs > 0 && H > 0 && W > 0 && C == 4, "ds_cfg_step: only C == 4 latents are supported (got C=%d)", C);
+  DS_REQUIRE(!views || (0 < rows->tile_h && rows->tile_h <= H && 0 < rows->tile_w && rows->tile_w <= W),
+             "ds_cfg_step: the view (%d x %d) must fit the canvas (%d x %d)", rows->tile_h, rows->tile_w, H, W);
+  DS_REQUIRE(!views || (0 < rows->stride_h && rows->stride_h <= rows->tile_h && 0 < rows->stride_w &&
+                        rows->stride_w <= rows->tile_w),
+             "ds_cfg_step: the stride (%d, %d) must be in (0, view size]", rows->stride_h, rows->stride_w);
+  DS_REQUIRE((reinterpret_cast<uintptr_t>(latents) & 15) == 0 && (reinterpret_cast<uintptr_t>(noise_pred) & 7) == 0 &&
+                 (reinterpret_cast<uintptr_t>(model_in) & 7) == 0,
+             "ds_cfg_step: latents must be 16-byte and noise_pred / model_in 8-byte aligned");
   DS_REQUIRE(!inpaint || ((reinterpret_cast<uintptr_t>(image_latents) & 15) == 0 &&
                           (reinterpret_cast<uintptr_t>(noise) & 15) == 0),
              "ds_cfg_step: image_latents / noise must be 16-byte aligned");
@@ -697,135 +732,24 @@ extern "C" int ds_cfg_step(const void* noise_pred, float* latents, void* model_i
              guidance_rescale);
   DeviceInfo dev;
   if (!get_device(&dev)) return DS_ERR_CUDA;
-  using StepKernel = void (*)(const uint2*, float4*, uint2*, const float*, float, long long, const float4*,
-                              const float4*, const unsigned char*, const float*, float, float, int);
-  static constexpr StepKernel kKernels[2][3][2][2] = {  // [update][chunks - 1][inpaint][rescale]; 1 chunk never rescales
-      {{{cfg_step_kernel<false, 1, false, false>, nullptr},
-       {cfg_step_kernel<false, 1, true, false>, nullptr}},
-      {{cfg_step_kernel<false, 2, false, false>, cfg_step_kernel<false, 2, false, true>},
-       {cfg_step_kernel<false, 2, true, false>, cfg_step_kernel<false, 2, true, true>}},
-      {{cfg_step_kernel<false, 3, false, false>, cfg_step_kernel<false, 3, false, true>},
-       {cfg_step_kernel<false, 3, true, false>, cfg_step_kernel<false, 3, true, true>}}},
-      {{{cfg_step_kernel<true, 1, false, false>, nullptr},
-       {cfg_step_kernel<true, 1, true, false>, nullptr}},
-      {{cfg_step_kernel<true, 2, false, false>, cfg_step_kernel<true, 2, false, true>},
-       {cfg_step_kernel<true, 2, true, false>, cfg_step_kernel<true, 2, true, true>}},
-      {{cfg_step_kernel<true, 3, false, false>, cfg_step_kernel<true, 3, false, true>},
-       {cfg_step_kernel<true, 3, true, false>, cfg_step_kernel<true, 3, true, true>}}}};
-  const long long n_pix = static_cast<long long>(bs) * HW;
-  kKernels[update][chunks - 1][inpaint][rescale]<<<static_cast<unsigned>((n_pix + 255) / 256), 256, 0,
-                                                   static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
-      guidance, n_pix, reinterpret_cast<const float4*>(image_latents), reinterpret_cast<const float4*>(noise), mask,
-      // phi and 1 - phi (in double) each rounded to fp32 once: torch's values of the Python scalars for an fp32 tensor
-      rescale_factors, static_cast<float>(guidance_rescale), static_cast<float>(1.0 - guidance_rescale), HW);
-  DS_LAUNCH_OK("cfg_step_kernel");
-  return DS_OK;
-}
-
-extern "C" int ds_tile_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
-                            int update, int chunks, const float* image_latents, const float* noise, const uint8_t* mask,
-                            const float* rescale_factors, double guidance_rescale, int bs, int H, int W, int tile_h,
-                            int tile_w, int stride_h, int stride_w, int C, void* stream) {
-  const bool inpaint = image_latents || noise || mask;
-  const bool rescale = rescale_factors != nullptr;
-  DS_REQUIRE(noise_pred && latents && model_in && coef, "ds_tile_step: NULL pointer");
-  DS_REQUIRE(!inpaint || (image_latents && noise && mask),
-             "ds_tile_step: image_latents / noise / mask must all be given or all be NULL");
-  DS_REQUIRE(update == 0 || update == 1, "ds_tile_step: update must be 0 (DDIM) or 1 (Euler), got %d", update);
-  DS_REQUIRE(1 <= chunks && chunks <= 3,
-             "ds_tile_step: chunks must be 2 or 3 (CFG, CFG + PAG) or 1 (no guidance), got %d", chunks);
-  DS_REQUIRE(chunks > 1 || !rescale, "ds_tile_step: rescale_factors must be NULL with 1 chunk (no guidance)");
-  DS_REQUIRE(bs > 0 && C == 4, "ds_tile_step: only C == 4 latents are supported (got C=%d)", C);
-  DS_REQUIRE(0 < tile_h && tile_h <= H && 0 < tile_w && tile_w <= W,
-             "ds_tile_step: the view (%d x %d) must fit the canvas (%d x %d)", tile_h, tile_w, H, W);
-  DS_REQUIRE(0 < stride_h && stride_h <= tile_h && 0 < stride_w && stride_w <= tile_w,
-             "ds_tile_step: the stride (%d, %d) must be in (0, view size]", stride_h, stride_w);
-  DS_REQUIRE(!inpaint || ((reinterpret_cast<uintptr_t>(image_latents) & 15) == 0 &&
-                          (reinterpret_cast<uintptr_t>(noise) & 15) == 0),
-             "ds_tile_step: image_latents / noise must be 16-byte aligned");
-  DS_REQUIRE(rescale ? std::isfinite(guidance_rescale) : guidance_rescale == 0.0,
-             "ds_tile_step: guidance_rescale must be finite, and 0 when rescale_factors is NULL (got %g)",
-             guidance_rescale);
-  DeviceInfo dev;
-  if (!get_device(&dev)) return DS_ERR_CUDA;
-  // n views per axis: ceil((dim - size) / stride) + 1, the last one flush with the far edge
-  const TileAxis ay{H, tile_h, stride_h, (H - tile_h + stride_h - 1) / stride_h + 1};
-  const TileAxis ax{W, tile_w, stride_w, (W - tile_w + stride_w - 1) / stride_w + 1};
-  using TileKernel = void (*)(const uint2*, float4*, uint2*, const float*, float, TileAxis, TileAxis, int,
-                              const float4*, const float4*, const unsigned char*, const float*, float, float);
-  static constexpr TileKernel kKernels[2][3][2][2] = {  // [update][chunks - 1][inpaint][rescale]; 1 chunk never rescales
-      {{{tile_step_kernel<false, 1, false, false>, nullptr},
-       {tile_step_kernel<false, 1, true, false>, nullptr}},
-      {{tile_step_kernel<false, 2, false, false>, tile_step_kernel<false, 2, false, true>},
-       {tile_step_kernel<false, 2, true, false>, tile_step_kernel<false, 2, true, true>}},
-      {{tile_step_kernel<false, 3, false, false>, tile_step_kernel<false, 3, false, true>},
-       {tile_step_kernel<false, 3, true, false>, tile_step_kernel<false, 3, true, true>}}},
-      {{{tile_step_kernel<true, 1, false, false>, nullptr},
-       {tile_step_kernel<true, 1, true, false>, nullptr}},
-      {{tile_step_kernel<true, 2, false, false>, tile_step_kernel<true, 2, false, true>},
-       {tile_step_kernel<true, 2, true, false>, tile_step_kernel<true, 2, true, true>}},
-      {{tile_step_kernel<true, 3, false, false>, tile_step_kernel<true, 3, false, true>},
-       {tile_step_kernel<true, 3, true, false>, tile_step_kernel<true, 3, true, true>}}}};
   const long long n_canvas = static_cast<long long>(bs) * H * W;
-  kKernels[update][chunks - 1][inpaint][rescale]<<<static_cast<unsigned>((n_canvas + 255) / 256), 256, 0,
-                                                   static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
-      guidance, ay, ax, bs, reinterpret_cast<const float4*>(image_latents), reinterpret_cast<const float4*>(noise),
-      mask, rescale_factors, static_cast<float>(guidance_rescale), static_cast<float>(1.0 - guidance_rescale));
-  DS_LAUNCH_OK("tile_step_kernel");
-  return DS_OK;
-}
-
-extern "C" int ds_region_step(const void* noise_pred, float* latents, void* model_in, const float* coef,
-                              float guidance, int update, int chunks, const float* image_latents, const float* noise,
-                              const uint8_t* mask, const float* rescale_factors, double guidance_rescale,
-                              const uint8_t* cover, int n_regions, int bs, int HW, int C, void* stream) {
-  const bool inpaint = image_latents || noise || mask;
-  const bool rescale = rescale_factors != nullptr;
-  DS_REQUIRE(noise_pred && latents && model_in && coef && cover, "ds_region_step: NULL pointer");
-  DS_REQUIRE(!inpaint || (image_latents && noise && mask),
-             "ds_region_step: image_latents / noise / mask must all be given or all be NULL");
-  DS_REQUIRE(update == 0 || update == 1, "ds_region_step: update must be 0 (DDIM) or 1 (Euler), got %d", update);
-  DS_REQUIRE(1 <= chunks && chunks <= 3,
-             "ds_region_step: chunks must be 2 or 3 (CFG, CFG + PAG) or 1 (no guidance), got %d", chunks);
-  DS_REQUIRE(chunks > 1 || !rescale, "ds_region_step: rescale_factors must be NULL with 1 chunk (no guidance)");
-  DS_REQUIRE(1 <= n_regions && n_regions <= 8, "ds_region_step: n_regions must be in [1, 8], got %d", n_regions);
-  DS_REQUIRE(bs > 0 && HW > 0 && C == 4, "ds_region_step: only C == 4 latents are supported (got C=%d)", C);
-  DS_REQUIRE((reinterpret_cast<uintptr_t>(latents) & 15) == 0 && (reinterpret_cast<uintptr_t>(noise_pred) & 7) == 0 &&
-                 (reinterpret_cast<uintptr_t>(model_in) & 7) == 0,
-             "ds_region_step: latents must be 16-byte and noise_pred / model_in 8-byte aligned");
-  DS_REQUIRE(!inpaint || ((reinterpret_cast<uintptr_t>(image_latents) & 15) == 0 &&
-                          (reinterpret_cast<uintptr_t>(noise) & 15) == 0),
-             "ds_region_step: image_latents / noise must be 16-byte aligned");
-  DS_REQUIRE(rescale ? std::isfinite(guidance_rescale) : guidance_rescale == 0.0,
-             "ds_region_step: guidance_rescale must be finite, and 0 when rescale_factors is NULL (got %g)",
-             guidance_rescale);
-  DeviceInfo dev;
-  if (!get_device(&dev)) return DS_ERR_CUDA;
-  using RegionKernel = void (*)(const uint2*, float4*, uint2*, const float*, float, const unsigned char*, int, int,
-                                int, const float4*, const float4*, const unsigned char*, const float*, float, float);
-  static constexpr RegionKernel kKernels[2][3][2][2] = {  // [update][chunks - 1][inpaint][rescale]; 1 chunk never rescales
-      {{{region_step_kernel<false, 1, false, false>, nullptr},
-       {region_step_kernel<false, 1, true, false>, nullptr}},
-      {{region_step_kernel<false, 2, false, false>, region_step_kernel<false, 2, false, true>},
-       {region_step_kernel<false, 2, true, false>, region_step_kernel<false, 2, true, true>}},
-      {{region_step_kernel<false, 3, false, false>, region_step_kernel<false, 3, false, true>},
-       {region_step_kernel<false, 3, true, false>, region_step_kernel<false, 3, true, true>}}},
-      {{{region_step_kernel<true, 1, false, false>, nullptr},
-       {region_step_kernel<true, 1, true, false>, nullptr}},
-      {{region_step_kernel<true, 2, false, false>, region_step_kernel<true, 2, false, true>},
-       {region_step_kernel<true, 2, true, false>, region_step_kernel<true, 2, true, true>}},
-      {{region_step_kernel<true, 3, false, false>, region_step_kernel<true, 3, false, true>},
-       {region_step_kernel<true, 3, true, false>, region_step_kernel<true, 3, true, true>}}}};
-  const long long n_canvas = static_cast<long long>(bs) * HW;
-  kKernels[update][chunks - 1][inpaint][rescale]<<<static_cast<unsigned>((n_canvas + 255) / 256), 256, 0,
-                                                   static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const uint2*>(noise_pred), reinterpret_cast<float4*>(latents), static_cast<uint2*>(model_in), coef,
-      guidance, cover, n_regions + 1, bs, HW, reinterpret_cast<const float4*>(image_latents),
-      reinterpret_cast<const float4*>(noise), mask, rescale_factors, static_cast<float>(guidance_rescale),
-      static_cast<float>(1.0 - guidance_rescale));
-  DS_LAUNCH_OK("region_step_kernel");
+  const auto s = static_cast<cudaStream_t>(stream);
+  if (views) {
+    const ds_step_rows& v = *rows;
+    // n views per axis: ceil((dim - size) / stride) + 1, the last one flush with the far edge
+    const TileAxis ay{H, v.tile_h, v.stride_h, (H - v.tile_h + v.stride_h - 1) / v.stride_h + 1};
+    const TileAxis ax{W, v.tile_w, v.stride_w, (W - v.tile_w + v.stride_w - 1) / v.stride_w + 1};
+    launch_step(TileRows{ay, ax, bs}, n_canvas, update, chunks, inpaint, rescale, noise_pred, latents, model_in, coef,
+                guidance, image_latents, noise, mask, rescale_factors, guidance_rescale, s);
+  } else if (regions) {
+    launch_step(RegionRows{static_cast<const unsigned char*>(rows->cover), rows->n_regions + 1, bs, H * W}, n_canvas,
+                update, chunks, inpaint, rescale, noise_pred, latents, model_in, coef, guidance, image_latents, noise,
+                mask, rescale_factors, guidance_rescale, s);
+  } else {
+    launch_step(PlainRows{bs, H * W}, n_canvas, update, chunks, inpaint, rescale, noise_pred, latents, model_in, coef,
+                guidance, image_latents, noise, mask, rescale_factors, guidance_rescale, s);
+  }
+  DS_LAUNCH_OK("cfg_step_kernel");
   return DS_OK;
 }
 

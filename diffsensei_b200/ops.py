@@ -15,7 +15,7 @@ import torch
 
 from . import _lib
 from ._lib import (EPI_GEGLU, EPI_GELU, EPI_NONE, EPI_QUICKGELU, EPI_SILU, Conv3x3Args, CrossIpArgs, DsEngineError, GemmArgs,
-                   check, lib)
+                   StepRows, check, lib)
 
 bf16, f32 = torch.bfloat16, torch.float32
 
@@ -695,38 +695,53 @@ def timestep_embedding(t: torch.Tensor, dim: int, out: Optional[torch.Tensor] = 
 
 
 def cfg_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
-              guidance: float, euler: bool, inpaint=None, rescale=None) -> None:
-    """The fused end of a denoise step (``ds_cfg_step``), in place.  noise_pred bf16 [k*bs,H,W,4] holds k = 2 chunks
+              guidance: float, euler: bool, inpaint=None, rescale=None, tiles=None, regions=None) -> None:
+    """The fused end of a denoise step (``ds_cfg_step``), in place.  noise_pred bf16 [k*rows,h,w,4] holds k = 2 chunks
     [uncond ; text] (CFG) or k = 3 [uncond ; text ; perturbed] (CFG + perturbed-attention guidance):
     eps = u + guidance (t - u) [+ s (t - p)]; or k = 1, the text chunk alone (no guidance, after a CFG cutoff):
     eps = t, ``guidance`` unused and ``rescale`` must be None.  latents fp32 NHWC [bs,H,W,4] <- DDIM or (``euler``) Euler update;
-    model_in bf16 [k*bs,H,W,4] <- cat[x]*k (DDIM) or cat[x / coef[2]]*k (Euler).  ``inpaint`` None or
+    model_in bf16, noise_pred's shape <- x (DDIM) or x / coef[2] (Euler) in every chunk.  ``inpaint`` None or
     (image_latents, noise, mask): fp32 NHWC [bs,H,W,4] twice and uint8 [bs,H,W]; where mask is 0 the latents become
-    c0 * image_latents + c1 * noise.  ``rescale`` None or (factors, guidance_rescale): factors fp32 [bs] from
-    ``cfg_rescale_factors`` of this noise_pred and coef, and eps of sample b becomes
-    phi * (eps * factors[b]) + (1 - phi) * eps (diffusers' ``rescale_noise_cfg``).  coef: the step's fp32 row on the
+    c0 * image_latents + c1 * noise.  ``rescale`` None or (factors, guidance_rescale): factors fp32 [rows] from
+    ``cfg_rescale_factors`` of this noise_pred and coef, and eps of row n becomes
+    phi * (eps * factors[n]) + (1 - phi) * eps (diffusers' ``rescale_noise_cfg``).  coef: the step's fp32 row on the
     device, exactly DDIM {alpha_prod_t, alpha_prod_t_prev} / Euler {sigma_i, sigma_{i+1}, sqrt(sigma_{i+1}^2 + 1)},
-    then {c0, c1} with ``inpaint``, then s with 3 chunks."""
-    _req(noise_pred, bf16, "cfg_step.noise_pred", 4)
-    _req(latents, f32, "cfg_step.latents", 4)
-    _req(model_in, bf16, "cfg_step.model_in", 4)
-    _req(coef, f32, "cfg_step.coef", 1)
+    then {c0, c1} with ``inpaint``, then s with 3 chunks.
+
+    The rows: without a layout, rows = bs and (h, w) = (H, W), row b the canvas sample b.  ``tiles``, a
+    ``tiles.TileGrid`` over (H, W): the canvas denoised as its V overlapping views, rows = bs*V of (tile_h, tile_w),
+    row b*V + v view v of sample b; each canvas pixel becomes the mean, in view order, of the updates its covering views
+    give it (MultiDiffusion), and every covering view gets the next UNet input.  ``regions``, (cover, R): the canvas
+    denoised under per-region prompts, cover uint8 [bs,H,W] with bit r - 1 set where region r (1 .. R, R <= 8) covers
+    the pixel, the background covering the pixels whose cover is 0; rows = bs*(R + 1) of (H, W), row b*(R + 1) + r
+    sample b under prompt r (r = 0 the background); each canvas pixel becomes the mean, in row order, of the updates
+    of its covering rows, and all rows get the next UNet input.  The inpaint blend follows the mean."""
+    if tiles is not None and regions is not None:
+        raise DsEngineError("cfg_step: tiles and regions are exclusive")
+    what = "tile_step" if tiles is not None else "region_step" if regions is not None else "cfg_step"
+    _req(noise_pred, bf16, f"{what}.noise_pred", 4)
+    _req(latents, f32, f"{what}.latents", 4)
+    _req(model_in, bf16, f"{what}.model_in", 4)
+    _req(coef, f32, f"{what}.coef", 1)
     bs, H, W, Cc = latents.shape
-    chunks = noise_pred.shape[0] // bs if bs else 0
+    per_sample, view, layout, fits = 1, (H, W), None, True
+    if tiles is not None:
+        per_sample, view = tiles.n_views, (tiles.tile_h, tiles.tile_w)
+        layout = StepRows(tiles.tile_h, tiles.tile_w, tiles.stride_h, tiles.stride_w, None, 0)
+        fits = (H, W) == (tiles.height, tiles.width)
+    elif regions is not None:
+        cover, n_regions = regions
+        _req(cover, torch.uint8, f"{what}.cover", 3)
+        n_regions = int(n_regions)
+        per_sample = n_regions + 1
+        layout = StepRows(0, 0, 0, 0, cover.data_ptr(), n_regions)
+        fits = 1 <= n_regions <= 8 and cover.shape == (bs, H, W)
+    rows = bs * per_sample
+    chunks = noise_pred.shape[0] // rows if rows else 0
     ncoef = (3 if euler else 2) + (0 if inpaint is None else 2) + (chunks == 3)
-    if chunks not in (1, 2, 3) or noise_pred.shape != (chunks * bs, H, W, Cc) or model_in.shape != noise_pred.shape \
-            or coef.numel() != ncoef:
-        raise DsEngineError("cfg_step: shape mismatch")
-    ptrs, factors, phi = _step_state("cfg_step", latents, bs, inpaint, rescale)
-    check(lib.ds_cfg_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(),
-                          float(guidance), int(bool(euler)), chunks, *ptrs, factors, float(phi), bs, H * W, Cc,
-                          _stream()), "ds_cfg_step")
-
-
-def _step_state(what: str, latents: torch.Tensor, rows: int, inpaint, rescale):
-    """The inpaint pointers (latent-shaped image latents and noise, a [bs, H, W] mask; NULLs without) and the rescale
-    factors (``rows`` values) and value of a step launch, checked."""
-    bs, H, W, _ = latents.shape
+    if not fits or chunks not in (1, 2, 3) or noise_pred.shape != (chunks * rows, *view, Cc) or \
+            model_in.shape != noise_pred.shape or coef.numel() != ncoef:
+        raise DsEngineError(f"{what}: shape mismatch")
     ptrs = [None] * 3
     if inpaint is not None:
         image_latents, noise, mask = inpaint
@@ -743,62 +758,9 @@ def _step_state(what: str, latents: torch.Tensor, rows: int, inpaint, rescale):
         if factors.numel() != rows:
             raise DsEngineError(f"{what}: rescale factors must hold one value per sample")
         factors = factors.data_ptr()
-    return ptrs, factors, phi
-
-
-def tile_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
-               guidance: float, euler: bool, tiles, inpaint=None, rescale=None) -> None:
-    """``cfg_step_`` on a canvas denoised as the overlapping views of ``tiles`` (a ``tiles.TileGrid``; ``ds_tile_step``),
-    in place.  latents fp32 NHWC [bs,H,W,4] is the canvas, (H, W) the grid's; noise_pred and model_in bf16
-    [k*bs*V, tile_h, tile_w, 4] hold k chunks of the V views of every canvas sample, row c*bs*V + b*V + v.  Each canvas
-    pixel becomes the mean, in view order, of the updates its covering views give it (MultiDiffusion), then the inpaint
-    blend; every covering view's rows of model_in get the next UNet input.  ``inpaint`` canvas-sized as in
-    ``cfg_step_``; ``rescale`` factors fp32 [bs*V], one per view row.  coef as in ``cfg_step_``."""
-    _req(noise_pred, bf16, "tile_step.noise_pred", 4)
-    _req(latents, f32, "tile_step.latents", 4)
-    _req(model_in, bf16, "tile_step.model_in", 4)
-    _req(coef, f32, "tile_step.coef", 1)
-    bs, H, W, Cc = latents.shape
-    rows = bs * tiles.n_views
-    chunks = noise_pred.shape[0] // rows if rows else 0
-    ncoef = (3 if euler else 2) + (0 if inpaint is None else 2) + (chunks == 3)
-    if (H, W) != (tiles.height, tiles.width) or chunks not in (1, 2, 3) or \
-            noise_pred.shape != (chunks * rows, tiles.tile_h, tiles.tile_w, Cc) or \
-            model_in.shape != noise_pred.shape or coef.numel() != ncoef:
-        raise DsEngineError("tile_step: shape mismatch")
-    ptrs, factors, phi = _step_state("tile_step", latents, rows, inpaint, rescale)
-    check(lib.ds_tile_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(),
-                           float(guidance), int(bool(euler)), chunks, *ptrs, factors, float(phi), bs, H, W,
-                           tiles.tile_h, tiles.tile_w, tiles.stride_h, tiles.stride_w, Cc, _stream()), "ds_tile_step")
-
-
-def region_step_(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coef: torch.Tensor,
-                 guidance: float, euler: bool, regions, inpaint=None, rescale=None) -> None:
-    """``cfg_step_`` on a canvas denoised under per-region prompts (``ds_region_step``), in place.  ``regions`` is
-    (cover, R): cover uint8 [bs,H,W], bit r - 1 set where region r (1 .. R, R <= 8) covers the pixel; the background
-    covers the pixels whose cover is 0.  latents fp32 NHWC [bs,H,W,4] is the canvas; noise_pred and model_in bf16
-    [k*bs*R',H,W,4], R' = R + 1, hold k chunks of R' rows per canvas sample, row c*bs*R' + b*R' + r (r = 0 the
-    background).  Each canvas pixel becomes the mean, in row order, of the updates its covering rows give it, then the
-    inpaint blend; all R' rows of model_in get the next UNet input.  ``inpaint`` canvas-sized as in ``cfg_step_``;
-    ``rescale`` factors fp32 [bs*R'], one per row.  coef as in ``cfg_step_``."""
-    cover, n_regions = regions
-    _req(noise_pred, bf16, "region_step.noise_pred", 4)
-    _req(latents, f32, "region_step.latents", 4)
-    _req(model_in, bf16, "region_step.model_in", 4)
-    _req(coef, f32, "region_step.coef", 1)
-    _req(cover, torch.uint8, "region_step.cover", 3)
-    bs, H, W, Cc = latents.shape
-    n_regions = int(n_regions)
-    rows = bs * (n_regions + 1)
-    chunks = noise_pred.shape[0] // rows if rows else 0
-    ncoef = (3 if euler else 2) + (0 if inpaint is None else 2) + (chunks == 3)
-    if not 1 <= n_regions <= 8 or chunks not in (1, 2, 3) or noise_pred.shape != (chunks * rows, H, W, Cc) or \
-            model_in.shape != noise_pred.shape or cover.shape != (bs, H, W) or coef.numel() != ncoef:
-        raise DsEngineError("region_step: shape mismatch")
-    ptrs, factors, phi = _step_state("region_step", latents, rows, inpaint, rescale)
-    check(lib.ds_region_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(),
-                             float(guidance), int(bool(euler)), chunks, *ptrs, factors, float(phi), cover.data_ptr(),
-                             n_regions, bs, H * W, Cc, _stream()), "ds_region_step")
+    check(lib.ds_cfg_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), coef.data_ptr(),
+                          float(guidance), int(bool(euler)), chunks, *ptrs, factors, float(phi), layout, bs, H, W, Cc,
+                          _stream()), "ds_cfg_step")
 
 
 def cfg_rescale_factors(noise_pred: torch.Tensor, coef: torch.Tensor, guidance: float,

@@ -551,11 +551,11 @@ class DiffSenseiPipeline:
         diffusers' ``rescale_noise_cfg`` on the guided eps of every sample before the scheduler step.  ``tiles``: a
         ``TileGrid`` (MultiDiffusion): ``latents`` is the canvas and the conditions (and ``adapter`` may not be given)
         have one row per view of every sample, row b * V + v of each chunk, ``aspect_ratio`` the view's; the UNet runs
-        the view rows in slices of at most ``max_batch_panels`` view-samples, and ``ds_tile_step`` averages the views'
-        updates on the canvas.  ``regions``: (cover uint8 (bs, h, w), R), regional prompts (MultiDiffusion's
+        the view rows in slices of at most ``max_batch_panels`` view-samples, and ``ds_cfg_step`` over the views averages
+        their updates on the canvas.  ``regions``: (cover uint8 (bs, h, w), R), regional prompts (MultiDiffusion's
         region-based generation): ``latents`` is the canvas and the conditions have R' = R + 1 rows per sample, row
         b * R' + r of each chunk (r = 0 the background); the UNet runs the rows in slices as with ``tiles`` and
-        ``ds_region_step`` averages, per pixel, the updates of the rows whose region covers it (bit r - 1 of the cover
+        ``ds_cfg_step`` over the cover averages, per pixel, the updates of the rows whose region covers it (bit r - 1 of the cover
         for row r, the background where the cover is 0).  ``callback_on_step_end``: diffusers' step-end callback, called as
         ``callback(pipe, i, t, {"latents": fp32 NCHW latents})`` after each step (and its inpaint blend); the latents it
         returns become the loop's (``DenoiseStepper.set_latents``), and once it sets ``pipe._interrupt`` the remaining
@@ -813,8 +813,8 @@ class DiffSenseiPipeline:
         A panel with ``tile_size`` (an int or ``(height, width)`` in pixels; ``tile_overlap``, default 256) is denoised
         as overlapping views of that size, MultiDiffusion (Bar-Tal et al. 2023) as diffusers'
         ``StableDiffusionPanoramaPipeline`` runs it (``tiles.TileGrid``; ``_tile_rows`` gives each view's conditions):
-        every step the UNet runs all views, ``max_batch_panels`` view-samples per call, and ``ds_tile_step`` averages
-        the views' updated latents on the canvas before the inpaint blend.  A tiled panel is a denoise of its own; its
+        every step the UNet runs all views, ``max_batch_panels`` view-samples per call, and ``ds_cfg_step`` over the
+        views averages their updated latents on the canvas before the inpaint blend.  A tiled panel is a denoise of its own; its
         noise, image and mask are canvas-sized as untiled, and the canvas is decoded whole.
 
         ``callback_on_step_end`` (diffusers' contract) is called as ``callback(pipe, i, t, callback_kwargs)`` after each
@@ -1395,11 +1395,11 @@ class DenoiseStepper:
     With ``tiles`` (a ``TileGrid``, MultiDiffusion) the fp32 master latents are the canvas and ``model_in`` holds the
     k chunks of its view rows (row b * V + v of each chunk; ``load_panel`` gathers the first input on the host); a
     step runs the UNet on the view rows in slices of at most k * ``max_batch_panels`` rows, one after another into
-    slices of one eps buffer, then ``ds_tile_step`` (with the factors of every view row when rescaling).  Every kernel
+    slices of one eps buffer, then ``ds_cfg_step`` over the views (with the factors of every view row when rescaling).  Every kernel
     gives a row the same bits whatever batch surrounds it, so the slicing changes no bit.
     With ``regions`` = (cover, R) (regional prompts) the fp32 master latents are the canvas, ``model_in`` holds R + 1
     copies of every sample in each chunk (row b * (R + 1) + r), the UNet runs them in slices as with ``tiles``, and
-    the step is ``ds_region_step`` over the cover, a per-panel buffer ``load_panel`` refills.
+    the step is ``ds_cfg_step`` over the cover, a per-panel buffer ``load_panel`` refills.
     With ``cfg_cutoff`` = k inside the run (diffusers' ``SDXLCFGCutoffCallback``) steps k + 1 .. run without guidance:
     the UNet on the text chunk's rows alone (their conditions, time-embedding rows, dialog boxes and adapter rows; the
     same slicing and chains as the full launch) and the 1-chunk step (eps = text eps, no rescale; the inpaint blend,

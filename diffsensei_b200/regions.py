@@ -3,7 +3,7 @@
 A panel with ``regions`` is denoised under R' = 1 + R prompts at once.  Row 0 is the panel's own prompt (the
 background) and rows 1 .. R are the regions in the order given; in every chunk UNet row ``b * R' + r`` is sample b
 under prompt r, and its input is the whole canvas.  After every step each latent pixel becomes the mean of the updates
-of the rows that cover it (``ds_region_step``).  The cover is one byte per latent pixel, bit r - 1 set where region r
+of the rows that cover it (``ds_cfg_step`` over the cover).  The cover is one byte per latent pixel, bit r - 1 set where region r
 covers it; the background covers exactly the pixels no region covers.  Covers are binary: a ``box`` covers the latent
 pixels whose ``torch.linspace(0, 1, n)`` coordinates lie in it (the rule the masked IP attention applies to character
 boxes, ``ip_mask.cuh``), a ``mask`` the pixels the inpaint mask processor sets (``preprocess_latent_mask``).

@@ -18,8 +18,9 @@ step's PAG scale (``pag_scales``) to that table.
 and rejects any class or value whose arithmetic is not implemented here.
 
 The per-step update itself runs on the GPU, fused with the guidance blend, the optional guidance rescale, the inpaint
-blend and the next step's input scaling (``fused_step_``, ``ds_cfg_step``, or ``ds_tile_step`` / ``ds_region_step`` on a tiled / regional canvas); these classes produce the timesteps, the per-step coefficient table
-the kernel reads (``coefficient_table``) and the divisor of the first step's UNet input (``model_input_divisors``).
+blend and the next step's input scaling (``fused_step_``, ``ds_cfg_step``, on a plain, tiled or regional canvas); these
+classes produce the timesteps, the per-step coefficient table the kernel reads (``coefficient_table``) and the divisor
+of the first step's UNet input (``model_input_divisors``).
 """
 from __future__ import annotations
 
@@ -114,15 +115,10 @@ class DDIMScheduler:
         """The guidance blend + DDIM update (``ops.cfg_step_``): ``coef`` is a row of ``step_table``, with the PAG
         scale appended for a 3-chunk ``noise_pred``; ``inpaint`` None or (image_latents, noise, mask); ``rescale``
         None or (factors, guidance_rescale), the guided eps rescaled first (``ops.cfg_rescale_factors``).  ``tiles``:
-        a ``TileGrid`` when ``latents`` is a canvas denoised as its views (``ops.tile_step_``); ``regions``: (cover, R)
-        when it is a canvas denoised under per-region prompts (``ops.region_step_``).  A 1-chunk ``noise_pred`` (the
-        text rows alone, after a CFG cutoff) steps with the text eps and no guidance."""
-        if tiles is not None:
-            ops.tile_step_(noise_pred, latents, model_in, coef, guidance, False, tiles, inpaint, rescale)
-        elif regions is not None:
-            ops.region_step_(noise_pred, latents, model_in, coef, guidance, False, regions, inpaint, rescale)
-        else:
-            ops.cfg_step_(noise_pred, latents, model_in, coef, guidance, euler=False, inpaint=inpaint, rescale=rescale)
+        a ``TileGrid`` when ``latents`` is a canvas denoised as its views; ``regions``: (cover, R) when it is a canvas
+        denoised under per-region prompts.  A 1-chunk ``noise_pred`` (the text rows alone, after a CFG cutoff) steps
+        with the text eps and no guidance."""
+        ops.cfg_step_(noise_pred, latents, model_in, coef, guidance, False, inpaint, rescale, tiles, regions)
 
     def set_begin_index(self, begin_index: int = 0) -> None:
         """The loop's first step (img2img); DDIM's arithmetic does not depend on it, only add_noise's timestep."""
@@ -193,12 +189,7 @@ class EulerDiscreteScheduler:
     def fused_step_(self, noise_pred, latents, model_in, coef, guidance: float, inpaint=None, rescale=None,
                     tiles=None, regions=None) -> None:
         """The guidance blend + Euler update + the next step's scale_model_input (``ops.cfg_step_``); see DDIM's."""
-        if tiles is not None:
-            ops.tile_step_(noise_pred, latents, model_in, coef, guidance, True, tiles, inpaint, rescale)
-        elif regions is not None:
-            ops.region_step_(noise_pred, latents, model_in, coef, guidance, True, regions, inpaint, rescale)
-        else:
-            ops.cfg_step_(noise_pred, latents, model_in, coef, guidance, euler=True, inpaint=inpaint, rescale=rescale)
+        ops.cfg_step_(noise_pred, latents, model_in, coef, guidance, True, inpaint, rescale, tiles, regions)
 
     def set_begin_index(self, begin_index: int = 0) -> None:
         """diffusers' ``set_begin_index``: the loop starts at sigma_{begin_index} (img2img)."""

@@ -2,7 +2,7 @@
 ``StableDiffusionPanoramaPipeline`` lays it out (``get_views(..., window_size, stride)``), on the host.
 
 A panel with ``tile_size`` is denoised as overlapping views of the tile's size: every step runs the UNet on every
-view and the step kernel (``ds_tile_step``) averages the views' updated latents on the canvas.  Departure from
+view and the step kernel (``ds_cfg_step`` over the views) averages the views' updated latents on the canvas.  Departure from
 ``get_views``: when the stride does not land on the far edge, one more view flush with that edge is added (diffusers
 leaves the remainder uncovered, ``count == 0``, which turns it to zero); duplicates are dropped.  Every view has the
 tile's size.

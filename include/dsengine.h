@@ -347,13 +347,25 @@ int ds_timestep_embedding(const float* t, void* out, int rows, int dim, void* st
  * optionally followed by the inpaint blend.                                        [HBM-bound]
  * Replaces src/pipelines/pipeline_diffsensei.py:315-317,332-337 (chunk, the guidance blend, scheduler.step, the
  * torch.cat([latents] * chunks) and scheduler.scale_model_input for the next step).
+ * The same step runs on a canvas whose UNet rows are laid out as views or regions (MultiDiffusion, Bar-Tal et al.
+ * 2023): `rows` NULL (or all zero) is the plain layout, one row per canvas sample; otherwise exactly one of
+ *   views   (tile_h > 0) : the canvas denoised as overlapping tile_h x tile_w views (diffusers'
+ *                          StableDiffusionPanoramaPipeline); per axis n = ceil((dim - tile) / stride) + 1 views, view k at
+ *                          min(k * stride, dim - tile) (the last flush with the far edge); V = n_h * n_w in row-major
+ *                          order; 0 < stride <= tile <= dim.  Row b * V + v is view v of canvas sample b.
+ *   regions (cover)      : the canvas denoised under per-region prompts (sec. 4.2); cover uint8 [bs][H][W], bit r - 1
+ *                          set <=> region r covers the pixel (bits >= n_regions are ignored), the background covers
+ *                          exactly the pixels whose byte is 0; n_regions 1 .. 8, R' = n_regions + 1.  Row b * R' + r is
+ *                          canvas sample b under prompt r (r = 0: the background), every row the whole canvas.
  *   update        : 0 = DDIMScheduler (eta = 0), 1 = EulerDiscreteScheduler (s_churn = 0); epsilon prediction
  *   chunks        : 2 = CFG, noise_pred [uncond ; text]; 3 = CFG + perturbed-attention guidance (diffusers' PAGMixin
  *                   under classifier-free guidance), noise_pred [uncond ; text ; perturbed]; 1 = no guidance (the steps
  *                   after a CFG cutoff), noise_pred [text]: eps = e_text exactly, guidance unused, rescale_factors NULL
- *   noise_pred    : bf16 NHWC [chunks*bs][H][W][4]
- *   latents       : fp32 [bs][H][W][4] updated in place (fp32 master copy)
- *   model_in      : bf16 NHWC [chunks*bs][H][W][4], the next UNet input in every chunk: x_new (DDIM),
+ *   noise_pred    : bf16 NHWC [chunks * rows][h][w][4], 8-byte aligned; chunk c of row n is row c * rows + n, where
+ *                   rows = bs (plain), bs * V (views) or bs * R' (regions) and h x w = tile_h x tile_w for views, else
+ *                   H x W
+ *   latents       : fp32 [bs][H][W][4] updated in place (fp32 master copy, the canvas), 16-byte aligned
+ *   model_in      : bf16 NHWC, noise_pred's shape, 8-byte aligned: the next UNet input in every chunk: x_new (DDIM),
  *                   x_new / sqrt(sigma_next^2 + 1) (Euler)
  *   image_latents : fp32 NHWC [bs][H][W][4] (z, scaling_factor * posterior sample), 16-byte aligned
  *   noise         : fp32 NHWC [bs][H][W][4] (n, the noise the start latents were drawn with), 16-byte aligned
@@ -362,21 +374,25 @@ int ds_timestep_embedding(const float* t, void* out, int rows, int dim, void* st
  *   coef          : device pointer to this step's row, columns in this order:
  *                   DDIM {alpha_prod_t, alpha_prod_t_prev} or Euler {sigma, sigma_next, sqrt(sigma_next^2 + 1)},
  *                   then {c0, c1} when inpainting, then s when chunks == 3
- *   rescale_factors : NULL (no rescale; guidance_rescale must then be 0) or fp32 [bs], the factors
- *                   ds_cfg_rescale_factors wrote for this noise_pred and coef row
+ *   rescale_factors : NULL (no rescale; guidance_rescale must then be 0) or fp32 [rows], one factor per row, the
+ *                   factors ds_cfg_rescale_factors wrote for this noise_pred and coef row
  *   guidance_rescale: phi of diffusers' rescale_noise_cfg as the caller's double (finite; on for phi > 0 in diffusers)
- * The arithmetic, per element:
+ * The arithmetic, per element of a row:
  *   eps   = e_uncond + guidance * (e_text - e_uncond)      [+ s * (e_text - e_perturbed) with 3 chunks]
  *   rescale (rescale_factors given): eps = fp32(phi) * (eps * r_b) + fp32(1 - phi) * eps, r_b the factor of the
- *            pixel's sample, 1 - phi evaluated in double: torch's fp32 values of the Python scalars
+ *            pixel's row, 1 - phi evaluated in double: torch's fp32 values of the Python scalars
  *   DDIM  : x0 = (x - sqrt(1-a_t) * eps) / sqrt(a_t);  x_new = sqrt(a_prev) * x0 + sqrt(1-a_prev) * eps
  *   Euler : x0 = x - sigma * eps;  d = (x - x0) / sigma;  x_new = x + d * (sigma_next - sigma)
+ * Per canvas pixel x: the plain layout's x_new is its row's.  With views or regions each covering row, in row order,
+ * gives x_r from x and that row's eps (and factor), and x_new = (0 + x_r1 + x_r2 + ...) / count in fp32, each sum and
+ * the division rounded on their own.  Then
  *   inpaint: init = c0 * z + c1 * n (add_noise of the image latents at the next timestep; {1, 0} on the last step);
  *            x_new = mask ? x_new : init, and the next UNet input is computed from the blended x_new
+ * and the canvas and the next UNet input are written, into every chunk of every covering view, or of all R' rows.
  * Rounding: every operation is rounded on its own in diffusers' eager fp32 order, except DDIM with 2 chunks and no
  * rescale, where the compiler may contract multiply-adds into FMAs (1 chunk: op by op, diffusers' eager
- * scheduler.step(noise_pred_text)).  A pixel with mask != 0 is the result without
- * inpaint bit for bit.
+ * scheduler.step(noise_pred_text)).  A pixel with mask != 0 is the result without inpaint bit for bit.  No atomics:
+ * every output element is written by one thread once.
  *
  * ds_cfg_rescale_factors: the per-sample factors of diffusers' rescale_noise_cfg (Lin et al. 2024, sec. 3.4), from
  * the same noise_pred / coef row / guidance / chunks the step then reads (s = coef[ncoef - 1] with 3 chunks):
@@ -387,52 +403,17 @@ int ds_timestep_embedding(const float* t, void* out, int rows, int dim, void* st
  *   std 0, so its factor is +inf (NaN if its text eps is constant too), and the rescaled step then writes inf / NaN
  *   into that sample, as diffusers does; there is no guard.
  * --------------------------------------------------------------------------------------------- */
+typedef struct {
+  int32_t tile_h, tile_w, stride_h, stride_w; /* views: tile_h > 0 */
+  const void* cover;                          /* regions: uint8 [bs][H][W] */
+  int32_t n_regions;
+} ds_step_rows;
 int ds_cfg_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance, int update,
                 int chunks, const float* image_latents, const float* noise, const uint8_t* mask,
-                const float* rescale_factors, double guidance_rescale, int bs, int HW, int C, void* stream);
+                const float* rescale_factors, double guidance_rescale, const ds_step_rows* rows, int bs, int H, int W,
+                int C, void* stream);
 int ds_cfg_rescale_factors(const void* noise_pred, const float* coef, int ncoef, float guidance, int chunks,
                            float* factors, int bs, int HW, int C, void* stream);
-
-/* ds_tile_step: ds_cfg_step on a canvas denoised as overlapping views (MultiDiffusion, Bar-Tal et al. 2023; diffusers'
- * StableDiffusionPanoramaPipeline).                                                [HBM-bound]
- *   latents       : fp32 NHWC [bs][H][W][4], the canvas (updated in place)
- *   noise_pred    : bf16 NHWC [chunks * bs * V][tile_h][tile_w][4], model_in the same shape; row c * bs * V + b * V + v
- *                   is chunk c of view v of canvas sample b
- *   views         : per axis n = ceil((dim - tile) / stride) + 1 views, view k at min(k * stride, dim - tile) (the last
- *                   flush with the far edge); V = n_h * n_w in row-major order; 0 < stride <= tile <= dim
- *   image_latents / noise / mask : canvas-sized as in ds_cfg_step (all three or none)
- *   rescale_factors : NULL or fp32 [bs * V], one factor per view row (ds_cfg_rescale_factors over the view rows)
- *   update, chunks, coef, guidance, guidance_rescale : as ds_cfg_step (chunks 1: the text chunk's view rows only)
- * Per canvas pixel: each covering view, in view order, gives x_v = ds_cfg_step's update of the canvas pixel from that
- * view's eps (and that view's factor); x_new = (0 + x_v1 + x_v2 + ...) / count in fp32, each sum and the division
- * rounded on their own (one view: ds_cfg_step's bits); then the inpaint blend on the canvas pixel; then the canvas and
- * the next UNet input (ds_cfg_step's) in every chunk of every covering view.  No atomics: every output element is
- * written by one thread once. */
-int ds_tile_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance, int update,
-                 int chunks, const float* image_latents, const float* noise, const uint8_t* mask,
-                 const float* rescale_factors, double guidance_rescale, int bs, int H, int W, int tile_h, int tile_w,
-                 int stride_h, int stride_w, int C, void* stream);
-
-/* ds_region_step: ds_cfg_step on a canvas denoised under per-region prompts (MultiDiffusion's region-based
- * generation, Bar-Tal et al. 2023 sec. 4.2).                                      [HBM-bound]
- *   latents       : fp32 NHWC [bs][HW][4], the canvas (updated in place)
- *   noise_pred    : bf16 NHWC [chunks * bs * R'][HW][4], model_in the same shape; R' = n_regions + 1; row
- *                   c * bs * R' + b * R' + r is chunk c of canvas sample b under prompt r (r = 0: the background)
- *   cover         : uint8 [bs][HW]; bit r - 1 set <=> region r covers the pixel (bits >= n_regions are ignored); the
- *                   background covers exactly the pixels whose byte is 0
- *   n_regions     : 1 .. 8
- *   image_latents / noise / mask : canvas-sized as in ds_cfg_step (all three or none)
- *   rescale_factors : NULL or fp32 [bs * R'], one factor per row (ds_cfg_rescale_factors over the rows)
- *   update, chunks, coef, guidance, guidance_rescale : as ds_cfg_step (chunks 1: the text chunk's rows only)
- * Per canvas pixel: each covering row, in row order, gives x_r = ds_cfg_step's update of the canvas pixel from that
- * row's eps (and that row's factor); x_new = (0 + x_r1 + x_r2 + ...) / count in fp32, each sum and the division
- * rounded on their own (one covering row: ds_cfg_step's bits); then the inpaint blend on the canvas pixel; then the
- * canvas and the next UNet input (ds_cfg_step's) in every chunk of all R' rows.  latents, image_latents and noise must
- * be 16-byte aligned, noise_pred and model_in 8-byte.  No atomics: every output element is written by one thread once. */
-int ds_region_step(const void* noise_pred, float* latents, void* model_in, const float* coef, float guidance,
-                   int update, int chunks, const float* image_latents, const float* noise, const uint8_t* mask,
-                   const float* rescale_factors, double guidance_rescale, const uint8_t* cover, int n_regions, int bs,
-                   int HW, int C, void* stream);
 
 /* Perceiver attention of the character Resampler: 16 latent queries x (n_kv) keys per (character, head),
  * q and k each pre-scaled by dim_head^-0.25, fp32 softmax (src/models/resampler.py:64-74).

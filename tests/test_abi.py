@@ -35,7 +35,7 @@ def test_struct_layout_matches_header_field_order():
     from diffsensei_b200 import _lib
     src = open(os.path.join(ROOT, "include", "dsengine.h")).read()
     for struct_name, cls in (("ds_gemm_args", _lib.GemmArgs), ("ds_conv3x3_args", _lib.Conv3x3Args),
-                             ("ds_cross_ip_args", _lib.CrossIpArgs)):
+                             ("ds_cross_ip_args", _lib.CrossIpArgs), ("ds_step_rows", _lib.StepRows)):
         body = re.search(r"typedef struct \{([^{}]*)\} " + struct_name + ";", src).group(1)
         body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
         names = []

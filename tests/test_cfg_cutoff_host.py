@@ -204,17 +204,18 @@ def test_stepper_key_changes_only_with_a_cutoff_inside_the_run(monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------------ ABI
-def test_abi_accepts_one_chunk_and_refuses_its_rescale():
+def test_abi_accepts_one_chunk_and_refuses_its_rescale_in_every_layout():
     """The argument checks run before any device query; each call fails a later check, so nothing launches."""
     from diffsensei_b200 import _lib
     lib = _lib.lib
-    cfg = lambda chunks, factors, phi, C: (16, 16, 16, 16, 7.5, 0, chunks, None, None, None, factors, phi, 1, 64, C,
-                                           None)
-    tile = lambda chunks, factors, phi, stride: (16, 16, 16, 16, 7.5, 1, chunks, None, None, None, factors, phi, 1,
-                                                 16, 16, 8, 8, stride, stride, 4, None)
-    region = lambda chunks, factors, phi, C: (16, 16, 16, 16, 7.5, 0, chunks, None, None, None, factors, phi, 16, 2,
-                                              1, 64, C, None)
-    for fn, args, later in ((lib.ds_cfg_step, cfg, 3), (lib.ds_tile_step, tile, 0), (lib.ds_region_step, region, 3)):
+    cfg = lambda chunks, factors, phi, C: (16, 16, 16, 16, 7.5, 0, chunks, None, None, None, factors, phi, None, 1,
+                                           16, 16, C, None)
+    tile = lambda chunks, factors, phi, stride: (16, 16, 16, 16, 7.5, 1, chunks, None, None, None, factors, phi,
+                                                 _lib.StepRows(8, 8, stride, stride, None, 0), 1, 16, 16, 4, None)
+    region = lambda chunks, factors, phi, C: (16, 16, 16, 16, 7.5, 0, chunks, None, None, None, factors, phi,
+                                              _lib.StepRows(0, 0, 0, 0, 16, 2), 1, 16, 16, C, None)
+    for args, later in ((cfg, 3), (tile, 0), (region, 3)):
+        fn = lib.ds_cfg_step
         assert fn(*args(1, None, 0.0, later)) == 1
         err = lib.ds_last_error()
         assert b"chunks" not in err and (b"C == 4" in err or b"stride" in err), err

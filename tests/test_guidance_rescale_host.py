@@ -54,14 +54,14 @@ def test_stepper_key_holds_the_value_only_when_on(monkeypatch):
     assert key(guidance_rescale=0.7) == on
 
 
-def test_abi_refuses_a_rescale_value_without_factors_and_a_non_finite_one():
-    """The argument checks of ds_cfg_step run before any device query (a NULL-free call with dummy pointers)."""
+def test_step_abi_refuses_a_rescale_value_without_factors_and_a_non_finite_one():
+    """The argument checks of ds_cfg_step run before any device query (dummy, aligned pointers)."""
     from diffsensei_b200 import _lib
     lib = _lib.lib
-    args = lambda factors, phi: (1, 1, 1, 1, 7.5, 0, 2, None, None, None, factors, phi, 1, 16, 4, None)
+    args = lambda factors, phi: (16, 16, 16, 16, 7.5, 0, 2, None, None, None, factors, phi, None, 1, 4, 4, 4, None)
     assert lib.ds_cfg_step(*args(None, 0.7)) == 1
     assert b"guidance_rescale" in lib.ds_last_error()
-    assert lib.ds_cfg_step(*args(1, math.nan)) == 1
+    assert lib.ds_cfg_step(*args(16, math.nan)) == 1
     assert b"guidance_rescale" in lib.ds_last_error()
     assert lib.ds_cfg_rescale_factors(1, 1, 3, 7.5, 4, 1, 1, 16, 4, None) == 1
     assert b"chunks" in lib.ds_last_error()

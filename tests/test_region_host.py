@@ -252,17 +252,19 @@ def test_stepper_key_is_unchanged_with_regions_off(monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------------ ABI
-def test_abi_checks_its_arguments():
-    """ds_region_step's argument checks run before any device query (dummy, aligned pointers)."""
+def test_abi_checks_a_region_layout():
+    """ds_cfg_step's argument checks on a region layout run before any device query (dummy, aligned pointers)."""
     from diffsensei_b200 import _lib
     lib = _lib.lib
 
     def call(**kw):
         a = dict(noise_pred=16, latents=16, model_in=16, coef=16, guidance=7.5, update=0, chunks=2, image_latents=None,
-                 noise=None, mask=None, rescale=None, guidance_rescale=0.0, cover=16, n_regions=2, bs=1, HW=64, C=4,
+                 noise=None, mask=None, rescale=None, guidance_rescale=0.0, cover=16, n_regions=2, bs=1, H=8, W=8, C=4,
                  stream=None)
         a.update(kw)
-        return lib.ds_region_step(*a.values()), lib.ds_last_error()
+        rows = _lib.StepRows(0, 0, 0, 0, a.pop("cover"), a.pop("n_regions"))
+        a = list(a.values())
+        return lib.ds_cfg_step(*a[:12], rows, *a[12:]), lib.ds_last_error()
     for kw, msg in [(dict(cover=None), b"NULL pointer"), (dict(noise_pred=None), b"NULL pointer"),
                     (dict(n_regions=0), b"n_regions must be in [1, 8]"), (dict(n_regions=9), b"n_regions"),
                     (dict(chunks=4), b"chunks must be 2 or 3"), (dict(update=2), b"update must be 0"),

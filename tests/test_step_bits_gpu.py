@@ -10,6 +10,16 @@ seeded CPU generators, so every build sees the same values.  The goldens were wr
 this one replaced:
 
     python tests/test_step_bits_gpu.py [OUT.json]     (on an H100; default OUT is tests/golden/step_bits.json)
+
+The second golden file, tests/golden/step_layout_bits.json, pins all 20 variants (DDIM / Euler x 1 / 2 / 3 chunks x
+inpaint off / on x guidance rescale off / on, rescale with 2 or 3 chunks only, its factors from ``cfg_rescale_factors``
+of the same eps) of the step on every row layout, through ``fused_step_(..., tiles=, regions=)``: the plain canvas, a
+view grid clipped at both far edges, a view equal to the canvas, a cover with pixels under 0, 1, 2 and 3 regions, and
+8 regions with every cover byte value, each at one shape whose pixel count is not a multiple of 256 on the first, a
+middle and the last step of a 30-step schedule.  Those goldens were written by the three separate step kernels
+(plain, tiled, regional) that the one kernel over a row layout replaced:
+
+    python tests/test_step_bits_gpu.py --layouts [OUT.json]     (default OUT is tests/golden/step_layout_bits.json)
 """
 import hashlib
 import json
@@ -22,6 +32,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 GOLDEN_FILE = os.path.join(HERE, "golden", "step_bits.json")
+LAYOUT_GOLDEN_FILE = os.path.join(HERE, "golden", "step_layout_bits.json")
 
 pytestmark = pytest.mark.gpu
 
@@ -90,6 +101,93 @@ def cfg_step_fn(ops, euler):
     return lambda eps, lat, mi, coef, inp: ops.cfg_step_(eps, lat, mi, coef, GUIDANCE, euler=euler, inpaint=inp)
 
 
+# ------------------------------------------------------------------------------------------------ row layouts
+LAYOUT_SHAPE = (2, 17, 23)                  # bs*HW = 782
+LAYOUTS = ["plain", "tiles_clipped", "tiles_whole", "regions_0123", "regions_r8"]
+LAYOUT_VARIANTS = [(euler, chunks, inpaint, rescale) for euler in (False, True) for chunks in (1, 2, 3)
+                   for inpaint in (False, True) for rescale in (False, True) if chunks > 1 or not rescale]
+PHI = 0.7
+
+
+def layout_case_name(layout, euler, chunks, inpaint, rescale, step):
+    return (f"{layout}_{'euler' if euler else 'ddim'}_c{chunks}{'_inpaint' if inpaint else ''}"
+            f"{'_rescale' if rescale else ''}_s{step}")
+
+
+def all_layout_cases():
+    return {layout_case_name(lay, *v, st): (lay, *v, st) for lay in LAYOUTS for v in LAYOUT_VARIANTS for st in STEPS}
+
+
+def layout_rows(layout):
+    """(keyword of ``fused_step_``, UNet rows per canvas sample, view height, view width), on the host."""
+    from diffsensei_b200.tiles import TileGrid
+    bs, H, W = LAYOUT_SHAPE
+    if layout.startswith("tiles"):
+        # 17 x 23 in 8 x 12 views at stride 5 x 7: ys 0, 5, 9 and xs 0, 7, 11, the last view on each axis clipped
+        grid = TileGrid(H, W, 8, 12, 5, 7) if layout == "tiles_clipped" else TileGrid(H, W, H, W, H, W)
+        return {"tiles": grid}, grid.n_views, grid.tile_h, grid.tile_w
+    if layout.startswith("regions"):
+        g = torch.Generator().manual_seed(7)
+        if layout == "regions_0123":
+            R, cover = 3, torch.randint(0, 8, (bs, H, W), generator=g, dtype=torch.uint8)
+        else:
+            R, cover = 8, (torch.randperm(bs * H * W, generator=g) % 256).to(torch.uint8).reshape(bs, H, W)
+        return {"regions": (cover, R)}, R + 1, H, W
+    return {}, 1, H, W
+
+
+def run_layout_case(layout, euler, chunks, inpaint, rescale, step):
+    """One step through the scheduler's ``fused_step_`` on ``layout``; returns (latents, model_in) on the device."""
+    from diffsensei_b200 import ops
+    from diffsensei_b200.scheduler import DDIMScheduler, EulerDiscreteScheduler
+    sch = EulerDiscreteScheduler() if euler else DDIMScheduler()
+    sch.set_timesteps(T_STEPS)
+    bs, H, W = LAYOUT_SHAPE
+    kw, per_sample, th, tw = layout_rows(layout)
+    if "regions" in kw:
+        kw = {"regions": (kw["regions"][0].to(DEV), kw["regions"][1])}
+    rows = bs * per_sample
+    coef = coef_row(euler, chunks, inpaint, step)
+    g = torch.Generator().manual_seed(1000 * step + 100 * LAYOUTS.index(layout) + 10 * chunks + 4 * euler +
+                                      2 * inpaint + rescale)
+    eps = torch.randn(chunks * rows, th, tw, 4, generator=g).to(bf16).to(DEV)
+    lat = (torch.randn(bs, H, W, 4, generator=g) * (float(coef[0]) if euler else 1.0)).to(DEV)
+    inp = None
+    if inpaint:
+        inp = (torch.randn(bs, H, W, 4, generator=g).to(DEV), torch.randn(bs, H, W, 4, generator=g).to(DEV),
+               (torch.rand(bs, H, W, generator=g) < 0.5).to(torch.uint8).to(DEV))
+    coef = coef.to(DEV)
+    res = (ops.cfg_rescale_factors(eps, coef, GUIDANCE, out=torch.empty(rows, device=DEV)), PHI) if rescale else None
+    mi = torch.full(eps.shape, float("nan"), dtype=bf16, device=DEV)
+    sch.fused_step_(eps, lat, mi, coef, GUIDANCE, inp, res, **kw)
+    torch.cuda.synchronize()
+    return lat, mi
+
+
+@pytest.fixture(scope="module")
+def layout_golden():
+    with open(LAYOUT_GOLDEN_FILE) as f:
+        return json.load(f)
+
+
+@pytest.mark.parametrize("name", sorted(all_layout_cases()))
+def test_step_layout_bits_match_golden(layout_golden, name):
+    lat, mi = run_layout_case(*all_layout_cases()[name])
+    assert torch.isfinite(lat).all() and torch.isfinite(mi.float()).all()
+    assert {"latents": bits(lat), "model_in": bits(mi)} == layout_golden[name]
+
+
+def test_layouts_cover_what_they_claim():
+    """The clipped grid ends flush with both far edges off its stride; the regions hold 0-3 and every byte."""
+    bs, H, W = LAYOUT_SHAPE
+    assert (bs * H * W) % 256 != 0
+    grid = layout_rows("tiles_clipped")[0]["tiles"]
+    assert grid.ys == [0, 5, 9] and grid.xs == [0, 7, 11]
+    cover = layout_rows("regions_0123")[0]["regions"][0]
+    assert {bin(v).count("1") for v in cover.unique().tolist()} == {0, 1, 2, 3}
+    assert len(layout_rows("regions_r8")[0]["regions"][0].unique()) == 256
+
+
 @pytest.fixture(scope="module")
 def golden():
     with open(GOLDEN_FILE) as f:
@@ -108,11 +206,17 @@ def test_step_bits_match_golden(golden, name):
 if __name__ == "__main__":
     sys.path.insert(0, ROOT)
     from diffsensei_b200 import ops as o
+    layouts = sys.argv[1:2] == ["--layouts"]
+    args = sys.argv[1 + layouts:]
+    if layouts:
+        runs = {name: (lambda c=case: run_layout_case(*c)) for name, case in all_layout_cases().items()}
+    else:
+        runs = {name: (lambda c=case: run_case(cfg_step_fn(o, c[0]), *c)) for name, case in all_cases().items()}
     out = {}
-    for name, (euler, chunks, inpaint, shape, step) in sorted(all_cases().items()):
-        lat, mi = run_case(cfg_step_fn(o, euler), euler, chunks, inpaint, shape, step)
+    for name in sorted(runs):
+        lat, mi = runs[name]()
         out[name] = {"latents": bits(lat), "model_in": bits(mi)}
         print(name, out[name], flush=True)
-    with open(sys.argv[1] if len(sys.argv) > 1 else GOLDEN_FILE, "w") as f:
+    with open(args[0] if args else (LAYOUT_GOLDEN_FILE if layouts else GOLDEN_FILE), "w") as f:
         json.dump(out, f, indent=1, sort_keys=True)
         f.write("\n")

@@ -193,12 +193,13 @@ def test_stepper_key_is_unchanged_with_tiling_off(monkeypatch):
     assert math.isclose(on[3], 32 / 48)
 
 
-def test_abi_checks_the_grid():
-    """ds_tile_step's argument checks run before any device query (dummy pointers)."""
+def test_abi_checks_a_view_layout():
+    """ds_cfg_step's checks of a view layout run before any device query (dummy pointers)."""
     from diffsensei_b200 import _lib
     lib = _lib.lib
-    args = lambda th, tw, sh, sw: (1, 1, 1, 1, 7.5, 0, 2, None, None, None, None, 0.0, 1, 16, 24, th, tw, sh, sw, 4,
-                                   None)
-    assert lib.ds_tile_step(*args(17, 8, 8, 8)) == 1 and b"fit the canvas" in lib.ds_last_error()
-    assert lib.ds_tile_step(*args(8, 8, 9, 8)) == 1 and b"stride" in lib.ds_last_error()
-    assert lib.ds_tile_step(*args(8, 8, 0, 8)) == 1 and b"stride" in lib.ds_last_error()
+    args = lambda th, tw, sh, sw, cover=None: (16, 16, 16, 16, 7.5, 0, 2, None, None, None, None, 0.0,
+                                               _lib.StepRows(th, tw, sh, sw, cover, 0), 1, 16, 24, 4, None)
+    assert lib.ds_cfg_step(*args(17, 8, 8, 8)) == 1 and b"fit the canvas" in lib.ds_last_error()
+    assert lib.ds_cfg_step(*args(8, 8, 9, 8)) == 1 and b"stride" in lib.ds_last_error()
+    assert lib.ds_cfg_step(*args(8, 8, 0, 8)) == 1 and b"stride" in lib.ds_last_error()
+    assert lib.ds_cfg_step(*args(8, 8, 8, 8, 16)) == 1 and b"both views and regions" in lib.ds_last_error()

@@ -5,7 +5,7 @@ An SDXL-size manga UNet with seeded random weights, a 1024 x 1024 panel (128 x 1
 DDIM, with 0, 1 and 3 regions (R' = 1, 2 and 4 UNet rows per chunk).  Measured, medians over ``--rounds`` rounds that
 alternate the three cases (round 0 a warm-up): the whole ``denoise`` call of ``--steps`` steps (host clock around a
 synchronised call, graph-captured stepper) and the captured step alone (CUDA events).  Then the step kernel alone,
-``ds_region_step`` on the canvas against ``ds_cfg_step`` on the same canvas, each as one CUDA graph of ``--iters``
+``ds_cfg_step`` over the regions on the canvas against ``ds_cfg_step`` on the plain canvas, each as one CUDA graph of ``--iters``
 launches replayed ``--rounds`` times, alternating (CUDA events).  The card's name, power limit and SM clocks are read
 with `nvidia-smi --query-gpu` (read only) in the same run.
 
@@ -49,8 +49,8 @@ def case_args(n_regions: int):
 
 
 def kernel_graph(sch, n_regions: int, iters: int):
-    """A CUDA graph of ``iters`` step-kernel launches on a 128 x 128 canvas: ``ds_cfg_step`` (0 regions) or
-    ``ds_region_step``, from a fixed eps."""
+    """A CUDA graph of ``iters`` step-kernel launches on a 128 x 128 canvas: ``ds_cfg_step`` (0 regions: the plain
+    layout), from a fixed eps."""
     from diffsensei_b200.scheduler import step_table
     h = w = SIZE // 8
     rows = n_regions + 1
@@ -129,7 +129,7 @@ def main():
             if r:
                 kern[R].append(round(us, 2))
     for R in cases:
-        res[f"regions_{R}"].update(step_kernel="ds_cfg_step" if R == 0 else "ds_region_step",
+        res[f"regions_{R}"].update(step_kernel="ds_cfg_step" if R == 0 else "ds_cfg_step (regions)",
                                    step_kernel_us_median=statistics.median(kern[R]), step_kernel_us_rounds=kern[R])
     res["gpu_after"] = gpu_info()
     print(json.dumps(res))

@@ -6,8 +6,8 @@ An SDXL-size manga UNet with seeded random weights, one sample, guidance 7.5, DD
 * a 1024 x 4096 strip (width x height; 512 x 128 latent), same tiles: 5 views.
 Measured, medians over ``--rounds`` (round 0 a warm-up): the whole ``denoise`` call of ``--steps`` steps (host clock
 around a synchronised call, graph-captured stepper), the captured step alone (CUDA events), and, with CUDA events
-over ``--iters`` launches, the step kernel alone: ``ds_tile_step`` on the tiled canvas against ``ds_cfg_step`` on the
-untiled one.  The card's name, power limit and SM clocks are read with `nvidia-smi --query-gpu` (read only) in the
+over ``--iters`` launches, the step kernel alone: ``ds_cfg_step`` over the views of the tiled canvas against
+``ds_cfg_step`` on the untiled one.  The card's name, power limit and SM clocks are read with `nvidia-smi --query-gpu` (read only) in the
 same run.
 
     python tools/tile_bench.py [--rounds 3] [--steps 4] [--iters 200]
@@ -115,7 +115,7 @@ def main():
                          "call_ms_median": statistics.median(calls), "call_ms_rounds": calls,
                          "step_ms_median": statistics.median(steps), "step_ms_rounds": steps,
                          "step_kernel_us": round(time_kernel(st, args.iters), 2),
-                         "step_kernel": "ds_cfg_step" if grid is None else "ds_tile_step"}
+                         "step_kernel": "ds_cfg_step" if grid is None else "ds_cfg_step (views)"}
             pipe._steppers.clear()
             torch.cuda.empty_cache()
         out["tiled_over_untiled_step"] = round(out["tiled"]["step_ms_median"] / out["untiled"]["step_ms_median"], 3)
