@@ -93,6 +93,7 @@ SIGNATURES = {
     "ds_resampler_attn": [_vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "ds_attention_small": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i64, _i64, _i64, _i64, _f, _i, _vp],
     "ds_embed_tokens": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],
+    "ds_prompt_emphasis": [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp],
     "ds_latent_pointwise": [_vp, _vp, _vp, _vp, _f, _i, _i, _vp],
     "ds_softmax_rows": [_vp, _vp, _i, _i, _i64, _i64, _f, _vp],
     "ds_image_postprocess": [_vp, _vp, _i, _i, _i, _vp],

@@ -42,10 +42,13 @@ constexpr int kAttnThreads = 384;
 constexpr int kQBytes = kQTile * kHd * 2;   // 16 KiB
 constexpr int kKVBytes = kKTile * kHd * 2;  // 8 KiB each for K and V
 constexpr int kStreamSmemBytes = kQBytes + kRing * 2 * kKVBytes + 1024 /*align*/ + 256 /*barriers*/;
-// cross-attention with resident keys: up to kResidentTiles K|V tiles of both sets together, two Q buffers
-constexpr int kResidentTiles = 4;
+// cross-attention with resident keys: up to kResidentTiles K|V tiles of both sets together, two Q buffers.  The
+// dynamic shared memory is sized at launch from the tiles present (cross_smem_bytes): 77 text + 80 IP keys take
+// 4 tiles, 97.25 KiB; a 4-chunk, 308-token prompt with the UNet's 80 IP keys 7 tiles; 8 tiles take 161.25 KiB.
+constexpr int kResidentTiles = 8;
 constexpr int kQBufs = 2;
-constexpr int kCrossSmemBytes = kResidentTiles * 2 * kKVBytes + kQBufs * kQBytes + 1024 + 256;
+constexpr int cross_smem_bytes(int tiles) { return tiles * 2 * kKVBytes + kQBufs * kQBytes + 1024 + 256; }
+static_assert(cross_smem_bytes(kResidentTiles) <= 227 * 1024, "resident key tiles exceed the opt-in shared memory");
 constexpr float kLog2e = 1.4426950408889634f;
 // Register budgets after setmaxnreg (the launch gives every thread 168): one TMA lane in the producer warpgroup, the
 // pipelined consumers hold O, two score tiles' worth of S / P and the softmax state.  128 * 40 + 256 * 232 <= 65536.
@@ -408,15 +411,15 @@ attn_cross_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
   uint8_t* sKV = smem;  // tile t (set 0's tiles, then set 1's): K at t * 16 KiB, V at t * 16 KiB + 8 KiB
-  uint8_t* sQ = sKV + kResidentTiles * 2 * kKVBytes;
+  const int tiles0 = (p.n_keys[0] + kKTile - 1) / kKTile;
+  const int tiles1 = (p.n_keys[1] + kKTile - 1) / kKTile;
+  uint8_t* sQ = sKV + (tiles0 + tiles1) * 2 * kKVBytes;
   uint64_t* kv_full = reinterpret_cast<uint64_t*>(sQ + kQBufs * kQBytes);
   uint64_t* kv_empty = kv_full + 1;
   uint64_t* q_full = kv_empty + 1;
   uint64_t* q_empty = q_full + kQBufs;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tiles0 = (p.n_keys[0] + kKTile - 1) / kKTile;
-  const int tiles1 = (p.n_keys[1] + kKTile - 1) / kKTile;
   const int item_lo = static_cast<int>(static_cast<long long>(blockIdx.x) * p.items / gridDim.x);
   const int item_hi = static_cast<int>(static_cast<long long>(blockIdx.x + 1) * p.items / gridDim.x);
 
@@ -517,13 +520,14 @@ static bool make_tok_map(CUtensorMap* m, const void* base, int cols, int ld, int
 
 using AttnKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, AttnParams);
 
-// attr_set: one flag per device, for the kernel's dynamic shared memory opt-in
-static int launch_attn(AttnKernel kernel, const char* name, int smem_bytes, bool* attr_set, dim3 grid,
-                       const CUtensorMap& tmQ, const CUtensorMap& tmK0, const CUtensorMap& tmK1, const AttnParams& p,
-                       cudaStream_t st) {
+// attr_set: one flag per device, for the kernel's dynamic shared memory opt-in (to max_smem_bytes, the most any launch
+// of the kernel takes)
+static int launch_attn(AttnKernel kernel, const char* name, int smem_bytes, int max_smem_bytes, bool* attr_set,
+                       dim3 grid, const CUtensorMap& tmQ, const CUtensorMap& tmK0, const CUtensorMap& tmK1,
+                       const AttnParams& p, cudaStream_t st) {
   bool& set = attr_set[device_slot()];
   if (!set) {
-    DS_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    DS_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_bytes));
     set = true;
   }
   cudaLaunchConfig_t cfg = {};
@@ -543,7 +547,7 @@ static int launch_attn(AttnKernel kernel, const char* name, int smem_bytes, bool
 static int launch_stream(const CUtensorMap& tmQ, const CUtensorMap& tmK0, const CUtensorMap& tmK1,
                          const AttnParams& p, int B, int heads, cudaStream_t st) {
   static bool attr_set[kMaxDevices] = {};
-  return launch_attn(attn_stream_kernel, "attn_stream_kernel", kStreamSmemBytes, attr_set,
+  return launch_attn(attn_stream_kernel, "attn_stream_kernel", kStreamSmemBytes, kStreamSmemBytes, attr_set,
                      dim3((p.Nq + kQTile - 1) / kQTile, heads, B), tmQ, tmK0, tmK1, p, st);
 }
 
@@ -665,6 +669,6 @@ extern "C" int ds_attention_cross_ip(const ds_cross_ip_args* a, void* stream) {
   p.items = static_cast<int>(items);
   const int ctas = static_cast<int>(items < dev.num_sms ? items : dev.num_sms);
   static bool attr_set[kMaxDevices] = {};
-  return launch_attn(attn_cross_kernel, "attn_cross_kernel", kCrossSmemBytes, attr_set, dim3(ctas), tmQ, tmT, tmI,
-                     p, st);
+  return launch_attn(attn_cross_kernel, "attn_cross_kernel", cross_smem_bytes(tiles), cross_smem_bytes(kResidentTiles),
+                     attr_set, dim3(ctas), tmQ, tmT, tmI, p, st);
 }

@@ -10,6 +10,8 @@
 //                        attention), so the attention is a plain CUDA-core kernel: K / V of one (batch, head) staged
 //                        in shared memory, one warp per query row, fp32 softmax.                   [latency-bound]
 //   ds_embed_tokens    : out[b][t][:] = token_embedding[ids[b][t]][:] + position_embedding[t][:]   (CLIPTextEmbeddings)
+//   ds_prompt_emphasis : AUTOMATIC1111's "Original" prompt emphasis on each encoder's chunk of hidden_states[-2],
+//                        written into the concatenated [chunks][L][C1 + C2] prompt embedding (prompt_weighting.py)
 #include "ds_common.cuh"
 #include "ds_host.h"
 
@@ -120,7 +122,101 @@ __global__ void embed_tokens_kernel(const int* __restrict__ ids, const uint4* __
   out[i] = o;
 }
 
+constexpr int kEmphasisThreads = 256;
+
+// One CTA per (entry, encoder).  z = the source chunk [L][C], w = its per-token weights [L]:
+//   m0 = mean(z), z' = z * w, m1 = mean(z'), out = z' * (m0 / m1)   (out = z' where m1 == 0),
+// fp32 throughout; each thread sums a fixed stride of elements and the CTA adds the 8 warp sums in warp order, so a
+// chunk's bits depend on nothing but the chunk.  A chunk whose weights are all 1 is copied unchanged.
+__global__ void __launch_bounds__(kEmphasisThreads)
+prompt_emphasis_kernel(const uint4* __restrict__ h1, const uint4* __restrict__ h2, const float* __restrict__ w1,
+                       const float* __restrict__ w2, const int* __restrict__ entries, uint4* __restrict__ out, int L,
+                       int C1, int C2) {
+  __shared__ float red[2][kEmphasisThreads / 32];
+  const int e = blockIdx.x, enc = blockIdx.y, tid = threadIdx.x;
+  const int src = entries[3 * e + enc], dst = entries[3 * e + 2];
+  const int cv = (enc ? C2 : C1) >> 3;
+  const int ldo = (C1 + C2) >> 3;
+  const uint4* z = (enc ? h2 : h1) + static_cast<long long>(src) * L * cv;
+  const float* w = (enc ? w2 : w1) + static_cast<long long>(src) * L;
+  uint4* o = out + static_cast<long long>(dst) * L * ldo + (enc ? C1 >> 3 : 0);
+  bool ones = true;
+  for (int t = tid; t < L; t += kEmphasisThreads) ones &= w[t] == 1.0f;
+  const int n = L * cv;
+  if (__syncthreads_and(ones)) {
+    for (int i = tid; i < n; i += kEmphasisThreads) {
+      const int t = i / cv;
+      o[static_cast<long long>(t) * ldo + (i - t * cv)] = __ldg(z + i);
+    }
+    return;
+  }
+  float s0 = 0.f, s1 = 0.f;
+  for (int i = tid; i < n; i += kEmphasisThreads) {
+    const float wt = w[i / cv];
+    const uint4 u = __ldg(z + i);
+    const uint32_t q[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float a = bf16_lo(q[k]), b = bf16_hi(q[k]);
+      s0 += a;
+      s0 += b;
+      s1 += __fmul_rn(a, wt);
+      s1 += __fmul_rn(b, wt);
+    }
+  }
+  s0 = warp_sum(s0);
+  s1 = warp_sum(s1);
+  if ((tid & 31) == 0) {
+    red[0][tid >> 5] = s0;
+    red[1][tid >> 5] = s1;
+  }
+  __syncthreads();
+  float t0 = 0.f, t1 = 0.f;
+#pragma unroll
+  for (int k = 0; k < kEmphasisThreads / 32; ++k) {
+    t0 += red[0][k];
+    t1 += red[1][k];
+  }
+  const float count = static_cast<float>(n) * 8.0f;
+  const float m0 = t0 / count, m1 = t1 / count;
+  const bool guard = m1 == 0.0f;
+  const float ratio = guard ? 1.0f : m0 / m1;
+  for (int i = tid; i < n; i += kEmphasisThreads) {
+    const int t = i / cv;
+    const float wt = w[t];
+    const uint4 u = __ldg(z + i);
+    const uint32_t q[4] = {u.x, u.y, u.z, u.w};
+    uint32_t r[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float a = __fmul_rn(bf16_lo(q[k]), wt), b = __fmul_rn(bf16_hi(q[k]), wt);
+      r[k] = guard ? pack_bf16(a, b) : pack_bf16(__fmul_rn(a, ratio), __fmul_rn(b, ratio));
+    }
+    o[static_cast<long long>(t) * ldo + (i - t * cv)] = make_uint4(r[0], r[1], r[2], r[3]);
+  }
+}
+
 }  // namespace ds
+
+extern "C" int ds_prompt_emphasis(const void* h1, const void* h2, const float* w1, const float* w2,
+                                  const int* entries, int n_entries, int L, int C1, int C2, void* out, void* stream) {
+  using namespace ds;
+  DS_REQUIRE(h1 && h2 && w1 && w2 && entries && out, "ds_prompt_emphasis: NULL pointer");
+  DS_REQUIRE(n_entries > 0 && L > 0 && C1 > 0 && C2 > 0 && C1 % 8 == 0 && C2 % 8 == 0,
+             "ds_prompt_emphasis: bad shape (n_entries, L > 0; C1, C2 > 0 and multiples of 8)");
+  DS_REQUIRE(n_entries <= 0x7fffffff / 3, "ds_prompt_emphasis: too many entries");
+  DS_REQUIRE((reinterpret_cast<uintptr_t>(h1) & 15) == 0 && (reinterpret_cast<uintptr_t>(h2) & 15) == 0 &&
+                 (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (reinterpret_cast<uintptr_t>(w1) & 3) == 0 &&
+                 (reinterpret_cast<uintptr_t>(w2) & 3) == 0 && (reinterpret_cast<uintptr_t>(entries) & 3) == 0,
+             "ds_prompt_emphasis: h1 / h2 / out must be 16-byte aligned, w1 / w2 / entries 4-byte aligned");
+  DeviceInfo dev;
+  if (!get_device(&dev)) return DS_ERR_CUDA;
+  prompt_emphasis_kernel<<<dim3(n_entries, 2), kEmphasisThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint4*>(h1), static_cast<const uint4*>(h2), w1, w2, entries, static_cast<uint4*>(out), L, C1,
+      C2);
+  DS_LAUNCH_OK("prompt_emphasis_kernel");
+  return DS_OK;
+}
 
 extern "C" int ds_attention_small(const void* q, const void* k, const void* v, void* out, int B, int Nq, int Nk,
                                   int heads, int head_dim, int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo,

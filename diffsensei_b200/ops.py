@@ -837,6 +837,37 @@ def embed_tokens(ids: torch.Tensor, tok_emb: torch.Tensor, pos_emb: torch.Tensor
     return out
 
 
+def prompt_emphasis(h1: torch.Tensor, h2: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, entries,
+                    chunks: int) -> torch.Tensor:
+    """Weighted prompt chunks into one concatenated embedding (ds_prompt_emphasis, AUTOMATIC1111's "Original"
+    emphasis): ``h1`` / ``h2`` bf16 [n1, L, C1] / [n2, L, C2] are the text encoders' ``hidden_states[-2]`` rows,
+    ``w1`` / ``w2`` fp32 [n1, L] / [n2, L] their per-token weights, ``entries`` (host ints, [E, 3]) one
+    (row of h1, row of h2, destination chunk) per output chunk.  Returns bf16 [chunks, L, C1 + C2]: chunk d holds
+    ``z' * mean(z) / mean(z')`` (``z' = z * w``) of its two rows side by side; a chunk no entry names stays
+    uninitialised."""
+    _req(h1, bf16, "prompt_emphasis.h1", 3)
+    _req(h2, bf16, "prompt_emphasis.h2", 3)
+    _req(w1, f32, "prompt_emphasis.w1", 2)
+    _req(w2, f32, "prompt_emphasis.w2", 2)
+    n1, L, C1 = h1.shape
+    n2, _, C2 = h2.shape
+    if h2.shape[1] != L or tuple(w1.shape) != (n1, L) or tuple(w2.shape) != (n2, L):
+        raise DsEngineError(f"prompt_emphasis: h1 {tuple(h1.shape)} / h2 {tuple(h2.shape)} / w1 {tuple(w1.shape)} / "
+                            f"w2 {tuple(w2.shape)} must be [n1, L, C1] / [n2, L, C2] / [n1, L] / [n2, L]")
+    table = torch.as_tensor(entries, dtype=torch.int32).reshape(-1, 3)
+    if table.shape[0] == 0 or table.device.type != "cpu":
+        raise DsEngineError("prompt_emphasis: entries must be a non-empty host table of (row 1, row 2, chunk)")
+    for col, hi, nm in ((0, n1, "row of h1"), (1, n2, "row of h2"), (2, int(chunks), "destination chunk")):
+        c = table[:, col]
+        if int(c.min()) < 0 or int(c.max()) >= hi:
+            raise DsEngineError(f"prompt_emphasis: entries' {nm} out of range [0, {hi})")
+    out = torch.empty(int(chunks), L, C1 + C2, dtype=bf16, device=h1.device)
+    dev_table = table.to(h1.device, non_blocking=False)
+    check(lib.ds_prompt_emphasis(h1.data_ptr(), h2.data_ptr(), w1.data_ptr(), w2.data_ptr(), dev_table.data_ptr(),
+                                 table.shape[0], L, C1, C2, out.data_ptr(), _stream()), "ds_prompt_emphasis")
+    return out
+
+
 # ---------------------------------------------------------------------------------------------- LLaMA decoder (agent)
 def gemv(x: torch.Tensor, w: torch.Tensor, residual: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
          out_fp32: bool = False) -> torch.Tensor:

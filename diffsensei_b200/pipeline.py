@@ -48,6 +48,7 @@ from . import callbacks, ops
 from .image_processor import (CLIPImageProcessor, VaeImageProcessor, ViTImageProcessor, adapter_image_info,
                               adapter_image_u8)
 from .lora import AdapterRegistry, lora_targets, normalize_lora, split_components
+from .prompt_weighting import plain_text, tokenize_chunks
 from .regions import NEGATIVE_KEYS, box_cover, check_regions, cover_byte, region_rows
 from .scheduler import DDIMScheduler, EulerDiscreteScheduler, get_timesteps, pag_scales, step_table, with_pag_column
 from .tiles import TILE_OVERLAP, TileGrid, check_tiles
@@ -67,7 +68,10 @@ PANEL_KEYS = frozenset({
     "dialog_bbox", "prompt_embeds", "negative_prompt_embeds", "pooled_prompt_embeds", "negative_pooled_prompt_embeds",
     "prompt_input_ids", "prompt_input_ids_2", "negative_prompt_input_ids", "negative_prompt_input_ids_2", "image",
     "mask_image", "padding_mask_crop", "adapter_image", "adapter_conditioning_scale", "tile_size", "tile_overlap",
-    "regions"})
+    "regions", "prompt_weighting"})
+# what prompt_weighting=True replaces: the embeddings and token ids of a panel's or a region's texts
+WEIGHTING_EXCLUDES = ("prompt_embeds", "negative_prompt_embeds", "pooled_prompt_embeds", "negative_pooled_prompt_embeds",
+                      "prompt_input_ids", "prompt_input_ids_2", "negative_prompt_input_ids", "negative_prompt_input_ids_2")
 PAGE_MAX_ROWS = 8       # samples per page denoise: a UNet batch of 16 rows, as __call__(num_samples=8)
 
 
@@ -665,6 +669,8 @@ class DiffSenseiPipeline:
                  tile_size=None, tile_overlap: int = TILE_OVERLAP,
                  # MultiDiffusion's region-based generation: [{"prompt": ..., "box": [x1, y1, x2, y2] or "mask": ...}]
                  regions=None,
+                 # AUTOMATIC1111's prompt emphasis "(word:1.3)" / "[word]" and prompts past 75 tokens (BREAK, chunks)
+                 prompt_weighting: bool = False,
                  # diffusers' per-step hook: callback(pipe, i, t, {"latents": ...}); pipe._interrupt = True stops
                  callback_on_step_end=None, callback_on_step_end_tensor_inputs=["latents"]):
         """A page of one panel: ``generate_page([panel], ...)[0]``, the panel holding this call's per-panel keywords
@@ -817,6 +823,11 @@ class DiffSenseiPipeline:
         views averages their updated latents on the canvas before the inpaint blend.  A tiled panel is a denoise of its own; its
         noise, image and mask are canvas-sized as untiled, and the canvas is decoded whole.
 
+        A panel with ``prompt_weighting=True`` reads its prompts (negatives and regions' included) with AUTOMATIC1111's
+        emphasis syntax and in 77-token chunks past 75 tokens (``prompt_weighting.py``): all its chunks join the page's
+        text-encoder calls, one ``ds_prompt_emphasis`` launch weights them, and every text of the panel is padded to its
+        chunk count k with the empty prompt's chunk; panels share a denoise only at the same 77 k text tokens.
+
         ``callback_on_step_end`` (diffusers' contract) is called as ``callback(pipe, i, t, callback_kwargs)`` after each
         step of every chunk's denoise, after the scheduler update and the inpaint blend; ``i`` counts the steps that
         denoise runs from 0, ``callback_kwargs["latents"]`` holds the chunk's fp32 NCHW latents (a tiled panel's whole
@@ -867,11 +878,18 @@ class DiffSenseiPipeline:
             if j.regions:
                 j.cover = self._region_cover(j)
         texts = jobs + [r for j in jobs for r in j.regions]          # the panels' prompts, then their regions'
+        weighted = [j for j in texts if j.chunks is not None]
+        chunk_ids = self._chunk_rows(weighted) if weighted else None   # every chunk of the page, one row each
         text = _stacked(lambda ids: (self.text_encoder(ids, output_hidden_states=True).hidden_states[-2],),
-                        [x for j in texts if j.ids is not None for x in (j.ids[0], j.ids[2]) if x is not None])
+                        [x for j in texts if j.ids is not None for x in (j.ids[0], j.ids[2]) if x is not None] +
+                        ([chunk_ids[0]] if weighted else []))
         text_2 = _stacked(lambda ids: (lambda o: (o.hidden_states[-2], o[0]))(
                           self.text_encoder_2(ids, output_hidden_states=True)),
-                          [x for j in texts if j.ids is not None for x in (j.ids[1], j.ids[3]) if x is not None])
+                          [x for j in texts if j.ids is not None for x in (j.ids[1], j.ids[3]) if x is not None] +
+                          ([chunk_ids[1]] if weighted else []))
+        if weighted:
+            (h1,), (h2, pooled) = text.pop(), text_2.pop()
+            self._emphasis(weighted, h1, h2, pooled, chunk_ids[2], chunk_ids[3])
         for j in texts:
             if j.ids is None:
                 continue
@@ -915,7 +933,9 @@ class DiffSenseiPipeline:
             (() if j.adapter_feats is None else ("adapter",))
         # a tiled panel, and a panel with regions, is a denoise of its own
         alone = lambda i: () if jobs[i].tiles is None and not jobs[i].regions else (("alone", i),)
-        shapes = [(j.ns,) + tuple(j.latents.shape[-2:]) + kind(j) + alone(i) for i, j in enumerate(jobs)]
+        # panels share a denoise only at one text length (prompt weighting and long prompt_embeds make it vary)
+        shapes = [(j.ns,) + tuple(j.latents.shape[-2:]) + kind(j) + alone(i) + (int(j.pe.shape[1]),)
+                  for i, j in enumerate(jobs)]
         for chunk in plan_page(shapes, max_batch_panels):
             tiles, regions = jobs[chunk[0]].tiles, jobs[chunk[0]].regions
             rows = [self._tile_rows(jobs[i]) if tiles is not None else self._region_rows(jobs[i]) if regions else
@@ -1001,6 +1021,7 @@ class DiffSenseiPipeline:
         only (tokenization included), so a bad panel fails before any GPU work."""
         g = lambda k, d=None: p.get(k, d)
         height, width = g("height"), g("width")
+        weighted = self._check_weighting(g)
         if g("mask_image") is not None and g("image") is None:
             raise ValueError("`mask_image` needs `image`: inpainting redraws the masked part of that image")
         if g("tile_size") is not None:
@@ -1059,7 +1080,8 @@ class DiffSenseiPipeline:
             if any(g(k) is not None for k in ("clip_pixel_values", "magi_pixel_values", "clip_image_embeds",
                                               "magi_image_embeds")):
                 raise ValueError("`ip_images` and pixel values / image embeddings can not be input together!")
-        ids = self._prompt_ids(g, ip_images, ip_image_embeds, ip_bbox)
+        ids = self._prompt_ids(g, ip_images, ip_image_embeds, ip_bbox, weighted)
+        region_jobs = [] if regions is None else self._region_jobs(regions, weighted)
         m = self.unet.cfg.max_num_ips
         clip_pv = magi_pv = None
         n_real = 0
@@ -1084,11 +1106,19 @@ class DiffSenseiPipeline:
         if num_ips != len(ip_bbox):
             raise ValueError(f"`ip_images` must have the same length as `ip_bbox`. But they are in length "
                              f"{num_ips} and {len(ip_bbox)}!")
+        chunks, k = None, 0
+        if weighted:        # every text of the panel is padded to the panel's chunk count
+            chunks, ids = ids, None
+            k = max(len(side[e][0]) for c in [chunks] + [r.chunks for r in region_jobs] for side in c
+                    if side is not None for e in range(2))
+            for r in region_jobs:
+                r.k = k
         return SimpleNamespace(
             ns=int(g("num_samples", 1)), height=height, width=width, generator=g("generator"), latents=g("latents"),
-            ids=ids, image=g("image"), mask_image=g("mask_image"), inpaint=None, crop=crop, mask_l=mask_l,
+            ids=ids, chunks=chunks, k=k, image=g("image"), mask_image=g("mask_image"), inpaint=None, crop=crop,
+            mask_l=mask_l,
             adapter_image=ad_image, adapter_scale=float(ad_scale), adapter_float=ad_image is not None and ad_float,
-            adapter_feats=None, tiles=tiles, regions=[] if regions is None else self._region_jobs(regions),
+            adapter_feats=None, tiles=tiles, regions=region_jobs,
             pe=g("prompt_embeds"), npe=g("negative_prompt_embeds"), pp=g("pooled_prompt_embeds"),
             npp=g("negative_pooled_prompt_embeds"), ip_images=ip_images, clip_pv=clip_pv, magi_pv=magi_pv,
             clip=g("clip_image_embeds"), magi=g("magi_image_embeds"), ip_image_embeds=ip_image_embeds,
@@ -1096,16 +1126,32 @@ class DiffSenseiPipeline:
             time_ids=list(g("original_size") or (height, width)) + list(g("crops_coords_top_left", (0, 0))) +
             list(g("target_size") or (height, width)))                   # _get_add_time_ids
 
-    def _prompt_ids(self, g, ip_images=(), ip_image_embeds=None, ip_bbox=()):
+    @staticmethod
+    def _check_weighting(g) -> bool:
+        """``prompt_weighting`` read with ``g(key)``: a bool, else ``ValueError`` naming the key."""
+        pw = g("prompt_weighting", False)
+        if not isinstance(pw, bool):
+            raise ValueError(f"`prompt_weighting` must be a bool, got {pw!r}")
+        return pw
+
+    def _prompt_ids(self, g, ip_images=(), ip_image_embeds=None, ip_bbox=(), weighted: bool = False):
         """The token ids of a panel's (or a region's) prompt keys, read with ``g(key)``: None when ``prompt_embeds``
         is given, else (ids, ids_2, negative_ids, negative_ids_2) from the strings (tokenized) or the ids, int64
-        tensors, the negatives None or both set.  Host only; raises as ``__call__`` does when neither can be
-        encoded."""
+        tensors, the negatives None or both set.  ``weighted`` (prompt weighting): the strings' chunks instead,
+        [positive, negative], each side ((ids, weights) under ``tokenizer``, (ids, weights) under ``tokenizer_2``)
+        (``prompt_weighting.tokenize_chunks``), the negative None without ``negative_prompt``.  Host only; raises as
+        ``__call__`` does when neither can be encoded."""
+        if weighted:
+            for k in WEIGHTING_EXCLUDES:
+                if g(k) is not None:
+                    raise ValueError(f"`prompt_weighting` can not be combined with `{k}`")
         if g("prompt_embeds") is not None:
             return None
         ids = None
         if g("prompt_input_ids") is None and isinstance(g("prompt"), str) and \
                 self.tokenizer is not None and self.tokenizer_2 is not None:
+            if weighted:
+                return self._prompt_chunks(g("prompt"), g("prompt_2"), g("negative_prompt"), g("negative_prompt_2"))
             ids = self.tokenize_prompt(g("prompt"), g("prompt_2"), g("negative_prompt"), g("negative_prompt_2"))
         elif g("prompt_input_ids") is not None:
             ids = (g("prompt_input_ids"), g("prompt_input_ids_2"), g("negative_prompt_input_ids"),
@@ -1122,7 +1168,63 @@ class DiffSenseiPipeline:
         return (as_ids(ids[0]), as_ids(ids[1] if ids[1] is not None else ids[0]), as_ids(ids[2]),
                 None if ids[2] is None else as_ids(ids[3] if ids[3] is not None else ids[2]))
 
-    def _region_jobs(self, regions) -> List[SimpleNamespace]:
+    def _prompt_chunks(self, prompt: str, prompt_2=None, negative_prompt=None, negative_prompt_2=None):
+        """``tokenize_prompt``'s defaults with prompt weighting: [positive, negative] chunks (``_prompt_ids``)."""
+        for name, p in (("prompt_2", prompt_2), ("negative_prompt", negative_prompt),
+                        ("negative_prompt_2", negative_prompt_2)):
+            if p is not None and not isinstance(p, str):
+                raise ValueError(f"`{name}` has to be of type `str` but is {type(p)}")
+        if self.text_encoder is None or self.text_encoder_2 is None:
+            raise ValueError("encode_prompt_ids needs text_encoder and text_encoder_2 engines")
+        side = lambda a, b: (tokenize_chunks(self.tokenizer, a), tokenize_chunks(self.tokenizer_2, b or a))
+        return [side(prompt, prompt_2), None if negative_prompt is None else side(negative_prompt, negative_prompt_2)]
+
+    def _chunk_rows(self, weighted):
+        """The encoder inputs of every chunk of the page's weighted texts (``chunks``), then the empty prompt's chunk,
+        the padding of texts with fewer chunks than their panel.  Sets each text's ``rows``: per side, None or the
+        first row of its chunks under each encoder.  Returns (ids, ids_2) int64 [n, 77] (host) and (weights,
+        weights_2) fp32 [n, 77] (device)."""
+        ids, ws = ([], []), ([], [])
+        for j in weighted:
+            j.rows = []
+            for side in j.chunks:
+                j.rows.append(None if side is None else (len(ids[0]), len(ids[1])))
+                for e in range(2 if side is not None else 0):
+                    ids[e].extend(side[e][0])
+                    ws[e].extend(side[e][1])
+        for e, tok in enumerate((self.tokenizer, self.tokenizer_2)):
+            i, w = tokenize_chunks(tok, "")
+            ids[e].extend(i)
+            ws[e].extend(w)
+        dev = self.unet.device
+        return (torch.tensor(ids[0]), torch.tensor(ids[1]), torch.tensor(ws[0], dtype=f32, device=dev),
+                torch.tensor(ws[1], dtype=f32, device=dev))
+
+    def _emphasis(self, weighted, h1, h2, pooled, w1, w2) -> None:
+        """Every weighted text's embeddings from its encoded chunks (``_chunk_rows``), in one ``ds_prompt_emphasis``
+        launch: ``pe`` [1, 77 k, C1 + C2] with chunk c at tokens 77 c .. 77 c + 76 (the empty prompt's chunk past the
+        text's own), ``pp`` the second encoder's pooled output of chunk 0 (unweighted, as AUTOMATIC1111); no negative
+        gives zeros at the positive's shape (``force_zeros_for_empty_prompt``)."""
+        empty = (h1.shape[0] - 1, h2.shape[0] - 1)
+        entries = []
+        for j in weighted:
+            for side, rows in zip(j.chunks, j.rows):
+                if side is not None:
+                    n, d = (len(side[0][0]), len(side[1][0])), len(entries)
+                    entries += [tuple(rows[e] + c if c < n[e] else empty[e] for e in range(2)) + (d + c,)
+                                for c in range(j.k)]
+        out = ops.prompt_emphasis(h1, h2, w1, w2, entries, len(entries))
+        d = 0
+        for j in weighted:
+            embeds = []
+            for side, rows in zip(j.chunks, j.rows):
+                embeds.append(None if side is None else
+                              (out[d:d + j.k].reshape(1, -1, out.shape[-1]), pooled[rows[1]:rows[1] + 1]))
+                d += 0 if side is None else j.k
+            (j.pe, j.pp), neg = embeds
+            j.npe, j.npp = (torch.zeros_like(j.pe), torch.zeros_like(j.pp)) if neg is None else neg
+
+    def _region_jobs(self, regions, weighted: bool = False) -> List[SimpleNamespace]:
         """The checked ``regions`` of a panel (``regions.check_regions``) with their prompts resolved by the panel's
         code (``_prompt_ids``); host only.  A region without any negative key takes the panel's negative conditioning
         (``own_negative`` False: ``_run_page`` copies it once the panel's is encoded)."""
@@ -1130,11 +1232,11 @@ class DiffSenseiPipeline:
         for k, r in enumerate(regions):
             g = lambda key, d=None: r.get(key, d)
             try:
-                ids = self._prompt_ids(g)
+                ids = self._prompt_ids(g, weighted=weighted)
             except (ValueError, NotImplementedError) as e:
                 raise type(e)(f"region {k}: {e}") from e
             out.append(SimpleNamespace(
-                ids=ids, pe=g("prompt_embeds"), npe=g("negative_prompt_embeds"), pp=g("pooled_prompt_embeds"),
+                ids=None if weighted else ids, chunks=ids if weighted else None, k=0, pe=g("prompt_embeds"), npe=g("negative_prompt_embeds"), pp=g("pooled_prompt_embeds"),
                 npp=g("negative_pooled_prompt_embeds"), box=g("box"), mask=g("mask"),
                 own_negative=any(g(key) is not None for key in NEGATIVE_KEYS)))
         return out
@@ -1354,7 +1456,8 @@ class DiffSenseiPipeline:
         chars = [(clip[k * m:(k + 1) * m].unsqueeze(0), magi[k * m:(k + 1) * m].unsqueeze(0), None)
                  for k in range(len(panels))]
         embeds = [img[:, nv:, :] for img, _ in self._character_embeds(chars)]         # gradio.py:96-97
-        prompts = [mllm_inputs(p["prompt"], tokenizer_mllm) for p in panels]
+        prompts = [mllm_inputs(plain_text(p["prompt"]) if p.get("prompt_weighting") else p["prompt"], tokenizer_mllm)
+                   for p in panels]
         outs = agent.generate_batch(tokenizer=tokenizer_mllm, input_ids=[ids[None] for ids, _ in prompts],
                                     image_embeds=embeds, ids_cmp_mask=[mask[None] for _, mask in prompts],
                                     max_new_tokens=max_new_tokens,

@@ -499,12 +499,24 @@ int ds_attention_single_head(const void* q, const void* k, const void* v, void* 
  *                        causal != 0: key j visible from query i iff j <= i (CLIP text), needs Nq == Nk.
  *   ds_embed_tokens    : out[b][t][:] = tok_emb[ids[b][t]][:] + pos_emb[t][:], bf16, ids int32 [B][L] (clamped to
  *                        the vocabulary) — CLIPTextEmbeddings.
+ *   ds_prompt_emphasis : AUTOMATIC1111's "Original" prompt emphasis, per chunk and encoder, into the concatenated
+ *                        prompt embedding.  h1 / h2: bf16 [n1][L][C1] / [n2][L][C2] (each text encoder's
+ *                        hidden_states[-2] rows), w1 / w2: fp32 [n1][L] / [n2][L] per-token weights, entries: int32
+ *                        [n_entries][3] = {row of h1, row of h2, destination chunk d} (device memory, rows in range:
+ *                        the caller checks them), out: bf16 [>= d + 1][L][C1 + C2].  For each entry and encoder, in
+ *                        fp32: m0 = mean(z), z' = z * w[:, None], m1 = mean(z'), and columns [0, C1) (encoder 1) or
+ *                        [C1, C1 + C2) (encoder 2) of out chunk d get z' * (m0 / m1), or z' where m1 == 0 (the
+ *                        weighting would otherwise give NaN).  The means are sums in a fixed order over the chunk
+ *                        alone; a chunk whose weights are all 1 is copied unchanged.  C1, C2 multiples of 8; h1, h2,
+ *                        out 16-byte aligned.
  * --------------------------------------------------------------------------------------------- */
 int ds_attention_small(const void* q, const void* k, const void* v, void* out, int B, int Nq, int Nk, int heads,
                        int head_dim, int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo, float scale, int causal,
                        void* stream);
 int ds_embed_tokens(const int* ids, const void* tok_emb, const void* pos_emb, void* out, int B, int L, int C, int vocab,
                     void* stream);
+int ds_prompt_emphasis(const void* h1, const void* h2, const float* w1, const float* w2, const int* entries,
+                       int n_entries, int L, int C1, int C2, void* out, void* stream);
 
 /* Image processors of prepare_ip_image_embeds (src/pipelines/pipeline_diffsensei.py:70-71,125-126: transformers'
  * CLIPImageProcessor / ViTImageProcessor, shipped defaults, PIL backend), bit-exact:
