@@ -39,11 +39,17 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 
 // bf16 pack on the INTEGER pipe: round-half-up on the 16 dropped mantissa bits (differs from RNE only on exact
 // ties, no bias that matters) + one PRMT, instead of cvt.rn.bf16x2.f32, which issues at the lower XU rate.
-// Inf stays Inf, NaN stays NaN; finite inputs only lose <= 0.5 ulp(bf16).
+// Finite inputs lose <= 0.5 ulp(bf16), except that those from half a bf16 ulp below 2^128 up round to +-Inf, as RNE
+// does.  +-Inf stay +-Inf.  A NaN is not rounded but truncated with its quiet bit set, so it stays a NaN of the same sign:
+// adding 0x8000 would carry a payload whose top mantissa bits are all ones into the exponent and the sign (the
+// 0x7FFFFFFF that fp32 arithmetic produces on sm_90 would pack to -0.0), and would turn a NaN whose payload lies in
+// the low 16 bits into Inf.  The NaN test is one FSETP; the integer form of it (mask, compare) costs one op more.
+__device__ __forceinline__ uint32_t bf16_bits_alu(float f) {
+  const uint32_t u = __float_as_uint(f);
+  return f != f ? (u | 0x00400000u) : u + 0x8000u;
+}
 __device__ __forceinline__ uint32_t pack_bf16_alu(float lo, float hi) {
-  const uint32_t a = __float_as_uint(lo) + 0x8000u;
-  const uint32_t b = __float_as_uint(hi) + 0x8000u;
-  return __byte_perm(a, b, 0x7632);  // {b.hi16, a.hi16}
+  return __byte_perm(bf16_bits_alu(lo), bf16_bits_alu(hi), 0x7632);  // {hi.hi16, lo.hi16}
 }
 
 // Items of a per-(sample, channel) reduction (gn_plan, ds_host.h): a launch has exactly one resident wave of CTAs
@@ -138,8 +144,11 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
 // ----------------------------------------------------------------------------------------------
 // x * sigmoid(x) with two MUFU ops (ex2 + rcp) instead of a full-precision divide
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
-// x * sigmoid(x) = 0.5 x (1 + tanh(x/2)) with ONE MUFU op (tanh.approx, abs err ~5e-4 on tanh => |err| <= 2.5e-4 |x|,
-// below the bf16 rounding of the result for |x| < 16).  Used where the op is otherwise XU-bound (GroupNorm apply).
+// x * sigmoid(x) = 0.5 x (1 + tanh(x/2)) with ONE MUFU op.  tanh.approx.f32 is documented to 2^-10.987 (~5e-4), so
+// |err| <= 2.5e-4 |x|.  That is below the bf16 rounding of the result (~2^-9 |silu(x)|) for x >= -1.5, but not
+// further down, where silu(x) -> 0 faster than |x|: at x = -6 silu is -0.0148 and the bound 1.5e-3, ~10 % or
+// some 25 bf16 ulps (tests/groupnorm_check.py carries it as its own term).  Used where the op is otherwise XU-bound
+// (GroupNorm apply).
 __device__ __forceinline__ float silu_tanh_f(float x) {
   float t;
   asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * x));

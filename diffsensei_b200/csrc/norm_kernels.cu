@@ -126,10 +126,11 @@ __global__ void chan_stats_kernel(const uint4* __restrict__ x, double* __restric
 // GroupNorm(+SiLU) apply from per-channel statistics; x = [x1 | x2] along channels (x2 may be NULL).
 // kU = independent 16-byte loads in flight per thread.
 template <bool kSilu, int kU>
-__global__ void gn_apply2_kernel(const uint4* __restrict__ x1, const uint4* __restrict__ x2, uint4* __restrict__ y,
-                                 const double* __restrict__ st1, const double* __restrict__ st2,
-                                 const float* __restrict__ gamma, const float* __restrict__ beta, int HW, int C1, int C2,
-                                 int groups, float eps, int items_per_sample, int ipx, int total_items) {
+__device__ __forceinline__ void gn_apply2_body(const uint4* __restrict__ x1, const uint4* __restrict__ x2,
+                                               uint4* __restrict__ y, const double* __restrict__ st1,
+                                               const double* __restrict__ st2, const float* __restrict__ gamma,
+                                               const float* __restrict__ beta, int HW, int C1, int C2, int groups,
+                                               float eps, int items_per_sample, int ipx, int total_items) {
   extern __shared__ double shd[];  // [C][2] channel sums of the current sample, then [groups][2] {mean, rstd}
   const int C = C1 + C2;
   const int cv = C >> 3, cv1 = C1 >> 3;
@@ -239,6 +240,26 @@ __global__ void gn_apply2_kernel(const uint4* __restrict__ x1, const uint4* __re
     }
     for (; p < p1; p += rpb) yb[static_cast<size_t>(p) * cv] = norm8(ldg_hint(xb + static_cast<size_t>(p) * scv, pol));
   }
+}
+
+template <bool kSilu, int kU>
+__global__ void gn_apply2_kernel(const uint4* __restrict__ x1, const uint4* __restrict__ x2, uint4* __restrict__ y,
+                                 const double* __restrict__ st1, const double* __restrict__ st2,
+                                 const float* __restrict__ gamma, const float* __restrict__ beta, int HW, int C1, int C2,
+                                 int groups, float eps, int items_per_sample, int ipx, int total_items) {
+  gn_apply2_body<kSilu, kU>(x1, x2, y, st1, st2, gamma, beta, HW, C1, C2, groups, eps, items_per_sample, ipx,
+                            total_items);
+}
+// Blocks of more than 512 threads (C > 4096): gn_apply2_kernel takes ~128 registers, and 65536 / 128 = 512 threads
+// exhaust the register file, so such a launch would fail.  This form is held to 64 registers, with 4 loads in flight.
+template <bool kSilu>
+__global__ void __launch_bounds__(1024)
+    gn_apply2_wide_kernel(const uint4* __restrict__ x1, const uint4* __restrict__ x2, uint4* __restrict__ y,
+                          const double* __restrict__ st1, const double* __restrict__ st2,
+                          const float* __restrict__ gamma, const float* __restrict__ beta, int HW, int C1, int C2,
+                          int groups, float eps, int items_per_sample, int ipx, int total_items) {
+  gn_apply2_body<kSilu, 4>(x1, x2, y, st1, st2, gamma, beta, HW, C1, C2, groups, eps, items_per_sample, ipx,
+                           total_items);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -367,9 +388,11 @@ extern "C" int ds_groupnorm_apply(const void* x1, const double* stats1, int C1, 
   GnPlan pl;
   DS_REQUIRE(gn_plan(B, HW, C, kGnApplyThreads, kGnUnroll, &pl), "ds_groupnorm_apply: tensor too large");
   const size_t smem = static_cast<size_t>(C) * 2 * sizeof(double) + static_cast<size_t>(groups) * 2 * sizeof(float);
-  auto* fn = apply_silu ? gn_apply2_kernel<true, kGnUnroll> : gn_apply2_kernel<false, kGnUnroll>;
-  static size_t attr[kMaxDevices][2] = {};
-  size_t& a = attr[device_slot()][apply_silu ? 1 : 0];
+  const bool wide = pl.threads > 512;
+  auto* fn = wide ? (apply_silu ? gn_apply2_wide_kernel<true> : gn_apply2_wide_kernel<false>)
+                  : (apply_silu ? gn_apply2_kernel<true, kGnUnroll> : gn_apply2_kernel<false, kGnUnroll>);
+  static size_t attr[kMaxDevices][4] = {};
+  size_t& a = attr[device_slot()][(wide ? 2 : 0) + (apply_silu ? 1 : 0)];
   if (smem > 48 * 1024 && smem > a) {
     DS_CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     a = smem;
