@@ -3,9 +3,10 @@
 // norm_kernels.cu / glue_kernels.cu):
 //   ds_latent_pointwise : latents / scaling_factor -> post_quant_conv (1x1, 4 -> 4) -> NHWC bf16
 //                         (src/pipelines/pipeline_diffsensei.py:346-361; diffusers AutoencoderKL.decode)
-//   ds_softmax_rows     : P = softmax(scale * S) row-wise, fp32 scores in, bf16 probabilities out — the mid-block
-//                         attention of the decoder has ONE head of width 512 over all H*W tokens (no flash kernel for
-//                         that head size: QK^T and PV run as plain wgmma GEMMs with this kernel between them)
+//   ds_softmax_rows     : P = softmax(scale * S) row-wise, fp32 scores in, bf16 probabilities out.  The decoder's
+//                         mid-block attention runs on ds_attention_single_head (vae_attention.cu); this kernel
+//                         remains only as the old QK^T GEMM -> softmax -> PV GEMM path that
+//                         tools/vae_attention_bench.py compares against
 //   ds_image_postprocess: (x / 2 + 0.5).clamp(0, 1), NHWC bf16 -> NCHW fp32 (VaeImageProcessor.postprocess/denormalize)
 // and one the encoder needs after its conv_out:
 //   ds_vae_posterior    : quant_conv (1x1, 8 -> 8) -> DiagonalGaussianDistribution sample / mode -> * scaling_factor

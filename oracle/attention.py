@@ -115,6 +115,20 @@ def attention_heads(q, k, v, heads: int, open_mask=None, dtype=torch.float64):
     return out
 
 
+def single_head_attention(q, k, v, dtype=torch.float64):
+    """ds_attention_single_head's operation: softmax(q k^T / sqrt(D)) v per image of q / k / v [B, N, D] ->
+    [B, N, D] in ``dtype`` on q's device; attention_heads(q, k, v, 1) in chunks of query rows, so that no [N, N]
+    matrix is live (at most 2^25 scores, 256 MiB in fp64, where the VAE's N reaches 65536)."""
+    B, n, d = q.shape
+    rows = max(1, (1 << 25) // k.shape[1])
+    out = torch.empty(B, n, d, dtype=dtype, device=q.device)
+    for b in range(B):
+        kb, vb = k[b].to(dtype), v[b].to(dtype)
+        for r in range(0, n, rows):
+            out[b, r:r + rows] = sdpa(q[b, r:r + rows].to(dtype), kb, vb)
+    return out
+
+
 def self_attention_abi(qkv, heads: int, dtype=torch.float64):
     """ds_attention_self's operation on its fused projection qkv [B, N, 3C] (q | k | v column blocks)."""
     c = qkv.shape[-1] // 3

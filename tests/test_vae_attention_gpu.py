@@ -1,6 +1,7 @@
-"""ds_attention_single_head — the VAE decoder's one-head attention of width 128 / 512 — against torch fp32, and the
-decoder / pipeline at latent sizes the old QK^T -> softmax_rows -> PV path refused (H*W not a multiple of 8, or more
-than 32768 tokens).  Bounds: kernel rel-L2 <= 1e-2 (BASELINE.md §3 per-op bound); decode as tests/test_vae_gpu.py."""
+"""ds_attention_single_head — the VAE decoder's one-head attention of width 128 / 512 — on strided views and bad
+arguments, and the decoder / pipeline at latent sizes the old QK^T -> softmax_rows -> PV path refused (H*W not a
+multiple of 8, or more than 32768 tokens).  Decode bounds as tests/test_vae_gpu.py.  The kernel's own values are
+checked per element against fp64 in tests/test_vae_attention_reference_gpu.py."""
 import numpy as np
 import pytest
 import torch
@@ -12,60 +13,12 @@ bf16, f32 = torch.bfloat16, torch.float32
 DEV = "cuda"
 
 
-def _ref(q, k, v):
-    """fp32 softmax(q k^T / sqrt(D)) v, in query-row chunks so no [N, N] matrix is built at large N."""
-    q, k, v = q.float(), k.float(), v.float()
-    D = q.shape[-1]
-    out = torch.empty_like(q)
-    rows = max(1, (1 << 28) // (4 * k.shape[1]))
-    for b in range(q.shape[0]):
-        for r in range(0, q.shape[1], rows):
-            s = q[b, r:r + rows] @ k[b].T * D ** -0.5
-            out[b, r:r + rows] = torch.softmax(s, dim=-1) @ v[b]
-    return out
-
-
 def _qkv(B, N, D, seed, q_scale=1.0):
     g = torch.Generator(device=DEV).manual_seed(seed)
     q = (torch.randn(B, N, D, generator=g, device=DEV) * q_scale).to(bf16)
     k = torch.randn(B, N, D, generator=g, device=DEV).to(bf16)
     v = torch.randn(B, N, D, generator=g, device=DEV).to(bf16)
     return q, k, v
-
-
-SHAPES = [(D, B, N) for D in (128, 512) for B in (1, 3) for N in (1, 7, 63, 64, 65, 1092, 1344, 3072, 16384)]
-SHAPES += [(512, 1, 34816), (512, 1, 65536)]
-
-
-@pytest.mark.parametrize("D,B,N", SHAPES)
-def test_kernel_matches_fp32(D, B, N):
-    from diffsensei_b200 import ops
-    torch.backends.cuda.matmul.allow_tf32 = False
-    q, k, v = _qkv(B, N, D, seed=N + D + B)
-    guard = 4096
-    buf = torch.full((B * N * D + guard,), 7.0, dtype=bf16, device=DEV)     # sentinel after the output
-    out = buf[:B * N * D].view(B, N, D)
-    ops.attention_single_head(q, k, v, out=out)
-    err = rel_l2(out, _ref(q, k, v))
-    assert err <= 1e-2, f"rel-L2 {err:.3e}"
-    assert bool((buf[B * N * D:] == 7.0).all()), "a row >= N was written"
-
-
-@pytest.mark.parametrize("D", [128, 512])
-def test_peaky_scores_rescale(D):
-    """Large-magnitude q: the row max moves up across many key tiles, so the online softmax rescales repeatedly."""
-    from diffsensei_b200 import ops
-    torch.backends.cuda.matmul.allow_tf32 = False
-    B, N = 2, 2500
-    q, k, v = _qkv(B, N, D, seed=11, q_scale=4.0)
-    # every query leans on one direction u and the keys lean on it more and more: scores rise by hundreds across the
-    # keys, so the running max is overtaken tile after tile
-    u = torch.randint(0, 2, (D,), generator=torch.Generator().manual_seed(12)).to(DEV).float() * 2 - 1
-    q = (q.float() + 8 * u).to(bf16)
-    k = (k.float() + torch.linspace(0, 3, N, device=DEV).view(1, N, 1) * u).to(bf16)
-    got = ops.attention_single_head(q, k, v)
-    err = rel_l2(got, _ref(q, k, v))
-    assert err <= 1e-2, f"rel-L2 {err:.3e}"
 
 
 @pytest.mark.parametrize("D", [128, 512])

@@ -68,11 +68,19 @@ def test_vae_helper_kernels():
         got = ops.softmax_rows(S.to(DEV), 0.37).float().cpu()
         want = torch.softmax(S * 0.37, dim=-1)
         assert rel_l2(got, want) < 5e-3 and torch.allclose(got.sum(-1), torch.ones(rows), atol=2e-2)
-    # latent_pointwise == (lat * inv_scale) through a 1x1 conv
-    lat, w, b = torch.randn(2, 4, 5, 7, generator=g), torch.randn(4, 4, generator=g), torch.randn(4, generator=g)
-    got = ops.latent_pointwise(lat.to(DEV), w.to(DEV), b.to(DEV), 1 / 0.13025).float().cpu()
-    want = torch.nn.functional.conv2d(lat / 0.13025, w.view(4, 4, 1, 1), b).permute(0, 2, 3, 1)
-    assert rel_l2(got, want) < 4e-3
+    # latent_pointwise == (lat * inv_scale) through a 1x1 conv, per element against fp64: z = lat * inv_scale and four
+    # fmaf per output round in fp32 (5 u of the sum of the terms' magnitudes, u = 2^-24), then one RNE bf16 rounding
+    # (2^-8 relative).  inv_scale enters as the fp32 the ABI takes.  B = 3 and 5 x 7 pixels: an odd H * W.
+    inv = float(torch.tensor(1 / 0.13025, dtype=f32))
+    lat, w, b = torch.randn(3, 4, 5, 7, generator=g) * 0.9, torch.randn(4, 4, generator=g), torch.randn(4, generator=g)
+    for bias in (b, None):
+        got = ops.latent_pointwise(lat.to(DEV), w.to(DEV), None if bias is None else bias.to(DEV), inv).cpu()
+        terms = lat.double().permute(0, 2, 3, 1)[..., None, :] * inv * w.double()             # [B, H, W, k, c]
+        bd = torch.zeros(4, dtype=torch.float64) if bias is None else bias.double()
+        want, mag = terms.sum(-1) + bd, terms.abs().sum(-1) + bd.abs()
+        assert got.dtype == bf16 and got.shape == (3, 5, 7, 4)
+        err, bound = (got.double() - want).abs(), 2.0 ** -8 * want.abs() + 5.5 * 2.0 ** -24 * mag
+        assert bool((err <= bound).all()), float((err / bound).max())
     # image_postprocess
     x = (torch.randn(2, 6, 5, 3, generator=g) * 1.5).to(bf16)
     got = ops.image_postprocess(x.to(DEV)).cpu()
